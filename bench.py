@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — training examples/sec of the xflow hot path on B200 (BASELINE.json metric).
+"""bench.py — training examples/sec of the xflow hot path on the H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workloads a,b,...] [--impl reference]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch per GPU: LRWorker::update / FMWorker::update (pull,
 forward, gradient, push) plus the server-side FTRL step it triggers.  The line's own numbers are the
@@ -23,6 +24,10 @@ GPUs (weak scaling: 65 536 rows per GPU, the id space stays what the config says
 
 --impl reference times only that CPU implementation (same rows per step, warm table, all host cores,
 key-range server shards in the in-process ps shim) and prints the same line with "impl": "reference".
+
+--dump-outputs DIR writes, per workload, what the device-resident timed path computed in its last step: the
+table rows it trained (every field) for a fixed, seeded sample of that step's keys, as DIR/<workload>_<field>.npy
+(float32).  The inputs depend only on the arguments, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -56,7 +61,8 @@ WORKLOADS = {
                  name="cfg5: FM k=16+FTRL, Zipf(1.05)-skewed ids in 1e8-feature space, 100 nnz/row, batch 65536 per GPU"),
 }
 MAIN = "headline_lr"
-RING = 8  # distinct batches cycled through (8 x 52 MB of keys > 126 MB L2; the tables are GBs)
+RING = 8  # distinct batches cycled through (8 x 52 MB of keys > 50 MB L2; the tables are GBs)
+DUMP_SAMPLE = 65536  # keys of the last timed batch whose rows --dump-outputs writes
 
 
 def load_peaks():
@@ -66,7 +72,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def config_of(wl, world):
@@ -137,6 +143,21 @@ class ClockSampler(threading.Thread):
         mhz = sorted(s[1] for s in win)
         return {"sm_mhz": float(mhz[len(mhz) // 2]) if mhz else None, "sm_max_mhz": float(self.max_mhz),
                 "reasons": sorted(seen), "samples": len(win)}
+
+
+def dump_outputs(out_dir, name, table, d_keys, world, rank, api):
+    """The rows of the keys of one trained batch: a seeded sample of its unique keys (this rank's shard only),
+    every field of the table exported as float32."""
+    keys = np.unique(d_keys.cpu().numpy().view(np.uint64))
+    keys = np.sort(np.random.default_rng(12345).choice(keys, min(DUMP_SAMPLE, keys.size), replace=False))
+    if world > 1:
+        keys = keys[np.array([api.shard_of(int(k), world) == rank for k in keys], bool)]
+    e = table.export(keys)
+    assert e["present"].all()
+    os.makedirs(out_dir, exist_ok=True)
+    fields = ("w", "nw", "zw") + (("v", "nv", "zv") if table.K else ())
+    for f in fields:
+        np.save(os.path.join(out_dir, "%s_%s.npy" % (name, f)), np.ascontiguousarray(e[f], np.float32))
 
 
 def make_ids(wl, seed, rows=B_ROWS):
@@ -356,6 +377,8 @@ def run_workload(name, wl, args, rank, world, local, comm, api, torch, stream, s
         st1 = tr.stats()
         launches = tr.launches() - l0
         sampler_windows = [(t_w0, t_w1)]
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, name, table, ring.dev[(args.warmup + args.steps - 1) % RING][1], world, rank, api)
         # ---------------- end-to-end, binary: page-locked host CSR of u32 ids, hashed on the device
         def one(i, addr):
             p = ring.pin[i % RING]
@@ -376,7 +399,7 @@ def run_workload(name, wl, args, rank, world, local, comm, api, torch, stream, s
         # ---------------- end-to-end, text (the headline e2e): what the reference arm does from its shard
         text = None
         if not args.no_text_e2e:
-            text = text_leg(api, tr, wl, rank, max(3, min(args.steps, 20)), 2, barrier)
+            text = text_leg(api, tr, wl, rank, args.steps, 2, barrier)
     ms, ms_bin = allmax(ms), allmax(ms_bin)
     steps = args.steps
     U = (st1["unique_keys"] - st0["unique_keys"]) / max(steps, 1)
@@ -392,22 +415,9 @@ def run_workload(name, wl, args, rank, world, local, comm, api, torch, stream, s
     else:
         kern = [("xf_k_step_lr_lazy (pull+forward+gradient+optimizer in one kernel)", b_step + b_update, t_a)]
     dom = max(kern, key=lambda k: k[2])
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        try:
-            import re
-            kname = re.search(r"xf_k_\w+", dom[0]).group(0)
-            traffic = json.load(open(tpath)).get(name, {}).get(kname)
-        except Exception:
-            traffic = None
     out["roofline"] = {
         "bound": "hbm", "kernel": dom[0], "achieved": dom[1] / dom[2] / 1e9 if dom[2] else None, "peak": peak, "unit": "GB/s",
-        "frac": dom[1] / dom[2] / 1e9 / peak if dom[2] else None, "traffic": traffic,
-        "traffic_source": (("ncu --set full capture of this workload (profiles/traffic.json)" if world == 1 else
-                            "ncu --set full of the owner kernel with this workload's per-GPU token count on one GPU acting as "
-                            "its own peer (profiles/traffic.json, profiles/r02_multigpu.md); S launches together")
-                           if traffic else None),
+        "frac": dom[1] / dom[2] / 1e9 / peak if dom[2] else None,
         "peak_source": peak_src, "algorithmic_bytes_per_launch": dom[1], "avg_launch_ms": dom[2] * 1e3,
         "kernels": [{"kernel": n, "algorithmic_bytes": b, "avg_ms": t * 1e3, "gbs": b / t / 1e9 if t else None} for n, b, t in kern],
         "step_algorithmic_bytes": b_step + b_update, "step_gbs": (b_step + b_update) / (ms * 1e-3 / steps) / 1e9,
@@ -456,7 +466,11 @@ def main():
     ap.add_argument("--no-extras", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-text-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write the table rows the last timed step trained (seeded key sample) as DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
 
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * xflow_b200 — C ABI of the B200-native drop-in for xflow's data-parallel hot path.
+ * xflow_b200 — C ABI of the H100-native drop-in for xflow's data-parallel hot path.
  *
  * Plain C: pointers, sizes and POD structs only (no torch / STL types).  Every entry point below is
  * what the reference's FFI for this path binds; the comment on each names the reference interface it

@@ -12,5 +12,13 @@ CASES = {
     "syn_fm_ftrl_k8_e1": dict(data="syn", model="fm", opt="ftrl", epochs=1, K=8, block_mb=1, preinit=True),
 }
 
+# runs of the reference on the synthetic shards with its wall-clock seeded FM init (pinned time), stored as
+# digests of its final table: (model, opt, K, epochs); block_mb = 1
+FRESH_RUNS = [("lr", "ftrl", 0, 3), ("lr", "sgd", 0, 3), ("fm", "sgd", 6, 2), ("fm", "ftrl", 4, 2)]
+
+
+def fresh_run_name(model, opt, K, epochs):
+    return "%s_%s_k%d_e%d" % (model, opt, K, epochs)
+
 SYN = dict(seed=7, rows=3000, nnz_per_row=48, id_space=20000, dist="zipf", zipf_s=1.2)
 SYN_TEST = dict(seed=8, rows=500, nnz_per_row=48, id_space=20000, dist="zipf", zipf_s=1.2)

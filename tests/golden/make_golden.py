@@ -8,7 +8,10 @@ reference's final table (w and, for FTRL, n and z; v rows for FM), the initial t
 replays a pre-initialised latent table, the reference's predictions (as printed to pred_0_0.txt,
 6 significant digits) and its logloss / auc line.  The synthetic text inputs are regenerated from a
 seed by xflow_b200.datagen (bit-reproducible), the bundled 200-row shards are copied as data fixtures.
+fresh_runs.json holds digests of the reference's final tables for the FRESH_RUNS cases (see fresh_runs).
 """
+import hashlib
+import json
 import os
 import shutil
 import sys
@@ -25,7 +28,7 @@ from xflow_b200 import datagen  # noqa: E402
 
 REF_DATA = "/root/reference/data"
 
-from cases import CASES, SYN, SYN_TEST  # noqa: E402
+from cases import CASES, FRESH_RUNS, SYN, SYN_TEST, fresh_run_name  # noqa: E402
 
 
 def materialise_data(kind, tmp):
@@ -38,6 +41,37 @@ def materialise_data(kind, tmp):
         datagen.write_text(tr + "-00000", *datagen.make_ids(**SYN))
         datagen.write_text(te + "-00000", *datagen.make_ids(**SYN_TEST))
     return tr, te
+
+
+def table_keys(prefixes):
+    """The keys a run on these shards leaves in the table: every key of the train and test shards (a predict
+    pull inserts, lr_worker.cc:47) and key 0 of the init push."""
+    ks = [k for p in prefixes for _, k, _ in O.load_blocks(p + "-00000", 1 << 20)]
+    return np.unique(np.concatenate(ks + [np.zeros(1, np.uint64)]))
+
+
+def digest(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def fresh_runs(tmp):
+    """fresh_runs.json: per FRESH_RUNS case, SHA-256 of the key list and of every field of the reference's final
+    table (its exact bits; the full tables would be ~1 MB of fixtures)."""
+    train, test = materialise_data("syn", tmp)
+    keys = table_keys((train, test))
+    out = {}
+    for model, opt, K, epochs in FRESH_RUNS:
+        run = tempfile.mkdtemp()
+        O.run_ref(model, opt, train, test, epochs, run, core=1, block_mb=1, vdim=K or 10,
+                  dump=os.path.join(run, "d.bin"), fix_time=1.5e9)
+        d = O.read_dump(os.path.join(run, "d.bin"))
+        assert np.array_equal(d["keys"], keys)
+        out[fresh_run_name(model, opt, K, epochs)] = {
+            k: digest(d[k]) for k in ("keys", "w", "nw", "zw", "v", "nv", "zv") if k in d}
+        shutil.rmtree(run, ignore_errors=True)
+    with open(os.path.join(HERE, "fresh_runs.json"), "w") as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+        f.write("\n")
 
 
 def main():
@@ -78,6 +112,7 @@ def main():
             b"feature_with_a_long_name_0123456789"]
     np.savez(os.path.join(HERE, "std_hash.npz"), strings=np.array(strs, dtype="S64"),
              hashes=np.array([O.std_hash(s) for s in strs], np.uint64))
+    fresh_runs(tmp)
     shutil.rmtree(tmp, ignore_errors=True)
 
 

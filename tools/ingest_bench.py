@@ -1,6 +1,6 @@
 """File -> model throughput of the two ingest paths (SURVEY.md section 8f-1): host parser
 (xf_loader_next, one CPU core, like the reference's LoadData) against the device parser
-(xf_trainer_ingest_text).  Prints one JSON line; numbers for profiles/, not a bench.py metric."""
+(xf_trainer_ingest_text).  Prints one JSON line; not a bench.py metric."""
 import json
 import os
 import sys

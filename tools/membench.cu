@@ -1,10 +1,10 @@
 // Micro-benchmarks behind the round-2 kernel decisions: which access PRIMITIVES limit the table kernels?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/membench tools/membench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/membench tools/membench.cu
 //   tools/membench [table_MB=8192] [accesses_M=6.5]
 // Table of 32-byte rows (the LR row), `n` distinct-ish random rows per launch (one batch's worth).
-//   read        one 256-bit load per access
-//   rmw         load + 256-bit store
-//   lazy        load + CAS on the tag word + 256-bit store + f64 RED   (the "open + accumulate" of step_lazy.cu)
+//   read        one 32-byte load per access (two 128-bit loads, as xf_load_head)
+//   rmw         load + 32-byte store
+//   lazy        load + CAS on the tag word + 32-byte store + f64 RED   (the "open + accumulate" of step_lazy.cu)
 //   lazy_sync   the same with __syncwarp between the stages (warp-synchronous, like the row kernel)
 //   red         f64 RED only
 //   pf+read     prefetch.global.L2 of n2 rows in one kernel, then the read kernel over the same rows
@@ -20,11 +20,14 @@ __device__ __forceinline__ uint64_t mix(uint64_t x) {
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
+// a 32-byte sector as two 128-bit accesses (sm_90 has no 256-bit LDG / STG), as table.cuh does
 __device__ __forceinline__ void ld256(const uint8_t* p, uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d) {
-  asm volatile("ld.global.cg.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
 __device__ __forceinline__ void st256(uint8_t* p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
-  asm volatile("st.global.v4.u64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
+  asm volatile("st.global.v2.u64 [%0], {%1,%2};\n\tst.global.v2.u64 [%0+16], {%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c),
+               "l"(d) : "memory");
 }
 
 enum { M_READ = 0, M_RMW, M_LAZY, M_LAZY_SYNC, M_RED, M_PF, M_CHAIN2, M_CHAIN4, M_READ64, M_READ128, M_LD2, M_ST, M_LD_RED, M_RED2, M_CAS, M_LD_CAS_ST, M_LD_ST_RED, M_ST16, M_RED_F32, M_LD_ST16, M_CAS128, M_LD_CAS128, M_LD_CAS128_RED };
@@ -138,6 +141,8 @@ __global__ void __launch_bounds__(256) krow(uint8_t* base, uint64_t mask, uint64
   if (acc == 0x12345u) *sink = acc;
 }
 
+static int g_sms = 132;
+
 template <int MODE>
 static float run(const char* name, uint8_t* base, uint64_t nsect, uint64_t n, uint64_t* sink, int bps = 8, uint64_t seed0 = 77,
                  bool print = true, int reps = 3) {
@@ -147,7 +152,7 @@ static float run(const char* name, uint8_t* base, uint64_t nsect, uint64_t n, ui
   float best = 1e30f;
   for (int r = 0; r < reps; ++r) {
     cudaEventRecord(e0);
-    k<MODE><<<148 * bps, 256>>>(base, nsect - 1, n, seed0 + 1000 * r, 5 + r, sink);
+    k<MODE><<<g_sms * bps, 256>>>(base, nsect - 1, n, seed0 + 1000 * r, 5 + r, sink);
     cudaEventRecord(e1);
     cudaEventSynchronize(e1);
     float ms;
@@ -163,6 +168,7 @@ int main(int argc, char** argv) {
   double acc_m = argc > 2 ? atof(argv[2]) : 6.5;
   uint64_t n = (uint64_t)(acc_m * 1e6);
   uint64_t nsect = 1;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
   while (nsect * 32 < mb * 1048576ull) nsect <<= 1;
   uint8_t* base;
   uint64_t* sink;
@@ -227,7 +233,7 @@ int main(int argc, char** argv) {
       float best = 1e30f;
       for (int r = 0; r < 3; ++r) {
         cudaEventRecord(e0);
-        kern[v]<<<148 * 8, 256>>>(base, nrow - 1, n, 99 + r, sink);
+        kern[v]<<<g_sms * 8, 256>>>(base, nrow - 1, n, 99 + r, sink);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms; cudaEventElapsedTime(&ms, e0, e1);

@@ -1,9 +1,9 @@
-// Micro-benchmark: what can B200's HBM3e + L2 sustain for RANDOM 32-byte sector traffic?
+// Micro-benchmark: what can the H100's HBM3 + L2 sustain for RANDOM 32-byte sector traffic?
 // The xflow hot path is exactly that access pattern (one table row = one sector), so this number —
 // not the streaming-copy peak — is the practical ceiling of the probe and update kernels.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/randsector tools/randsector.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/randsector tools/randsector.cu
 //   tools/randsector [table_MB=1024] [accesses_M=16]
-// Prints G sectors/s and GB/s for: random 256-bit reads at several loads-in-flight per thread,
+// Prints G sectors/s and GB/s for: random 32-byte reads at several loads-in-flight per thread,
 // random read-modify-write of the sector, random f64 atomic adds, with 32 B and 64 B L2 fetch granularity.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,12 +16,16 @@ __device__ __forceinline__ uint64_t mix(uint64_t x) {
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
+// a 32-byte sector as two 128-bit accesses (sm_90 has no 256-bit LDG / STG), as table.cuh does
 __device__ __forceinline__ void ld256(const uint8_t* p, uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d) {
-  asm volatile("ld.global.cg.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
 __device__ __forceinline__ void st256(uint8_t* p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
-  asm volatile("st.global.v4.u64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d) : "memory");
+  asm volatile("st.global.v2.u64 [%0], {%1,%2};\n\tst.global.v2.u64 [%0+16], {%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c),
+               "l"(d) : "memory");
 }
+static int g_sms = 132;
 
 template <int MLP, int MODE>  // MODE 0 read, 1 read+write, 2 atomic f64 add
 __global__ void k_rand(uint8_t* base, uint64_t nsect_mask, uint64_t per_thread, uint64_t seed, uint64_t* sink) {
@@ -89,7 +93,7 @@ __global__ void k_ord(uint8_t* base, uint64_t nsect, uint64_t per_thread, uint64
 template <int MLP, int MODE, int ORDER>
 static void run_ord(const char* name, uint8_t* base, uint64_t nsect, uint64_t total, uint64_t S, uint64_t W,
                     uint64_t* sink) {
-  const int block = 256, grid = 148 * 8;
+  const int block = 256, grid = g_sms * 8;
   uint64_t threads = (uint64_t)block * grid;
   uint64_t per_thread = (total / threads / MLP) * MLP;
   if (per_thread == 0) per_thread = MLP;
@@ -117,7 +121,7 @@ static void run_ord(const char* name, uint8_t* base, uint64_t nsect, uint64_t to
 
 template <int MLP, int MODE>
 static void run(const char* name, uint8_t* base, uint64_t nsect, uint64_t total, uint64_t* sink) {
-  const int block = 256, grid = 148 * 8;
+  const int block = 256, grid = g_sms * 8;
   uint64_t threads = (uint64_t)block * grid;
   uint64_t per_thread = (total / threads / MLP) * MLP;
   if (per_thread == 0) per_thread = MLP;
@@ -145,6 +149,7 @@ int main(int argc, char** argv) {
   uint64_t mb = argc > 1 ? strtoull(argv[1], 0, 10) : 1024;
   uint64_t total = (argc > 2 ? strtoull(argv[2], 0, 10) : 16) * 1000000ull;
   uint64_t nsect = 1;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
   while (nsect * 32 < mb * 1048576ull) nsect <<= 1;
   uint8_t* base;
   uint64_t* sink;

@@ -233,9 +233,8 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   }
   XF_CUDA_TRY(cudaSetDevice(cfg->device));
   // L2 fetch granularity = one probing bucket (LR: 4 rows = one 128-byte line), so that the collision probes of
-  // a bucket find the line the first probe fetched.  It costs DRAM read traffic (ncu, headline LR batch: 340 MB at
-  // 32 B, 932 MB at 128 B, DRAM 33 % busy) and buys time: 0.447 ms against 0.522 ms per batch with 32-byte fetches
-  // — the kernels are bound by the request rate, not by DRAM bytes (DESIGN.md section 6).  A hint: the driver may
+  // a bucket (and the second half of a 32-byte sector) find the line the first load fetched.  It costs DRAM read
+  // traffic and buys time: the kernels are bound by the request rate, not by DRAM bytes (DESIGN.md section 6).  A hint: the driver may
   // ignore it.  XFLOW_L2_FETCH = 32 / 64 / 128 overrides.
   {
     int fetch = 128;

@@ -323,8 +323,7 @@ int xf_mg_create(xf_trainer* tr) {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
     // Routing and the DONE signal are what the OTHER ranks wait for.  Giving their streams the high priority
-    // (XFLOW_MG_ROUTE_PRIO=1) was measured at 2 GPUs: 163.6 M examples/s against 166.7 M at equal priority, twice
-    // each, so equal priority stays the default.
+    // (XFLOW_MG_ROUTE_PRIO=1) did not make the 2-GPU step faster, so equal priority stays the default.
     const char* rp = getenv("XFLOW_MG_ROUTE_PRIO");
     const int prio = (rp && *rp == '1') ? hi : lo;
     if (cudaStreamCreateWithPriority(&mg->st2, cudaStreamNonBlocking, prio) != cudaSuccess) { rc = XF_ERR_CUDA; break; }

@@ -1,4 +1,4 @@
-// sm_100a kernels of the xflow hot path.  All of them are HBM / L2-latency bound integer+float work
+// sm_90a kernels of the xflow hot path.  All of them are HBM / L2-latency bound integer+float work
 // on 32-byte table sectors (see table.cuh); there is no dense tile anywhere on this path (the
 // reference's FM term is a per-row scalar, fm_worker.cc:177-196), so no tensor-core code.
 //
@@ -100,7 +100,7 @@ xf_k_update(XfTableView t, const uint32_t* __restrict__ slots, uint64_t n, int t
   for (uint64_t base = gwarp * 32; base < n; base += nwarps * 32) {
     // Fused step: walk the touched array BACKWARDS.  The rows touched last by the step kernel are
     // the ones still resident (dirty) in L2; a forward walk meets them only after they have been
-    // evicted (LRU thrash: ncu showed 44 % L2 hits forward).
+    // evicted (LRU thrash).
     const uint64_t e_fwd = base + lane;
     const uint64_t e_i = (SLOTG && e_fwd < n) ? (n - 1 - e_fwd) : e_fwd;
     const uint64_t e_phys = (e_i < n_head) ? e_i : (uint64_t)extra_base + (e_i - n_head);
@@ -120,7 +120,7 @@ xf_k_update(XfTableView t, const uint32_t* __restrict__ slots, uint64_t n, int t
       pend = (cnt <= ngroups) ? 0u : (pend & ~((2u << __fns(pend, 0, ngroups)) - 1u));
 
       // Every load of the row is issued before anything is consumed: slot -> {head, accumulators, v, nv,
-      // zv} is then two DRAM latencies deep (measured: the dependent chain head -> v -> nv/zv cost 3.5x).
+      // zv} is then two DRAM latencies deep instead of a dependent chain head -> v -> nv/zv.
       // The latent loads are speculative: a row whose latent block is not materialised ignores them.
       const bool lat = K > 0 && (part & 2) && rowp != nullptr;
       float* vp = lat ? xf_row_v(rowp) : nullptr;
@@ -154,7 +154,7 @@ xf_k_update(XfTableView t, const uint32_t* __restrict__ slots, uint64_t n, int t
         accL = a.x;
         accA = a.y;
       }
-      // the group leader reads the head sector once (one 256-bit load) and shares key / flags
+      // the group leader reads the head sector once and shares key / flags
       XfHead h;
       h.key = 0; h.flags = 0; h.w = h.n = h.z = 0.f; h.g = 0.0;
       if (q == 0 && rowp != nullptr) h = xf_load_head(rowp);
@@ -569,7 +569,7 @@ int xf_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sm_count <= 0) g_sm_count = 148;
+    if (g_sm_count <= 0) g_sm_count = 132;  // H100 SXM
   }
   return g_sm_count;
 }
@@ -600,9 +600,9 @@ static void xf_launch_update_t(const XfTableView& t, const uint32_t* slots, uint
                                const float* gw, const float* gv, int part, unsigned long long* live_total,
                                cudaStream_t st, const uint32_t* n_dev = nullptr, const uint32_t* rows_dev = nullptr,
                                uint32_t extra_base = 0, uint32_t extra_n = 0, const float* v0_side = nullptr) {
-  // wide variant: whole-row loads / stores by one instruction.  Measured so far (profiles/r02_fm_update.md): fewer
-  // requests but only 2 rows in flight per warp and 90+ registers -> 3x SLOWER than the per-coordinate kernel;
-  // off unless XFLOW_UPDATE_WIDE=1 (A/B measurements)
+  // wide variant: whole-row loads / stores by one instruction: fewer requests but only 2 rows in flight per warp
+  // and 90+ registers, slower than the per-coordinate kernel when it was measured; off unless XFLOW_UPDATE_WIDE=1
+  // (A/B measurements)
   static const bool wide_on = [] { const char* e = getenv("XFLOW_UPDATE_WIDE"); return e && *e == '1'; }();
   if (wide_on && !t.canon && t.K > 0 && (t.K & 3) == 0 && t.stride <= 512 && (part & 2)) {
     int G = 1;

@@ -1,4 +1,4 @@
-// sm_100a kernels of the sharded (multi-GPU) step; layout and protocol in mg.cuh, stream schedule in
+// sm_90a kernels of the sharded (multi-GPU) step; layout and protocol in mg.cuh, stream schedule in
 // comm.cu.  Every exchange is done by the producing kernel itself with stores into the consumer's
 // memory over NVLink (cudaIpc-mapped slabs); xf_k_signal / xf_k_wait order them with step counters.
 //
@@ -207,7 +207,7 @@ xf_k_pull_tokens(XfTableView t, const uint64_t* __restrict__ in_keys, const uint
         float* sv = (s > 0 && side_v != nullptr) ? side_v + ((uint64_t)s * cap + i) * (uint64_t)K : nullptr;
         if ((h.flags & XF_FLAG_V_READY) && (K & 7) == 0) {
           const float* vp = reinterpret_cast<const float*>(xf_row(t, (uint64_t)r) + 32);
-          for (int k = 0; k < K; k += 8) {  // 256-bit loads: half as many row-touching instructions
+          for (int k = 0; k < K; k += 8) {  // a sector at a time
             float v[8];
             xf_ld8_l1(vp + k, v);
 #pragma unroll
@@ -340,8 +340,8 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
   const uint32_t nwarps = gridDim.x * wpb;
   // Two groups of 32 tokens per warp and iteration: both deposits are issued before any result is looked at, and
   // the coalesced inputs of the NEXT iteration (slot, row index, stashed state words) are requested before this
-  // iteration's atomics go out.  ncu on the first version (one group, nothing ahead): 27 G requests/s with 53
-  // long-scoreboard stall cycles per issue — a chain of four dependent round trips per 32 tokens.
+  // iteration's atomics go out.  The first version (one group, nothing ahead) stalled on a chain of four dependent
+  // round trips per 32 tokens.
   const bool have_stash = stash != nullptr;
   uint32_t s_n[2], r_n[2];
   uint4 b_n[2];

@@ -1,4 +1,4 @@
-// The fused worker step (sm_100a): what LRWorker::update / FMWorker::update do between reading a
+// The fused worker step (sm_90a): what LRWorker::update / FMWorker::update do between reading a
 // slice and returning from the last Push (src/model/lr/lr_worker.cc:121-177, fm/fm_worker.cc:126-245)
 // WITHOUT the reference's sort / unique / merge-join: the table row is the per-key accumulator.
 //
@@ -13,7 +13,7 @@
 //                (kernels.cu) walks that array                                                (Push)
 //
 // One warp per row, one lane per token, two tokens per lane in flight: keys for a 64-token chunk are
-// loaded first, then the two first-probe sectors (one 256-bit load each), then resolved; the two
+// loaded first, then the two first-probe sectors (xf_load_head), then resolved; the two
 // returning atomics of phase B are likewise issued back to back.  HBM / L2-latency bound integer and
 // float work on random sectors: no shared-memory tile, no tensor core — see DESIGN.md.
 #include <cuda_runtime.h>
@@ -41,7 +41,7 @@ __device__ __forceinline__ void xf_fm_token(const XfTableView& t, uint32_t slot,
   st = 0.f;
   qt = 0.f;
   if ((flags & XF_FLAG_V_READY) && (K & 7) == 0) {
-    // 256-bit loads: half as many row-touching instructions (the row starts 32-byte aligned)
+    // a sector at a time (the row starts 32-byte aligned)
     const float* vp = reinterpret_cast<const float*>(xf_row(t, slot) + 32);
     for (int k = 0; k < K; k += 8) {
       float v[8];
@@ -68,7 +68,7 @@ __device__ __forceinline__ void xf_fm_token(const XfTableView& t, uint32_t slot,
 
 // Hot-key cache (FM only): with skewed ids a handful of keys take a large share of all tokens (Zipf
 // 1.05 over 1e8 ids: the top key is ~8 % of the tokens of every batch) and their L2 atomics serialise
-// the whole kernel (measured: 3.7 ms per cfg5-shaped batch, 17 contended atomics per token).  Each CTA
+// the whole kernel (17 contended atomics per token on a cfg5-shaped batch).  Each CTA
 // therefore keeps NC direct-mapped accumulator rows in shared memory, claimed first-come with a CAS on
 // the tag; a token whose key owns (or obtains) an entry accumulates there with shared-memory atomics,
 // everything else goes to HBM as before.  The entries are flushed once, when the CTA has finished all

@@ -5,10 +5,10 @@
 // ("opening" the row for b).  Every other reader applies it on the fly (xf_apply_pending, table.cuh), so
 // the observable table is the reference's at every batch boundary.
 //
-// Why: on a multi-GB table every row-touching instruction costs about the same (~28 ps of chip time: load,
-// store or atomic, hit or miss — tools/membench.cu, profiles/r02_membench.md), so the kernel's time is
-// (row-touching instructions per token) x 28 ps x tokens.  The eager pair (step + update) needs 4.3 per token,
-// round 1's lazy protocol (load, CAS on the tag, 256-bit store, RED) also 4.3 in one launch; this one 2.3:
+// Why: on a multi-GB table every row-touching instruction costs about the same (load, store or atomic, hit or
+// miss — tools/membench.cu), so the kernel's time is (row-touching instructions per token) x a fixed cost x
+// tokens.  The eager pair (step + update) needs 4.3 per token, round 1's lazy protocol (load, CAS on the tag,
+// full-sector store, RED) also 4.3 in one launch; this one 2.3:
 //   phase A  load the row (1.3 with the collision probes) and compute, in registers, the weight the batch
 //            pulls: the row's state with the pending step applied (pure function of what was loaded)
 //   phase B  after the row reduction, ONE 128-bit CAS per distinct key of the token group deposits the
@@ -19,10 +19,9 @@
 // Inside a warp, tokens with the same slot elect one lane (__match_any_sync): one deposit of
 // count x residual per distinct key of a 32-token group.
 //
-// Tried and measured on the 1e8-id table (profiles/r02_lazy_experiments.md): bucketised probing (collision
-// probes inside one 128-byte line: -3 %, kept), L2 prefetch by dedicated warps running ahead (+23 % time: the
-// prefetches are requests too, removed), claim + publish in one CAS.128 with a separate RED (3.3 instructions
-// per token: 0.61 ms per headline batch against 0.72 ms for round 1's protocol).
+// Tried on the 1e8-id table: bucketised probing (collision probes inside one 128-byte line: faster, kept), L2
+// prefetch by dedicated warps running ahead (slower: the prefetches are requests too, removed), claim + publish
+// in one CAS.128 with a separate RED (3.3 instructions per token: between round 1's protocol and this one).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>

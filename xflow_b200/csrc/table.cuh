@@ -106,10 +106,10 @@ __host__ __device__ inline uint32_t xf_row_stride(int K, int opt, int canon = 0)
 // that share one 128-byte line (LR: 4 rows of 32 B; FM rows are longer than a line: B = 1 = plain linear
 // probing).  Probe i of a key visits its home bucket first — starting at a key-dependent slot and wrapping
 // inside the bucket — and then the following buckets slot by slot.  Why: a warp waits for the slowest of its
-// lanes, and every step of a linear-probing chain used to be one more DEPENDENT DRAM access (measured on the
-// 1e8-id table at load 0.37: the longest chain among the 64 tokens a warp has in flight averaged 5 DRAM round
-// trips, ncu long-scoreboard 51 cycles per issue).  Inside a bucket the further probes hit the line the first
-// one fetched (L2 fetch granularity = the bucket, xf_table_create); chains that leave the home bucket are rare
+// lanes, and every step of a linear-probing chain used to be one more DEPENDENT DRAM access (on the 1e8-id
+// table at load 0.37 the longest chain among the 64 tokens a warp has in flight is several DRAM round trips).
+// Inside a bucket the further probes hit the line the first one fetched (L2 fetch granularity = the bucket,
+// xf_table_create); chains that leave the home bucket are rare
 // (1.6 % of the keys at load 0.37 with B = 4, simulated; expected longest chain among 64 tokens 1.7 lines).
 __device__ __forceinline__ uint64_t xf_probe_slot(const XfTableView& t, uint64_t key, uint32_t i) {
   const uint64_t m = key * 0x9E3779B97F4A7C15ull;
@@ -169,11 +169,29 @@ struct XfHead {
   double g;
 };
 
+// One 32-byte sector as two 128-bit loads issued back to back (sm_90 has no 256-bit LDG): both are in flight at
+// once, and with the L2 fetch granularity at 128 B (xf_table_create) the second finds the line the first one
+// brought into L2.  Each half is one 16-byte access, which is what the lazy protocol's 128-bit CAS on bytes
+// 16..31 compares against.
+__device__ __forceinline__ void xf_ld32_cg(const void* p, uint64_t& q0, uint64_t& q1, uint64_t& q2, uint64_t& q3) {
+  asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+}
+__device__ __forceinline__ void xf_ld32_ca(const void* p, uint64_t& q0, uint64_t& q1, uint64_t& q2, uint64_t& q3) {
+  asm volatile("ld.global.ca.v2.u64 {%0,%1}, [%4];\n\tld.global.ca.v2.u64 {%2,%3}, [%4+16];"
+               : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+}
+// the whole sector written by two 128-bit stores (no read-for-fill: L2 merges them into one full sector)
+__device__ __forceinline__ void xf_st32(void* p, uint64_t q0, uint64_t q1, uint64_t q2, uint64_t q3) {
+  asm volatile("st.global.v2.u64 [%0], {%1,%2};\n\tst.global.v2.u64 [%0+16], {%3,%4};" ::"l"(p), "l"(q0), "l"(q1),
+               "l"(q2), "l"(q3)
+               : "memory");
+}
+
 __device__ __forceinline__ XfHead xf_load_head(const uint8_t* row) {
-  // one 32-byte sector = ONE 256-bit L2 load (sm_100 LDG.E.256; L1 is useless for random rows).
-  // Two 16-byte loads cost two L2 requests and, measured with ncu, up to two DRAM fetches.
+  // the row's first 32-byte sector straight from L2 (L1 is useless for random rows)
   uint64_t q0, q1, q2, q3;
-  asm volatile("ld.global.cg.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(row));
+  xf_ld32_cg(row, q0, q1, q2, q3);
   XfHead h;
   h.key = q0;
   h.g = __longlong_as_double((long long)q1);
@@ -189,10 +207,10 @@ __device__ __forceinline__ XfHead xf_load_head(const uint8_t* row) {
 // nothing else).  A stale copy can then differ from L2 only by showing EMPTY for a slot that was claimed
 // during this kernel — the insert CAS resolves that (xf_probe_from), and a row inserted during the kernel
 // still has its default parameters.  With skewed ids this keeps each SM's reads of the hot rows local:
-// through L2 every token of the hottest key queues on one slice (measured, DESIGN.md section 4).
+// through L2 every token of the hottest key queues on one slice (DESIGN.md section 4).
 __device__ __forceinline__ XfHead xf_load_head_l1(const uint8_t* row) {
   uint64_t q0, q1, q2, q3;
-  asm volatile("ld.global.ca.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(row));
+  xf_ld32_ca(row, q0, q1, q2, q3);
   XfHead h;
   h.key = q0;
   h.g = __longlong_as_double((long long)q1);
@@ -203,23 +221,23 @@ __device__ __forceinline__ XfHead xf_load_head_l1(const uint8_t* row) {
   return h;
 }
 
-// eight consecutive floats of a latent row with ONE 256-bit load through L1 (read-only-for-the-kernel data,
-// see xf_load_head_l1): a row access costs per instruction, not per byte (tools/membench.cu)
+// eight consecutive floats of a latent row (one 32-byte sector) through L1 (read-only-for-the-kernel data,
+// see xf_load_head_l1)
 __device__ __forceinline__ void xf_ld8_l1(const float* p, float (&o)[8]) {
   uint64_t q0, q1, q2, q3;
-  asm volatile("ld.global.ca.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+  xf_ld32_ca(p, q0, q1, q2, q3);
   o[0] = __uint_as_float((uint32_t)q0); o[1] = __uint_as_float((uint32_t)(q0 >> 32));
   o[2] = __uint_as_float((uint32_t)q1); o[3] = __uint_as_float((uint32_t)(q1 >> 32));
   o[4] = __uint_as_float((uint32_t)q2); o[5] = __uint_as_float((uint32_t)(q2 >> 32));
   o[6] = __uint_as_float((uint32_t)q3); o[7] = __uint_as_float((uint32_t)(q3 >> 32));
 }
 
-// full-sector store of the head (one 256-bit STG: no partial-sector write, no read-for-fill)
+// full-sector store of the head
 __device__ __forceinline__ void xf_store_head(uint8_t* row, const XfHead& h) {
   const uint64_t q1 = (uint64_t)__double_as_longlong(h.g);
   const uint64_t q2 = (uint64_t)__float_as_uint(h.w) | ((uint64_t)__float_as_uint(h.n) << 32);
   const uint64_t q3 = (uint64_t)__float_as_uint(h.z) | ((uint64_t)h.flags << 32);
-  asm volatile("st.global.v4.u64 [%0], {%1,%2,%3,%4};" ::"l"(row), "l"(h.key), "l"(q1), "l"(q2), "l"(q3) : "memory");
+  xf_st32(row, h.key, q1, q2, q3);
 }
 
 // Find `key` starting at its home slot `s` (= xf_home_slot) whose head `h` the caller has already loaded; if
@@ -312,7 +330,7 @@ __device__ __forceinline__ float xf_div_rows_plain(float g, double rows) { retur
 __device__ __forceinline__ float xf_div_rows(float g, double rows) {
   // A power-of-two row count (the usual batch size) makes the quotient an exact scaling: multiplying by
   // the exact reciprocal gives the same double, hence the same float, without a double division (the
-  // update kernel was instruction-bound on it, profiles/r01_ncu_full_fm_ftrl.md).
+  // update kernel was instruction-bound on it).
   const long long b = __double_as_longlong(rows);
   if ((b & 0x000FFFFFFFFFFFFFll) == 0ll && b > 0ll) {
     const double inv = __longlong_as_double((2046ll << 52) - b);  // 2^-e for rows = 2^e
@@ -400,7 +418,7 @@ __device__ __forceinline__ void xf_lazy_store(const XfTableView& t, uint8_t* row
   uint64_t q1 = 0ull;
   if (keep_w && ftrl && __float_as_uint(h.w) != __float_as_uint(xf_ftrl_w(t, h.z, h.n)))
     q1 = (uint64_t)__float_as_uint(h.w) | ((uint64_t)xf_lazy_check(q2) << 32);
-  asm volatile("st.global.v4.u64 [%0], {%1,%2,%3,%4};" ::"l"(rowp), "l"(h.key), "l"(q1), "l"(q2), "l"(0ull) : "memory");
+  xf_st32(rowp, h.key, q1, q2, 0ull);
 }
 // store a canonical head into a row of either kind
 __device__ __forceinline__ void xf_store_head_t(const XfTableView& t, uint8_t* rowp, const XfHead& h) {
@@ -409,10 +427,9 @@ __device__ __forceinline__ void xf_store_head_t(const XfTableView& t, uint8_t* r
 }
 
 // ---- lazy tables: fold + open + deposit with ONE 128-bit compare-and-swap ------------------------------------
-// Measured on B200 (tools/membench.cu, profiles/r02_membench.md): on a multi-GB table every instruction that
-// touches a random row costs about the same whatever it is — load, store, CAS or RED, hit or miss (the request
-// path saturates near 36 G requests/s) — so the number of row-touching instructions per token is what sets the
-// speed of these kernels.  Round 1's protocol needed four (load, CAS on the tag, 256-bit store, RED).  Here a
+// On a multi-GB table every instruction that touches a random row costs about the same whatever it is — load,
+// store, CAS or RED, hit or miss: the request path saturates first (tools/membench.cu measures it) — so the number
+// of row-touching instructions per token is what sets the speed of these kernels.  Round 1's protocol needed four (load, CAS on the tag, 256-bit store, RED).  Here a
 // token needs two: the load, and this deposit — which for the FIRST token of a batch on a row is a CAS.128 of
 // {state, tag, g}: (pending state, p, sum_p) -> (state after the step of p, seq, its own residual), and for a
 // later token of the same batch (duplicate keys) a 64-bit integer add into g.  Nobody ever waits or polls.
