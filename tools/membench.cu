@@ -2,13 +2,18 @@
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/membench tools/membench.cu
 //   tools/membench [table_MB=8192] [accesses_M=6.5]
 // Table of 32-byte rows (the LR row), `n` distinct-ish random rows per launch (one batch's worth).
-//   read        one 32-byte load per access (two 128-bit loads, as xf_load_head)
+//   read        one 32-byte load per access (two 128-bit loads from one lane, as xf_load_head)
+//   read pair   the same rows, each 128-bit load instruction serving two lanes' halves of one row (xf_ld32_pair)
 //   rmw         load + 32-byte store
 //   lazy        load + CAS on the tag word + 32-byte store + f64 RED   (the "open + accumulate" of step_lazy.cu)
 //   lazy_sync   the same with __syncwarp between the stages (warp-synchronous, like the row kernel)
 //   red         f64 RED only
 //   pf+read     prefetch.global.L2 of n2 rows in one kernel, then the read kernel over the same rows
 //   chain-k     k dependent loads per access (probe chains)
+// On one H100 80GB HBM3 (SXM, power limit 400 W), 8 GiB table, 6.5 M rows per launch, best of 3, the same at L2
+// fetch granularity 32, 64 and 128 B (to within 1 %), in G rows/s: read 21.9, read pair 30.4-30.7 (1.40x),
+// CAS.128 only 12.0, load + CAS.128 10.3-10.4, read pair + CAS.128 10.3-10.5.  A paired look costs fewer requests
+// than a one-lane one, but a row that is also CAS'd is bound by the atomic.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -25,20 +30,50 @@ __device__ __forceinline__ void ld256(const uint8_t* p, uint64_t& a, uint64_t& b
   asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
                : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
+// The same 32-byte rows read by lane PAIRS (as xf_ld32_pair in table.cuh): lanes 2i and 2i+1 each load one 16-byte
+// half of the even lane's row in one instruction and of the odd lane's row in a second one, then swap halves.  Still
+// two LDG.128 per lane, but each instruction touches 16 rows instead of 32.  p == nullptr: no row (returns zeros).
+__device__ __forceinline__ void ld256_pair(const uint8_t* p, uint64_t& a, uint64_t& b, uint64_t& c, uint64_t& d) {
+  const uint32_t odd = threadIdx.x & 1u;
+  const uint8_t* o = (const uint8_t*)__shfl_xor_sync(0xffffffffu, (unsigned long long)p, 1);
+  const uint8_t* r0 = odd ? o : p;
+  const uint8_t* r1 = odd ? p : o;
+  uint64_t x0 = 0, x1 = 0, y0 = 0, y1 = 0;
+  asm volatile("{\n .reg .pred p0, p1;\n setp.ne.u64 p0, %4, 0;\n setp.ne.u64 p1, %5, 0;\n"
+               " @p0 ld.global.cg.v2.u64 {%0,%1}, [%6];\n @p1 ld.global.cg.v2.u64 {%2,%3}, [%7];\n}"
+               : "+l"(x0), "+l"(x1), "+l"(y0), "+l"(y1)
+               : "l"(r0), "l"(r1), "l"(r0 + 16 * odd), "l"(r1 + 16 * odd));
+  const uint64_t m0 = odd ? y0 : x0, m1 = odd ? y1 : x1;  // this lane's half of its own row
+  const uint64_t t0 = __shfl_xor_sync(0xffffffffu, odd ? x0 : y0, 1), t1 = __shfl_xor_sync(0xffffffffu, odd ? x1 : y1, 1);
+  a = odd ? t0 : m0; b = odd ? t1 : m1; c = odd ? m0 : t0; d = odd ? m1 : t1;
+}
 __device__ __forceinline__ void st256(uint8_t* p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
   asm volatile("st.global.v2.u64 [%0], {%1,%2};\n\tst.global.v2.u64 [%0+16], {%3,%4};" ::"l"(p), "l"(a), "l"(b), "l"(c),
                "l"(d) : "memory");
 }
 
-enum { M_READ = 0, M_RMW, M_LAZY, M_LAZY_SYNC, M_RED, M_PF, M_CHAIN2, M_CHAIN4, M_READ64, M_READ128, M_LD2, M_ST, M_LD_RED, M_RED2, M_CAS, M_LD_CAS_ST, M_LD_ST_RED, M_ST16, M_RED_F32, M_LD_ST16, M_CAS128, M_LD_CAS128, M_LD_CAS128_RED };
+enum { M_READ = 0, M_RMW, M_LAZY, M_LAZY_SYNC, M_RED, M_PF, M_CHAIN2, M_CHAIN4, M_READ64, M_READ128, M_LD2, M_ST, M_LD_RED, M_RED2, M_CAS, M_LD_CAS_ST, M_LD_ST_RED, M_ST16, M_RED_F32, M_LD_ST16, M_CAS128, M_LD_CAS128, M_LD_CAS128_RED, M_READ_PAIR, M_READ_PAIR_CAS128 };
 
 template <int MODE>
 __global__ void __launch_bounds__(256) k(uint8_t* base, uint64_t mask, uint64_t n, uint64_t seed, uint32_t tag, uint64_t* sink) {
   uint64_t acc = 0;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+  const bool pair = MODE == M_READ_PAIR || MODE == M_READ_PAIR_CAS128;
+  const uint64_t n_it = pair ? (n + 31) & ~31ull : n;  // the pair modes keep whole warps in the loop
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_it; i += (uint64_t)gridDim.x * blockDim.x) {
     uint8_t* p = base + ((mix(seed + i) & mask) << 5);
     uint64_t a, b, c, d;
-    if (MODE == M_PF) {
+    if (pair) {
+      ld256_pair(i < n ? p : nullptr, a, b, c, d);
+      acc += a ^ b ^ c ^ d;
+      if (MODE == M_READ_PAIR_CAS128 && i < n) {
+        uint64_t o0, o1;
+        const uint64_t n0 = c + 1, n1 = (d & 0xFFFFFFFFull) | ((uint64_t)tag << 32);
+        asm volatile("{\n .reg .b128 cmp, swp, old;\n mov.b128 cmp, {%2, %3};\n mov.b128 swp, {%4, %5};\n"
+                     " atom.global.cas.b128 old, [%6], cmp, swp;\n mov.b128 {%0, %1}, old;\n}"
+                     : "=l"(o0), "=l"(o1) : "l"(c), "l"(d), "l"(n0), "l"(n1), "l"(p + 16) : "memory");
+        acc += o0 ^ o1;
+      }
+    } else if (MODE == M_PF) {
       asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
     } else if (MODE == M_RED) {
       atomicAdd(reinterpret_cast<double*>(p + 24), 1.0);
@@ -176,11 +211,11 @@ int main(int argc, char** argv) {
   cudaMalloc(&sink, 8);
   cudaMemset(base, 0, nsect * 32);
   for (int fetch = 32; fetch <= 128; fetch *= 2) {
-    if (fetch == 64) continue;
     cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, fetch);
     printf("table %llu MiB, %llu accesses per launch, L2 fetch granularity %d B\n", (unsigned long long)(nsect * 32 >> 20),
            (unsigned long long)n, fetch);
     for (int bps = 2; bps <= 8; bps *= 2) run<M_READ>("read", base, nsect, n, sink, bps);
+    for (int bps = 2; bps <= 8; bps *= 2) run<M_READ_PAIR>("read pair", base, nsect, n, sink, bps);
     run<M_READ64>("read 64-B group (2 loads)", base, nsect, n, sink);
     run<M_READ128>("read 128-B group (4 loads)", base, nsect, n, sink);
     for (int bps = 4; bps <= 8; bps *= 2) run<M_RMW>("rmw (load + store)", base, nsect, n, sink, bps);
@@ -199,6 +234,7 @@ int main(int argc, char** argv) {
     run<M_LD_ST_RED>("load + store + RED", base, nsect, n, sink);
     run<M_CAS128>("CAS.128 only", base, nsect, n, sink);
     run<M_LD_CAS128>("load + CAS.128", base, nsect, n, sink);
+    run<M_READ_PAIR_CAS128>("read pair + CAS.128", base, nsect, n, sink);
     run<M_LD_CAS128_RED>("load + CAS.128 + RED.u64", base, nsect, n, sink);
     run<M_CHAIN2>("chain of 2 dependent loads", base, nsect, 2 * n / 2, sink);
     run<M_CHAIN4>("chain of 4 dependent loads", base, nsect, n, sink);

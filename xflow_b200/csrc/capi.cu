@@ -233,9 +233,9 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   }
   XF_CUDA_TRY(cudaSetDevice(cfg->device));
   // L2 fetch granularity = one probing bucket (LR: 4 rows = one 128-byte line), so that the collision probes of
-  // a bucket (and the second half of a 32-byte sector) find the line the first load fetched.  It costs DRAM read
-  // traffic and buys time: the kernels are bound by the request rate, not by DRAM bytes (DESIGN.md section 6).  A hint: the driver may
-  // ignore it.  XFLOW_L2_FETCH = 32 / 64 / 128 overrides.
+  // a bucket find the line the first load fetched.  It costs DRAM read traffic; the kernels are bound by the request
+  // rate, not by DRAM bytes, and on the H100 32, 64 and 128 B time the same on every N = 1 bench workload (DESIGN.md
+  // section 6).  A hint: the driver may ignore it.  XFLOW_L2_FETCH = 32 / 64 / 128 overrides.
   {
     int fetch = 128;
     const char* fe = getenv("XFLOW_L2_FETCH");

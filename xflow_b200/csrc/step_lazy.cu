@@ -10,7 +10,10 @@
 // tokens.  The eager pair (step + update) needs 4.3 per token, round 1's lazy protocol (load, CAS on the tag,
 // full-sector store, RED) also 4.3 in one launch; this one 2.3:
 //   phase A  load the row (1.3 with the collision probes) and compute, in registers, the weight the batch
-//            pulls: the row's state with the pending step applied (pure function of what was loaded)
+//            pulls: the row's state with the pending step applied (pure function of what was loaded).
+//            sm_90 has no 256-bit load: a 32-byte row read by one lane is two 128-bit loads, i.e. two requests,
+//            so the probe runs convergent across the warp, one look per round for every unresolved token, and
+//            every look is a lane-pair load (xf_ld32_pair, table.cuh) that costs one request per row.
 //   phase B  after the row reduction, ONE 128-bit CAS per distinct key of the token group deposits the
 //            residual, publishes the new state and stamps the row for this batch (xf_lazy_deposit, table.cuh);
 //            a key that another token of the batch has opened already gets a 64-bit integer add instead.
@@ -22,6 +25,9 @@
 // Tried on the 1e8-id table: bucketised probing (collision probes inside one 128-byte line: faster, kept), L2
 // prefetch by dedicated warps running ahead (slower: the prefetches are requests too, removed), claim + publish
 // in one CAS.128 with a separate RED (3.3 instructions per token: between round 1's protocol and this one).
+// On the H100 the rule above holds only in part: a lane-pair row look runs at 1.4x the rate of a one-lane one,
+// not 2x, and an atomic costs about 2.5 paired looks (tools/membench.cu), so phase B's CAS.128 sets most of the
+// kernel's time.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -32,6 +38,34 @@
 #define XF_NO_SLOT 0xFFFFFFFFu
 #define XF_LAZY_CACHED 2  // 64-token chunks whose group leaders keep their look at the row for phase B
 
+// One step of xf_probe_from<true> for a token of `key` whose probe number i is at slot s and whose look at that
+// row is (q0..q3).  Returns true when the token is resolved: found (slot = s), inserted (q0..q3 = what xf_k_fill
+// left in the row with the key claimed, *created = true), or out of probes (slot stays XF_NO_SLOT, *t.error = 1).
+// Otherwise s and i move on to the next probe slot, which the caller loads.
+__device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key, uint64_t& s, uint32_t& i, uint64_t& q0,
+                                             uint64_t& q1, uint64_t& q2, uint64_t& q3, uint32_t& slot, bool& created) {
+  if (q0 == key) { slot = (uint32_t)s; return true; }
+  if (q0 == XF_EMPTY_KEY) {
+    const unsigned long long old =
+        atomicCAS(reinterpret_cast<unsigned long long*>(xf_row(t, s)), (unsigned long long)XF_EMPTY_KEY, (unsigned long long)key);
+    if (old == XF_EMPTY_KEY) {
+      created = true;
+      q0 = key; q1 = q2 = q3 = 0ull;  // lazy rows: g is the integer 0, no state, no tag
+      slot = (uint32_t)s;
+      return true;
+    }
+    if (old == key) {  // raced with another inserter of the same key: the other fields are still what was loaded
+      q0 = key;
+      slot = (uint32_t)s;
+      return true;
+    }
+    // a different key took the slot: on to the next one
+  }
+  if (++i == XF_MAX_PROBE) { *t.error = 1; return true; }
+  s = xf_probe_slot(t, key, i);
+  return false;
+}
+
 __global__ void __launch_bounds__(256, 3)
 xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
                   const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
@@ -39,6 +73,9 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
                   unsigned long long* __restrict__ unique_total) {
   __shared__ float s_abs[8];
   __shared__ unsigned int s_open;
+  // the group leaders' looks at their rows, from phase A to phase B.  In registers they took the kernel past the
+  // 80 registers that 3 CTAs of 256 threads per SM leave it, and it spilled.
+  __shared__ uint64_t s_q2[2 * XF_LAZY_CACHED][256], s_q3[2 * XF_LAZY_CACHED][256], s_q2n[2 * XF_LAZY_CACHED][256];
   if (threadIdx.x == 0) s_open = 0;
   if (blockIdx.x == 0 && threadIdx.x == 0 && mode == 0) rows_by_seq[seq] = (uint32_t)B;  // read by later batches only
   __syncthreads();
@@ -56,13 +93,12 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
     float wsum = 0.f;
     // first XF_LAZY_CACHED chunks (rows <= 128 tokens), per half: if this lane leads its group of equal slots,
     // the slot, the group size, and the row's second half as it looked (old) and as it will be published (new)
+    // (the old and new second halves live in shared memory: s_q2 / s_q3 / s_q2n, indexed like lead_s)
     uint32_t lead_s[2 * XF_LAZY_CACHED];
     uint32_t cnt_c[XF_LAZY_CACHED];  // 8 bits per half
-    uint64_t q2_c[2 * XF_LAZY_CACHED], q3_c[2 * XF_LAZY_CACHED], q2n_c[2 * XF_LAZY_CACHED];
 #pragma unroll
     for (int c = 0; c < XF_LAZY_CACHED; ++c) {
       lead_s[2 * c] = lead_s[2 * c + 1] = XF_NO_SLOT;
-      q2_c[2 * c] = q2_c[2 * c + 1] = q3_c[2 * c] = q3_c[2 * c + 1] = q2n_c[2 * c] = q2n_c[2 * c + 1] = 0ull;
       cnt_c[c] = 0;
     }
 
@@ -73,23 +109,32 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       const bool v0 = j0 < end, v1 = j1 < end;
       const uint64_t k0 = v0 ? __ldcs(keys + j0) : 0ull;
       const uint64_t k1 = v1 ? __ldcs(keys + j1) : 0ull;
-      const uint64_t p0 = xf_home_slot(t, k0), p1 = xf_home_slot(t, k1);
-      XfHead h0, h1;
-      h0.key = h1.key = XF_EMPTY_KEY;
-      h0.flags = h1.flags = 0u;
-      h0.w = h0.n = h0.z = h1.w = h1.n = h1.z = 0.f;
-      h0.g = h1.g = 0.0;
-      if (v0) h0 = xf_load_head(xf_row(t, p0));
-      if (v1) h1 = xf_load_head(xf_row(t, p1));
-      uint32_t s0 = XF_NO_SLOT, s1 = XF_NO_SLOT;
-      if (v0) { const int64_t r = xf_probe_from<true>(t, k0, p0, h0); if (r >= 0) s0 = (uint32_t)r; }
-      if (v1) { const int64_t r = xf_probe_from<true>(t, k1, p1, h1); if (r >= 0) s1 = (uint32_t)r; }
+      uint64_t p0 = xf_home_slot(t, k0), p1 = xf_home_slot(t, k1);
+      // the probe (xf_probe_from<true>), one look per round for every token of the warp that is still unresolved,
+      // so that every look is a lane-pair load
+      uint64_t a0, a1, a2, a3, b0, b1, b2, b3;
+      xf_ld32_pair(v0 ? xf_row(t, p0) : nullptr, a0, a1, a2, a3);
+      xf_ld32_pair(v1 ? xf_row(t, p1) : nullptr, b0, b1, b2, b3);
+      uint32_t s0 = XF_NO_SLOT, s1 = XF_NO_SLOT, i0 = 0, i1 = 0;
+      bool u0 = v0, u1 = v1;
+      for (;;) {
+        bool c0 = false, c1 = false;
+        if (u0) u0 = !xf_lazy_look(t, k0, p0, i0, a0, a1, a2, a3, s0, c0);
+        if (u1) u1 = !xf_lazy_look(t, k1, p1, i1, b0, b1, b2, b3, s1, c1);
+        const unsigned created = __popc(__ballot_sync(0xffffffffu, c0)) + __popc(__ballot_sync(0xffffffffu, c1));
+        if (created && lane == 0) atomicAdd(t.size, (unsigned long long)created);
+        if (!__any_sync(0xffffffffu, u0 || u1)) break;
+        uint64_t x0, x1, x2, x3;
+        xf_ld32_pair(u0 ? xf_row(t, p0) : nullptr, x0, x1, x2, x3);
+        if (u0) { a0 = x0; a1 = x1; a2 = x2; a3 = x3; }
+        xf_ld32_pair(u1 ? xf_row(t, p1) : nullptr, x0, x1, x2, x3);
+        if (u1) { b0 = x0; b1 = x1; b2 = x2; b3 = x3; }
+      }
       // the weight this batch pulls = the row with its pending step applied (computed, not stored)
-      const uint64_t a2 = xf_raw_q2(h0), a3 = xf_raw_q3(h0), b2 = xf_raw_q2(h1), b3 = xf_raw_q3(h1);
       uint64_t a2n = a2, b2n = b2;
       float w0 = 0.f, w1 = 0.f;
-      if (s0 != XF_NO_SLOT) w0 = xf_lazy_fold(t, xf_raw_q1(h0), a2, a3, mode == 1 ? 0xFFFFFFFFu : seq, a2n);
-      if (s1 != XF_NO_SLOT) w1 = xf_lazy_fold(t, xf_raw_q1(h1), b2, b3, mode == 1 ? 0xFFFFFFFFu : seq, b2n);
+      if (s0 != XF_NO_SLOT) w0 = xf_lazy_fold(t, a1, a2, a3, mode == 1 ? 0xFFFFFFFFu : seq, a2n);
+      if (s1 != XF_NO_SLOT) w1 = xf_lazy_fold(t, b1, b2, b3, mode == 1 ? 0xFFFFFFFFu : seq, b2n);
       wsum += w0;
       wsum += w1;
       if (mode == 1) continue;
@@ -107,10 +152,12 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
         if (ch == c) {
           lead_s[2 * c] = L0 ? s0 : XF_NO_SLOT;
           lead_s[2 * c + 1] = L1 ? s1 : XF_NO_SLOT;
-          q2_c[2 * c] = a2; q3_c[2 * c] = a3; q2n_c[2 * c] = a2n;
-          q2_c[2 * c + 1] = b2; q3_c[2 * c + 1] = b3; q2n_c[2 * c + 1] = b2n;
           cnt_c[c] = (L0 ? (uint32_t)__popc(grp0) : 0u) | ((L1 ? (uint32_t)__popc(grp1) : 0u) << 8);
         }
+      if (ch < XF_LAZY_CACHED) {
+        if (L0) { s_q2[2 * ch][threadIdx.x] = a2; s_q3[2 * ch][threadIdx.x] = a3; s_q2n[2 * ch][threadIdx.x] = a2n; }
+        if (L1) { s_q2[2 * ch + 1][threadIdx.x] = b2; s_q3[2 * ch + 1][threadIdx.x] = b3; s_q2n[2 * ch + 1][threadIdx.x] = b2n; }
+      }
     }
 
     const float wx = xf_warp_sum(wsum);
@@ -126,11 +173,13 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
     const long long lf = xf_fix_of(loss);
 #pragma unroll
     for (int c = 0; c < XF_LAZY_CACHED; ++c) {
+      const int x = threadIdx.x;
       if (lead_s[2 * c] != XF_NO_SLOT &&
-          xf_lazy_deposit(t, xf_row(t, lead_s[2 * c]), q2_c[2 * c], q3_c[2 * c], q2n_c[2 * c], seq, lf * (long long)(cnt_c[c] & 0xFFu)))
+          xf_lazy_deposit(t, xf_row(t, lead_s[2 * c]), s_q2[2 * c][x], s_q3[2 * c][x], s_q2n[2 * c][x], seq,
+                          lf * (long long)(cnt_c[c] & 0xFFu)))
         ++open_acc;
       if (lead_s[2 * c + 1] != XF_NO_SLOT &&
-          xf_lazy_deposit(t, xf_row(t, lead_s[2 * c + 1]), q2_c[2 * c + 1], q3_c[2 * c + 1], q2n_c[2 * c + 1], seq,
+          xf_lazy_deposit(t, xf_row(t, lead_s[2 * c + 1]), s_q2[2 * c + 1][x], s_q3[2 * c + 1][x], s_q2n[2 * c + 1][x], seq,
                           lf * (long long)(cnt_c[c] >> 8)))
         ++open_acc;
     }

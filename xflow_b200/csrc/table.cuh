@@ -169,10 +169,11 @@ struct XfHead {
   double g;
 };
 
-// One 32-byte sector as two 128-bit loads issued back to back (sm_90 has no 256-bit LDG): both are in flight at
-// once, and with the L2 fetch granularity at 128 B (xf_table_create) the second finds the line the first one
-// brought into L2.  Each half is one 16-byte access, which is what the lazy protocol's 128-bit CAS on bytes
-// 16..31 compares against.
+// One 32-byte sector as two 128-bit loads from the same lane (sm_90 has no 256-bit LDG).  That is two
+// instructions, and so two memory requests, per row: on a random multi-GB table it costs twice what one row look
+// could (tools/membench.cu, "read" against "read pair"); xf_ld32_pair below reads the same rows with each
+// instruction serving half the lanes' rows.  Each half is one 16-byte access, which is what the lazy protocol's
+// 128-bit CAS on bytes 16..31 compares against.
 __device__ __forceinline__ void xf_ld32_cg(const void* p, uint64_t& q0, uint64_t& q1, uint64_t& q2, uint64_t& q3) {
   asm volatile("ld.global.cg.v2.u64 {%0,%1}, [%4];\n\tld.global.cg.v2.u64 {%2,%3}, [%4+16];"
                : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
@@ -180,6 +181,27 @@ __device__ __forceinline__ void xf_ld32_cg(const void* p, uint64_t& q0, uint64_t
 __device__ __forceinline__ void xf_ld32_ca(const void* p, uint64_t& q0, uint64_t& q1, uint64_t& q2, uint64_t& q3) {
   asm volatile("ld.global.ca.v2.u64 {%0,%1}, [%4];\n\tld.global.ca.v2.u64 {%2,%3}, [%4+16];"
                : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+}
+// The row at `mine` (nullptr: none; the result is then zero) read by lane PAIRS, through L2: lanes 2i and 2i+1
+// each load one 16-byte half of the even lane's row in one instruction and of the odd lane's row in a second, then
+// swap halves, so each lane ends up with its own whole row.  Still two LDG.128 per lane, but each instruction
+// touches 16 rows rather than 32, which halves the requests per row (tools/membench.cu).  Both loads are issued
+// before the swap, so they are in flight together.  All 32 lanes of the warp must call it together.
+__device__ __forceinline__ void xf_ld32_pair(const uint8_t* mine, uint64_t& q0, uint64_t& q1, uint64_t& q2, uint64_t& q3) {
+  const uint32_t odd = threadIdx.x & 1u;
+  const uint8_t* other = (const uint8_t*)__shfl_xor_sync(0xffffffffu, (unsigned long long)mine, 1);
+  const uint8_t* r0 = odd ? other : mine;  // the even lane's row
+  const uint8_t* r1 = odd ? mine : other;  // the odd lane's row
+  uint64_t x0 = 0, x1 = 0, y0 = 0, y1 = 0;
+  asm volatile("{\n .reg .pred p0, p1;\n setp.ne.u64 p0, %4, 0;\n setp.ne.u64 p1, %5, 0;\n"
+               " @p0 ld.global.cg.v2.u64 {%0,%1}, [%6];\n @p1 ld.global.cg.v2.u64 {%2,%3}, [%7];\n}"
+               : "+l"(x0), "+l"(x1), "+l"(y0), "+l"(y1)
+               : "l"(r0), "l"(r1), "l"(r0 + 16 * odd), "l"(r1 + 16 * odd));
+  const uint64_t m0 = odd ? y0 : x0, m1 = odd ? y1 : x1;  // this lane's half of its own row
+  const uint64_t t0 = __shfl_xor_sync(0xffffffffu, odd ? x0 : y0, 1);
+  const uint64_t t1 = __shfl_xor_sync(0xffffffffu, odd ? x1 : y1, 1);
+  q0 = odd ? t0 : m0; q1 = odd ? t1 : m1;
+  q2 = odd ? m0 : t0; q3 = odd ? m1 : t1;
 }
 // the whole sector written by two 128-bit stores (no read-for-fill: L2 merges them into one full sector)
 __device__ __forceinline__ void xf_st32(void* p, uint64_t q0, uint64_t q1, uint64_t q2, uint64_t q3) {
