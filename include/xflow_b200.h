@@ -133,6 +133,42 @@ XF_DLL int xf_table_dump_text(xf_table* t, const char* path, int nonzero_only, u
 XF_DLL int xf_table_set_stream(xf_table* t, void* cuda_stream);
 XF_DLL int xf_table_sync(xf_table* t);
 
+/* Feature admission (McMahan et al., "Ad Click Prediction: a View from the Trenches", section 5.1).  A per-table
+ * policy for the keys that TRAINING STEPS insert; explicit pull / push / import / load, xf_table_touch_decimal_ids,
+ * xf_trainer_init_push and the ps-lite functors still insert as `store[key]` does.  The table numbers its training
+ * batches b = 0, 1, 2, ...; in batch b a token whose key is absent from the table is
+ *   XF_ADMIT_ALL      inserted (the default: today's behaviour);
+ *   XF_ADMIT_POISSON  inserted iff u24(key, b) < floor(probability * 2^24), u24 = the top 24 bits of
+ *                     splitmix64(key ^ splitmix64(seed + b)) (all tokens of one key in one batch decide alike);
+ *   XF_ADMIT_BLOOM    inserted iff min_j cell[c_j] >= threshold, over the key's cells
+ *                     c_j = top log2_cells bits of splitmix64(key ^ splitmix64(seed + (j+1) * 0x9E3779B97F4A7C15)),
+ *                     j < hashes, in 2^log2_cells one-byte counters as they stood BEFORE batch b.  After the step
+ *                     every rejected token adds 1 to each of its cells (once per j), saturating at 255; then, if
+ *                     decay_batches > 0 and (b+1) % decay_batches == 0, every cell is halved.
+ * A rejected token reads as a row of zeros that nobody updates: w = 0 (FM: v = 0), no gradient, no optimizer step,
+ * not counted in unique_keys.  An admitted key starts as an inserted key always does.  With a policy other than
+ * XF_ADMIT_ALL, predict never inserts: an absent key contributes 0.
+ * Single-GPU tables only: refused on canonical tables (canonical_fm = 1), on tables with num_shards > 1, and by
+ * xf_trainer_create with a multi-rank comm.  The filter lives in device memory owned by the table (2^log2_cells
+ * bytes) and is NOT part of xf_table_save / xf_table_load: a resumed run starts with an empty filter. */
+enum { XF_ADMIT_ALL = 0, XF_ADMIT_POISSON = 1, XF_ADMIT_BLOOM = 2 };
+typedef struct xf_admission_config {
+  int mode;                /* XF_ADMIT_* */
+  float probability;       /* POISSON: 0..1 */
+  uint32_t threshold;      /* BLOOM: 1..255 occurrences before a key is admitted */
+  uint32_t log2_cells;     /* BLOOM: 10..36 (2^log2_cells bytes of filter) */
+  uint32_t hashes;         /* BLOOM: 1..8 */
+  uint64_t decay_batches;  /* BLOOM: halve the filter every decay_batches training batches; 0 = never */
+  uint64_t seed;
+} xf_admission_config;
+/* mode XF_ADMIT_ALL, probability 1, threshold 2, log2_cells 30, hashes 3, decay_batches 0, seed 0 */
+XF_DLL int xf_admission_config_default(xf_admission_config* cfg);
+/* replaces the table's policy and clears the filter (XF_ADMIT_ALL frees it); on failure the table is unchanged */
+XF_DLL int xf_table_set_admission(xf_table* t, const xf_admission_config* cfg);
+/* since the table was created: training batches, rejected tokens, keys inserted by admission (any pointer may be
+ * NULL; reads device counters, waits for the table's stream) */
+XF_DLL int xf_table_admission_stats(xf_table* t, uint64_t* batches, uint64_t* rejected_tokens, uint64_t* admitted_keys);
+
 /* bucketing rule of ps::Postoffice::GetServerKeyRanges (postoffice.cc:134-143) + DefaultSlicer
  * (kv_app.h:405-460): shard = min(key / floor((2^64-1)/S), S-1).  Pure host function. */
 XF_DLL int xf_shard_of(uint64_t key, int num_shards);

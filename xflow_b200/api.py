@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libxflow_b200.so")
 MODEL_LR, MODEL_FM, MODEL_FM_CANONICAL, MODEL_MVM = 0, 1, 2, 3
 OPT_FTRL, OPT_SGD = 0, 1
 VINIT_DEFAULT, VINIT_COUNTER, VINIT_ZERO = 0, 1, 3
+ADMIT_ALL, ADMIT_POISSON, ADMIT_BLOOM = 0, 1, 2
 COMM_ID_BYTES = 128
 
 _lib = None
@@ -28,6 +29,11 @@ class TableConfig(C.Structure):
                 ("beta", C.c_float), ("lambda1", C.c_float), ("lambda2", C.c_float),
                 ("learning_rate", C.c_float), ("v_init", C.c_int), ("seed", C.c_uint64),
                 ("capacity", C.c_uint64), ("shard_index", C.c_int), ("num_shards", C.c_int), ("canonical_fm", C.c_int)]
+
+
+class AdmissionConfig(C.Structure):
+    _fields_ = [("mode", C.c_int), ("probability", C.c_float), ("threshold", C.c_uint32), ("log2_cells", C.c_uint32),
+                ("hashes", C.c_uint32), ("decay_batches", C.c_uint64), ("seed", C.c_uint64)]
 
 
 class TrainerConfig(C.Structure):
@@ -60,6 +66,9 @@ SIGNATURES = {
     "xf_table_load": (_i, [_vp, C.c_char_p]),
     "xf_table_set_stream": (_i, [_vp, _vp]),
     "xf_table_sync": (_i, [_vp]),
+    "xf_admission_config_default": (_i, [_vp]),
+    "xf_table_set_admission": (_i, [_vp, _vp]),
+    "xf_table_admission_stats": (_i, [_vp, _vp, _vp, _vp]),
     "xf_shard_of": (_i, [_u64, _i]),
     "xf_trainer_create": (_i, [_vp, _vp, _vp, _vp]),
     "xf_trainer_destroy": (_i, [_vp]),
@@ -324,6 +333,25 @@ class Table:
 
     def sync(self):
         _check(lib().xf_table_sync(self.h))
+
+    def set_admission(self, mode, probability=None, threshold=None, log2_cells=None, hashes=None, decay_batches=None,
+                      seed=None):
+        """Feature admission of the keys training steps insert (ADMIT_ALL / ADMIT_POISSON / ADMIT_BLOOM); replaces
+        the policy and clears the filter.  Unset fields keep xf_admission_config_default's values."""
+        cfg = AdmissionConfig()
+        _check(lib().xf_admission_config_default(C.byref(cfg)))
+        cfg.mode = mode
+        for k, v in dict(probability=probability, threshold=threshold, log2_cells=log2_cells, hashes=hashes,
+                         decay_batches=decay_batches, seed=seed).items():
+            if v is not None:
+                setattr(cfg, k, v)
+        _check(lib().xf_table_set_admission(self.h, C.byref(cfg)))
+
+    def admission_stats(self):
+        """Training batches, rejected tokens and keys admitted since the table was created."""
+        a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        _check(lib().xf_table_admission_stats(self.h, C.byref(a), C.byref(b), C.byref(c)))
+        return dict(batches=a.value, rejected_tokens=b.value, admitted_keys=c.value)
 
 
 class Comm:

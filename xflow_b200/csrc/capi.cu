@@ -294,12 +294,103 @@ XF_DLL int xf_table_destroy(xf_table* t) {
   cudaFree(t->d_size);
   cudaFree(t->d_error);
   if (t->d_rows_by_seq) cudaFree(t->d_rows_by_seq);
+  if (t->d_filter) cudaFree(t->d_filter);
+  if (t->d_admit) cudaFree(t->d_admit);
   if (t->h_size_ring) cudaFreeHost(t->h_size_ring);
   for (int i = 0; i < 4; ++i) if (t->size_ev[i]) cudaEventDestroy(t->size_ev[i]);
   t->s_keys.release(); t->s_slots.release(); t->s_w.release(); t->s_v.release();
   t->s_nw.release(); t->s_zw.release(); t->s_nv.release(); t->s_zv.release(); t->s_present.release();
   if (t->own_stream && t->stream) cudaStreamDestroy(t->stream);
   delete t;
+  return XF_OK;
+}
+
+// -------------------------------------------------------------------------------------------------
+// feature admission (admit.cu; semantics in include/xflow_b200.h)
+// -------------------------------------------------------------------------------------------------
+XF_DLL int xf_admission_config_default(xf_admission_config* cfg) {
+  if (!cfg) return XF_ERR_ARG;
+  memset(cfg, 0, sizeof(*cfg));
+  cfg->mode = XF_ADMIT_ALL;
+  cfg->probability = 1.0f;
+  cfg->threshold = 2;
+  cfg->log2_cells = 30;
+  cfg->hashes = 3;
+  cfg->decay_batches = 0;
+  cfg->seed = 0;
+  return XF_OK;
+}
+
+XF_DLL int xf_table_set_admission(xf_table* t, const xf_admission_config* cfg) {
+  if (!t || !cfg) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (cfg->mode != XF_ADMIT_ALL && cfg->mode != XF_ADMIT_POISSON && cfg->mode != XF_ADMIT_BLOOM) {
+    xf_set_error("admission mode %d is not XF_ADMIT_ALL, XF_ADMIT_POISSON or XF_ADMIT_BLOOM", cfg->mode);
+    return XF_ERR_ARG;
+  }
+  if (cfg->mode == XF_ADMIT_POISSON && !(cfg->probability >= 0.0f && cfg->probability <= 1.0f)) {
+    xf_set_error("admission probability %g is outside [0, 1]", (double)cfg->probability);
+    return XF_ERR_ARG;
+  }
+  if (cfg->mode == XF_ADMIT_BLOOM) {
+    if (cfg->threshold < 1 || cfg->threshold > 255) { xf_set_error("admission threshold %u is outside 1..255", cfg->threshold); return XF_ERR_ARG; }
+    if (cfg->log2_cells < 10 || cfg->log2_cells > 36) { xf_set_error("admission log2_cells %u is outside 10..36", cfg->log2_cells); return XF_ERR_ARG; }
+    if (cfg->hashes < 1 || cfg->hashes > XF_ADM_MAX_HASHES) { xf_set_error("admission hashes %u is outside 1..8", cfg->hashes); return XF_ERR_ARG; }
+  }
+  if (cfg->mode != XF_ADMIT_ALL && t->cfg.canonical_fm) {
+    xf_set_error("feature admission does not serve canonical tables (canonical_fm = 1)");
+    return XF_ERR_ARG;
+  }
+  if (cfg->mode != XF_ADMIT_ALL && t->cfg.num_shards > 1) {
+    xf_set_error("feature admission needs a single-shard table (this one is shard %d of %d)", t->cfg.shard_index,
+                 t->cfg.num_shards);
+    return XF_ERR_ARG;
+  }
+  XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
+  XF_CUDA_TRY(cudaStreamSynchronize(t->stream));  // steps in flight may still read the old filter
+  // allocate first, so that a failure leaves the table as it was
+  if (!t->d_admit && cfg->mode != XF_ADMIT_ALL) {
+    unsigned long long* c = nullptr;
+    if (cudaMalloc(&c, 4 * sizeof(unsigned long long)) != cudaSuccess) {
+      cudaGetLastError();
+      xf_set_error("cannot allocate the admission counters");
+      return XF_ERR_CUDA;
+    }
+    XF_CUDA_TRY(cudaMemsetAsync(c, 0, 4 * sizeof(unsigned long long), t->stream));
+    t->d_admit = c;
+  }
+  uint8_t* filter = nullptr;
+  if (cfg->mode == XF_ADMIT_BLOOM) {
+    const size_t bytes = (size_t)1 << cfg->log2_cells;
+    if (cudaMalloc(&filter, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      xf_set_error("cannot allocate the admission filter (2^%u bytes)", cfg->log2_cells);
+      return XF_ERR_CUDA;
+    }
+    if (cudaMemsetAsync(filter, 0, bytes, t->stream) != cudaSuccess) {
+      cudaGetLastError();
+      cudaFree(filter);
+      xf_set_error("cannot clear the admission filter");
+      return XF_ERR_CUDA;
+    }
+  }
+  if (t->d_filter) cudaFree(t->d_filter);
+  t->d_filter = filter;
+  t->admit = *cfg;
+  if (t->d_admit) XF_CUDA_TRY(cudaMemsetAsync(t->d_admit + 2, 0, 2 * sizeof(unsigned long long), t->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(t->stream));
+  return XF_OK;
+}
+
+XF_DLL int xf_table_admission_stats(xf_table* t, uint64_t* batches, uint64_t* rejected_tokens, uint64_t* admitted_keys) {
+  if (!t) return XF_ERR_ARG;
+  unsigned long long c[2] = {0ull, 0ull};
+  if (t->d_admit) {
+    XF_CUDA_TRY(cudaMemcpyAsync(c, t->d_admit, sizeof(c), cudaMemcpyDeviceToHost, t->stream));
+    XF_CUDA_TRY(cudaStreamSynchronize(t->stream));
+  }
+  if (batches) *batches = t->admit_batches;
+  if (rejected_tokens) *rejected_tokens = c[0];
+  if (admitted_keys) *admitted_keys = c[1];
   return XF_OK;
 }
 
@@ -714,6 +805,11 @@ XF_DLL int xf_trainer_create(xf_trainer** out, xf_table* table, xf_comm* comm, c
   // kernels of comm.cu under ncu, which cannot wrap a multi-rank command)
   const char* force_mg = getenv("XFLOW_MG_FORCE");
   if (comm && (xf_comm_nranks(comm) > 1 || (force_mg && *force_mg == '1'))) {
+    if (table->admit.mode != XF_ADMIT_ALL) {
+      xf_set_error("feature admission is single-GPU only: the sharded step cannot serve a table with a policy");
+      delete tr;
+      return XF_ERR_ARG;
+    }
     if (table->cfg.num_shards != xf_comm_nranks(comm) || table->cfg.shard_index != xf_comm_rank(comm)) {
       xf_set_error("table shard (%d of %d) does not match comm rank (%d of %d)", table->cfg.shard_index,
                    table->cfg.num_shards, xf_comm_rank(comm), xf_comm_nranks(comm));
@@ -740,7 +836,7 @@ XF_DLL int xf_trainer_destroy(xf_trainer* tr) {
     b.h_row_ptr.release(); b.h_keys.release(); b.h_labels.release();
     cudaEventDestroy(b.copied); cudaEventDestroy(b.consumed); cudaEventDestroy(b.staged);
   }
-  tr->touched.release(); tr->loss.release(); tr->pctr.release();
+  tr->touched.release(); tr->loss.release(); tr->pctr.release(); tr->rejected.release();
   cudaStreamSynchronize(tr->ing_copy_stream);
   cudaStreamSynchronize(tr->ing_stream);
   for (int i = 0; i < 2; ++i) {
@@ -772,11 +868,55 @@ static int xf_check_batch(xf_trainer* tr, uint32_t rows, uint32_t nnz) {
   return XF_OK;
 }
 
+// The admission policy a step of `mode` asks (xf_table_set_admission): Poisson and Bloom decide in the step kernel;
+// predict inserts nothing.  Bloom steps append their rejected tokens to the trainer's list for the count pass.
+static int xf_admit_view(xf_trainer* tr, int mode, XfAdmitView& a) {
+  xf_table* t = tr->table;
+  const xf_admission_config& c = t->admit;
+  memset(&a, 0, sizeof(a));
+  a.mode = mode == 1 ? XF_ADM_NEVER : c.mode;
+  a.p24 = (uint32_t)floor((double)c.probability * 16777216.0);
+  a.batch_mix = xf_splitmix64(c.seed + t->admit_batches);
+  a.threshold = c.threshold;
+  a.log2_cells = c.log2_cells;
+  a.hashes = c.hashes;
+  a.seed = c.seed;
+  a.cells = t->d_filter;
+  a.admitted = t->d_admit + 1;
+  a.rej_n = t->d_admit;  // Poisson: only counted
+  if (c.mode == XF_ADMIT_BLOOM) {
+    XF_TRY(tr->rejected.ensure((size_t)tr->cfg.max_nnz * sizeof(uint64_t)));
+    a.rej_n = t->d_admit + 2 + (t->admit_batches & 1);
+    a.rej_keys = tr->rejected.as<uint64_t>();
+  }
+  return XF_OK;
+}
+
+// after a training step: the Bloom filter counts the step's rejected tokens and decays; the batch number moves on
+static void xf_admit_after_step(xf_trainer* tr, const XfAdmitView* adm, uint32_t nnz) {
+  xf_table* t = tr->table;
+  if (adm && t->admit.mode == XF_ADMIT_BLOOM) {
+    const uint64_t b = t->admit_batches;
+    xf_launch_admit_count(*adm, t->d_filter, adm->rej_keys, adm->rej_n, nnz, t->d_admit, t->d_admit + 2 + ((b + 1) & 1),
+                          t->stream);
+    ++tr->launches;
+    if (t->admit.decay_batches && (b + 1) % t->admit.decay_batches == 0) {
+      xf_launch_admit_decay(t->d_filter, t->admit.log2_cells, t->stream);
+      ++tr->launches;
+    }
+  }
+  ++t->admit_batches;
+}
+
 // the step proper, on device-resident CSR; mode 0 = train, 1 = predict
 static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                const uint8_t* d_labels, uint32_t rows, uint32_t nnz, int mode, float* d_abs,
                                const float* d_vals = nullptr, const uint8_t* d_fields = nullptr) {
   xf_table* t = tr->table;
+  if (tr->mg && t->admit.mode != XF_ADMIT_ALL) {
+    xf_set_error("feature admission is single-GPU only: the sharded step cannot serve a table with a policy");
+    return XF_ERR_ARG;
+  }
   if (rows == 0 && !tr->mg) return XF_OK;     // sharded: an empty batch still takes part in the exchange
   if (!tr->mg) XF_TRY(t->ensure_room(nnz));  // the sharded path sizes the shard from what it receives
   cudaStream_t st = t->stream;
@@ -794,18 +934,25 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     if (tr->mg) return xf_mg_step(tr, d_row_ptr, d_keys, d_labels, rows, nnz, mode, d_abs, pe);
     XF_CUDA_TRY(cudaEventRecord(pe[0], st));
   }
+  XfAdmitView adm_v;
+  const XfAdmitView* adm = nullptr;  // nullptr: every absent key is inserted (the kernels without admission)
+  if (t->admit.mode != XF_ADMIT_ALL) {
+    XF_TRY(xf_admit_view(tr, mode, adm_v));
+    adm = &adm_v;
+  }
   if (t->view.lazy) {
     // one kernel: the optimizer step of earlier batches is folded in as rows are touched
     if (mode == 0) XF_TRY(t->next_seq());
     xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, t->seq, t->d_rows_by_seq,
                            (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                           mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, st);
+                           mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, adm, st);
     ++tr->launches;
     if (prof) {
       XF_CUDA_TRY(cudaEventRecord(pe[1], st));
       XF_CUDA_TRY(cudaEventRecord(pe[2], st));
       XF_CUDA_TRY(cudaEventRecord(pe[3], st));
     }
+    if (mode == 0) xf_admit_after_step(tr, adm, nnz);
     XF_CUDA_TRY(cudaGetLastError());
     return XF_OK;
   }
@@ -825,7 +972,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   else
     xf_launch_step(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(), nnz,
                    (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                   mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, st);
+                   mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, adm, st);
   ++tr->launches;
   if (prof) {
     XF_CUDA_TRY(cudaEventRecord(pe[1], st));
@@ -838,6 +985,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     ++tr->launches;
   }
   if (prof) XF_CUDA_TRY(cudaEventRecord(pe[3], st));
+  if (mode == 0) xf_admit_after_step(tr, adm, nnz);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }

@@ -75,6 +75,11 @@ struct xf_table {
   // (kv_app.h:110-165) those entry points may be called from several threads: serialised by this mutex
   std::mutex host_mu;
   XfDevBuf s_keys, s_slots, s_w, s_v, s_nw, s_zw, s_nv, s_zv, s_present;
+  // feature admission (xf_table_set_admission, admit.cu): the policy, the Bloom filter, the training-batch number b
+  xf_admission_config admit{};                // mode XF_ADMIT_ALL
+  uint8_t* d_filter = nullptr;                // 2^log2_cells one-byte counters (XF_ADMIT_BLOOM only)
+  unsigned long long* d_admit = nullptr;      // {rejected tokens, admitted keys, rejected-list length of even / odd b}
+  uint64_t admit_batches = 0;
 
   int alloc_table(uint64_t capacity);
   int ensure_room(uint64_t incoming_keys);
@@ -98,6 +103,7 @@ struct xf_trainer {
   XfBatchBuf buf[2];
   uint64_t step_index = 0;
   XfDevBuf touched, loss, pctr;
+  XfDevBuf rejected;                    // keys of the rejected tokens of the current step (max_nnz; Bloom admission only)
   unsigned long long* d_unique_total = nullptr;
   float* d_abs_loss = nullptr;          // 2 slots
   float* h_abs_loss = nullptr;          // pinned, 2 slots

@@ -12,7 +12,13 @@ int xf_tps_for(int K);
 void xf_launch_fill(const XfTableView& t, cudaStream_t st);
 void xf_launch_step(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels,
                     int B, int mode, uint32_t* touched, uint32_t nnz, float* loss_out, float* pctr_out,
-                    float* abs_loss_sum, cudaStream_t st);
+                    float* abs_loss_sum, const XfAdmitView* adm, cudaStream_t st);
+// feature admission (admit.cu): after a step on the table's stream, count the batch's rejected tokens into the
+// Bloom filter (n = *rej_n of them in rej_keys, at most nnz), add n to *rejected_total and zero *next_rej_n
+void xf_launch_admit_count(const XfAdmitView& a, uint8_t* cells, const uint64_t* rej_keys, const unsigned long long* rej_n,
+                           uint32_t nnz, unsigned long long* rejected_total, unsigned long long* next_rej_n, cudaStream_t st);
+// halve every counter of the Bloom filter (2^log2_cells bytes)
+void xf_launch_admit_decay(uint8_t* cells, uint32_t log2_cells, cudaStream_t st);
 // FM step: shared-memory hot-key cache; its flush uses touched[nnz .. nnz + xf_step_touched_extra)
 uint32_t xf_step_touched_extra(int K, int B);
 // touched[j] (one entry per token position) = slot of the key first touched by token j, else 0xFFFFFFFF
@@ -35,7 +41,7 @@ int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm);
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
-                            cudaStream_t st);
+                            const XfAdmitView* adm, cudaStream_t st);
 
 // lazy tables: fold all pending steps (sequence numbers restart afterwards)
 void xf_launch_flush_pending(const XfTableView& t, cudaStream_t st);

@@ -2,7 +2,8 @@
 // slice and returning from the last Push (src/model/lr/lr_worker.cc:121-177, fm/fm_worker.cc:126-245)
 // WITHOUT the reference's sort / unique / merge-join: the table row is the per-key accumulator.
 //
-//   CSR slice -> probe/insert every token's key (Pull semantics: missing keys are created)
+//   CSR slice -> probe/insert every token's key (Pull semantics: missing keys are created; with a feature-admission
+//                policy only the keys it admits, admit.cu)
 //             -> w (and for FM the latent row reduced to sum_k v, sum_k v^2) from the row just found
 //             -> per-row warp-segmented sums -> clamped sigmoid -> residual  (calculate_loss)
 //             -> every token adds its contribution to its key's gradient accumulators with L2
@@ -77,12 +78,14 @@ __device__ __forceinline__ void xf_fm_token(const XfTableView& t, uint32_t slot,
 // Per (group of) token(s) the step adds three doubles to the key: G (the w-gradient), L = loss and
 // Aq = loss * S (the factorised latent gradient, table.cuh); loss * S is exact in double.
 //   mode: 0 = train, 1 = predict (forward only; the Pull still inserts missing keys, lr_worker.cc:47)
-template <bool FM, int VEC>
+// ADMIT: absent keys are inserted only if the admission policy `adm` admits them (xf_probe_from); a rejected token
+// adds nothing to its row's sums and never reaches the hot-key cache or touched[] (its slot stays XF_NO_SLOT).
+template <bool FM, int VEC, bool ADMIT>
 __global__ void __launch_bounds__(256)
 xf_k_step(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
           const uint8_t* __restrict__ labels, int B, int mode, uint32_t* __restrict__ touched,
           float* __restrict__ loss_out, float* __restrict__ pctr_out, float* __restrict__ abs_loss_sum,
-          int log2nc, uint32_t touched_base) {
+          int log2nc, uint32_t touched_base, XfAdmitView adm) {
   __shared__ float s_abs[8];
   extern __shared__ __align__(16) unsigned char xf_smem[];
   float abs_acc = 0.f;
@@ -124,14 +127,16 @@ xf_k_step(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* _
       if (v0) h0 = FM ? xf_load_head_l1(xf_row(t, p0)) : xf_load_head(xf_row(t, p0));
       if (v1) h1 = FM ? xf_load_head_l1(xf_row(t, p1)) : xf_load_head(xf_row(t, p1));
       uint32_t s0 = XF_NO_SLOT, s1 = XF_NO_SLOT;
+      bool r0 = false, r1 = false;
       if (v0) {
-        const int64_t r = xf_probe_from<true>(t, k0, p0, h0);
+        const int64_t r = xf_probe_from<true, ADMIT>(t, k0, p0, h0, &adm, &r0);
         if (r >= 0) { s0 = (uint32_t)r; wsum += h0.w; }
       }
       if (v1) {
-        const int64_t r = xf_probe_from<true>(t, k1, p1, h1);
+        const int64_t r = xf_probe_from<true, ADMIT>(t, k1, p1, h1, &adm, &r1);
         if (r >= 0) { s1 = (uint32_t)r; wsum += h1.w; }
       }
+      if (ADMIT) xf_admit_append(adm, r0, k0, r1, k1);
       if (FM) {
         float st, qt;
         if (s0 != XF_NO_SLOT) { xf_fm_token<VEC>(t, s0, h0.flags, k0, st, qt); ssum += st; qsum += qt; }
@@ -280,21 +285,29 @@ uint32_t xf_step_touched_extra(int K, int B) {
 
 void xf_launch_step(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels,
                     int B, int mode, uint32_t* touched, uint32_t nnz, float* loss_out, float* pctr_out,
-                    float* abs_loss_sum, cudaStream_t st) {
+                    float* abs_loss_sum, const XfAdmitView* adm, cudaStream_t st) {
   if (B <= 0) return;
   const int block = 256;
   const int grid = xf_grid_for((uint64_t)B * 32, block, 8);
   const int lg = xf_step_cache_log2(t.K);
   const size_t smem = lg >= 0 ? ((size_t)1 << lg) * 28 : 0;
-#define XF_STEP_ARGS t, row_ptr, keys, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, lg, nnz
-  if (t.K == 0) {
-    xf_k_step<false, 1><<<grid, block, 0, st>>>(XF_STEP_ARGS);
-  } else {
-    switch (xf_vec_for(t.K)) {
-      case 4: xf_k_step<true, 4><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;
-      case 2: xf_k_step<true, 2><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;
-      default: xf_k_step<true, 1><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;
-    }
+#define XF_STEP_ARGS t, row_ptr, keys, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, lg, nnz, a
+#define XF_STEP_LAUNCH(A)                                                                  \
+  if (t.K == 0) {                                                                          \
+    xf_k_step<false, 1, A><<<grid, block, 0, st>>>(XF_STEP_ARGS);                          \
+  } else {                                                                                 \
+    switch (xf_vec_for(t.K)) {                                                             \
+      case 4: xf_k_step<true, 4, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;       \
+      case 2: xf_k_step<true, 2, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;       \
+      default: xf_k_step<true, 1, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;      \
+    }                                                                                      \
   }
+  const XfAdmitView a = adm ? *adm : XfAdmitView{};
+  if (adm) {
+    XF_STEP_LAUNCH(true)
+  } else {
+    XF_STEP_LAUNCH(false)
+  }
+#undef XF_STEP_LAUNCH
 #undef XF_STEP_ARGS
 }

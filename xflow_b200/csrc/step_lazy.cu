@@ -42,10 +42,18 @@
 // row is (q0..q3).  Returns true when the token is resolved: found (slot = s), inserted (q0..q3 = what xf_k_fill
 // left in the row with the key claimed, *created = true), or out of probes (slot stays XF_NO_SLOT, *t.error = 1).
 // Otherwise s and i move on to the next probe slot, which the caller loads.
+// ADMIT: an absent key asks the admission policy before its CAS; a key it does not admit resolves with slot =
+// XF_NO_SLOT (it pulls w = 0 and takes no part in phase B) and *rejected = true (predict: false, nothing counted).
+template <bool ADMIT>
 __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key, uint64_t& s, uint32_t& i, uint64_t& q0,
-                                             uint64_t& q1, uint64_t& q2, uint64_t& q3, uint32_t& slot, bool& created) {
+                                             uint64_t& q1, uint64_t& q2, uint64_t& q3, uint32_t& slot, bool& created,
+                                             const XfAdmitView& adm, bool& rejected) {
   if (q0 == key) { slot = (uint32_t)s; return true; }
   if (q0 == XF_EMPTY_KEY) {
+    if (ADMIT && !xf_admit(adm, key)) {
+      rejected = adm.mode != XF_ADM_NEVER;
+      return true;
+    }
     const unsigned long long old =
         atomicCAS(reinterpret_cast<unsigned long long*>(xf_row(t, s)), (unsigned long long)XF_EMPTY_KEY, (unsigned long long)key);
     if (old == XF_EMPTY_KEY) {
@@ -66,11 +74,13 @@ __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key,
   return false;
 }
 
+// ADMIT = false is the kernel without an admission policy (every absent key is inserted); ADMIT = true asks `adm`.
+template <bool ADMIT>
 __global__ void __launch_bounds__(256, 3)
 xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
                   const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
                   float* __restrict__ loss_out, float* __restrict__ pctr_out, float* __restrict__ abs_loss_sum,
-                  unsigned long long* __restrict__ unique_total) {
+                  unsigned long long* __restrict__ unique_total, XfAdmitView adm) {
   __shared__ float s_abs[8];
   __shared__ unsigned int s_open;
   // the group leaders' looks at their rows, from phase A to phase B.  In registers they took the kernel past the
@@ -116,13 +126,16 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       xf_ld32_pair(v0 ? xf_row(t, p0) : nullptr, a0, a1, a2, a3);
       xf_ld32_pair(v1 ? xf_row(t, p1) : nullptr, b0, b1, b2, b3);
       uint32_t s0 = XF_NO_SLOT, s1 = XF_NO_SLOT, i0 = 0, i1 = 0;
-      bool u0 = v0, u1 = v1;
+      bool u0 = v0, u1 = v1, r0 = false, r1 = false;
       for (;;) {
         bool c0 = false, c1 = false;
-        if (u0) u0 = !xf_lazy_look(t, k0, p0, i0, a0, a1, a2, a3, s0, c0);
-        if (u1) u1 = !xf_lazy_look(t, k1, p1, i1, b0, b1, b2, b3, s1, c1);
+        if (u0) u0 = !xf_lazy_look<ADMIT>(t, k0, p0, i0, a0, a1, a2, a3, s0, c0, adm, r0);
+        if (u1) u1 = !xf_lazy_look<ADMIT>(t, k1, p1, i1, b0, b1, b2, b3, s1, c1, adm, r1);
         const unsigned created = __popc(__ballot_sync(0xffffffffu, c0)) + __popc(__ballot_sync(0xffffffffu, c1));
-        if (created && lane == 0) atomicAdd(t.size, (unsigned long long)created);
+        if (created && lane == 0) {
+          atomicAdd(t.size, (unsigned long long)created);
+          if (ADMIT) atomicAdd(adm.admitted, (unsigned long long)created);
+        }
         if (!__any_sync(0xffffffffu, u0 || u1)) break;
         uint64_t x0, x1, x2, x3;
         xf_ld32_pair(u0 ? xf_row(t, p0) : nullptr, x0, x1, x2, x3);
@@ -130,6 +143,7 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
         xf_ld32_pair(u1 ? xf_row(t, p1) : nullptr, x0, x1, x2, x3);
         if (u1) { b0 = x0; b1 = x1; b2 = x2; b3 = x3; }
       }
+      if (ADMIT) xf_admit_append(adm, r0, k0, r1, k1);
       // the weight this batch pulls = the row with its pending step applied (computed, not stored)
       uint64_t a2n = a2, b2n = b2;
       float w0 = 0.f, w1 = 0.f;
@@ -210,9 +224,13 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
-                            cudaStream_t st) {
+                            const XfAdmitView* adm, cudaStream_t st) {
   if (B <= 0) return;
   const int grid = xf_grid_for((uint64_t)B * 32, 256, 8);
-  xf_k_step_lr_lazy<<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, loss_out, pctr_out,
-                                           abs_loss_sum, unique_total);
+  if (adm)
+    xf_k_step_lr_lazy<true><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, loss_out, pctr_out,
+                                                  abs_loss_sum, unique_total, *adm);
+  else
+    xf_k_step_lr_lazy<false><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, loss_out, pctr_out,
+                                                   abs_loss_sum, unique_total, XfAdmitView{});
 }

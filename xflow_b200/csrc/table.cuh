@@ -85,6 +85,24 @@ struct XfTableView {
   // accumulators A[k] = sum_occ loss x S_k behind the optimizer state
   int canon;
 };
+// Feature admission (admit.cu): which ABSENT keys a training step may insert.  Only the admitting instantiations
+// of the step kernels take it; a token whose key is absent and not admitted is "rejected": it reads as a row of
+// zeros, updates nothing, and its key is appended to the rejected-token list for the Bloom filter's count pass.
+#define XF_ADM_POISSON 1  // = XF_ADMIT_POISSON: admit iff top 24 bits of splitmix64(key ^ batch_mix) < p24
+#define XF_ADM_BLOOM 2    // = XF_ADMIT_BLOOM: admit iff min over the key's cells >= threshold
+#define XF_ADM_NEVER 3    // predict with a policy set: insert nothing, count nothing
+#define XF_ADM_MAX_HASHES 8
+struct XfAdmitView {
+  int mode;
+  uint32_t p24;                          // floor(p * 2^24)
+  uint64_t batch_mix;                    // splitmix64(seed + b), b = the table's training-batch number
+  uint32_t threshold, log2_cells, hashes;
+  uint64_t seed;                         // the policy's seed (the Bloom cells: xf_admit_cell)
+  const uint8_t* cells;                  // 2^log2_cells one-byte saturating counters
+  unsigned long long* rej_n;             // append position of the rejected-token list (Poisson: the stats counter)
+  uint64_t* rej_keys;                    // the list (nullptr: count only)
+  unsigned long long* admitted;          // keys inserted by admission (stats)
+};
 #define XF_TAG_LOCKED 0xFFFFFFFFu  // never a batch number (the sequence ring is far smaller)
 #define XF_FIX_SCALE 134217728.0          // 2^27: residual sums of lazy tables are 48-bit integers of this unit
 #define XF_FIX_INV 7.450580596923828125e-9  // 2^-27  (|sum of a key's residuals in one batch| < 2^20)
@@ -131,6 +149,34 @@ __host__ __device__ __forceinline__ uint64_t xf_splitmix64(uint64_t x) {
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
+// ---- admission hashes; must stay bit-identical to tests/admission_model.py (bloom_cells, poisson_admits)
+// cell j of `key`: the top log2_cells bits of splitmix64(key ^ splitmix64(seed + (j + 1) * 0x9E3779B97F4A7C15))
+__host__ __device__ __forceinline__ uint64_t xf_admit_cell(uint64_t key, uint64_t seed, uint32_t j, uint32_t log2_cells) {
+  return xf_splitmix64(key ^ xf_splitmix64(seed + (uint64_t)(j + 1) * 0x9E3779B97F4A7C15ull)) >> (64 - log2_cells);
+}
+__device__ __forceinline__ bool xf_admit(const XfAdmitView& a, uint64_t key) {
+  if (a.mode == XF_ADM_POISSON) return (uint32_t)(xf_splitmix64(key ^ a.batch_mix) >> 40) < a.p24;
+  if (a.mode != XF_ADM_BLOOM) return false;
+  uint32_t m = 255u;
+  for (uint32_t j = 0; j < a.hashes; ++j) m = min(m, (uint32_t)__ldcg(a.cells + xf_admit_cell(key, a.seed, j, a.log2_cells)));
+  return m >= a.threshold;
+}
+// Warp-aggregated append of the rejected tokens (r0: k0, r1: k1) to the list: one atomic per warp and chunk that has
+// rejections, none otherwise.  All 32 lanes of the warp must call it together.
+__device__ __forceinline__ void xf_admit_append(const XfAdmitView& a, bool r0, uint64_t k0, bool r1, uint64_t k1) {
+  const unsigned m0 = __ballot_sync(0xffffffffu, r0), m1 = __ballot_sync(0xffffffffu, r1);
+  if ((m0 | m1) == 0u) return;
+  const unsigned lane = threadIdx.x & 31u;
+  unsigned long long base = 0ull;
+  if (lane == 0u) base = atomicAdd(a.rej_n, (unsigned long long)(__popc(m0) + __popc(m1)));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (a.rej_keys) {
+    const unsigned lt = (1u << lane) - 1u;
+    if (r0) a.rej_keys[base + __popc(m0 & lt)] = k0;
+    if (r1) a.rej_keys[base + __popc(m0) + __popc(m1 & lt)] = k1;
+  }
+}
+
 __device__ __forceinline__ float xf_counter_normal(uint64_t key, uint32_t k, uint64_t seed) {
   uint64_t base = xf_splitmix64(key ^ xf_splitmix64(seed + 0x632BE59BD9B4E019ull * (uint64_t)(k + 1)));
   uint32_t sum = 0;
@@ -266,12 +312,19 @@ __device__ __forceinline__ void xf_store_head(uint8_t* row, const XfHead& h) {
 // INSERT, claim an empty slot for it when absent (store[key] semantics).  Returns the slot index, or -1 (not found
 // without INSERT, or probe overflow -> *t.error = 1).  On return `h` is the row's first sector as it
 // was when the key matched (or the default contents on insert).
-template <bool INSERT>
-__device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t key, uint64_t s, XfHead& h) {
+// ADMIT (INSERT only): an absent key is inserted only if the policy `*adm` admits it; otherwise the call returns -1
+// and sets *rejected (unless the policy is XF_ADM_NEVER).  Every token of one key decides the same way in a batch.
+template <bool INSERT, bool ADMIT = false>
+__device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t key, uint64_t s, XfHead& h,
+                                                 const XfAdmitView* adm = nullptr, bool* rejected = nullptr) {
   for (int probes = 0; probes < XF_MAX_PROBE; ++probes) {
     if (h.key == key) return (int64_t)s;
     if (h.key == XF_EMPTY_KEY) {
       if (!INSERT) return -1;
+      if (ADMIT && !xf_admit(*adm, key)) {
+        *rejected = adm->mode != XF_ADM_NEVER;
+        return -1;
+      }
       unsigned long long old =
           atomicCAS(reinterpret_cast<unsigned long long*>(xf_row(t, s)), (unsigned long long)XF_EMPTY_KEY,
                     (unsigned long long)key);
@@ -279,7 +332,10 @@ __device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t 
         // we created the entry: count it (warp-aggregated) and report default contents
         unsigned m = __activemask();
         int leader = __ffs(m) - 1;
-        if ((int)(threadIdx.x & 31) == leader) atomicAdd(t.size, (unsigned long long)__popc(m));
+        if ((int)(threadIdx.x & 31) == leader) {
+          atomicAdd(t.size, (unsigned long long)__popc(m));
+          if (ADMIT) atomicAdd(adm->admitted, (unsigned long long)__popc(m));
+        }
         h.key = key; h.flags = 0; h.w = 0.f; h.n = 0.f; h.z = 0.f;
         h.g = t.lazy ? 0.0 : -0.0;  // what xf_k_fill left in the row (lazy: the integer 0)
         return (int64_t)s;

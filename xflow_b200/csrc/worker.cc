@@ -42,6 +42,49 @@ void must(int rc, const char* what) {
 }
 }  // namespace
 
+// Feature admission of the tables' training steps (xf_table_set_admission): XFLOW_ADMIT = bloom:<n> (a key gets a row
+// once it has occurred n times, counted in a counting Bloom filter of 2^XFLOW_ADMIT_LOG2_CELLS bytes, default 30,
+// 3 hashes, halved every XFLOW_ADMIT_DECAY batches, default 0 = never) or poisson:<p> (inserted with probability p).
+// Unset: every key is inserted.  Single GPU only.
+static xf_admission_config AdmissionFromEnv(int world) {
+  xf_admission_config c;
+  xf_admission_config_default(&c);
+  const char* e = getenv("XFLOW_ADMIT");
+  if (!e || !*e) return c;
+  const std::string s(e);
+  const size_t colon = s.find(':');
+  const std::string kind = s.substr(0, colon), arg = colon == std::string::npos ? "" : s.substr(colon + 1);
+  char* end = nullptr;
+  if (kind == "bloom") {
+    const long n = strtol(arg.c_str(), &end, 10);
+    if (arg.empty() || *end || n < 1 || n > 255) throw std::runtime_error("XFLOW_ADMIT=bloom:<n> needs 1 <= n <= 255, got '" + s + "'");
+    c.mode = XF_ADMIT_BLOOM;
+    c.threshold = (uint32_t)n;
+    const char* lg = getenv("XFLOW_ADMIT_LOG2_CELLS");
+    if (lg && *lg) {
+      const long v = strtol(lg, &end, 10);
+      if (*end || v < 10 || v > 36) throw std::runtime_error(std::string("XFLOW_ADMIT_LOG2_CELLS must be 10..36, got '") + lg + "'");
+      c.log2_cells = (uint32_t)v;
+    }
+    const char* d = getenv("XFLOW_ADMIT_DECAY");
+    if (d && *d) {
+      const long long v = strtoll(d, &end, 10);
+      if (*end || v < 0) throw std::runtime_error(std::string("XFLOW_ADMIT_DECAY must be a batch count >= 0, got '") + d + "'");
+      c.decay_batches = (uint64_t)v;
+    }
+  } else if (kind == "poisson") {
+    const double p = strtod(arg.c_str(), &end);
+    if (arg.empty() || *end || !(p >= 0.0 && p <= 1.0)) throw std::runtime_error("XFLOW_ADMIT=poisson:<p> needs 0 <= p <= 1, got '" + s + "'");
+    c.mode = XF_ADMIT_POISSON;
+    c.probability = (float)p;
+  } else {
+    throw std::runtime_error("XFLOW_ADMIT must be bloom:<n> or poisson:<p>, got '" + s + "'");
+  }
+  c.seed = (uint64_t)env_int("XFLOW_SEED", 0);
+  if (world > 1) throw std::runtime_error("XFLOW_ADMIT is single-GPU only: unset it or run with XFLOW_WORLD = 1");
+  return c;
+}
+
 int MyRank() { return env_int("XFLOW_RANK", env_int("RANK", 0)); }
 int NumWorkers() { return env_int("XFLOW_WORLD", env_int("WORLD_SIZE", 1)); }
 
@@ -72,6 +115,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   if (rank_ < 0 || rank_ >= world_)
     throw std::runtime_error("rank " + std::to_string(rank_) + " needs XFLOW_WORLD / WORLD_SIZE > rank: a worker with rank > 0 "
                              "has no servers to talk to on its own");
+  AdmissionFromEnv(world_);  // a malformed XFLOW_ADMIT, or one with XFLOW_WORLD > 1, fails here
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -113,6 +157,15 @@ static xf_table* make_table(Optimizer opt, int K, int device, int rank, int worl
   cfg.capacity = (uint64_t)1 << env_int("XFLOW_TABLE_LOG2", 20);
   xf_table* t = nullptr;
   must(xf_table_create(&t, &cfg), "xf_table_create");
+  const xf_admission_config adm = AdmissionFromEnv(world);
+  if (adm.mode != XF_ADMIT_ALL) {
+    const int rc = xf_table_set_admission(t, &adm);
+    if (rc != XF_OK) {
+      const std::string err = xf_last_error();
+      xf_table_destroy(t);
+      throw std::runtime_error("xf_table_set_admission: " + err);
+    }
+  }
   return t;
 }
 
