@@ -110,7 +110,8 @@ def oracle_case_run(case, syn_data, exact=False):
     return t.export(g["keys"]), lab, p
 
 
-def check_fm_first_step(rp, keys, lab, K, v0_of, loss, export_of, alpha=0.05, beta=1.0, l1=5e-5, l2=10.0):
+def check_fm_first_step(rp, keys, lab, K, v0_of, loss, export_of, alpha=0.05, beta=1.0, l1=5e-5, l2=10.0,
+                        k_fold_w=False):
     """Closed form of the FIRST FM + FTRL step on a fresh table (w = 0, n = z = 0, v = v0) in float64,
     compared with an implementation's residuals and exported state.  Tolerances are noise-aware: a sum
     over a key's occurrences is accepted within a few float32 ulps of the sum of the |terms| (both the
@@ -153,6 +154,10 @@ def check_fm_first_step(rp, keys, lab, K, v0_of, loss, export_of, alpha=0.05, be
     # w: g = K * L / B ; from the zero state n = g^2, z = g
     gw = K * L / B
     tol_gw = 1e-5 * np.abs(gw) + 8 * eps * K * magL / B + 1e-30
+    if k_fold_w:
+        # fm_worker.cc:140 forms a token's w-gradient as K sequential float adds of its residual: up to K ulps of
+        # K |residual| each, which at K ~ 100 and above outgrows the 8 ulps above
+        tol_gw = tol_gw + K * eps * K * magL / B
     within(e["zw"], gw, tol_gw, "zw after step 1")
     within(e["nw"], gw ** 2, 2 * np.abs(gw) * tol_gw + tol_gw ** 2 + 1e-5 * gw ** 2, "nw after step 1")
     # v: g = (Aq - v L) / B ; n = g^2 ; z = g - |g| / alpha * v ; v' from (z, n)
@@ -170,6 +175,72 @@ def check_fm_first_step(rp, keys, lab, K, v0_of, loss, export_of, alpha=0.05, be
     bad = decided & (np.abs(got_v - vn) > tol_v)
     assert not bad.any(), "v after step 1: %d/%d outside tolerance" % (int(bad.sum()), bad.size)
     return uk, e
+
+
+def ftrl64(g, w, n, z, alpha=0.05, beta=1.0, l1=5e-5, l2=10.0):
+    """One FTRL-proximal step (ftrl.h:59-74) in float64."""
+    n2 = n + g * g
+    z2 = z + g - (np.sqrt(n2) - np.sqrt(n)) / alpha * w
+    w2 = np.where(np.abs(z2) <= l1, 0.0, (z2 - np.sign(z2) * l1) / -((beta + np.sqrt(n2)) / alpha + l2))
+    return w2, n2, z2
+
+
+class CanonicalFM64:
+    """float64 numpy model of XF_MODEL_FM_CANONICAL (step_fmc.cu; SURVEY 8f-4): the textbook FM with feature values,
+    y = sum w x + 1/2 sum_k[(sum v_k x)^2 - sum (v_k x)^2], gradients / rows, one FTRL or SGD step (learning rate
+    1e-3) per touched key.  A key enters with the w and v a pull of the device table gives it (insert-on-pull)."""
+
+    def __init__(self, K, opt, pull):
+        self.K, self.opt, self.pull = K, opt, pull
+        self.state = {}  # key -> [w, nw, zw, v[K], nv[K], zv[K]]
+
+    def _enter(self, uk):
+        new = np.array([k for k in uk if int(k) not in self.state], np.uint64)
+        if new.size:
+            w0, v0 = self.pull(new)
+            for k, a, b in zip(new, w0, v0):
+                self.state[int(k)] = [float(a), 0.0, 0.0, b.astype(np.float64), np.zeros(self.K), np.zeros(self.K)]
+
+    def step(self, rp, keys, x, lab):
+        """One training step; returns the residuals of the rows."""
+        K, B = self.K, lab.size
+        uk, inv = np.unique(keys, return_inverse=True)
+        self._enter(uk)
+        W = np.array([self.state[int(k)][0] for k in uk])
+        V = np.stack([self.state[int(k)][3] for k in uk]) if uk.size else np.zeros((0, K))
+        row_of = np.repeat(np.arange(B), np.diff(rp).astype(np.int64))
+        x64 = x.astype(np.float64)
+        wx = np.zeros(B); np.add.at(wx, row_of, W[inv] * x64)
+        S = np.zeros((B, K)); np.add.at(S, row_of, V[inv] * x64[:, None])
+        Q = np.zeros(B); np.add.at(Q, row_of, ((V[inv] * x64[:, None]) ** 2).sum(1))
+        y = wx + 0.5 * ((S ** 2).sum(1) - Q)
+        with np.errstate(over="ignore"):
+            e = np.power(2.718281828, np.clip(y, -30, 30))
+        p = np.where(y < -30, 1e-6, np.where(y > 30, 1.0, e / (1 + e)))
+        loss = p - lab
+        r = loss[row_of] * x64
+        gw = np.zeros(uk.size); np.add.at(gw, inv, r)
+        A = np.zeros((uk.size, K)); np.add.at(A, inv, r[:, None] * S[row_of])
+        L2 = np.zeros(uk.size); np.add.at(L2, inv, r * x64)
+        gv = (A - V * L2[:, None]) / B
+        gw = gw / B
+        for i, k in enumerate(uk):
+            s = self.state[int(k)]
+            if self.opt == "ftrl":
+                s[0], s[1], s[2] = ftrl64(gw[i], s[0], s[1], s[2])
+                s[3], s[4], s[5] = ftrl64(gv[i], s[3], s[4], s[5])
+            else:
+                s[0] -= 1e-3 * gw[i]
+                s[3] = s[3] - 1e-3 * gv[i]
+        return loss
+
+    def keys(self):
+        return np.array(sorted(self.state), np.uint64)
+
+    def export(self, keys):
+        """{w, nw, zw, v, nv, zv}: [n, 1] or [n, K] float64 arrays of the given keys (all known to the model)."""
+        return {k: np.array([np.atleast_1d(self.state[int(q)][j]) for q in keys]).reshape(len(keys), -1)
+                for j, k in enumerate(("w", "nw", "zw", "v", "nv", "zv"))}
 
 
 def build_and_run_ps_compat(tmp_dir):

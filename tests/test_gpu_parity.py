@@ -10,7 +10,8 @@ import numpy as np
 import pytest
 
 from cases import CASES
-from common import check_fm_first_step, assert_close, assert_close_noise_aware, data_prefixes, golden, oracle_case_run
+from common import (CanonicalFM64, check_fm_first_step, assert_close, assert_close_noise_aware, data_prefixes, ftrl64,
+                    golden, oracle_case_run)
 from oracle import oracle as O
 from xflow_b200 import api, datagen
 
@@ -493,13 +494,6 @@ def test_device_metric_matches_host_metric():
     lib.xf_metric_destroy(m)
 
 
-def _ftrl64(g, w, n, z, alpha=0.05, beta=1.0, l1=5e-5, l2=10.0):
-    n2 = n + g * g
-    z2 = z + g - (np.sqrt(n2) - np.sqrt(n)) / alpha * w
-    w2 = np.where(np.abs(z2) <= l1, 0.0, (z2 - np.sign(z2) * l1) / -((beta + np.sqrt(n2)) / alpha + l2))
-    return w2, n2, z2
-
-
 @pytest.mark.parametrize("K,opt", [(8, "ftrl"), (16, "sgd"), (4, "ftrl")])
 def test_canonical_fm_with_values_matches_float64_model(K, opt):
     """XF_MODEL_FM_CANONICAL (step_fmc.cu; SURVEY 8f-4, NOT the reference's model): the textbook FM with feature
@@ -510,53 +504,17 @@ def test_canonical_fm_with_values_matches_float64_model(K, opt):
     t = api.Table(latent_dim=K, optimizer=gopt, v_init=api.VINIT_COUNTER, seed=4, canonical_fm=1)
     tr = api.Trainer(t, model=api.MODEL_FM_CANONICAL, max_rows=B, max_nnz=B * d * 2, keep_loss=True)
     rng = np.random.default_rng(K)
-    state = {}
-
-    def rows_of(uk):
-        for k in uk:
-            if int(k) not in state:
-                state[int(k)] = None
-        new = np.array([k for k in uk if state[int(k)] is None], np.uint64)
-        if new.size:
-            w0, v0 = t.pull(new)                       # insert-on-pull: default w, counter-based v
-            for k, a, b in zip(new, w0, v0):
-                state[int(k)] = [float(a), 0.0, 0.0, b.astype(np.float64), np.zeros(K), np.zeros(K)]
-
+    model = CanonicalFM64(K, opt, t.pull)                 # insert-on-pull: default w, counter-based v
     for step in range(3):
         rp, keys, lab = datagen.make_csr_keys(70 + step, B, d, space, api.hash_decimal_ids, ragged=(step == 1))
         x = (rng.random(keys.size) * 1.5 + 0.25).astype(np.float32)
         x[::7] *= -1.0
-        uk, inv = np.unique(keys, return_inverse=True)
-        rows_of(uk)
-        W = np.array([state[int(k)][0] for k in uk]); V = np.stack([state[int(k)][3] for k in uk])
-        row_of = np.repeat(np.arange(B), np.diff(rp).astype(np.int64))
-        x64 = x.astype(np.float64)
-        wx = np.zeros(B); np.add.at(wx, row_of, W[inv] * x64)
-        S = np.zeros((B, K)); np.add.at(S, row_of, V[inv] * x64[:, None])
-        Q = np.zeros(B); np.add.at(Q, row_of, ((V[inv] * x64[:, None]) ** 2).sum(1))
-        y = wx + 0.5 * ((S ** 2).sum(1) - Q)
-        p = np.where(y < -30, 1e-6, np.where(y > 30, 1.0, np.power(2.718281828, y) / (1 + np.power(2.718281828, y))))
-        loss = p - lab
+        loss = model.step(rp, keys, x, lab)
         tr.step_host_values(rp, keys, x, lab)
         assert_close(tr.get_loss(B), loss, "canonical FM residuals, step %d" % step, rel=2e-5, abs_floor=2e-6)
-        r = loss[row_of] * x64
-        gw = np.zeros(uk.size); np.add.at(gw, inv, r)
-        A = np.zeros((uk.size, K)); np.add.at(A, inv, r[:, None] * S[row_of])
-        L2 = np.zeros(uk.size); np.add.at(L2, inv, r * x64)
-        gv = (A - V * L2[:, None]) / B
-        gw = gw / B
-        for i, k in enumerate(uk):
-            s = state[int(k)]
-            if opt == "ftrl":
-                s[0], s[1], s[2] = _ftrl64(gw[i], s[0], s[1], s[2])
-                s[3], s[4], s[5] = _ftrl64(gv[i], s[3], s[4], s[5])
-            else:
-                s[0] -= 1e-3 * gw[i]
-                s[3] = s[3] - 1e-3 * gv[i]
-    allk = np.array(sorted(state), np.uint64)
+    allk = model.keys()
     e = t.export(allk)
-    ref = {k: np.array([np.atleast_1d(state[int(q)][j]) for q in allk]).reshape(allk.size, -1)
-           for j, k in enumerate(("w", "nw", "zw", "v", "nv", "zv"))}
+    ref = model.export(allk)
     for k in ("w", "v") + (("nw", "zw", "nv", "zv") if opt == "ftrl" else ()):
         assert_close(e[k].reshape(allk.size, -1), ref[k], "canonical FM %s" % k, rel=2e-4, abs_floor=2e-7)
     # forward only, with values
@@ -618,7 +576,7 @@ def test_defined_mvm_matches_float64_model(K, opt, with_vals):
         g = A / B
         for i in np.nonzero(touched)[0]:
             if opt == "ftrl":
-                V[i], NV[i], ZV[i] = _ftrl64(g[i], V[i], NV[i], ZV[i])
+                V[i], NV[i], ZV[i] = ftrl64(g[i], V[i], NV[i], ZV[i])
             else:
                 V[i] = V[i] - lr * g[i]
     e = t.export(allk)

@@ -274,8 +274,8 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
     // XFLOW_SEQ_RING: ring size override (tests exercise the flush with a tiny ring)
     const char* ring = getenv("XFLOW_SEQ_RING");
     t->rows_cap = (ring && atoi(ring) >= 4 && atoi(ring) <= 65535) ? (size_t)atoi(ring) : (size_t)65535;  // tags are 16 bits
-    XF_CUDA_TRY(cudaMalloc(&t->d_rows_by_seq, t->rows_cap * sizeof(uint32_t)));
-    XF_CUDA_TRY(cudaMemsetAsync(t->d_rows_by_seq, 0, t->rows_cap * sizeof(uint32_t), t->stream));
+    XF_CUDA_TRY(cudaMalloc(&t->d_rows_by_seq, t->rows_cap * sizeof(uint64_t)));
+    XF_CUDA_TRY(cudaMemsetAsync(t->d_rows_by_seq, 0, t->rows_cap * sizeof(uint64_t), t->stream));
     v.rows_by_seq = t->d_rows_by_seq;
   }
   int r = t->alloc_table(cfg->capacity ? cfg->capacity : (1ull << 20));
@@ -943,7 +943,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   if (t->view.lazy) {
     // one kernel: the optimizer step of earlier batches is folded in as rows are touched
     if (mode == 0) XF_TRY(t->next_seq());
-    xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, t->seq, t->d_rows_by_seq,
+    xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, nnz, mode, t->seq, t->d_rows_by_seq,
                            (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
                            mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, adm, st);
     ++tr->launches;

@@ -65,9 +65,9 @@ struct xf_table {
   uint64_t cum_incoming = 0, known_size = 0, known_at = 0;
   uint64_t launches = 0;
   int refs = 1;              // the creator + every trainer bound to the table (destroy order is free)
-  // lazy ("update on next touch") tables: batch sequence number and the per-batch row counts
+  // lazy ("update on next touch") tables: batch sequence number and the per-batch row counts and fixed-point units
   uint32_t seq = 0;
-  uint32_t* d_rows_by_seq = nullptr;
+  uint64_t* d_rows_by_seq = nullptr;
   size_t rows_cap = 0;
   int next_seq();            // advances seq; flushes all pending steps and restarts when the ring is used up
   int reserve_seqs(int n);   // makes sure the next n numbers come without a restart (flushes now if they would not)

@@ -39,7 +39,7 @@ void xf_launch_list_keys(const XfTableView& t, uint64_t* keys_out, unsigned long
                          cudaStream_t st);
 int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm);
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
-                            const uint8_t* labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
+                            const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
                             const XfAdmitView* adm, cudaStream_t st);
 
@@ -67,7 +67,7 @@ void xf_launch_bcast_rowv(const float* src, uint32_t n_words, int S, const XfPee
                           uint64_t dst_word_off, cudaStream_t st);
 void xf_launch_push_tokens_lr(const XfTableView& t, const uint32_t* slots, const uint32_t* in_rows, const float* rowv,
                               const uint32_t* meta_s, uint32_t cap, uint64_t work_bound, uint32_t seq,
-                              uint32_t* rows_by_seq, unsigned long long* uniq_remote, const void* stash,
+                              uint64_t* rows_by_seq, unsigned long long* uniq_remote, const void* stash,
                               cudaStream_t st);
 uint32_t xf_acc_touched_extra(int K, uint64_t work_bound);
 void xf_launch_acc_tokens(const XfTableView& t, const uint32_t* slots, const uint32_t* in_rows, const void* rowv,

@@ -327,11 +327,14 @@ __global__ void xf_k_bcast_rowv(const uint32_t* __restrict__ src, uint32_t n_wor
 __global__ void __launch_bounds__(256)
 xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uint32_t* __restrict__ in_rows,
                     const float* __restrict__ rowv, const uint32_t* __restrict__ meta_s, uint32_t cap, uint32_t seq,
-                    uint32_t* rows_by_seq, unsigned long long* uniq_remote, const uint4* __restrict__ stash) {
+                    uint64_t* rows_by_seq, unsigned long long* uniq_remote, const uint4* __restrict__ stash) {
   __shared__ unsigned int s_open;
   if (threadIdx.x == 0) s_open = 0;
   const uint32_t n = min(__ldg(meta_s), cap);
-  if (blockIdx.x == 0 && threadIdx.x == 0) rows_by_seq[seq] = __ldg(meta_s + 1);  // read by later launches only
+  // the source's tokens for this shard bound every key's residual sum of this push: they set its fixed-point unit
+  const int fs = xf_fix_shift(n);
+  if (blockIdx.x == 0 && threadIdx.x == 0)  // read by later launches only
+    rows_by_seq[seq] = (uint64_t)__ldg(meta_s + 1) | ((uint64_t)fs << 32);
   __syncthreads();
   unsigned int open_acc = 0;
   const int lane = threadIdx.x & 31;
@@ -389,7 +392,7 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
       // tokens of this group that hit the same row: the lowest lane deposits the group's residuals
       const unsigned grp = __match_any_sync(0xffffffffu, valid ? s[u] : (0xFFFFFF00u | (uint32_t)lane));
       lead[u] = valid && lane == __ffs(grp) - 1;
-      fix[u] = valid ? xf_fix_of(l[u]) : 0ll;
+      fix[u] = valid ? xf_fix_of(l[u], fs) : 0ll;
       if (__any_sync(0xffffffffu, valid && __popc(grp) > 1)) {
         long long sum = 0ll;
         for (int b = 0; b < 32; ++b) {
@@ -589,7 +592,7 @@ void xf_launch_bcast_rowv(const float* src, uint32_t n_words, int S, const XfPee
 }
 void xf_launch_push_tokens_lr(const XfTableView& t, const uint32_t* slots, const uint32_t* in_rows, const float* rowv,
                               const uint32_t* meta_s, uint32_t cap, uint64_t work_bound, uint32_t seq,
-                              uint32_t* rows_by_seq, unsigned long long* uniq_remote, const void* stash,
+                              uint64_t* rows_by_seq, unsigned long long* uniq_remote, const void* stash,
                               cudaStream_t st) {
   const int grid = xf_grid_for(work_bound ? work_bound : 1, 256, 8);
   xf_k_push_tokens_lr<<<grid, 256, 0, st>>>(t, slots, in_rows, rowv, meta_s, cap, seq, rows_by_seq, uniq_remote,

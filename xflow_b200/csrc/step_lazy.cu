@@ -78,7 +78,7 @@ __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key,
 template <bool ADMIT>
 __global__ void __launch_bounds__(256, 3)
 xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
-                  const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
+                  const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint64_t* rows_by_seq, int fix_shift,
                   float* __restrict__ loss_out, float* __restrict__ pctr_out, float* __restrict__ abs_loss_sum,
                   unsigned long long* __restrict__ unique_total, XfAdmitView adm) {
   __shared__ float s_abs[8];
@@ -87,7 +87,8 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
   // 80 registers that 3 CTAs of 256 threads per SM leave it, and it spilled.
   __shared__ uint64_t s_q2[2 * XF_LAZY_CACHED][256], s_q3[2 * XF_LAZY_CACHED][256], s_q2n[2 * XF_LAZY_CACHED][256];
   if (threadIdx.x == 0) s_open = 0;
-  if (blockIdx.x == 0 && threadIdx.x == 0 && mode == 0) rows_by_seq[seq] = (uint32_t)B;  // read by later batches only
+  if (blockIdx.x == 0 && threadIdx.x == 0 && mode == 0)  // read by later batches only
+    rows_by_seq[seq] = (uint64_t)(uint32_t)B | ((uint64_t)fix_shift << 32);
   __syncthreads();
   float abs_acc = 0.f;
   unsigned int open_acc = 0;
@@ -184,7 +185,7 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
     if (lane == 0 && loss_out) loss_out[row] = loss;
     abs_acc += fabsf(loss);
     // ---------------- phase B: one deposit per distinct key of a token group: count x residual, integer, exact
-    const long long lf = xf_fix_of(loss);
+    const long long lf = xf_fix_of(loss, fix_shift);
 #pragma unroll
     for (int c = 0; c < XF_LAZY_CACHED; ++c) {
       const int x = threadIdx.x;
@@ -222,15 +223,16 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
 }
 
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
-                            const uint8_t* labels, int B, int mode, uint32_t seq, uint32_t* rows_by_seq,
+                            const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
                             const XfAdmitView* adm, cudaStream_t st) {
   if (B <= 0) return;
   const int grid = xf_grid_for((uint64_t)B * 32, 256, 8);
+  const int fs = xf_fix_shift(nnz);  // nnz bounds every key's residual sum in this batch
   if (adm)
-    xf_k_step_lr_lazy<true><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, loss_out, pctr_out,
-                                                  abs_loss_sum, unique_total, *adm);
+    xf_k_step_lr_lazy<true><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, loss_out,
+                                                  pctr_out, abs_loss_sum, unique_total, *adm);
   else
-    xf_k_step_lr_lazy<false><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, loss_out, pctr_out,
-                                                   abs_loss_sum, unique_total, XfAdmitView{});
+    xf_k_step_lr_lazy<false><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, loss_out,
+                                                   pctr_out, abs_loss_sum, unique_total, XfAdmitView{});
 }
