@@ -169,6 +169,46 @@ XF_DLL int xf_table_set_admission(xf_table* t, const xf_admission_config* cfg);
  * NULL; reads device counters, waits for the table's stream) */
 XF_DLL int xf_table_admission_stats(xf_table* t, uint64_t* batches, uint64_t* rejected_tokens, uint64_t* admitted_keys);
 
+/* Feature eviction: per-key stamps of the last training batch, and sweeps that drop idle keys or keep a key budget.
+ * Batch numbers b are admission's: 0, 1, 2, ... per non-empty training step on the table (an empty batch is not one).
+ * With tracking on, every present key k carries a stamp last(k), a 32-bit batch number:
+ *   - a training step of batch b sets last(k) = b for every key one of its tokens reads from a row, including the
+ *     keys the step inserts or admits; a token that admission rejects stamps nothing (its key has no row);
+ *   - any other insertion (predict's insert-on-pull, xf_table_pull / _push / _import / _load,
+ *     xf_table_touch_decimal_ids, xf_trainer_init_push, the ps-lite functors) sets last(k) = the number of training
+ *     batches run so far;
+ *   - reading or updating an existing key outside a training step (predict, pull, push, import, export) leaves its
+ *     stamp alone;
+ *   - when tracking starts, every key already present gets the number of training batches run so far.
+ * A sweep (xf_table_evict) runs at the current batch number B, stream-ordered after everything enqueued on the
+ * table's stream.  It removes
+ *   1. with max_idle_batches = T > 0: every key with last(k) < B - T (no training batch among the last T touched
+ *      it; nothing when B <= T);
+ *   2. with max_keys = N > 0: of the keys left, all but the N most recently touched, where a larger stamp is more
+ *      recent and, between equal stamps, the smaller 64-bit key is.  Exactly min(N, keys left) keys survive.
+ * An evicted key is absent, as if never inserted: its optimizer state (a lazy row's pending step included) goes with
+ * it, its next training touch asks the admission policy again, and its next insertion starts from default contents.
+ * Surviving rows are copied as they are.  The sweep rebuilds the table at the smallest power-of-two capacity >= the
+ * floor (the larger of the creation capacity and the largest xf_table_reserve) that holds the survivors at load
+ * <= 0.5, never above the current capacity; the old and the new table are both allocated while it runs, as in
+ * growth.  A sweep that would remove nothing and keep the capacity does nothing.
+ * The stamps are one uint32_t per slot of device memory beside the rows (+12.5 % for LR rows, +1.6 % for FM K = 16
+ * FTRL rows); they are not part of xf_table_save (a loaded key is an insertion).  A table that has run 2^32 - 1
+ * training batches refuses further tracked training steps.  Single-GPU tables only: refused on canonical tables
+ * (canonical_fm = 1), on tables with num_shards > 1, and by xf_trainer_create / the step with a multi-rank comm. */
+typedef struct xf_eviction_config {
+  uint64_t max_idle_batches;  /* > 0: a sweep drops keys no training batch touched among the last max_idle_batches */
+  uint64_t max_keys;          /* > 0: a sweep then keeps only the max_keys most recently touched keys */
+} xf_eviction_config;
+/* starts (or keeps) per-key stamps and sets the sweep's limits; both 0 = track only; cfg = NULL stops tracking and
+ * frees them.  Calling it again replaces the limits and keeps the stamps.  On failure the table is unchanged. */
+XF_DLL int xf_table_set_eviction(xf_table* t, const xf_eviction_config* cfg);
+/* one sweep now (waits for the table's stream); *evicted = keys removed (may be NULL).  XF_ERR_STATE without
+ * tracking.  On failure (allocation included) the table is unchanged. */
+XF_DLL int xf_table_evict(xf_table* t, uint64_t* evicted);
+/* out[i] = last(keys[i]), or UINT64_MAX for an absent key; never inserts.  XF_ERR_STATE without tracking. */
+XF_DLL int xf_table_last_touch(xf_table* t, const uint64_t* keys, uint64_t n, uint64_t* out);
+
 /* bucketing rule of ps::Postoffice::GetServerKeyRanges (postoffice.cc:134-143) + DefaultSlicer
  * (kv_app.h:405-460): shard = min(key / floor((2^64-1)/S), S-1).  Pure host function. */
 XF_DLL int xf_shard_of(uint64_t key, int num_shards);

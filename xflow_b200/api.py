@@ -36,6 +36,10 @@ class AdmissionConfig(C.Structure):
                 ("hashes", C.c_uint32), ("decay_batches", C.c_uint64), ("seed", C.c_uint64)]
 
 
+class EvictionConfig(C.Structure):
+    _fields_ = [("max_idle_batches", C.c_uint64), ("max_keys", C.c_uint64)]
+
+
 class TrainerConfig(C.Structure):
     _fields_ = [("model", C.c_int), ("max_rows", C.c_uint32), ("max_nnz", C.c_uint32), ("keep_loss", C.c_int)]
 
@@ -69,6 +73,9 @@ SIGNATURES = {
     "xf_admission_config_default": (_i, [_vp]),
     "xf_table_set_admission": (_i, [_vp, _vp]),
     "xf_table_admission_stats": (_i, [_vp, _vp, _vp, _vp]),
+    "xf_table_set_eviction": (_i, [_vp, _vp]),
+    "xf_table_evict": (_i, [_vp, _vp]),
+    "xf_table_last_touch": (_i, [_vp, _vp, _u64, _vp]),
     "xf_shard_of": (_i, [_u64, _i]),
     "xf_trainer_create": (_i, [_vp, _vp, _vp, _vp]),
     "xf_trainer_destroy": (_i, [_vp]),
@@ -352,6 +359,30 @@ class Table:
         a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
         _check(lib().xf_table_admission_stats(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(batches=a.value, rejected_tokens=b.value, admitted_keys=c.value)
+
+    def set_eviction(self, max_idle_batches=0, max_keys=0):
+        """Feature eviction: start (or keep) per-key stamps of the last training batch and set the limits a sweep
+        (evict) applies: drop keys no training batch touched among the last max_idle_batches, then keep only the
+        max_keys most recently touched.  0 = no such limit; calling again replaces the limits and keeps the stamps."""
+        cfg = EvictionConfig(max_idle_batches, max_keys)
+        _check(lib().xf_table_set_eviction(self.h, C.byref(cfg)))
+
+    def stop_eviction(self):
+        """Stop tracking and free the stamps."""
+        _check(lib().xf_table_set_eviction(self.h, None))
+
+    def evict(self):
+        """One sweep now (waits for the table's stream); returns the number of keys removed."""
+        n = C.c_uint64()
+        _check(lib().xf_table_evict(self.h, C.byref(n)))
+        return n.value
+
+    def last_touch(self, keys):
+        """The batch number that last touched each key (np.uint64), UINT64_MAX for an absent key; never inserts."""
+        keys = np.ascontiguousarray(keys, np.uint64)
+        out = np.empty(keys.size, np.uint64)
+        _check(lib().xf_table_last_touch(self.h, _p(keys), keys.size, _p(out)))
+        return out
 
 
 class Comm:

@@ -101,7 +101,15 @@ int xf_table::alloc_table(uint64_t capacity) {
   const uint32_t stride = xf_row_stride(cfg.latent_dim, cfg.optimizer, cfg.canonical_fm);
   uint8_t* base = nullptr;
   XF_CUDA_TRY(cudaMalloc(&base, capacity * (uint64_t)stride));
+  uint32_t* stamp = nullptr;
+  if (d_stamp != nullptr && cudaMalloc(&stamp, capacity * sizeof(uint32_t)) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(base);
+    xf_set_error("cannot allocate the eviction stamps of %llu slots", (unsigned long long)capacity);
+    return XF_ERR_CUDA;
+  }
   view.base = base;
+  if (stamp) d_stamp = stamp;  // tracking on: the new table's stamps (the rebuild fills them)
   view.mask = capacity - 1;
   uint32_t lg = 0;
   while ((1ull << lg) < capacity) ++lg;
@@ -136,15 +144,19 @@ int xf_table::check_error() {
   return XF_OK;
 }
 
-int xf_table::grow(uint64_t new_capacity) {
+int xf_table::grow(uint64_t new_capacity) { return rebuild(new_capacity, XfKeep{0u, 0, 0u, 0ull}); }
+
+int xf_table::rebuild(uint64_t new_capacity, const XfKeep& keep) {
   XfTableView old = view;
+  uint32_t* old_stamp = d_stamp;
   const int rc = alloc_table(new_capacity);  // on failure the old table (and its size counter) stay as they are
-  if (rc != XF_OK) { view = old; return rc; }
+  if (rc != XF_OK) { view = old; d_stamp = old_stamp; return rc; }
   XF_CUDA_TRY(cudaMemsetAsync(d_size, 0, sizeof(unsigned long long), stream));  // the rehash re-counts every key
-  xf_launch_rehash(old, view, stream);
+  xf_launch_rehash(old, view, keep, old_stamp, d_stamp, stream);
   ++launches;
   XF_CUDA_TRY(cudaStreamSynchronize(stream));
   XF_CUDA_TRY(cudaFree(old.base));
+  if (old_stamp) XF_CUDA_TRY(cudaFree(old_stamp));
   return XF_OK;
 }
 
@@ -280,6 +292,7 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   }
   int r = t->alloc_table(cfg->capacity ? cfg->capacity : (1ull << 20));
   if (r != XF_OK) { delete t; return r; }
+  t->cap_floor = t->view.mask + 1;
   XF_CUDA_TRY(cudaStreamSynchronize(t->stream));
   *out = t;
   return XF_OK;
@@ -291,6 +304,8 @@ XF_DLL int xf_table_destroy(xf_table* t) {
   cudaSetDevice(t->cfg.device);
   cudaStreamSynchronize(t->stream);
   if (t->view.base) cudaFree(t->view.base);
+  if (t->d_stamp) cudaFree(t->d_stamp);
+  t->s_hist.release();
   cudaFree(t->d_size);
   cudaFree(t->d_error);
   if (t->d_rows_by_seq) cudaFree(t->d_rows_by_seq);
@@ -384,7 +399,7 @@ XF_DLL int xf_table_set_admission(xf_table* t, const xf_admission_config* cfg) {
 XF_DLL int xf_table_admission_stats(xf_table* t, uint64_t* batches, uint64_t* rejected_tokens, uint64_t* admitted_keys) {
   if (!t) return XF_ERR_ARG;
   unsigned long long c[2] = {0ull, 0ull};
-  if (t->d_admit) {
+  if (t->d_admit && (rejected_tokens || admitted_keys)) {  // the batch number alone is host state
     XF_CUDA_TRY(cudaMemcpyAsync(c, t->d_admit, sizeof(c), cudaMemcpyDeviceToHost, t->stream));
     XF_CUDA_TRY(cudaStreamSynchronize(t->stream));
   }
@@ -442,6 +457,7 @@ XF_DLL int xf_table_reserve(xf_table* t, uint64_t n_keys) {
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
   uint64_t want = xf_pow2_at_least(n_keys * 2);
   if (want > t->view.mask + 1) XF_TRY(t->grow(want));
+  t->cap_floor = std::max(t->cap_floor, want);  // eviction sweeps do not shrink below a reservation
   return XF_OK;
 }
 
@@ -450,7 +466,7 @@ XF_DLL int xf_table_pull_device(xf_table* t, const uint64_t* d_keys, uint64_t n,
   if (n == 0) return XF_OK;
   XF_TRY(t->ensure_room(n));
   XF_TRY(t->s_slots.ensure(n * sizeof(uint32_t)));
-  xf_launch_probe(t->view, d_keys, n, true, t->s_slots.as<uint32_t>(), d_w_out, t->stream);
+  xf_launch_probe(t->view, d_keys, n, true, t->s_slots.as<uint32_t>(), d_w_out, t->stream, t->stamps());
   ++t->launches;
   if (d_v_out && t->view.K > 0) {
     xf_launch_gather_v(t->view, t->s_slots.as<uint32_t>(), d_keys, n, d_v_out, t->stream);
@@ -466,7 +482,7 @@ XF_DLL int xf_table_push_device(xf_table* t, const uint64_t* d_keys, uint64_t n,
   if (d_gv && t->view.K == 0) d_gv = nullptr;
   XF_TRY(t->ensure_room(n));
   XF_TRY(t->s_slots.ensure(n * sizeof(uint32_t)));
-  xf_launch_probe(t->view, d_keys, n, true, t->s_slots.as<uint32_t>(), nullptr, t->stream);
+  xf_launch_probe(t->view, d_keys, n, true, t->s_slots.as<uint32_t>(), nullptr, t->stream, t->stamps());
   xf_launch_update_pushed(t->view, t->s_slots.as<uint32_t>(), n, d_gw, d_gv, t->stream);
   t->launches += 2;
   XF_CUDA_TRY(cudaGetLastError());
@@ -562,7 +578,7 @@ XF_DLL int xf_table_import(xf_table* t, const uint64_t* keys, uint64_t n, const 
   XF_TRY(xf_h2d_opt(t->s_v, K ? v : nullptr, n * K, t->stream, &dv));
   XF_TRY(xf_h2d_opt(t->s_nv, K ? nv : nullptr, n * K, t->stream, &dnv));
   XF_TRY(xf_h2d_opt(t->s_zv, K ? zv : nullptr, n * K, t->stream, &dzv));
-  xf_launch_probe(t->view, t->s_keys.as<uint64_t>(), n, true, t->s_slots.as<uint32_t>(), nullptr, t->stream);
+  xf_launch_probe(t->view, t->s_keys.as<uint64_t>(), n, true, t->s_slots.as<uint32_t>(), nullptr, t->stream, t->stamps());
   xf_launch_import(t->view, t->s_slots.as<uint32_t>(), n, dw, dnw, dzw, dv, dnv, dzv, t->stream);
   t->launches += 2;
   XF_CUDA_TRY(cudaGetLastError());
@@ -810,6 +826,11 @@ XF_DLL int xf_trainer_create(xf_trainer** out, xf_table* table, xf_comm* comm, c
       delete tr;
       return XF_ERR_ARG;
     }
+    if (table->d_stamp) {
+      xf_set_error("feature eviction is single-GPU only: the sharded step cannot stamp the keys it touches");
+      delete tr;
+      return XF_ERR_ARG;
+    }
     if (table->cfg.num_shards != xf_comm_nranks(comm) || table->cfg.shard_index != xf_comm_rank(comm)) {
       xf_set_error("table shard (%d of %d) does not match comm rank (%d of %d)", table->cfg.shard_index,
                    table->cfg.num_shards, xf_comm_rank(comm), xf_comm_nranks(comm));
@@ -917,8 +938,20 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     xf_set_error("feature admission is single-GPU only: the sharded step cannot serve a table with a policy");
     return XF_ERR_ARG;
   }
+  const bool stamp = t->d_stamp != nullptr;  // feature eviction: the tracking kernels
+  if (tr->mg && stamp) {
+    xf_set_error("feature eviction is single-GPU only: the sharded step cannot stamp the keys it touches");
+    return XF_ERR_ARG;
+  }
+  if (stamp && mode == 0 && rows > 0 && t->admit_batches >= 0xFFFFFFFFull) {
+    xf_set_error("the table has run 2^32 - 1 training batches: 32-bit eviction stamps cannot number the next one "
+                 "(xf_table_set_eviction(t, NULL) stops tracking)");
+    return XF_ERR_STATE;
+  }
   if (rows == 0 && !tr->mg) return XF_OK;     // sharded: an empty batch still takes part in the exchange
   if (!tr->mg) XF_TRY(t->ensure_room(nnz));  // the sharded path sizes the shard from what it receives
+  // taken after ensure_room: a growth there replaces the stamp array
+  const XfStampView sv = t->stamps();
   cudaStream_t st = t->stream;
   const bool prof = tr->profile && mode == 0;
   cudaEvent_t* pe = nullptr;
@@ -945,7 +978,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     if (mode == 0) XF_TRY(t->next_seq());
     xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, nnz, mode, t->seq, t->d_rows_by_seq,
                            (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                           mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, adm, st);
+                           mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, adm, sv, st);
     ++tr->launches;
     if (prof) {
       XF_CUDA_TRY(cudaEventRecord(pe[1], st));
@@ -972,7 +1005,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   else
     xf_launch_step(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(), nnz,
                    (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                   mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, adm, st);
+                   mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, adm, sv, st);
   ++tr->launches;
   if (prof) {
     XF_CUDA_TRY(cudaEventRecord(pe[1], st));
@@ -981,7 +1014,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   if (mode == 0) {
     // Push + server-side optimizer: one FTRL/SGD step per touched key with g / rows
     xf_launch_update_touched(t->view, tr->touched.as<uint32_t>(), (uint64_t)nnz + extra, (double)rows,
-                             tr->d_unique_total, st);
+                             tr->d_unique_total, sv, st);
     ++tr->launches;
   }
   if (prof) XF_CUDA_TRY(cudaEventRecord(pe[3], st));

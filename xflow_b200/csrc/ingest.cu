@@ -40,7 +40,7 @@ XF_DLL int xf_hash_decimal_ids_device(const uint32_t* d_ids, uint64_t n, uint64_
 // Pre-population: what a Pull of the ids [first, first + n) by any worker leaves behind — their keys
 // exist in the table with default contents (store[key], ftrl.h:56 / sgd.h:48).  Sharded tables keep only
 // the keys of their own range (postoffice.cc:134-143).  Ids are hashed as their decimal strings.
-__global__ void xf_k_touch_ids(XfTableView t, uint64_t first, uint64_t n, uint64_t width, int S, int shard) {
+__global__ void xf_k_touch_ids(XfTableView t, uint64_t first, uint64_t n, uint64_t width, int S, int shard, XfStampView sv) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     uint64_t v = first + i;
     char rev[20];
@@ -54,7 +54,7 @@ __global__ void xf_k_touch_ids(XfTableView t, uint64_t first, uint64_t n, uint64
       if ((int)(q < (uint64_t)S ? q : (uint64_t)S - 1) != shard) continue;
     }
     XfHead h;
-    xf_probe<true>(t, key, &h);
+    xf_probe<true, true>(t, key, &h, &sv);  // an inserted key is stamped when the table tracks stamps
   }
 }
 
@@ -67,7 +67,8 @@ XF_DLL int xf_table_touch_decimal_ids(xf_table* t, uint64_t first_id, uint64_t c
   for (uint64_t done = 0; done < count; done += chunk) {
     const uint64_t n = count - done < chunk ? count - done : chunk;
     XF_TRY(t->ensure_room(S > 1 ? n / (uint64_t)S + n / (8 * (uint64_t)S) + 65536 : n));
-    xf_k_touch_ids<<<xf_grid_for(n, 256, 8), 256, 0, t->stream>>>(t->view, first_id + done, n, width, S, t->cfg.shard_index);
+    xf_k_touch_ids<<<xf_grid_for(n, 256, 8), 256, 0, t->stream>>>(t->view, first_id + done, n, width, S, t->cfg.shard_index,
+                                                                        t->stamps());
     ++t->launches;
     XF_CUDA_TRY(cudaGetLastError());
   }

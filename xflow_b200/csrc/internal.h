@@ -80,10 +80,19 @@ struct xf_table {
   uint8_t* d_filter = nullptr;                // 2^log2_cells one-byte counters (XF_ADMIT_BLOOM only)
   unsigned long long* d_admit = nullptr;      // {rejected tokens, admitted keys, rejected-list length of even / odd b}
   uint64_t admit_batches = 0;
+  // feature eviction (xf_table_set_eviction, evict.cu): the sweep's limits and the stamps, one uint32_t per slot beside
+  // the rows (nullptr = tracking off); kernels that may stamp get stamps(): the array and the current batch number
+  xf_eviction_config evict{};
+  uint32_t* d_stamp = nullptr;
+  XfStampView stamps() const { return XfStampView{d_stamp, (uint32_t)(admit_batches < 0xFFFFFFFFull ? admit_batches : 0xFFFFFFFFull)}; }
+  uint64_t cap_floor = 0;     // no sweep shrinks the table below this: the creation capacity, the largest reserve
+  XfDevBuf s_hist;            // the sweep's 2^16-bin histogram
 
-  int alloc_table(uint64_t capacity);
+  int alloc_table(uint64_t capacity);  // a fresh table (with a stamp array if tracking is on); on failure view is kept
   int ensure_room(uint64_t incoming_keys);
   int grow(uint64_t new_capacity);
+  // rebuild at new_capacity with the rows `keep` keeps (grow keeps all): old + new are allocated at the peak
+  int rebuild(uint64_t new_capacity, const XfKeep& keep);
   int check_error();
 };
 

@@ -12,7 +12,7 @@ int xf_tps_for(int K);
 void xf_launch_fill(const XfTableView& t, cudaStream_t st);
 void xf_launch_step(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels,
                     int B, int mode, uint32_t* touched, uint32_t nnz, float* loss_out, float* pctr_out,
-                    float* abs_loss_sum, const XfAdmitView* adm, cudaStream_t st);
+                    float* abs_loss_sum, const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st);
 // feature admission (admit.cu): after a step on the table's stream, count the batch's rejected tokens into the
 // Bloom filter (n = *rej_n of them in rej_keys, at most nnz), add n to *rejected_total and zero *next_rej_n
 void xf_launch_admit_count(const XfAdmitView& a, uint8_t* cells, const uint64_t* rej_keys, const unsigned long long* rej_n,
@@ -21,27 +21,45 @@ void xf_launch_admit_count(const XfAdmitView& a, uint8_t* cells, const uint64_t*
 void xf_launch_admit_decay(uint8_t* cells, uint32_t log2_cells, cudaStream_t st);
 // FM step: shared-memory hot-key cache; its flush uses touched[nnz .. nnz + xf_step_touched_extra)
 uint32_t xf_step_touched_extra(int K, int B);
-// touched[j] (one entry per token position) = slot of the key first touched by token j, else 0xFFFFFFFF
+// touched[j] (one entry per token position) = slot of the key first touched by token j, else 0xFFFFFFFF;
+// sv.stamp != nullptr (feature eviction): the rows updated get stamp[slot] = sv.now
 void xf_launch_update_touched(const XfTableView& t, const uint32_t* touched, uint64_t nnz, double rows,
-                              unsigned long long* unique_total, cudaStream_t st);
+                              unsigned long long* unique_total, const XfStampView& sv, cudaStream_t st);
 void xf_launch_update_pushed(const XfTableView& t, const uint32_t* slots, uint64_t n, const float* gw,
                              const float* gv, cudaStream_t st);
+// a key it inserts gets stamp = sv.now when sv.stamp != nullptr (feature eviction)
 void xf_launch_probe(const XfTableView& t, const uint64_t* keys, uint64_t n, bool insert, uint32_t* slots,
-                     float* w_out, cudaStream_t st);
+                     float* w_out, cudaStream_t st, const XfStampView& sv = XfStampView{nullptr, 0u});
 void xf_launch_gather_v(const XfTableView& t, const uint32_t* slots, const uint64_t* keys, uint64_t n,
                         float* v_out, cudaStream_t st);
 void xf_launch_import(const XfTableView& t, const uint32_t* slots, uint64_t n, const float* w, const float* nw,
                       const float* zw, const float* v, const float* nv, const float* zv, cudaStream_t st);
 void xf_launch_export(const XfTableView& t, const uint32_t* slots, const uint64_t* keys, uint64_t n, float* w,
                       float* nw, float* zw, float* v, float* nv, float* zv, uint8_t* present, cudaStream_t st);
-void xf_launch_rehash(const XfTableView& src, const XfTableView& dst, cudaStream_t st);
+// re-insert the rows of `src` that `keep` keeps into `dst` (growth: all of them), with their stamps
+void xf_launch_rehash(const XfTableView& src, const XfTableView& dst, const XfKeep& keep, const uint32_t* src_stamp,
+                      uint32_t* dst_stamp, cudaStream_t st);
+// feature eviction (evict.cu): stamp every slot with `value` (tracking starts); out[i] = stamp of slots[i], or
+// UINT64_MAX for 0xFFFFFFFF; the histogram passes of the sweep's radix select
+void xf_launch_stamp_fill(uint32_t* stamp, uint64_t n, uint32_t value, cudaStream_t st);
+void xf_launch_gather_stamps(const uint32_t* stamp, const uint32_t* slots, uint64_t n, uint64_t* out, cudaStream_t st);
+struct XfEvictPass {
+  int what;          // 0: high 16 bits of the stamp; 1: its low 16 bits, among stamps with high bits `hi`;
+                     // 2: the 16-bit key digit at `shift`, among keys of stamp `s_star` whose bits above it are `prefix`
+  uint32_t cutoff;   // only stamps >= cutoff count
+  uint32_t hi, s_star;
+  uint64_t prefix;
+  int shift;
+};
+void xf_launch_evict_hist(const XfTableView& t, const uint32_t* stamp, const XfEvictPass& p, unsigned int* hist,
+                          cudaStream_t st);
 void xf_launch_list_keys(const XfTableView& t, uint64_t* keys_out, unsigned long long* count, uint64_t max_out,
                          cudaStream_t st);
 int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm);
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
-                            const XfAdmitView* adm, cudaStream_t st);
+                            const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st);
 
 // lazy tables: fold all pending steps (sequence numbers restart afterwards)
 void xf_launch_flush_pending(const XfTableView& t, cudaStream_t st);

@@ -80,12 +80,14 @@ __device__ __forceinline__ void xf_fm_token(const XfTableView& t, uint32_t slot,
 //   mode: 0 = train, 1 = predict (forward only; the Pull still inserts missing keys, lr_worker.cc:47)
 // ADMIT: absent keys are inserted only if the admission policy `adm` admits them (xf_probe_from); a rejected token
 // adds nothing to its row's sums and never reaches the hot-key cache or touched[] (its slot stays XF_NO_SLOT).
-template <bool FM, int VEC, bool ADMIT>
+// STAMP (feature eviction): a key this kernel inserts is stamped with sv.now; the training step's other keys
+// are stamped by the optimizer pass over touched[] (xf_k_update).
+template <bool FM, int VEC, bool ADMIT, bool STAMP>
 __global__ void __launch_bounds__(256)
 xf_k_step(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
           const uint8_t* __restrict__ labels, int B, int mode, uint32_t* __restrict__ touched,
           float* __restrict__ loss_out, float* __restrict__ pctr_out, float* __restrict__ abs_loss_sum,
-          int log2nc, uint32_t touched_base, XfAdmitView adm) {
+          int log2nc, uint32_t touched_base, XfAdmitView adm, XfStampView sv) {
   __shared__ float s_abs[8];
   extern __shared__ __align__(16) unsigned char xf_smem[];
   float abs_acc = 0.f;
@@ -129,11 +131,11 @@ xf_k_step(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* _
       uint32_t s0 = XF_NO_SLOT, s1 = XF_NO_SLOT;
       bool r0 = false, r1 = false;
       if (v0) {
-        const int64_t r = xf_probe_from<true, ADMIT>(t, k0, p0, h0, &adm, &r0);
+        const int64_t r = xf_probe_from<true, ADMIT, STAMP>(t, k0, p0, h0, &adm, &r0, &sv);
         if (r >= 0) { s0 = (uint32_t)r; wsum += h0.w; }
       }
       if (v1) {
-        const int64_t r = xf_probe_from<true, ADMIT>(t, k1, p1, h1, &adm, &r1);
+        const int64_t r = xf_probe_from<true, ADMIT, STAMP>(t, k1, p1, h1, &adm, &r1, &sv);
         if (r >= 0) { s1 = (uint32_t)r; wsum += h1.w; }
       }
       if (ADMIT) xf_admit_append(adm, r0, k0, r1, k1);
@@ -285,28 +287,33 @@ uint32_t xf_step_touched_extra(int K, int B) {
 
 void xf_launch_step(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels,
                     int B, int mode, uint32_t* touched, uint32_t nnz, float* loss_out, float* pctr_out,
-                    float* abs_loss_sum, const XfAdmitView* adm, cudaStream_t st) {
+                    float* abs_loss_sum, const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st) {
   if (B <= 0) return;
   const int block = 256;
   const int grid = xf_grid_for((uint64_t)B * 32, block, 8);
   const int lg = xf_step_cache_log2(t.K);
   const size_t smem = lg >= 0 ? ((size_t)1 << lg) * 28 : 0;
-#define XF_STEP_ARGS t, row_ptr, keys, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, lg, nnz, a
-#define XF_STEP_LAUNCH(A)                                                                  \
+#define XF_STEP_ARGS t, row_ptr, keys, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, lg, nnz, a, sv
+#define XF_STEP_LAUNCH(A, S)                                                               \
   if (t.K == 0) {                                                                          \
-    xf_k_step<false, 1, A><<<grid, block, 0, st>>>(XF_STEP_ARGS);                          \
+    xf_k_step<false, 1, A, S><<<grid, block, 0, st>>>(XF_STEP_ARGS);                       \
   } else {                                                                                 \
     switch (xf_vec_for(t.K)) {                                                             \
-      case 4: xf_k_step<true, 4, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;       \
-      case 2: xf_k_step<true, 2, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;       \
-      default: xf_k_step<true, 1, A><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;      \
+      case 4: xf_k_step<true, 4, A, S><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;    \
+      case 2: xf_k_step<true, 2, A, S><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;    \
+      default: xf_k_step<true, 1, A, S><<<grid, block, smem, st>>>(XF_STEP_ARGS); break;   \
     }                                                                                      \
   }
   const XfAdmitView a = adm ? *adm : XfAdmitView{};
-  if (adm) {
-    XF_STEP_LAUNCH(true)
+  const bool stamp = sv.stamp != nullptr;
+  if (adm && stamp) {
+    XF_STEP_LAUNCH(true, true)
+  } else if (adm) {
+    XF_STEP_LAUNCH(true, false)
+  } else if (stamp) {
+    XF_STEP_LAUNCH(false, true)
   } else {
-    XF_STEP_LAUNCH(false)
+    XF_STEP_LAUNCH(false, false)
   }
 #undef XF_STEP_LAUNCH
 #undef XF_STEP_ARGS

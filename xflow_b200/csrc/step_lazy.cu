@@ -44,10 +44,11 @@
 // Otherwise s and i move on to the next probe slot, which the caller loads.
 // ADMIT: an absent key asks the admission policy before its CAS; a key it does not admit resolves with slot =
 // XF_NO_SLOT (it pulls w = 0 and takes no part in phase B) and *rejected = true (predict: false, nothing counted).
-template <bool ADMIT>
+// STAMP (feature eviction): a key this look inserts is stamped with sv.now.
+template <bool ADMIT, bool STAMP>
 __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key, uint64_t& s, uint32_t& i, uint64_t& q0,
                                              uint64_t& q1, uint64_t& q2, uint64_t& q3, uint32_t& slot, bool& created,
-                                             const XfAdmitView& adm, bool& rejected) {
+                                             const XfAdmitView& adm, bool& rejected, const XfStampView& sv) {
   if (q0 == key) { slot = (uint32_t)s; return true; }
   if (q0 == XF_EMPTY_KEY) {
     if (ADMIT && !xf_admit(adm, key)) {
@@ -57,6 +58,7 @@ __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key,
     const unsigned long long old =
         atomicCAS(reinterpret_cast<unsigned long long*>(xf_row(t, s)), (unsigned long long)XF_EMPTY_KEY, (unsigned long long)key);
     if (old == XF_EMPTY_KEY) {
+      if (STAMP) sv.stamp[s] = sv.now;
       created = true;
       q0 = key; q1 = q2 = q3 = 0ull;  // lazy rows: g is the integer 0, no state, no tag
       slot = (uint32_t)s;
@@ -75,12 +77,14 @@ __device__ __forceinline__ bool xf_lazy_look(const XfTableView& t, uint64_t key,
 }
 
 // ADMIT = false is the kernel without an admission policy (every absent key is inserted); ADMIT = true asks `adm`.
-template <bool ADMIT>
+// STAMP = true (feature eviction) stores stamp[slot] = sv.now where a key is inserted and where a training
+// batch opens a row (the deposit that returns true: once per key and batch); STAMP = false is the kernel without it.
+template <bool ADMIT, bool STAMP>
 __global__ void __launch_bounds__(256, 3)
 xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
                   const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint64_t* rows_by_seq, int fix_shift,
                   float* __restrict__ loss_out, float* __restrict__ pctr_out, float* __restrict__ abs_loss_sum,
-                  unsigned long long* __restrict__ unique_total, XfAdmitView adm) {
+                  unsigned long long* __restrict__ unique_total, XfAdmitView adm, XfStampView sv) {
   __shared__ float s_abs[8];
   __shared__ unsigned int s_open;
   // the group leaders' looks at their rows, from phase A to phase B.  In registers they took the kernel past the
@@ -130,8 +134,8 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       bool u0 = v0, u1 = v1, r0 = false, r1 = false;
       for (;;) {
         bool c0 = false, c1 = false;
-        if (u0) u0 = !xf_lazy_look<ADMIT>(t, k0, p0, i0, a0, a1, a2, a3, s0, c0, adm, r0);
-        if (u1) u1 = !xf_lazy_look<ADMIT>(t, k1, p1, i1, b0, b1, b2, b3, s1, c1, adm, r1);
+        if (u0) u0 = !xf_lazy_look<ADMIT, STAMP>(t, k0, p0, i0, a0, a1, a2, a3, s0, c0, adm, r0, sv);
+        if (u1) u1 = !xf_lazy_look<ADMIT, STAMP>(t, k1, p1, i1, b0, b1, b2, b3, s1, c1, adm, r1, sv);
         const unsigned created = __popc(__ballot_sync(0xffffffffu, c0)) + __popc(__ballot_sync(0xffffffffu, c1));
         if (created && lane == 0) {
           atomicAdd(t.size, (unsigned long long)created);
@@ -159,8 +163,14 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       const bool L0 = s0 != XF_NO_SLOT && lane == __ffs(grp0) - 1, L1 = s1 != XF_NO_SLOT && lane == __ffs(grp1) - 1;
       if (ch >= XF_LAZY_CACHED) {
         // long rows (> 128 tokens): nothing is remembered for phase B; open the row now with an empty deposit
-        if (L0 && xf_lazy_deposit(t, xf_row(t, s0), a2, a3, a2n, seq, 0ll)) ++open_acc;
-        if (L1 && xf_lazy_deposit(t, xf_row(t, s1), b2, b3, b2n, seq, 0ll)) ++open_acc;
+        if (L0 && xf_lazy_deposit(t, xf_row(t, s0), a2, a3, a2n, seq, 0ll)) {
+          ++open_acc;
+          if (STAMP) sv.stamp[s0] = sv.now;
+        }
+        if (L1 && xf_lazy_deposit(t, xf_row(t, s1), b2, b3, b2n, seq, 0ll)) {
+          ++open_acc;
+          if (STAMP) sv.stamp[s1] = sv.now;
+        }
       }
 #pragma unroll
       for (int c = 0; c < XF_LAZY_CACHED; ++c)
@@ -191,12 +201,16 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       const int x = threadIdx.x;
       if (lead_s[2 * c] != XF_NO_SLOT &&
           xf_lazy_deposit(t, xf_row(t, lead_s[2 * c]), s_q2[2 * c][x], s_q3[2 * c][x], s_q2n[2 * c][x], seq,
-                          lf * (long long)(cnt_c[c] & 0xFFu)))
+                          lf * (long long)(cnt_c[c] & 0xFFu))) {
         ++open_acc;
+        if (STAMP) sv.stamp[lead_s[2 * c]] = sv.now;
+      }
       if (lead_s[2 * c + 1] != XF_NO_SLOT &&
           xf_lazy_deposit(t, xf_row(t, lead_s[2 * c + 1]), s_q2[2 * c + 1][x], s_q3[2 * c + 1][x], s_q2n[2 * c + 1][x], seq,
-                          lf * (long long)(cnt_c[c] >> 8)))
+                          lf * (long long)(cnt_c[c] >> 8))) {
         ++open_acc;
+        if (STAMP) sv.stamp[lead_s[2 * c + 1]] = sv.now;
+      }
     }
     for (int ch = XF_LAZY_CACHED; ch < chunks; ++ch) {
       // long rows (> 128 tokens): the rows were opened in phase A
@@ -225,14 +239,18 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
-                            const XfAdmitView* adm, cudaStream_t st) {
+                            const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st) {
   if (B <= 0) return;
   const int grid = xf_grid_for((uint64_t)B * 32, 256, 8);
   const int fs = xf_fix_shift(nnz);  // nnz bounds every key's residual sum in this batch
-  if (adm)
-    xf_k_step_lr_lazy<true><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, loss_out,
-                                                  pctr_out, abs_loss_sum, unique_total, *adm);
-  else
-    xf_k_step_lr_lazy<false><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, loss_out,
-                                                   pctr_out, abs_loss_sum, unique_total, XfAdmitView{});
+  const XfAdmitView a = adm ? *adm : XfAdmitView{};
+#define XF_LAZY_LAUNCH(A, S)                                                                                    \
+  xf_k_step_lr_lazy<A, S><<<grid, 256, 0, st>>>(t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, loss_out, \
+                                                pctr_out, abs_loss_sum, unique_total, a, sv)
+  const bool stamp = sv.stamp != nullptr;
+  if (adm && stamp) XF_LAZY_LAUNCH(true, true);
+  else if (adm) XF_LAZY_LAUNCH(true, false);
+  else if (stamp) XF_LAZY_LAUNCH(false, true);
+  else XF_LAZY_LAUNCH(false, false);
+#undef XF_LAZY_LAUNCH
 }

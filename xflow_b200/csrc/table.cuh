@@ -106,6 +106,25 @@ struct XfAdmitView {
   uint64_t* rej_keys;                    // the list (nullptr: count only)
   unsigned long long* admitted;          // keys inserted by admission (stats)
 };
+// Feature eviction (evict.cu): which keys a sweep keeps, as one predicate on (stamp, key).  Order: a larger stamp is
+// more recent, and between equal stamps the smaller key is.  A key is kept iff stamp >= cutoff and, if bounded, it is
+// at least as recent as the boundary (s_star, k_star).  Growth keeps every key (cutoff 0, not bounded).
+struct XfKeep {
+  uint32_t cutoff;
+  int bounded;
+  uint32_t s_star;
+  uint64_t k_star;
+};
+// Feature eviction (xf_table_set_eviction, evict.cu): stamp[slot] = the training-batch number that last touched the
+// slot's key (nullptr: tracking off); now = the table's batch number when the kernel was launched.  A kernel
+// parameter of its own, passed last: inside XfTableView it changed how ptxas allocates the FM step's registers.
+struct XfStampView {
+  uint32_t* stamp;
+  uint32_t now;
+};
+__host__ __device__ __forceinline__ bool xf_keeps(const XfKeep& k, uint32_t stamp, uint64_t key) {
+  return stamp >= k.cutoff && (!k.bounded || stamp > k.s_star || (stamp == k.s_star && key <= k.k_star));
+}
 #define XF_TAG_LOCKED 0xFFFFFFFFu  // never a batch number (the sequence ring is far smaller)
 #define XF_FIX_MAX_SHIFT 27    // the finest unit of a lazy table's residual sums: 2^-27
 #define XF_TAG_MASK 0xFFFFull  // lazy rows: low 16 bits of the word at byte 24
@@ -327,9 +346,11 @@ __device__ __forceinline__ void xf_store_head(uint8_t* row, const XfHead& h) {
 // was when the key matched (or the default contents on insert).
 // ADMIT (INSERT only): an absent key is inserted only if the policy `*adm` admits it; otherwise the call returns -1
 // and sets *rejected (unless the policy is XF_ADM_NEVER).  Every token of one key decides the same way in a batch.
-template <bool INSERT, bool ADMIT = false>
+// STAMP (INSERT only): the inserting thread stamps the new key with sv->now when the table tracks stamps.
+template <bool INSERT, bool ADMIT = false, bool STAMP = false>
 __device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t key, uint64_t s, XfHead& h,
-                                                 const XfAdmitView* adm = nullptr, bool* rejected = nullptr) {
+                                                 const XfAdmitView* adm = nullptr, bool* rejected = nullptr,
+                                                 const XfStampView* sv = nullptr) {
   for (int probes = 0; probes < XF_MAX_PROBE; ++probes) {
     if (h.key == key) return (int64_t)s;
     if (h.key == XF_EMPTY_KEY) {
@@ -349,6 +370,7 @@ __device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t 
           atomicAdd(t.size, (unsigned long long)__popc(m));
           if (ADMIT) atomicAdd(adm->admitted, (unsigned long long)__popc(m));
         }
+        if (STAMP && sv->stamp != nullptr) sv->stamp[s] = sv->now;
         h.key = key; h.flags = 0; h.w = 0.f; h.n = 0.f; h.z = 0.f;
         h.g = t.lazy ? 0.0 : -0.0;  // what xf_k_fill left in the row (lazy: the integer 0)
         return (int64_t)s;
@@ -367,11 +389,12 @@ __device__ __forceinline__ int64_t xf_probe_from(const XfTableView& t, uint64_t 
   return -1;
 }
 
-template <bool INSERT>
-__device__ __forceinline__ int64_t xf_probe(const XfTableView& t, uint64_t key, XfHead* head) {
+template <bool INSERT, bool STAMP = false>
+__device__ __forceinline__ int64_t xf_probe(const XfTableView& t, uint64_t key, XfHead* head,
+                                            const XfStampView* sv = nullptr) {
   const uint64_t s = xf_home_slot(t, key);
   XfHead h = xf_load_head(xf_row(t, s));
-  const int64_t r = xf_probe_from<INSERT>(t, key, s, h);
+  const int64_t r = xf_probe_from<INSERT, false, STAMP>(t, key, s, h, nullptr, nullptr, sv);
   *head = h;
   return r;
 }

@@ -85,6 +85,47 @@ static xf_admission_config AdmissionFromEnv(int world) {
   return c;
 }
 
+// Feature eviction (xf_table_set_eviction): XFLOW_EVICT_IDLE = T drops keys no training batch touched among the last
+// T, XFLOW_EVICT_MAX_KEYS = N keeps the N most recently touched; the worker sweeps after every training step that makes
+// the table's batch number a multiple of XFLOW_EVICT_EVERY = E (required with a limit).  Unset: no tracking.  Single
+// GPU only.  *every = E (0: eviction off).
+static uint64_t env_count(const char* name, bool positive) {
+  const char* v = getenv(name);
+  if (!v || !*v) return 0;
+  char* end = nullptr;
+  const unsigned long long n = strtoull(v, &end, 10);
+  if (*end || *v == '-' || (positive && n == 0))
+    throw std::runtime_error(std::string(name) + " must be a count " + (positive ? "> 0" : ">= 0") + ", got '" + v + "'");
+  return (uint64_t)n;
+}
+static xf_eviction_config EvictionFromEnv(int world, uint64_t* every) {
+  xf_eviction_config c;
+  c.max_idle_batches = env_count("XFLOW_EVICT_IDLE", false);
+  c.max_keys = env_count("XFLOW_EVICT_MAX_KEYS", false);
+  *every = env_count("XFLOW_EVICT_EVERY", true);
+  const bool limit = c.max_idle_batches > 0 || c.max_keys > 0;
+  if (limit && *every == 0)
+    throw std::runtime_error("XFLOW_EVICT_IDLE / XFLOW_EVICT_MAX_KEYS need XFLOW_EVICT_EVERY = <batches between sweeps>");
+  if (!limit && *every > 0) throw std::runtime_error("XFLOW_EVICT_EVERY needs XFLOW_EVICT_IDLE or XFLOW_EVICT_MAX_KEYS");
+  if (limit && world > 1) throw std::runtime_error("XFLOW_EVICT_* is single-GPU only: unset it or run with XFLOW_WORLD = 1");
+  return c;
+}
+
+// the table's training-batch number (host state, no device sync)
+static uint64_t TableBatches(xf_table* t) {
+  uint64_t b = 0;
+  if (xf_table_admission_stats(t, &b, nullptr, nullptr) != XF_OK) throw std::runtime_error(std::string("xf_table_admission_stats: ") + xf_last_error());
+  return b;
+}
+// after a training step that started at batch number `before`: sweep if the step made the number a multiple of E
+static void SweepIfDue(xf_table* t, uint64_t before) {
+  static const uint64_t every = [] { uint64_t e = 0; EvictionFromEnv(1, &e); return e; }();
+  if (!every) return;
+  const uint64_t b = TableBatches(t);
+  if (b != before && b % every == 0 && xf_table_evict(t, nullptr) != XF_OK)
+    throw std::runtime_error(std::string("xf_table_evict: ") + xf_last_error());
+}
+
 int MyRank() { return env_int("XFLOW_RANK", env_int("RANK", 0)); }
 int NumWorkers() { return env_int("XFLOW_WORLD", env_int("WORLD_SIZE", 1)); }
 
@@ -116,6 +157,8 @@ Server::Server(Optimizer opt, int latent_dim, int device)
     throw std::runtime_error("rank " + std::to_string(rank_) + " needs XFLOW_WORLD / WORLD_SIZE > rank: a worker with rank > 0 "
                              "has no servers to talk to on its own");
   AdmissionFromEnv(world_);  // a malformed XFLOW_ADMIT, or one with XFLOW_WORLD > 1, fails here
+  uint64_t every = 0;
+  EvictionFromEnv(world_, &every);  // likewise XFLOW_EVICT_*
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -164,6 +207,16 @@ static xf_table* make_table(Optimizer opt, int K, int device, int rank, int worl
       const std::string err = xf_last_error();
       xf_table_destroy(t);
       throw std::runtime_error("xf_table_set_admission: " + err);
+    }
+  }
+  uint64_t every = 0;
+  const xf_eviction_config ev = EvictionFromEnv(world, &every);
+  if (every) {
+    const int rc = xf_table_set_eviction(t, &ev);
+    if (rc != XF_OK) {
+      const std::string err = xf_last_error();
+      xf_table_destroy(t);
+      throw std::runtime_error("xf_table_set_eviction: " + err);
     }
   }
   return t;
@@ -237,8 +290,10 @@ void WorkerBase::update(int start, int end) {
     rp = slice_row_ptr_.data();
   }
   ensure_trainer(rows, nnz);
+  const uint64_t before = TableBatches(table_);
   must(xf_trainer_step_host(trainer_, rp, cur_keys_ + base, cur_labels_ + start, rows, nnz, nullptr),
        "xf_trainer_step_host");
+  SweepIfDue(table_, before);
   rows_trained += rows;
 }
 
@@ -344,7 +399,9 @@ void WorkerBase::batch_training() {
       run_blocks(collective_blocks, [&](uint32_t rows) {
         const uint32_t thread_size = rows / (uint32_t)core_num;  // :190 — remainder rows are dropped, as in the reference
         for (uint32_t i = 0; i < (uint32_t)core_num; ++i) {      // :192-196
+          const uint64_t before = TableBatches(table_);
           must(xf_trainer_step_ingested(trainer_, i * thread_size, (i + 1) * thread_size), "xf_trainer_step_ingested");
+          SweepIfDue(table_, before);
           rows_trained += thread_size;
         }
       });
