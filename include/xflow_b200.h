@@ -35,7 +35,8 @@ enum {
   XF_OK = 0,
   XF_ERR_ARG = -1,       /* bad argument */
   XF_ERR_CUDA = -2,      /* CUDA runtime error (incl. "no device") */
-  XF_ERR_FULL = -3,      /* table probe overflow and growth impossible */
+  XF_ERR_FULL = -3,      /* no room: capacity past 2^31 slots, or a probe sequence overflowed (sticky, see
+                            "Probe overflow" above xf_table_pull) */
   XF_ERR_IO = -4,        /* file open / read failure (reference: exit(1), io.h:33-36) */
   XF_ERR_COMM = -5,      /* NCCL failure */
   XF_ERR_STATE = -6
@@ -84,6 +85,22 @@ XF_DLL int xf_table_config_default(xf_table_config* cfg);
 /* replaces: new ps::KVServer<float>(0/1) + set_request_handle(FTRL/SGD handle)  (server.h:22-31) */
 XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg);
 XF_DLL int xf_table_destroy(xf_table* t);
+
+/* Keys.  Any u64 but 2^64 - 1, which marks an empty slot of the table (the reference has no server range that holds
+ * it either).  The entry points that take keys from HOST memory refuse it with XF_ERR_ARG, naming it, before anything
+ * is enqueued: xf_table_pull, _push, _import, _export, _last_touch, and xf_trainer_step_host / _predict_host with
+ * their _values and _fields forms.  The device-pointer entry points (xf_table_pull_device / _push_device,
+ * xf_trainer_step_device*), the _async steps, the id and text-ingest paths do not look: that would be one more pass
+ * over every batch on the paths that carry the bulk of the training data, and a key hashed on the device is 2^64 - 1
+ * with probability 2^-64 per id.  There the key is the caller's contract.
+ *
+ * Probe overflow.  A lookup visits at most 8192 slots (XF_MAX_PROBE) of its key's probe sequence.  Growth keeps the
+ * load at or below 0.75, so hashed keys never come near that; but keys that share one probe sequence form a single
+ * chain whatever the capacity, and once 8192 of them are present, inserting or even looking up another key of that
+ * sequence overflows, at any capacity.  The call reports XF_ERR_FULL ("table probe sequence overflowed"); a training
+ * step reports it at the next call that checks the table: xf_trainer_sync, xf_table_sync, a predict, or a table call
+ * below that returns data to the host.  The key or token that overflowed is skipped.  The error is sticky: nothing
+ * clears it, and every later such call on the table returns XF_ERR_FULL. */
 
 /* replaces: KVWorker<float>::Pull + Wait (kv_app.h:147-165) served by KVServerFTRLHandle_w/_v pull
  * branch (ftrl.h:49-52,75-77,108-111,142-144 ; sgd.h).  keys: n host u64 (any order, duplicates allowed

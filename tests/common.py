@@ -243,6 +243,45 @@ class CanonicalFM64:
                 for j, k in enumerate(("w", "nw", "zw", "v", "nv", "zv"))}
 
 
+class MVM64:
+    """float64 numpy model of XF_MODEL_MVM (step_mvm.cu; SURVEY 8f-4): y = sum_k prod_{fields present}
+    (sum_{tokens of the field} v_k x), gradient of a token = residual * x * product of the OTHER fields' sums, one FTRL
+    or SGD step (learning rate `lr`) per touched key on v.  State: V, NV, ZV [n, K] of the keys `idx` indexes."""
+
+    def __init__(self, V0, opt, lr):
+        self.V = np.asarray(V0, np.float64).copy()
+        self.NV = np.zeros_like(self.V)
+        self.ZV = np.zeros_like(self.V)
+        self.opt, self.lr = opt, lr
+
+    def step(self, idx, rp, fields, x, lab):
+        """One training step on tokens whose keys are rows `idx` of the state; returns the residuals of the rows."""
+        V, B, K = self.V, lab.size, self.V.shape[1]
+        row_of = np.repeat(np.arange(B), np.diff(rp).astype(np.int64))
+        x64 = np.ones(idx.size) if x is None else x.astype(np.float64)
+        S = np.zeros((B, 32, K)); np.add.at(S, (row_of, fields.astype(np.int64)), V[idx] * x64[:, None])
+        present = np.zeros((B, 32), bool); present[row_of, fields.astype(np.int64)] = True
+        Sp = np.where(present[:, :, None], S, 1.0)
+        y = np.where(present.any(1), Sp.prod(1).sum(1), 0.0)
+        p = np.where(y < -30, 1e-6, np.where(y > 30, 1.0, np.power(2.718281828, y) / (1 + np.power(2.718281828, y))))
+        loss = p - lab
+        # product over the other fields of the row, per token
+        excl = np.ones((idx.size, K))
+        for f in range(32):
+            other = present[row_of, f] & (fields != f)
+            excl[other] *= S[row_of[other], f]
+        gtok = loss[row_of, None] * x64[:, None] * excl
+        A = np.zeros_like(V); np.add.at(A, idx, gtok)
+        touched = np.zeros(V.shape[0], bool); touched[idx] = True
+        g = A / B
+        for i in np.nonzero(touched)[0]:
+            if self.opt == "ftrl":
+                V[i], self.NV[i], self.ZV[i] = ftrl64(g[i], V[i], self.NV[i], self.ZV[i])
+            else:
+                V[i] = V[i] - self.lr * g[i]
+        return loss
+
+
 def build_and_run_ps_compat(tmp_dir):
     """Compile tests/cxx/ps_compat_check.cc against the shipped headers + library and run it."""
     import subprocess

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 from cases import CASES
-from common import (CanonicalFM64, check_fm_first_step, assert_close, assert_close_noise_aware, data_prefixes, ftrl64,
+from common import (MVM64, CanonicalFM64, check_fm_first_step, assert_close, assert_close_noise_aware, data_prefixes,
                     golden, oracle_case_run)
 from oracle import oracle as O
 from xflow_b200 import api, datagen
@@ -552,33 +552,12 @@ def test_defined_mvm_matches_float64_model(K, opt, with_vals):
     allk = np.unique(np.concatenate([b[1] for b in batches]))
     V0 = rng.normal(0.0, 0.6, (allk.size, K)).astype(np.float32)
     t.import_(allk, v=V0)
-    V = V0.astype(np.float64); NV = np.zeros_like(V); ZV = np.zeros_like(V)
+    model = MVM64(V0, opt, lr)
     for step, (rp, keys, fields, x, lab) in enumerate(batches):
-        idx = np.searchsorted(allk, keys)
-        row_of = np.repeat(np.arange(B), np.diff(rp).astype(np.int64))
-        x64 = np.ones(keys.size) if x is None else x.astype(np.float64)
-        S = np.zeros((B, 32, K)); np.add.at(S, (row_of, fields.astype(np.int64)), V[idx] * x64[:, None])
-        present = np.zeros((B, 32), bool); present[row_of, fields.astype(np.int64)] = True
-        Sp = np.where(present[:, :, None], S, 1.0)
-        y = np.where(present.any(1), Sp.prod(1).sum(1), 0.0)
-        p = np.where(y < -30, 1e-6, np.where(y > 30, 1.0, np.power(2.718281828, y) / (1 + np.power(2.718281828, y))))
-        loss = p - lab
+        loss = model.step(np.searchsorted(allk, keys), rp, fields, x, lab)
         tr.step_host_fields(rp, keys, fields, x, lab)
         assert_close(tr.get_loss(B), loss, "MVM residuals, step %d" % step, rel=5e-5, abs_floor=5e-6)
-        # product over the other fields of the row, per token
-        excl = np.ones((keys.size, K))
-        for f in range(32):
-            other = present[row_of, f] & (fields != f)
-            excl[other] *= S[row_of[other], f]
-        gtok = loss[row_of, None] * x64[:, None] * excl
-        A = np.zeros_like(V); np.add.at(A, idx, gtok)
-        touched = np.zeros(allk.size, bool); touched[idx] = True
-        g = A / B
-        for i in np.nonzero(touched)[0]:
-            if opt == "ftrl":
-                V[i], NV[i], ZV[i] = ftrl64(g[i], V[i], NV[i], ZV[i])
-            else:
-                V[i] = V[i] - lr * g[i]
+    V, NV, ZV = model.V, model.NV, model.ZV
     e = t.export(allk)
     assert e["present"].all()
     if opt == "ftrl":

@@ -22,6 +22,19 @@ void xf_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 XF_DLL const char* xf_last_error(void) { return g_err; }
+
+// 2^64 - 1 is XF_EMPTY_KEY, the mark of an empty slot, and never a key: a probe for it stops at the first free slot of
+// its chain and takes that slot for the key's row without claiming it, so what it writes there would show up in the
+// next key to land in the slot.  The entry points that take keys from host memory refuse it before enqueuing anything.
+int xf_check_host_keys(const uint64_t* keys, uint64_t n, const char* fn) {
+  for (uint64_t i = 0; i < n; ++i)
+    if (keys[i] == XF_EMPTY_KEY) {
+      xf_set_error("%s: key %llu (2^64 - 1) at position %llu is reserved: it marks an empty table slot", fn,
+                   (unsigned long long)keys[i], (unsigned long long)i);
+      return XF_ERR_ARG;
+    }
+  return XF_OK;
+}
 XF_DLL int xf_version(void) { return 100; }
 XF_DLL int xf_device_count(void) {
   int n = 0;
@@ -491,6 +504,7 @@ XF_DLL int xf_table_push_device(xf_table* t, const uint64_t* d_keys, uint64_t n,
 
 XF_DLL int xf_table_pull(xf_table* t, const uint64_t* keys, uint64_t n, float* w_out, float* v_out) {
   if (!t || (!keys && n)) return XF_ERR_ARG;
+  XF_TRY(xf_check_host_keys(keys, n, "xf_table_pull"));
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   if (n == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
@@ -533,6 +547,7 @@ XF_DLL int xf_table_push(xf_table* t, const uint64_t* keys, uint64_t n, const fl
   if (!t || (!keys && n)) return XF_ERR_ARG;
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   if (n == 0) return XF_OK;
+  XF_TRY(xf_check_host_keys(keys, n, "xf_table_push"));
   XF_TRY(xf_check_unique_keys(keys, n));
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
   const int K = t->view.K;
@@ -563,6 +578,7 @@ static int xf_h2d_opt(XfDevBuf& b, const float* src, size_t count, cudaStream_t 
 XF_DLL int xf_table_import(xf_table* t, const uint64_t* keys, uint64_t n, const float* w, const float* nw,
                            const float* zw, const float* v, const float* nv, const float* zv) {
   if (!t || (!keys && n)) return XF_ERR_ARG;
+  XF_TRY(xf_check_host_keys(keys, n, "xf_table_import"));
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   if (n == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
@@ -588,6 +604,7 @@ XF_DLL int xf_table_import(xf_table* t, const uint64_t* keys, uint64_t n, const 
 XF_DLL int xf_table_export(xf_table* t, const uint64_t* keys, uint64_t n, float* w, float* nw, float* zw,
                            float* v, float* nv, float* zv, uint8_t* present) {
   if (!t || (!keys && n)) return XF_ERR_ARG;
+  XF_TRY(xf_check_host_keys(keys, n, "xf_table_export"));
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   if (n == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));
@@ -1080,6 +1097,7 @@ XF_DLL int xf_trainer_step_host(xf_trainer* tr, const uint32_t* row_ptr, const u
                                 const uint8_t* labels, uint32_t rows, uint32_t nnz, float* mean_abs_loss) {
   if (!tr || !row_ptr || (!keys && nnz) || !labels) return XF_ERR_ARG;
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host"));
   if (rows == 0 && !tr->mg) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);
@@ -1108,6 +1126,7 @@ XF_DLL int xf_trainer_predict_host(xf_trainer* tr, const uint32_t* row_ptr, cons
                                    uint32_t nnz, float* pctr_out) {
   if (!tr || !row_ptr || (!keys && nnz) || !pctr_out) return XF_ERR_ARG;
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host"));
   if (rows == 0 && !tr->mg) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);
@@ -1153,6 +1172,7 @@ XF_DLL int xf_trainer_step_host_values(xf_trainer* tr, const uint32_t* row_ptr, 
   if (!tr || !row_ptr || (!keys && nnz) || !labels) return XF_ERR_ARG;
   if (tr->cfg.model != XF_MODEL_FM_CANONICAL) { xf_set_error("feature values need XF_MODEL_FM_CANONICAL"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_values"));
   if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);
@@ -1181,6 +1201,7 @@ XF_DLL int xf_trainer_predict_host_values(xf_trainer* tr, const uint32_t* row_pt
   if (!tr || !row_ptr || (!keys && nnz) || !pctr_out) return XF_ERR_ARG;
   if (tr->cfg.model != XF_MODEL_FM_CANONICAL) { xf_set_error("feature values need XF_MODEL_FM_CANONICAL"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host_values"));
   if (rows == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);
@@ -1217,6 +1238,7 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
   if (!tr || !row_ptr || (!keys && nnz) || (!fields && nnz) || !labels) return XF_ERR_ARG;
   if (tr->cfg.model != XF_MODEL_MVM) { xf_set_error("field ids need XF_MODEL_MVM"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_fields"));
   if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);
@@ -1248,6 +1270,7 @@ XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_pt
   if (!tr || !row_ptr || (!keys && nnz) || (!fields && nnz) || !pctr_out) return XF_ERR_ARG;
   if (tr->cfg.model != XF_MODEL_MVM) { xf_set_error("field ids need XF_MODEL_MVM"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host_fields"));
   if (rows == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int slot = (int)(tr->step_index & 1);

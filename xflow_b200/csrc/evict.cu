@@ -222,6 +222,7 @@ XF_DLL int xf_table_evict(xf_table* t, uint64_t* evicted) {
 XF_DLL int xf_table_last_touch(xf_table* t, const uint64_t* keys, uint64_t n, uint64_t* out) {
   if (!t || ((!keys || !out) && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
   if (!t->d_stamp) { xf_set_error("xf_table_last_touch needs eviction tracking (xf_table_set_eviction)"); return XF_ERR_STATE; }
+  XF_TRY(xf_check_host_keys(keys, n, "xf_table_last_touch"));
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   if (n == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(t->cfg.device));

@@ -12,6 +12,8 @@
 #include "table.cuh"
 
 void xf_set_error(const char* fmt, ...);
+// XF_ERR_ARG, naming the key, if any of the n host keys is the reserved empty-slot marker 2^64 - 1 (capi.cu)
+int xf_check_host_keys(const uint64_t* keys, uint64_t n, const char* fn);
 
 #define XF_CUDA_TRY(expr)                                                              \
   do {                                                                                 \
