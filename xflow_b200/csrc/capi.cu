@@ -990,45 +990,36 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     XF_TRY(xf_admit_view(tr, mode, adm_v));
     adm = &adm_v;
   }
+  float* loss_out = (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr;
+  float* pctr_out = mode == 1 ? tr->pctr.as<float>() : nullptr;
+  uint32_t extra = 0;  // eager: touched[] positions past the tokens (the FM hot-key cache's flushes)
   if (t->view.lazy) {
     // one kernel: the optimizer step of earlier batches is folded in as rows are touched
     if (mode == 0) XF_TRY(t->next_seq());
     xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, nnz, mode, t->seq, t->d_rows_by_seq,
-                           (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                           mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, tr->d_unique_total, adm, sv, st);
-    ++tr->launches;
-    if (prof) {
-      XF_CUDA_TRY(cudaEventRecord(pe[1], st));
-      XF_CUDA_TRY(cudaEventRecord(pe[2], st));
-      XF_CUDA_TRY(cudaEventRecord(pe[3], st));
-    }
-    if (mode == 0) xf_admit_after_step(tr, adm, nnz);
-    XF_CUDA_TRY(cudaGetLastError());
-    return XF_OK;
+                           loss_out, pctr_out, d_abs, tr->d_unique_total, adm, sv, st);
+  } else {
+    const bool mvm = tr->cfg.model == XF_MODEL_MVM;
+    const bool canon = tr->cfg.model == XF_MODEL_FM_CANONICAL || mvm;
+    if (mvm && !d_fields && nnz) { xf_set_error("XF_MODEL_MVM steps need the tokens' field ids (xf_trainer_step_host_fields)"); return XF_ERR_ARG; }
+    extra = canon ? 0u : xf_step_touched_extra(t->view.K, (int)rows);
+    XF_TRY(tr->touched.ensure(((size_t)nnz + extra) * 4));
+    if (mvm)
+      xf_launch_step_mvm(t->view, d_row_ptr, d_keys, d_fields, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
+                         loss_out, pctr_out, d_abs, st);
+    else if (canon)
+      xf_launch_step_fmc(t->view, d_row_ptr, d_keys, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
+                         loss_out, pctr_out, d_abs, st);
+    else
+      xf_launch_step(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(), nnz, loss_out,
+                     pctr_out, d_abs, adm, sv, st);
   }
-  const bool mvm = tr->cfg.model == XF_MODEL_MVM;
-  const bool canon = tr->cfg.model == XF_MODEL_FM_CANONICAL || mvm;
-  if (mvm && !d_fields && nnz) { xf_set_error("XF_MODEL_MVM steps need the tokens' field ids (xf_trainer_step_host_fields)"); return XF_ERR_ARG; }
-  const uint32_t extra = canon ? 0u : xf_step_touched_extra(t->view.K, (int)rows);
-  XF_TRY(tr->touched.ensure(((size_t)nnz + extra) * 4));
-  if (mvm)
-    xf_launch_step_mvm(t->view, d_row_ptr, d_keys, d_fields, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
-                       (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                       mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, st);
-  else if (canon)
-    xf_launch_step_fmc(t->view, d_row_ptr, d_keys, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
-                       (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                       mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, st);
-  else
-    xf_launch_step(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(), nnz,
-                   (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr,
-                   mode == 1 ? tr->pctr.as<float>() : nullptr, d_abs, adm, sv, st);
   ++tr->launches;
   if (prof) {
     XF_CUDA_TRY(cudaEventRecord(pe[1], st));
     XF_CUDA_TRY(cudaEventRecord(pe[2], st));
   }
-  if (mode == 0) {
+  if (!t->view.lazy && mode == 0) {
     // Push + server-side optimizer: one FTRL/SGD step per touched key with g / rows
     xf_launch_update_touched(t->view, tr->touched.as<uint32_t>(), (uint64_t)nnz + extra, (double)rows,
                              tr->d_unique_total, sv, st);
@@ -1040,15 +1031,20 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   return XF_OK;
 }
 
+// the counters of xf_trainer_stats after a training step
+static void xf_count_step(xf_trainer* tr, uint32_t rows, uint32_t nnz) {
+  ++tr->n_steps;
+  tr->n_rows += rows;
+  tr->n_nnz += nnz;
+  tr->last_rows = rows;
+}
+
 XF_DLL int xf_trainer_step_device(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                   const uint8_t* d_labels, uint32_t rows, uint32_t nnz) {
   if (!tr || !d_row_ptr || !d_keys || !d_labels) return XF_ERR_ARG;
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_step_device_impl(tr, d_row_ptr, d_keys, d_labels, rows, nnz, 0, nullptr));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
+  xf_count_step(tr, rows, nnz);
   return XF_OK;
 }
 
@@ -1063,12 +1059,11 @@ static bool xf_is_pinned(const void* p) {
 
 // stage one host array into buffer set `b` (pinned source: DMA directly; pageable: copy through the
 // set's pinned staging) and enqueue the H2D on the copy stream
-static int xf_stage(xf_trainer* tr, XfDevBuf& dev, XfPinBuf& pin, const void* src, size_t bytes, bool staging_free) {
+static int xf_stage(xf_trainer* tr, XfDevBuf& dev, XfPinBuf& pin, const void* src, size_t bytes) {
   if (bytes == 0) return XF_OK;
   XF_TRY(dev.ensure(bytes));
   const void* from = src;
   if (!xf_is_pinned(src)) {
-    (void)staging_free;
     XF_TRY(pin.ensure(bytes));
     memcpy(pin.p, src, bytes);
     from = pin.p;
@@ -1077,20 +1072,87 @@ static int xf_stage(xf_trainer* tr, XfDevBuf& dev, XfPinBuf& pin, const void* sr
   return XF_OK;
 }
 
+// The batch's CSR into buffer set `b` on the copy stream, with the table stream waiting for it.  keys (8 B per
+// token) are staged like the other arrays; ids (4 B per token, page-locked, xf_trainer_step_host_ids_async) are
+// hashed to keys on the device.  labels == NULL (predict): none are copied.
 static int xf_upload_batch(xf_trainer* tr, XfBatchBuf& b, const uint32_t* row_ptr, const uint64_t* keys,
-                           const uint8_t* labels, uint32_t rows, uint32_t nnz) {
+                           const uint32_t* ids, const uint8_t* labels, uint32_t rows, uint32_t nnz) {
   // the device buffers of this set may still be read by the step issued two calls ago
   XF_CUDA_TRY(cudaStreamWaitEvent(tr->copy_stream, b.consumed, 0));
-  // its pinned staging may still be the source of that step's H2D
-  XF_CUDA_TRY(cudaEventSynchronize(b.staged));
-  XF_TRY(xf_stage(tr, b.row_ptr, b.h_row_ptr, row_ptr, ((size_t)rows + 1) * 4, true));
-  XF_TRY(xf_stage(tr, b.keys, b.h_keys, keys, (size_t)nnz * 8, true));
-  if (labels) XF_TRY(xf_stage(tr, b.labels, b.h_labels, labels, (size_t)rows, true));
-  XF_CUDA_TRY(cudaEventRecord(b.staged, tr->copy_stream));
+  if (ids) {
+    XF_TRY(b.row_ptr.ensure(((size_t)rows + 1) * 4));
+    XF_TRY(b.ids.ensure((size_t)nnz * 4));
+    XF_TRY(b.keys.ensure((size_t)nnz * 8));
+    XF_TRY(b.labels.ensure(rows));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.row_ptr.p, row_ptr, ((size_t)rows + 1) * 4, cudaMemcpyHostToDevice, tr->copy_stream));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.ids.p, ids, (size_t)nnz * 4, cudaMemcpyHostToDevice, tr->copy_stream));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.labels.p, labels, rows, cudaMemcpyHostToDevice, tr->copy_stream));
+    XF_TRY(xf_launch_hash_ids(b.ids.as<uint32_t>(), nnz, b.keys.as<uint64_t>(), tr->copy_stream));
+    ++tr->launches;
+  } else {
+    // its pinned staging may still be the source of that step's H2D
+    XF_CUDA_TRY(cudaEventSynchronize(b.staged));
+    XF_TRY(xf_stage(tr, b.row_ptr, b.h_row_ptr, row_ptr, ((size_t)rows + 1) * 4));
+    XF_TRY(xf_stage(tr, b.keys, b.h_keys, keys, (size_t)nnz * 8));
+    if (labels) XF_TRY(xf_stage(tr, b.labels, b.h_labels, labels, (size_t)rows));
+    XF_CUDA_TRY(cudaEventRecord(b.staged, tr->copy_stream));
+  }
   XF_CUDA_TRY(cudaEventRecord(b.copied, tr->copy_stream));
   XF_CUDA_TRY(cudaStreamWaitEvent(tr->table->stream, b.copied, 0));
   tr->input_ready = b.copied;  // the sharded path starts its dedup on another stream
   return XF_OK;
+}
+
+// A batch in host memory through the next buffer set into a step of `mode` (0 = train, 1 = predict).  vals /
+// fields (optional) go by a plain stream-ordered copy on the table stream: they are a small part of a batch.  A
+// training step first clears the set's abs-loss word, and is counted; *slot (may be NULL) = the set used.
+static int xf_step_host_impl(xf_trainer* tr, int mode, const uint32_t* row_ptr, const uint64_t* keys,
+                             const uint32_t* ids, const uint8_t* labels, uint32_t rows, uint32_t nnz, int* slot,
+                             const float* vals = nullptr, const uint8_t* fields = nullptr) {
+  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
+  const int s = (int)(tr->step_index & 1);
+  XfBatchBuf& b = tr->buf[s];
+  ++tr->step_index;
+  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, ids, labels, rows, nnz));
+  cudaStream_t st = tr->table->stream;
+  if (!labels) XF_TRY(b.labels.ensure((size_t)rows + 1));  // unused by mode 1 but must be a valid pointer
+  const float* d_vals = nullptr;
+  if (vals && nnz) {
+    XF_TRY(b.vals.ensure((size_t)nnz * 4));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.vals.p, vals, (size_t)nnz * 4, cudaMemcpyHostToDevice, st));
+    d_vals = b.vals.as<float>();
+  }
+  const uint8_t* d_fields = nullptr;
+  if (fields && nnz) {
+    XF_TRY(b.fields.ensure((size_t)nnz));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.fields.p, fields, (size_t)nnz, cudaMemcpyHostToDevice, st));
+    d_fields = b.fields.as<uint8_t>();
+  }
+  float* d_abs = mode == 0 ? tr->d_abs_loss + s : nullptr;
+  if (d_abs) XF_CUDA_TRY(cudaMemsetAsync(d_abs, 0, sizeof(float), st));
+  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz,
+                             mode, d_abs, d_vals, d_fields));
+  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
+  if (mode == 0) xf_count_step(tr, rows, nnz);
+  if (slot) *slot = s;
+  return XF_OK;
+}
+
+// the mean |pctr - label| of the training step just run in buffer set `slot`; waits for the table stream
+static int xf_read_abs_loss(xf_trainer* tr, int slot, uint32_t rows, float* mean_abs_loss) {
+  cudaStream_t st = tr->table->stream;
+  XF_CUDA_TRY(cudaMemcpyAsync(tr->h_abs_loss + slot, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  if (mean_abs_loss) *mean_abs_loss = rows ? tr->h_abs_loss[slot] / (float)rows : 0.f;
+  return XF_OK;
+}
+
+// the predictions of the step just run, to the host; waits for the table stream and reports its sticky error
+static int xf_read_pctr(xf_trainer* tr, float* pctr_out, uint32_t rows) {
+  cudaStream_t st = tr->table->stream;
+  XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, tr->pctr.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  return tr->table->check_error();
 }
 
 XF_DLL int xf_trainer_step_host(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
@@ -1099,26 +1161,9 @@ XF_DLL int xf_trainer_step_host(xf_trainer* tr, const uint32_t* row_ptr, const u
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host"));
   if (rows == 0 && !tr->mg) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, labels, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss + slot, 0, sizeof(float), st));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows,
-                             nnz, 0, tr->d_abs_loss + slot));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  if (mean_abs_loss) {
-    XF_CUDA_TRY(cudaMemcpyAsync(tr->h_abs_loss + slot, tr->d_abs_loss + slot, sizeof(float),
-                                cudaMemcpyDeviceToHost, st));
-    XF_CUDA_TRY(cudaStreamSynchronize(st));
-    *mean_abs_loss = rows ? tr->h_abs_loss[slot] / (float)rows : 0.f;
-  }
+  int slot;
+  XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, nullptr, labels, rows, nnz, &slot));
+  if (mean_abs_loss) XF_TRY(xf_read_abs_loss(tr, slot, rows, mean_abs_loss));
   return XF_OK;
 }
 
@@ -1128,19 +1173,8 @@ XF_DLL int xf_trainer_predict_host(xf_trainer* tr, const uint32_t* row_ptr, cons
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host"));
   if (rows == 0 && !tr->mg) return XF_OK;
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, nullptr, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  XF_TRY(b.labels.ensure((size_t)rows + 1));  // unused by mode 1 but must be a valid pointer
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows,
-                             nnz, 1, nullptr));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, tr->pctr.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
-  XF_CUDA_TRY(cudaStreamSynchronize(st));
-  return tr->table->check_error();
+  XF_TRY(xf_step_host_impl(tr, 1, row_ptr, keys, nullptr, nullptr, rows, nnz, nullptr));
+  return xf_read_pctr(tr, pctr_out, rows);
 }
 
 // ---- the same entry points with feature values (XF_MODEL_FM_CANONICAL, step_fmc.cu)
@@ -1150,20 +1184,7 @@ XF_DLL int xf_trainer_step_device_values(xf_trainer* tr, const uint32_t* d_row_p
   if (tr->cfg.model != XF_MODEL_FM_CANONICAL) { xf_set_error("feature values need XF_MODEL_FM_CANONICAL"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_step_device_impl(tr, d_row_ptr, d_keys, d_labels, rows, nnz, 0, nullptr, d_vals));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  return XF_OK;
-}
-
-static int xf_upload_vals(xf_trainer* tr, XfBatchBuf& b, const float* vals, uint32_t nnz, const float** d_vals) {
-  *d_vals = nullptr;
-  if (!vals || !nnz) return XF_OK;
-  XF_TRY(b.vals.ensure((size_t)nnz * 4));
-  // pageable or pinned: a plain stream-ordered copy on the table stream (the values are a small part of a batch)
-  XF_CUDA_TRY(cudaMemcpyAsync(b.vals.p, vals, (size_t)nnz * 4, cudaMemcpyHostToDevice, tr->table->stream));
-  *d_vals = b.vals.as<float>();
+  xf_count_step(tr, rows, nnz);
   return XF_OK;
 }
 
@@ -1174,25 +1195,9 @@ XF_DLL int xf_trainer_step_host_values(xf_trainer* tr, const uint32_t* row_ptr, 
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_values"));
   if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, labels, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  const float* d_vals = nullptr;
-  XF_TRY(xf_upload_vals(tr, b, vals, nnz, &d_vals));
-  XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss + slot, 0, sizeof(float), st));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz, 0,
-                             tr->d_abs_loss + slot, d_vals));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  XF_CUDA_TRY(cudaMemcpyAsync(tr->h_abs_loss + slot, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost, st));
-  XF_CUDA_TRY(cudaStreamSynchronize(st));  // also: `vals` may be reused by the caller
-  if (mean_abs_loss) *mean_abs_loss = tr->h_abs_loss[slot] / (float)rows;
+  int slot;
+  XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, nullptr, labels, rows, nnz, &slot, vals));
+  XF_TRY(xf_read_abs_loss(tr, slot, rows, mean_abs_loss));  // also: `vals` may be reused by the caller
   return tr->table->check_error();
 }
 
@@ -1203,32 +1208,14 @@ XF_DLL int xf_trainer_predict_host_values(xf_trainer* tr, const uint32_t* row_pt
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host_values"));
   if (rows == 0) return XF_OK;
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, nullptr, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  XF_TRY(b.labels.ensure((size_t)rows + 1));
-  const float* d_vals = nullptr;
-  XF_TRY(xf_upload_vals(tr, b, vals, nnz, &d_vals));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz, 1,
-                             nullptr, d_vals));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, tr->pctr.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
-  XF_CUDA_TRY(cudaStreamSynchronize(st));
-  return tr->table->check_error();
+  XF_TRY(xf_step_host_impl(tr, 1, row_ptr, keys, nullptr, nullptr, rows, nnz, nullptr, vals));
+  return xf_read_pctr(tr, pctr_out, rows);
 }
 
 // ---- the defined multi-view machine (XF_MODEL_MVM, step_mvm.cu): the batch with the tokens' field ids
-static int xf_upload_fields(xf_trainer* tr, XfBatchBuf& b, const uint8_t* fields, uint32_t nnz, const uint8_t** d_fields) {
-  *d_fields = nullptr;
-  if (!nnz) return XF_OK;
+static int xf_check_fields(const uint8_t* fields, uint32_t nnz) {
   for (uint32_t j = 0; j < nnz; ++j)
     if (fields[j] >= XF_MVM_FIELDS) { xf_set_error("field id %u of token %u: XF_MODEL_MVM takes field ids below %d", (unsigned)fields[j], j, XF_MVM_FIELDS); return XF_ERR_ARG; }
-  XF_TRY(b.fields.ensure((size_t)nnz));
-  XF_CUDA_TRY(cudaMemcpyAsync(b.fields.p, fields, (size_t)nnz, cudaMemcpyHostToDevice, tr->table->stream));
-  *d_fields = b.fields.as<uint8_t>();
   return XF_OK;
 }
 
@@ -1240,27 +1227,10 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_fields"));
   if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, labels, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  const float* d_vals = nullptr;
-  const uint8_t* d_fields = nullptr;
-  XF_TRY(xf_upload_vals(tr, b, vals, nnz, &d_vals));
-  XF_TRY(xf_upload_fields(tr, b, fields, nnz, &d_fields));
-  XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss + slot, 0, sizeof(float), st));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz, 0,
-                             tr->d_abs_loss + slot, d_vals, d_fields));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  XF_CUDA_TRY(cudaMemcpyAsync(tr->h_abs_loss + slot, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost, st));
-  XF_CUDA_TRY(cudaStreamSynchronize(st));  // also: `fields` / `vals` may be reused by the caller
-  if (mean_abs_loss) *mean_abs_loss = tr->h_abs_loss[slot] / (float)rows;
+  XF_TRY(xf_check_fields(fields, nnz));
+  int slot;
+  XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, nullptr, labels, rows, nnz, &slot, vals, fields));
+  XF_TRY(xf_read_abs_loss(tr, slot, rows, mean_abs_loss));  // also: `fields` / `vals` may be reused by the caller
   return tr->table->check_error();
 }
 
@@ -1272,23 +1242,9 @@ XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_pt
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host_fields"));
   if (rows == 0) return XF_OK;
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, nullptr, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  XF_TRY(b.labels.ensure((size_t)rows + 1));
-  const float* d_vals = nullptr;
-  const uint8_t* d_fields = nullptr;
-  XF_TRY(xf_upload_vals(tr, b, vals, nnz, &d_vals));
-  XF_TRY(xf_upload_fields(tr, b, fields, nnz, &d_fields));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz, 1,
-                             nullptr, d_vals, d_fields));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, tr->pctr.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
-  XF_CUDA_TRY(cudaStreamSynchronize(st));
-  return tr->table->check_error();
+  XF_TRY(xf_check_fields(fields, nnz));
+  XF_TRY(xf_step_host_impl(tr, 1, row_ptr, keys, nullptr, nullptr, rows, nnz, nullptr, vals, fields));
+  return xf_read_pctr(tr, pctr_out, rows);
 }
 
 XF_DLL int xf_trainer_init_push(xf_trainer* tr) {
@@ -1348,77 +1304,38 @@ XF_DLL int xf_trainer_wait_uploads(xf_trainer* tr) {
   return XF_OK;
 }
 
+// xf_trainer_step_host_async / _ids_async: page-locked buffers only, and nothing waits for the device; the batch's
+// loss sum goes to pinned_abs_loss_sum (optional) by an asynchronous copy
+static int xf_step_async(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys, const uint32_t* ids,
+                         const uint8_t* labels, uint32_t rows, uint32_t nnz, float* pinned_abs_loss_sum, const char* fn) {
+  XF_TRY(xf_check_batch(tr, rows, nnz));
+  if (rows == 0 && !tr->mg) return XF_OK;
+  if (!xf_is_pinned(row_ptr) || !xf_is_pinned(ids ? (const void*)ids : keys) || !xf_is_pinned(labels) ||
+      (pinned_abs_loss_sum && !xf_is_pinned(pinned_abs_loss_sum))) {
+    xf_set_error("%s needs page-locked host buffers", fn);
+    return XF_ERR_ARG;
+  }
+  int slot;
+  XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, ids, labels, rows, nnz, &slot));
+  if (pinned_abs_loss_sum)
+    XF_CUDA_TRY(cudaMemcpyAsync(pinned_abs_loss_sum, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost,
+                                tr->table->stream));
+  return XF_OK;
+}
+
 XF_DLL int xf_trainer_step_host_async(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
                                       const uint8_t* labels, uint32_t rows, uint32_t nnz,
                                       float* pinned_abs_loss_sum) {
   if (!tr || !row_ptr || (!keys && nnz) || !labels) return XF_ERR_ARG;
-  XF_TRY(xf_check_batch(tr, rows, nnz));
-  if (rows == 0 && !tr->mg) return XF_OK;
-  if (!xf_is_pinned(row_ptr) || !xf_is_pinned(keys) || !xf_is_pinned(labels) ||
-      (pinned_abs_loss_sum && !xf_is_pinned(pinned_abs_loss_sum))) {
-    xf_set_error("xf_trainer_step_host_async needs page-locked host buffers");
-    return XF_ERR_ARG;
-  }
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  XF_TRY(xf_upload_batch(tr, b, row_ptr, keys, labels, rows, nnz));
-  cudaStream_t st = tr->table->stream;
-  XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss + slot, 0, sizeof(float), st));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows,
-                             nnz, 0, tr->d_abs_loss + slot));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  if (pinned_abs_loss_sum)
-    XF_CUDA_TRY(cudaMemcpyAsync(pinned_abs_loss_sum, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost, st));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  return XF_OK;
+  return xf_step_async(tr, row_ptr, keys, nullptr, labels, rows, nnz, pinned_abs_loss_sum, "xf_trainer_step_host_async");
 }
 
 XF_DLL int xf_trainer_step_host_ids_async(xf_trainer* tr, const uint32_t* row_ptr, const uint32_t* ids,
                                           const uint8_t* labels, uint32_t rows, uint32_t nnz,
                                           float* pinned_abs_loss_sum) {
   if (!tr || !row_ptr || (!ids && nnz) || !labels) return XF_ERR_ARG;
-  XF_TRY(xf_check_batch(tr, rows, nnz));
-  if (rows == 0 && !tr->mg) return XF_OK;
-  if (!xf_is_pinned(row_ptr) || !xf_is_pinned(ids) || !xf_is_pinned(labels) ||
-      (pinned_abs_loss_sum && !xf_is_pinned(pinned_abs_loss_sum))) {
-    xf_set_error("xf_trainer_step_host_ids_async needs page-locked host buffers");
-    return XF_ERR_ARG;
-  }
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
-  const int slot = (int)(tr->step_index & 1);
-  XfBatchBuf& b = tr->buf[slot];
-  ++tr->step_index;
-  // upload row_ptr, ids (4 B/token instead of 8 B keys) and labels; hash on the device
-  XF_CUDA_TRY(cudaStreamWaitEvent(tr->copy_stream, b.consumed, 0));
-  XF_TRY(b.row_ptr.ensure(((size_t)rows + 1) * 4));
-  XF_TRY(b.ids.ensure((size_t)nnz * 4));
-  XF_TRY(b.keys.ensure((size_t)nnz * 8));
-  XF_TRY(b.labels.ensure(rows));
-  XF_CUDA_TRY(cudaMemcpyAsync(b.row_ptr.p, row_ptr, ((size_t)rows + 1) * 4, cudaMemcpyHostToDevice, tr->copy_stream));
-  XF_CUDA_TRY(cudaMemcpyAsync(b.ids.p, ids, (size_t)nnz * 4, cudaMemcpyHostToDevice, tr->copy_stream));
-  XF_CUDA_TRY(cudaMemcpyAsync(b.labels.p, labels, rows, cudaMemcpyHostToDevice, tr->copy_stream));
-  XF_TRY(xf_launch_hash_ids(b.ids.as<uint32_t>(), nnz, b.keys.as<uint64_t>(), tr->copy_stream));
-  ++tr->launches;
-  XF_CUDA_TRY(cudaEventRecord(b.copied, tr->copy_stream));
-  cudaStream_t st = tr->table->stream;
-  XF_CUDA_TRY(cudaStreamWaitEvent(st, b.copied, 0));
-  tr->input_ready = b.copied;
-  XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss + slot, 0, sizeof(float), st));
-  XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows,
-                             nnz, 0, tr->d_abs_loss + slot));
-  XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
-  if (pinned_abs_loss_sum)
-    XF_CUDA_TRY(cudaMemcpyAsync(pinned_abs_loss_sum, tr->d_abs_loss + slot, sizeof(float), cudaMemcpyDeviceToHost, st));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->n_nnz += nnz;
-  tr->last_rows = rows;
-  return XF_OK;
+  return xf_step_async(tr, row_ptr, nullptr, ids, labels, rows, nnz, pinned_abs_loss_sum,
+                       "xf_trainer_step_host_ids_async");
 }
 
 // Two-phase ingest.  _begin copies the block to the device and parses it on the trainer's ingest streams
@@ -1524,7 +1441,7 @@ XF_DLL int xf_trainer_ingest_text(xf_trainer* tr, const char* text, uint64_t len
   return xf_trainer_ingest_end(tr, rows, nnz);
 }
 
-static int xf_ingested_range(xf_trainer* tr, uint32_t row_start, uint32_t row_end) {
+int xf_ingested_range(xf_trainer* tr, uint32_t row_start, uint32_t row_end) {
   if (!tr) return XF_ERR_ARG;
   if (row_start > row_end || row_end > tr->ing_rows) { xf_set_error("row range outside the ingested block"); return XF_ERR_ARG; }
   if (tr->mg && (row_start != 0 || row_end != tr->ing_rows)) {
@@ -1547,9 +1464,7 @@ XF_DLL int xf_trainer_step_ingested(xf_trainer* tr, uint32_t row_start, uint32_t
   XF_TRY(xf_step_device_impl(tr, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(),
                              g.labels.as<uint8_t>() + row_start, rows, tr->ing_nnz, 0, nullptr));
   XF_CUDA_TRY(cudaEventRecord(g.consumed, tr->table->stream));
-  ++tr->n_steps;
-  tr->n_rows += rows;
-  tr->last_rows = rows;
+  xf_count_step(tr, rows, 0);  // a slice's tokens are not counted: its step is given the whole block's
   return XF_OK;
 }
 
@@ -1569,36 +1484,27 @@ XF_DLL int xf_trainer_ingested_export(xf_trainer* tr, uint32_t* row_ptr_out, uin
 
 // forward pass over a row range of the current ingested block; predictions stay in tr->pctr (metric.cu)
 int xf_trainer_forward_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end) {
+  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   xf_trainer::IngestSet& g = tr->ing[tr->ing_cur];
   return xf_step_device_impl(tr, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(),
                              g.labels.as<uint8_t>() + row_start, row_end - row_start, tr->ing_nnz, 1, nullptr);
 }
 
-// Forward pass over a row range of the current block.  Asynchronous when pinned result buffers are given
-// (xf_trainer_predict_ingested_async): the caller reads them after xf_trainer_sync.
-static int xf_predict_ingested_impl(xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
-                                    uint8_t* labels_out, bool sync) {
+XF_DLL int xf_trainer_predict_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
+                                       uint8_t* labels_out) {
   XF_TRY(xf_ingested_range(tr, row_start, row_end));
   if (row_end == row_start && !tr->mg) return XF_OK;
   if (!pctr_out) return XF_ERR_ARG;
-  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
+  XF_TRY(xf_trainer_forward_ingested(tr, row_start, row_end));
   xf_trainer::IngestSet& g = tr->ing[tr->ing_cur];
   const uint32_t rows = row_end - row_start;
   cudaStream_t st = tr->table->stream;
-  XF_TRY(xf_step_device_impl(tr, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(),
-                             g.labels.as<uint8_t>() + row_start, rows, tr->ing_nnz, 1, nullptr));
   if (rows) XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, tr->pctr.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
   if (labels_out && rows)
     XF_CUDA_TRY(cudaMemcpyAsync(labels_out, g.labels.as<uint8_t>() + row_start, rows, cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaEventRecord(g.consumed, st));
-  if (!sync) return XF_OK;
   XF_CUDA_TRY(cudaStreamSynchronize(st));
   return tr->table->check_error();
-}
-
-XF_DLL int xf_trainer_predict_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
-                                       uint8_t* labels_out) {
-  return xf_predict_ingested_impl(tr, row_start, row_end, pctr_out, labels_out, true);
 }
 
 XF_DLL int xf_trainer_set_profile(xf_trainer* tr, int on) {

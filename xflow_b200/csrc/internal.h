@@ -156,7 +156,9 @@ int xf_launch_parse(const char* d_text, uint64_t len, XfDevBuf& scratch, uint32_
                     cudaStream_t st);
 int xf_launch_hash_ids(const uint32_t* d_ids, uint32_t n, uint64_t* d_keys, cudaStream_t st);
 
-int xf_trainer_forward_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end);  // capi.cu
+// capi.cu: XF_ERR_ARG unless [row_start, row_end) lies in the current ingested block (sharded: is all of it)
+int xf_ingested_range(xf_trainer* tr, uint32_t row_start, uint32_t row_end);
+int xf_trainer_forward_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end);
 
 // multi-GPU pieces implemented in comm.cu
 int xf_mg_create(xf_trainer* tr);
