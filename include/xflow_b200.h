@@ -288,6 +288,49 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
 XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
                                           const uint8_t* fields, const float* vals, uint32_t rows, uint32_t nnz,
                                           float* pctr_out);
+/* Importance-weighted training (McMahan et al., "Ad Click Prediction: a View from the Trenches", section 6.1):
+ * per-row weights and negative subsampling for XF_MODEL_LR / XF_MODEL_FM.  Each row r of a training step has an
+ * effective weight e_r = c_r * s_r (float product, rounded to nearest):
+ *   c_r  the caller's weight (xf_trainer_step_host_weighted / _device_weighted); 1 for every other entry point;
+ *   s_r  the trainer's negative-sampling policy (xf_trainer_set_negative_sampling): 1 for a positive row (label != 0)
+ *        or without a policy; for a negative row inv = (float)(1.0 / rate) if the row is kept and 0 if it is dropped.
+ *        A negative row is kept iff the top 24 bits of splitmix64(seed ^ F_r) < floor(rate * 2^24), where
+ *        F_r = sum over the row's tokens of splitmix64(key) mod 2^64 (0 for a row without tokens).  The decision is a
+ *        function of the row alone, computed on the device: the same whatever the entry point, block cut or slice.
+ *        Since F_r ignores token order, rows with equal key multisets decide alike.
+ * The step then uses the weighted residual loss_r = e_r * (pctr_r - label_r) wherever it used pctr_r - label_r:
+ *   - the gradients are sum over the tokens of key i of loss_r (FM: and loss_r * (S_r - v_ik)), divided by the batch's
+ *     row count B as before.  B counts every row, skipped ones included, so that under subsampling the gradient stays
+ *     an unbiased estimate of the full batch's.  Weights of 1 give the unweighted step bit for bit.
+ *   - a row with e_r = 0 is skipped: its tokens do not probe, insert or ask the admission policy (the Bloom filter
+ *     does not count them), nothing is stamped, deposited or counted in unique_keys for it, and keep_loss reports 0
+ *     for it.  The batch is still a training batch (admission's and eviction's batch number moves on).
+ *   - lazy LR tables sum each batch's residuals per key in a fixed-point unit 2^-s; weighted, s = the same function of
+ *     W = sum over the trained rows of ceil(e_r) * tokens_r (instead of the token count), so every key's sum stays in
+ *     its field.  Sums stay exact while W < 2^47.  xf_trainer_step_host_weighted refuses a batch whose W could
+ *     reach 2^47 (XF_ERR_ARG, bounded with the policy's largest factor); device weights that do are outside the
+ *     step's range.
+ *   - *mean_abs_loss = sum_r e_r * |pctr_r - label_r| / B; xf_trainer_get_loss keeps reporting the UNWEIGHTED
+ *     pctr_r - label_r of the trained rows.
+ * Predict is unweighted.  A step with caller weights or a policy runs one more kernel (weight.cu) before the step
+ * kernel: xf_trainer_launches counts +1 per such step.  Refused (XF_ERR_ARG): canonical FM / MVM trainers, trainers
+ * that run the sharded step (a comm of more than one rank, or XFLOW_MG_FORCE=1), and host weights that are NaN,
+ * negative or infinite.  Weights in device memory are the caller's contract, as device keys are. */
+/* one step with row weights weights[rows] (host memory); otherwise xf_trainer_step_host */
+XF_DLL int xf_trainer_step_host_weighted(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
+                                         const uint8_t* labels, const float* weights, uint32_t rows, uint32_t nnz,
+                                         float* mean_abs_loss);
+/* the same on a batch and weights in device memory; asynchronous on the table's stream, like xf_trainer_step_device */
+XF_DLL int xf_trainer_step_device_weighted(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys,
+                                           const uint8_t* d_labels, const float* d_weights, uint32_t rows,
+                                           uint32_t nnz);
+/* Negative sampling for every later training step of the trainer, on every entry point (host, device, _async,
+ * _ids_async, _ingested and the _weighted pair): keep each negative row with probability `rate` (decided as above,
+ * with this policy's own seed) and weight it by 1 / rate.  rate = 1 turns the policy off; a rate outside
+ * [2^-24, 1] (NaN included) is refused. */
+XF_DLL int xf_trainer_set_negative_sampling(xf_trainer* tr, float rate, uint64_t seed);
+/* rows trained with e_r = 0 since the trainer was created (device counter; waits for the table's stream) */
+XF_DLL int xf_trainer_skipped_rows(xf_trainer* tr, uint64_t* skipped);
 /* the one-off "init push" of key 0 with zero gradient (lr_worker.cc:180-182, fm_worker.cc:248-252) */
 XF_DLL int xf_trainer_init_push(xf_trainer* tr);
 /* residuals (pctr - label) of the last step; needs keep_loss = 1 */

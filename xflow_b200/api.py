@@ -87,6 +87,10 @@ SIGNATURES = {
     "xf_trainer_predict_host_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "xf_trainer_step_host_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "xf_trainer_predict_host_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
+    "xf_trainer_step_host_weighted": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
+    "xf_trainer_step_device_weighted": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32]),
+    "xf_trainer_set_negative_sampling": (_i, [_vp, _f, _u64]),
+    "xf_trainer_skipped_rows": (_i, [_vp, _vp]),
     "xf_trainer_init_push": (_i, [_vp]),
     "xf_trainer_get_loss": (_i, [_vp, _vp, _u32]),
     "xf_trainer_stats": (_i, [_vp, _vp, _vp, _vp, _vp]),
@@ -435,6 +439,33 @@ class Trainer:
         _check(lib().xf_trainer_step_host(self.h, _p(row_ptr), _p(keys), _p(labels), labels.size, keys.size,
                                           C.byref(loss) if want_loss else None))
         return loss.value if want_loss else None
+
+    def step_host_weighted(self, row_ptr, keys, labels, weights, want_loss=True):
+        """One step on host CSR arrays with a weight per row (see xf_trainer_step_host_weighted)."""
+        row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
+        keys = np.ascontiguousarray(keys, np.uint64)
+        labels = np.ascontiguousarray(labels, np.uint8)
+        weights = np.ascontiguousarray(weights, np.float32)
+        if weights.size != labels.size:
+            raise ValueError("one weight per row: %d weights for %d rows" % (weights.size, labels.size))
+        loss = C.c_float()
+        _check(lib().xf_trainer_step_host_weighted(self.h, _p(row_ptr), _p(keys), _p(labels), _p(weights), labels.size,
+                                                   keys.size, C.byref(loss) if want_loss else None))
+        return loss.value if want_loss else None
+
+    def step_device_weighted(self, d_row_ptr, d_keys, d_labels, d_weights, rows, nnz):
+        _check(lib().xf_trainer_step_device_weighted(self.h, _p(d_row_ptr), _p(d_keys), _p(d_labels), _p(d_weights),
+                                                     rows, nnz))
+
+    def set_negative_sampling(self, rate, seed=0):
+        """Keep each negative row of every later training step with probability `rate`, weighted 1 / rate (1: off)."""
+        _check(lib().xf_trainer_set_negative_sampling(self.h, float(rate), int(seed)))
+
+    def skipped_rows(self):
+        """Rows trained with effective weight 0 since the trainer was created."""
+        n = C.c_uint64()
+        _check(lib().xf_trainer_skipped_rows(self.h, C.byref(n)))
+        return n.value
 
     def step_host_values(self, row_ptr, keys, vals, labels):
         """One step of the canonical FM (XF_MODEL_FM_CANONICAL) on host CSR arrays with feature values."""

@@ -1,6 +1,7 @@
 // C ABI layers 2 (parameter table) and 3 (fused worker step) of include/xflow_b200.h.
 // Host orchestration only — every byte of table state lives in HBM and is touched only by the
 // kernels in kernels.cu.  There is no CPU fallback anywhere in this file.
+#include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -31,6 +32,16 @@ int xf_check_host_keys(const uint64_t* keys, uint64_t n, const char* fn) {
     if (keys[i] == XF_EMPTY_KEY) {
       xf_set_error("%s: key %llu (2^64 - 1) at position %llu is reserved: it marks an empty table slot", fn,
                    (unsigned long long)keys[i], (unsigned long long)i);
+      return XF_ERR_ARG;
+    }
+  return XF_OK;
+}
+// A row weight scales the row's residual (xf_trainer_step_host_weighted): it must be a finite number >= 0.
+int xf_check_host_weights(const float* weights, uint64_t n, const char* fn) {
+  for (uint64_t i = 0; i < n; ++i)
+    if (!(weights[i] >= 0.f) || weights[i] == INFINITY) {
+      xf_set_error("%s: weight %g of row %llu: row weights must be finite and >= 0", fn, (double)weights[i],
+                   (unsigned long long)i);
       return XF_ERR_ARG;
     }
   return XF_OK;
@@ -830,6 +841,8 @@ XF_DLL int xf_trainer_create(xf_trainer** out, xf_table* table, xf_comm* comm, c
   XF_TRY(tr->pctr.ensure((size_t)cfg->max_rows * 4));
   XF_CUDA_TRY(cudaMalloc(&tr->d_unique_total, sizeof(unsigned long long)));
   XF_CUDA_TRY(cudaMalloc(&tr->d_abs_loss, 2 * sizeof(float)));
+  XF_CUDA_TRY(cudaMalloc(&tr->d_wstat, 2 * sizeof(unsigned long long)));
+  XF_CUDA_TRY(cudaMemsetAsync(tr->d_wstat, 0, 2 * sizeof(unsigned long long), table->stream));
   XF_CUDA_TRY(cudaHostAlloc(&tr->h_abs_loss, 2 * sizeof(float), cudaHostAllocDefault));
   XF_CUDA_TRY(cudaMemsetAsync(tr->d_unique_total, 0, sizeof(unsigned long long), table->stream));
   XF_CUDA_TRY(cudaMemsetAsync(tr->d_abs_loss, 0, 2 * sizeof(float), table->stream));
@@ -871,10 +884,11 @@ XF_DLL int xf_trainer_destroy(xf_trainer* tr) {
   for (int i = 0; i < 2; ++i) {
     XfBatchBuf& b = tr->buf[i];
     b.row_ptr.release(); b.keys.release(); b.labels.release(); b.ids.release(); b.vals.release(); b.fields.release();
+    b.weights.release();
     b.h_row_ptr.release(); b.h_keys.release(); b.h_labels.release();
     cudaEventDestroy(b.copied); cudaEventDestroy(b.consumed); cudaEventDestroy(b.staged);
   }
-  tr->touched.release(); tr->loss.release(); tr->pctr.release(); tr->rejected.release();
+  tr->touched.release(); tr->loss.release(); tr->pctr.release(); tr->rejected.release(); tr->row_w.release();
   cudaStreamSynchronize(tr->ing_copy_stream);
   cudaStreamSynchronize(tr->ing_stream);
   for (int i = 0; i < 2; ++i) {
@@ -888,7 +902,7 @@ XF_DLL int xf_trainer_destroy(xf_trainer* tr) {
   tr->ing_scratch.release();
   cudaStreamDestroy(tr->ing_stream);
   cudaStreamDestroy(tr->ing_copy_stream);
-  cudaFree(tr->d_unique_total); cudaFree(tr->d_abs_loss);
+  cudaFree(tr->d_unique_total); cudaFree(tr->d_abs_loss); cudaFree(tr->d_wstat);
   cudaFreeHost(tr->h_abs_loss);
   cudaStreamDestroy(tr->copy_stream);
   for (cudaEvent_t e : tr->prof_events) cudaEventDestroy(e);
@@ -946,10 +960,32 @@ static void xf_admit_after_step(xf_trainer* tr, const XfAdmitView* adm, uint32_t
   ++t->admit_batches;
 }
 
-// the step proper, on device-resident CSR; mode 0 = train, 1 = predict
+// Importance weighting of a training step (weight.cu): with caller weights d_w (may be NULL) or a negative-sampling
+// policy, the rows' effective weights and the lazy step's bound W; *wv stays {NULL, NULL} (the kernels without
+// weighting, nothing launched) when the step has neither.
+static int xf_row_weights(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys, const uint8_t* d_labels,
+                          const float* d_w, uint32_t rows, XfWeightView* wv) {
+  const bool sample = tr->neg_rate < 1.f;
+  *wv = XfWeightView{nullptr, nullptr};
+  if (!d_w && !sample) return XF_OK;
+  XF_TRY(tr->row_w.ensure((size_t)tr->cfg.max_rows * sizeof(float)));
+  cudaStream_t st = tr->table->stream;
+  XF_CUDA_TRY(cudaMemsetAsync(tr->d_wstat, 0, sizeof(unsigned long long), st));
+  const uint32_t p24 = (uint32_t)floor((double)tr->neg_rate * 16777216.0);
+  const float inv = (float)(1.0 / (double)tr->neg_rate);
+  xf_launch_row_weights(d_row_ptr, d_keys, d_labels, d_w, (int)rows, sample, p24, inv, tr->neg_seed,
+                        tr->row_w.as<float>(), tr->d_wstat, tr->d_wstat + 1, st);
+  ++tr->launches;
+  *wv = XfWeightView{tr->row_w.as<float>(), tr->d_wstat};
+  return XF_OK;
+}
+
+// the step proper, on device-resident CSR; mode 0 = train, 1 = predict.  d_w: the rows' weights (training only; NULL:
+// all 1), see xf_row_weights.
 static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                const uint8_t* d_labels, uint32_t rows, uint32_t nnz, int mode, float* d_abs,
-                               const float* d_vals = nullptr, const uint8_t* d_fields = nullptr) {
+                               const float* d_vals = nullptr, const uint8_t* d_fields = nullptr,
+                               const float* d_w = nullptr) {
   xf_table* t = tr->table;
   if (tr->mg && t->admit.mode != XF_ADMIT_ALL) {
     xf_set_error("feature admission is single-GPU only: the sharded step cannot serve a table with a policy");
@@ -990,6 +1026,8 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     XF_TRY(xf_admit_view(tr, mode, adm_v));
     adm = &adm_v;
   }
+  XfWeightView wv{nullptr, nullptr};
+  if (mode == 0) XF_TRY(xf_row_weights(tr, d_row_ptr, d_keys, d_labels, d_w, rows, &wv));
   float* loss_out = (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr;
   float* pctr_out = mode == 1 ? tr->pctr.as<float>() : nullptr;
   uint32_t extra = 0;  // eager: touched[] positions past the tokens (the FM hot-key cache's flushes)
@@ -997,7 +1035,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     // one kernel: the optimizer step of earlier batches is folded in as rows are touched
     if (mode == 0) XF_TRY(t->next_seq());
     xf_launch_step_lr_lazy(t->view, d_row_ptr, d_keys, d_labels, (int)rows, nnz, mode, t->seq, t->d_rows_by_seq,
-                           loss_out, pctr_out, d_abs, tr->d_unique_total, adm, sv, st);
+                           loss_out, pctr_out, d_abs, tr->d_unique_total, adm, sv, wv, st);
   } else {
     const bool mvm = tr->cfg.model == XF_MODEL_MVM;
     const bool canon = tr->cfg.model == XF_MODEL_FM_CANONICAL || mvm;
@@ -1012,7 +1050,7 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
                          loss_out, pctr_out, d_abs, st);
     else
       xf_launch_step(t->view, d_row_ptr, d_keys, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(), nnz, loss_out,
-                     pctr_out, d_abs, adm, sv, st);
+                     pctr_out, d_abs, adm, sv, wv, st);
   }
   ++tr->launches;
   if (prof) {
@@ -1108,7 +1146,8 @@ static int xf_upload_batch(xf_trainer* tr, XfBatchBuf& b, const uint32_t* row_pt
 // training step first clears the set's abs-loss word, and is counted; *slot (may be NULL) = the set used.
 static int xf_step_host_impl(xf_trainer* tr, int mode, const uint32_t* row_ptr, const uint64_t* keys,
                              const uint32_t* ids, const uint8_t* labels, uint32_t rows, uint32_t nnz, int* slot,
-                             const float* vals = nullptr, const uint8_t* fields = nullptr) {
+                             const float* vals = nullptr, const uint8_t* fields = nullptr,
+                             const float* weights = nullptr) {
   XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
   const int s = (int)(tr->step_index & 1);
   XfBatchBuf& b = tr->buf[s];
@@ -1128,10 +1167,16 @@ static int xf_step_host_impl(xf_trainer* tr, int mode, const uint32_t* row_ptr, 
     XF_CUDA_TRY(cudaMemcpyAsync(b.fields.p, fields, (size_t)nnz, cudaMemcpyHostToDevice, st));
     d_fields = b.fields.as<uint8_t>();
   }
+  const float* d_w = nullptr;  // row weights (xf_trainer_step_host_weighted): like vals
+  if (weights && rows) {
+    XF_TRY(b.weights.ensure((size_t)rows * 4));
+    XF_CUDA_TRY(cudaMemcpyAsync(b.weights.p, weights, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+    d_w = b.weights.as<float>();
+  }
   float* d_abs = mode == 0 ? tr->d_abs_loss + s : nullptr;
   if (d_abs) XF_CUDA_TRY(cudaMemsetAsync(d_abs, 0, sizeof(float), st));
   XF_TRY(xf_step_device_impl(tr, b.row_ptr.as<uint32_t>(), b.keys.as<uint64_t>(), b.labels.as<uint8_t>(), rows, nnz,
-                             mode, d_abs, d_vals, d_fields));
+                             mode, d_abs, d_vals, d_fields, d_w));
   XF_CUDA_TRY(cudaEventRecord(b.consumed, st));
   if (mode == 0) xf_count_step(tr, rows, nnz);
   if (slot) *slot = s;
@@ -1175,6 +1220,80 @@ XF_DLL int xf_trainer_predict_host(xf_trainer* tr, const uint32_t* row_ptr, cons
   if (rows == 0 && !tr->mg) return XF_OK;
   XF_TRY(xf_step_host_impl(tr, 1, row_ptr, keys, nullptr, nullptr, rows, nnz, nullptr));
   return xf_read_pctr(tr, pctr_out, rows);
+}
+
+// ---- importance weighting (weight.cu): row weights and negative sampling
+// the trainers that can weight their rows: LR / FM on a single GPU
+static int xf_check_weighting(xf_trainer* tr, const char* fn) {
+  if (tr->cfg.model != XF_MODEL_LR && tr->cfg.model != XF_MODEL_FM) {
+    xf_set_error("%s: importance weighting needs XF_MODEL_LR or XF_MODEL_FM (canonical FM and MVM are not weighted)", fn);
+    return XF_ERR_ARG;
+  }
+  if (tr->mg) {
+    xf_set_error("%s: importance weighting is single-GPU only: the sharded step cannot weight its rows", fn);
+    return XF_ERR_ARG;
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_trainer_step_host_weighted(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
+                                         const uint8_t* labels, const float* weights, uint32_t rows, uint32_t nnz,
+                                         float* mean_abs_loss) {
+  if (!tr || !row_ptr || (!keys && nnz) || !labels || (!weights && rows)) return XF_ERR_ARG;
+  XF_TRY(xf_check_weighting(tr, "xf_trainer_step_host_weighted"));
+  XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_weighted"));
+  XF_TRY(xf_check_host_weights(weights, rows, "xf_trainer_step_host_weighted"));
+  if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
+  if (tr->table->view.lazy) {
+    // the lazy step sums each key's weighted residuals in a 48-bit fixed-point field whose unit comes from
+    // W = sum ceil(e_r) * tokens_r (weight.cu): refuse a batch whose W could reach 2^47, where no unit keeps it exact
+    // (bounded with the largest factor the sampling policy can give a row)
+    const double smax = tr->neg_rate < 1.f ? (double)(float)(1.0 / (double)tr->neg_rate) : 1.0;
+    double W = 0.0;
+    for (uint32_t r = 0; r < rows; ++r) W += ceil((double)weights[r] * smax) * (double)(row_ptr[r + 1] - row_ptr[r]);
+    if (W >= 140737488355328.0) {
+      xf_set_error("xf_trainer_step_host_weighted: weights too large for a lazy table: sum over rows of ceil(weight) x "
+                   "tokens is %.6g, the residual sums hold less than 2^47", W);
+      return XF_ERR_ARG;
+    }
+  }
+  int slot;
+  XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, nullptr, labels, rows, nnz, &slot, nullptr, nullptr, weights));
+  if (mean_abs_loss) XF_TRY(xf_read_abs_loss(tr, slot, rows, mean_abs_loss));
+  return XF_OK;
+}
+
+XF_DLL int xf_trainer_step_device_weighted(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys,
+                                           const uint8_t* d_labels, const float* d_weights, uint32_t rows,
+                                           uint32_t nnz) {
+  if (!tr || !d_row_ptr || !d_keys || !d_labels || !d_weights) return XF_ERR_ARG;
+  XF_TRY(xf_check_weighting(tr, "xf_trainer_step_device_weighted"));
+  XF_TRY(xf_check_batch(tr, rows, nnz));
+  XF_TRY(xf_step_device_impl(tr, d_row_ptr, d_keys, d_labels, rows, nnz, 0, nullptr, nullptr, nullptr, d_weights));
+  xf_count_step(tr, rows, nnz);
+  return XF_OK;
+}
+
+XF_DLL int xf_trainer_set_negative_sampling(xf_trainer* tr, float rate, uint64_t seed) {
+  if (!tr) return XF_ERR_ARG;
+  XF_TRY(xf_check_weighting(tr, "xf_trainer_set_negative_sampling"));
+  if (!(rate > 0.f && rate <= 1.f) || (double)rate < 1.0 / 16777216.0) {
+    xf_set_error("xf_trainer_set_negative_sampling: rate %g must lie in [2^-24, 1]", (double)rate);
+    return XF_ERR_ARG;
+  }
+  tr->neg_rate = rate;
+  tr->neg_seed = seed;
+  return XF_OK;
+}
+
+XF_DLL int xf_trainer_skipped_rows(xf_trainer* tr, uint64_t* skipped) {
+  if (!tr || !skipped) return XF_ERR_ARG;
+  unsigned long long n = 0;
+  XF_CUDA_TRY(cudaMemcpyAsync(&n, tr->d_wstat + 1, sizeof(n), cudaMemcpyDeviceToHost, tr->table->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(tr->table->stream));
+  *skipped = n;
+  return XF_OK;
 }
 
 // ---- the same entry points with feature values (XF_MODEL_FM_CANONICAL, step_fmc.cu)

@@ -14,6 +14,8 @@
 void xf_set_error(const char* fmt, ...);
 // XF_ERR_ARG, naming the key, if any of the n host keys is the reserved empty-slot marker 2^64 - 1 (capi.cu)
 int xf_check_host_keys(const uint64_t* keys, uint64_t n, const char* fn);
+// XF_ERR_ARG, naming the row, if any of the n host row weights is NaN, negative or infinite (capi.cu)
+int xf_check_host_weights(const float* weights, uint64_t n, const char* fn);
 
 #define XF_CUDA_TRY(expr)                                                              \
   do {                                                                                 \
@@ -99,7 +101,7 @@ struct xf_table {
 };
 
 struct XfBatchBuf {
-  XfDevBuf row_ptr, keys, labels, ids, vals, fields;
+  XfDevBuf row_ptr, keys, labels, ids, vals, fields, weights;
   XfPinBuf h_row_ptr, h_keys, h_labels;
   cudaEvent_t copied = nullptr;   // H2D of this buffer finished (copy stream)
   cudaEvent_t consumed = nullptr; // kernels reading this buffer finished (compute stream)
@@ -121,6 +123,13 @@ struct xf_trainer {
   uint64_t n_steps = 0, n_rows = 0, n_nnz = 0;
   uint32_t last_rows = 0;
   uint64_t launches = 0;
+  // importance weighting (xf_trainer_set_negative_sampling, the _weighted steps; weight.cu): the negative-sampling
+  // policy (rate 1: none), the rows' effective weights of the current step (max_rows floats, allocated on first use)
+  // and {W of the current step, rows skipped since creation}
+  float neg_rate = 1.f;
+  uint64_t neg_seed = 0;
+  XfDevBuf row_w;
+  unsigned long long* d_wstat = nullptr;
   // device-side ingest (xf_trainer_ingest_begin / _end): two sets of {raw text, the block's CSR}, so that
   // block i+1 is copied and parsed on the ingest stream while block i is being trained on the table stream
   struct IngestSet {

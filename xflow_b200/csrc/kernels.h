@@ -12,7 +12,14 @@ int xf_tps_for(int K);
 void xf_launch_fill(const XfTableView& t, cudaStream_t st);
 void xf_launch_step(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels,
                     int B, int mode, uint32_t* touched, uint32_t nnz, float* loss_out, float* pctr_out,
-                    float* abs_loss_sum, const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st);
+                    float* abs_loss_sum, const XfAdmitView* adm, const XfStampView& sv, const XfWeightView& wv,
+                    cudaStream_t st);
+// importance weighting (weight.cu): e_out[r] = the effective weight of row r of a training batch; *W += the lazy
+// step's fixed-point bound, *skipped += the rows with e = 0.  caller_w may be NULL (all 1); sample: the negative-
+// sampling policy (keep a negative row iff top24(splitmix64(seed ^ F_r)) < p24, with weight inv)
+void xf_launch_row_weights(const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* labels, const float* caller_w,
+                           int B, bool sample, uint32_t p24, float inv, uint64_t seed, float* e_out,
+                           unsigned long long* W, unsigned long long* skipped, cudaStream_t st);
 // feature admission (admit.cu): after a step on the table's stream, count the batch's rejected tokens into the
 // Bloom filter (n = *rej_n of them in rej_keys, at most nnz), add n to *rejected_total and zero *next_rej_n
 void xf_launch_admit_count(const XfAdmitView& a, uint8_t* cells, const uint64_t* rej_keys, const unsigned long long* rej_n,
@@ -59,7 +66,7 @@ int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm);
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,
-                            const XfAdmitView* adm, const XfStampView& sv, cudaStream_t st);
+                            const XfAdmitView* adm, const XfStampView& sv, const XfWeightView& wv, cudaStream_t st);
 
 // lazy tables: fold all pending steps (sequence numbers restart afterwards)
 void xf_launch_flush_pending(const XfTableView& t, cudaStream_t st);

@@ -122,6 +122,13 @@ struct XfStampView {
   uint32_t* stamp;
   uint32_t now;
 };
+// Importance weighting (weight.cu): e[row] = the effective weight of each row of the step (0: the row is skipped) and
+// *W = sum over trained rows of ceil(e) x tokens, the bound the lazy step derives its fixed-point unit from.  Only the
+// weighting instantiations of the step kernels read it; a kernel parameter of its own, passed last, like XfStampView.
+struct XfWeightView {
+  const float* e;
+  const unsigned long long* W;
+};
 __host__ __device__ __forceinline__ bool xf_keeps(const XfKeep& k, uint32_t stamp, uint64_t key) {
   return stamp >= k.cutoff && (!k.bounded || stamp > k.s_star || (stamp == k.s_star && key <= k.k_star));
 }

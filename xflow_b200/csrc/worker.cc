@@ -111,6 +111,21 @@ static xf_eviction_config EvictionFromEnv(int world, uint64_t* every) {
   return c;
 }
 
+// Negative sampling of the trainers' steps (xf_trainer_set_negative_sampling): XFLOW_NEG_SAMPLE = r keeps each negative
+// row with probability r and weights it by 1 / r, decided per row from its keys and XFLOW_SEED.  Unset or 1: every row
+// is trained with weight 1.  Single GPU only.
+static float NegSampleFromEnv(int world) {
+  const char* e = getenv("XFLOW_NEG_SAMPLE");
+  if (!e || !*e) return 1.f;
+  char* end = nullptr;
+  const double r = strtod(e, &end);
+  if (*end || !(r > 0.0 && r <= 1.0) || (float)r < 1.0f / 16777216.0f)
+    throw std::runtime_error(std::string("XFLOW_NEG_SAMPLE must be a rate in [2^-24, 1], got '") + e + "'");
+  if (world > 1)
+    throw std::runtime_error("XFLOW_NEG_SAMPLE is single-GPU only: unset it or run with XFLOW_WORLD = 1");
+  return (float)r;
+}
+
 // the table's training-batch number (host state, no device sync)
 static uint64_t TableBatches(xf_table* t) {
   uint64_t b = 0;
@@ -159,6 +174,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   AdmissionFromEnv(world_);  // a malformed XFLOW_ADMIT, or one with XFLOW_WORLD > 1, fails here
   uint64_t every = 0;
   EvictionFromEnv(world_, &every);  // likewise XFLOW_EVICT_*
+  NegSampleFromEnv(world_);         // and XFLOW_NEG_SAMPLE
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -272,6 +288,10 @@ void WorkerBase::ensure_trainer(uint32_t rows, uint32_t nnz) {
   cfg.max_nnz = nnz + nnz / 4 + 16;
   cfg.keep_loss = 0;
   must(xf_trainer_create(&trainer_, table_, comm_, &cfg), "xf_trainer_create");
+  const float neg_rate = NegSampleFromEnv(1);  // XFLOW_WORLD > 1 was refused at Server creation
+  if (neg_rate < 1.f)
+    must(xf_trainer_set_negative_sampling(trainer_, neg_rate, (uint64_t)env_int("XFLOW_SEED", 0)),
+         "xf_trainer_set_negative_sampling");
   trainer_rows_ = cfg.max_rows;
   trainer_nnz_ = cfg.max_nnz;
 }
