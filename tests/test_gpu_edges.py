@@ -6,7 +6,7 @@ float64 model for the canonical FM):
   B. latent widths K = 1 ... 1024: VEC = 1, 2 and 4, the sector path, chunk counts that are not a power of two and
      K / VEC > 32 in xf_k_update, through fused steps and through Pull / Push; canonical FM at K = 32, 64, 128;
   C. rows longer than 128 tokens (phase B's re-probe from chunk 2 on), with and without admission;
-  D. the process-wide settings XFLOW_FM_CACHE_LOG2 and XFLOW_UPDATE_WIDE, in a child process (edge_child.py)."""
+  D. the process-wide setting XFLOW_FM_CACHE_LOG2, in a child process (edge_child.py)."""
 import os
 import subprocess
 import sys
@@ -399,12 +399,6 @@ def _child(tmp_path, env, what):
 @pytest.mark.parametrize("log2", ["0", "10"])
 def test_fm_cache_size_setting_matches_oracle(log2, tmp_path):
     got = _child(tmp_path, {"XFLOW_FM_CACHE_LOG2": log2}, "fm_steps")
-    _check_fm_steps(got)
-
-
-def test_wide_update_setting_matches_oracle(tmp_path):
-    got = _child(tmp_path, {"XFLOW_UPDATE_WIDE": "1"}, "wide")
-    assert got["pull_push_ok"].all(), got["pull_push_ok"]
     _check_fm_steps(got)
 
 

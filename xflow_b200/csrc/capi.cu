@@ -271,13 +271,8 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   // L2 fetch granularity = one probing bucket (LR: 4 rows = one 128-byte line), so that the collision probes of
   // a bucket find the line the first load fetched.  It costs DRAM read traffic; the kernels are bound by the request
   // rate, not by DRAM bytes, and on the H100 32, 64 and 128 B time the same on every N = 1 bench workload (DESIGN.md
-  // section 6).  A hint: the driver may ignore it.  XFLOW_L2_FETCH = 32 / 64 / 128 overrides.
-  {
-    int fetch = 128;
-    const char* fe = getenv("XFLOW_L2_FETCH");
-    if (fe && (atoi(fe) == 32 || atoi(fe) == 64 || atoi(fe) == 128)) fetch = atoi(fe);
-    if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)fetch) != cudaSuccess) cudaGetLastError();
-  }
+  // section 6).  A hint: the driver may ignore it.
+  if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 128) != cudaSuccess) cudaGetLastError();
   xf_table* t = new xf_table;
   t->cfg = *cfg;
   memset(&t->view, 0, sizeof(t->view));

@@ -320,22 +320,15 @@ int xf_mg_create(xf_trainer* tr) {
     if (cudaMalloc(&mg->slab, mg->L.total) != cudaSuccess) { cudaGetLastError(); xf_set_error("cannot allocate the %llu-byte exchange slab", (unsigned long long)mg->L.total); rc = XF_ERR_CUDA; break; }
     // flags, meta and counters start at zero; the rest is written before it is read
     if (cudaMemsetAsync(mg->slab, 0, mg->L.off_in_keys, st) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    // Routing and the DONE signal are what the OTHER ranks wait for.  Giving their streams the high priority
-    // (XFLOW_MG_ROUTE_PRIO=1) did not make the 2-GPU step faster, so equal priority stays the default.
-    const char* rp = getenv("XFLOW_MG_ROUTE_PRIO");
-    const int prio = (rp && *rp == '1') ? hi : lo;
-    if (cudaStreamCreateWithPriority(&mg->st2, cudaStreamNonBlocking, prio) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
-    if (cudaStreamCreateWithPriority(&mg->st3, cudaStreamNonBlocking, prio) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
+    // Routing and the DONE signal are what the OTHER ranks wait for; a high priority for their streams did not
+    // make the 2-GPU step faster, so they run at the default priority.
+    if (cudaStreamCreateWithFlags(&mg->st2, cudaStreamNonBlocking) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
+    if (cudaStreamCreateWithFlags(&mg->st3, cudaStreamNonBlocking) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
     if (cudaEventCreateWithFlags(&mg->ev_meta, cudaEventDisableTiming) != cudaSuccess) { rc = XF_ERR_CUDA; break; }
     if ((rc = mg->slots.ensure((size_t)S * mg->cap * 4)) != XF_OK) break;
     if ((rc = mg->rowv_local.ensure((size_t)mg->max_rows * 8 + 16)) != XF_OK) break;
     const bool lazy = tr->table->view.lazy != 0;
-    {
-      const char* se = getenv("XFLOW_MG_STASH");  // A/B: 0 = the Push handler loads the rows itself
-      if (lazy && !(se && *se == '0') && (rc = mg->stash.ensure((size_t)S * mg->cap * 16)) != XF_OK) break;
-    }
+    if (lazy && (rc = mg->stash.ensure((size_t)S * mg->cap * 16)) != XF_OK) break;
     if (!lazy) {
       mg->touched_extra = xf_acc_touched_extra(mg->K, (uint64_t)mg->cap);
       if ((rc = mg->touched.ensure(((size_t)mg->cap + 2 * (size_t)mg->touched_extra) * 4)) != XF_OK) break;
@@ -550,8 +543,7 @@ int xf_mg_step(xf_trainer* tr, const uint32_t* d_row_ptr, const uint64_t* d_keys
     if (t->view.lazy) {
       XF_TRY(t->next_seq());
       xf_launch_push_tokens_lr(t->view, slots_s, rows_s, reinterpret_cast<const float*>(rowv_s), meta_s, cap, work, t->seq,
-                               t->d_rows_by_seq, uniq_s,
-                               mg->stash.p ? (const uint8_t*)mg->stash.p + (size_t)s * cap * 16 : nullptr, st);
+                               t->d_rows_by_seq, uniq_s, (const uint8_t*)mg->stash.p + (size_t)s * cap * 16, st);
       ++tr->launches;
     } else {
       xf_launch_acc_tokens(t->view, slots_s, rows_s, rowv_s, meta_s, cap, work, mg->touched.as<uint32_t>(), st);

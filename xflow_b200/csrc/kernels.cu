@@ -247,161 +247,6 @@ xf_k_update(XfTableView t, const uint32_t* __restrict__ slots, uint64_t n, int t
 }
 
 // -------------------------------------------------------------------------------------------------
-// optimizer step over a list of rows, WIDE variant (K a multiple of 4, row <= 512 B: every FM config of
-// BASELINE.json).  On a multi-GB table the cost of a row access is per INSTRUCTION that touches the row, not
-// per byte (tools/membench.cu: a 256-byte row read by 4 lanes x 4 x 16 B = 1365 us per 6.5 M rows, by 16 lanes
-// x 16 B in ONE instruction = 267 us).  A group of G lanes (G = the row's 16-byte units rounded up to a power of
-// two) therefore loads the whole row with one instruction and stores it with one: lane 0 holds {key, g}, lane 1
-// {w, n, z, flags}, the next K/4 lanes the latent row, then {L, Aq}, then nv and zv.  The lanes that hold v do
-// the latent coordinates (nv / zv / accumulators reach them by shuffles, results go back the same way), lane 1
-// does w.  Same arithmetic, same options (SLOTG, pulled-v side buffer, device-side list length) as xf_k_update.
-// -------------------------------------------------------------------------------------------------
-template <bool SLOTG>
-__global__ void __launch_bounds__(256, 4)
-xf_k_update_wide(XfTableView t, const uint32_t* __restrict__ slots, uint64_t n, int G, double rows,
-                 const float* __restrict__ gw, const float* __restrict__ gv, int part,
-                 unsigned long long* __restrict__ live_total, const uint32_t* __restrict__ n_dev,
-                 const uint32_t* __restrict__ rows_dev, uint32_t extra_base, uint32_t extra_n,
-                 const float* __restrict__ v0_side, XfStampView sv) {
-  __shared__ unsigned int s_live;
-  if (threadIdx.x == 0) s_live = 0;
-  __syncthreads();
-  uint64_t n_head = n;
-  if (n_dev != nullptr) {
-    n_head = min((uint64_t)__ldg(n_dev), (uint64_t)extra_base);
-    n = n_head + extra_n;
-    rows = (double)__ldg(rows_dev);
-  }
-  unsigned int live_acc = 0;
-  const int K = t.K;
-  const bool ftrl = t.opt == XF_OPT_FTRL;
-  const int nV = K >> 2;                       // 16-byte units of v
-  const int units = (int)(t.stride >> 4);      // units of the whole row
-  const int u_acc = 2 + nV, u_nv = u_acc + 1, u_zv = u_nv + nV;
-  const unsigned lane = threadIdx.x & 31u;
-  const uint64_t gwarp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-  const int q = (int)(lane & (unsigned)(G - 1));
-  const int gi = (int)(lane / (unsigned)G);
-  const int ngroups = 32 / G;
-  const bool is_v = q >= 2 && q < 2 + nV;
-  const int jv = q - 2;                        // which quarter of v this lane holds (is_v)
-  // lanes this lane exchanges with
-  const int src_nv = is_v ? u_nv + jv : 0, src_zv = (is_v && ftrl) ? u_zv + jv : 0;
-  const bool is_nv = ftrl && q >= u_nv && q < u_nv + nV, is_zv = ftrl && q >= u_zv && q < u_zv + nV;
-  const int back = is_nv ? 2 + (q - u_nv) : (is_zv ? 2 + (q - u_zv) : 0);
-
-  for (uint64_t base = gwarp * 32; base < n; base += nwarps * 32) {
-    const uint64_t e_fwd = base + lane;
-    const uint64_t e_i = (SLOTG && e_fwd < n) ? (n - 1 - e_fwd) : e_fwd;  // backwards: see xf_k_update
-    const uint64_t e_phys = (e_i < n_head) ? e_i : (uint64_t)extra_base + (e_i - n_head);
-    const uint32_t s_lane = (e_fwd < n) ? __ldcs(slots + e_phys) : 0xFFFFFFFFu;
-    unsigned pend = __ballot_sync(0xffffffffu, s_lane != 0xFFFFFFFFu);
-    if (live_total != nullptr && lane == 0) live_acc += __popc(pend);
-    while (pend) {
-      const int cnt = __popc(pend);
-      const unsigned src = (gi < cnt) ? __fns(pend, 0, gi + 1) : 0u;
-      const uint32_t s = __shfl_sync(0xffffffffu, s_lane, (int)src);
-      const uint64_t i = __shfl_sync(0xffffffffu, (unsigned long long)e_i, (int)src);
-      const uint64_t i_phys = __shfl_sync(0xffffffffu, (unsigned long long)e_phys, (int)src);
-      const bool live = gi < cnt;
-      uint4* rowu = live ? reinterpret_cast<uint4*>(xf_row(t, s)) : nullptr;
-      pend = (cnt <= ngroups) ? 0u : (pend & ~((2u << __fns(pend, 0, ngroups)) - 1u));
-
-      // ---- the whole row, one instruction; the side inputs of the v lanes with it
-      uint4 u = make_uint4(0, 0, 0, 0);
-      if (live && q < units) u = __ldcg(rowu + q);
-      float4 side = make_float4(0.f, 0.f, 0.f, 0.f);  // SLOTG: v as pulled (sources >= 1) ; pushed: gv
-      if (live && is_v) {
-        if (SLOTG) {
-          if (v0_side != nullptr) {
-            const uint64_t tok = (i_phys < (uint64_t)extra_base) ? i_phys : (uint64_t)__ldg(slots + i_phys + extra_n);
-            side = __ldcg(reinterpret_cast<const float4*>(v0_side + tok * (uint64_t)K) + jv);
-          }
-        } else {
-          side = __ldcg(reinterpret_cast<const float4*>(gv + i * (uint64_t)K) + jv);
-        }
-      }
-      float gw_i = 0.f;
-      if (!SLOTG && live && q == 1 && (part & 1)) gw_i = __ldg(gw + i);
-
-      // ---- exchange inside the group (all lanes of the warp take part in every shuffle)
-      const uint32_t key_lo = __shfl_sync(0xffffffffu, u.x, 0, G), key_hi = __shfl_sync(0xffffffffu, u.y, 0, G);
-      const uint32_t g_lo = __shfl_sync(0xffffffffu, u.z, 0, G), g_hi = __shfl_sync(0xffffffffu, u.w, 0, G);
-      const uint32_t flags = __shfl_sync(0xffffffffu, u.w, 1, G);
-      const uint32_t aL0 = __shfl_sync(0xffffffffu, u.x, u_acc, G), aL1 = __shfl_sync(0xffffffffu, u.y, u_acc, G);
-      const uint32_t aA0 = __shfl_sync(0xffffffffu, u.z, u_acc, G), aA1 = __shfl_sync(0xffffffffu, u.w, u_acc, G);
-      uint4 un, uz;
-      un.x = __shfl_sync(0xffffffffu, u.x, src_nv, G); un.y = __shfl_sync(0xffffffffu, u.y, src_nv, G);
-      un.z = __shfl_sync(0xffffffffu, u.z, src_nv, G); un.w = __shfl_sync(0xffffffffu, u.w, src_nv, G);
-      uz.x = __shfl_sync(0xffffffffu, u.x, src_zv, G); uz.y = __shfl_sync(0xffffffffu, u.y, src_zv, G);
-      uz.z = __shfl_sync(0xffffffffu, u.z, src_zv, G); uz.w = __shfl_sync(0xffffffffu, u.w, src_zv, G);
-      const uint64_t key = (uint64_t)key_lo | ((uint64_t)key_hi << 32);
-      const double g_acc = __longlong_as_double((long long)((uint64_t)g_lo | ((uint64_t)g_hi << 32)));
-      const double accL = __longlong_as_double((long long)((uint64_t)aL0 | ((uint64_t)aL1 << 32)));
-      const double accA = __longlong_as_double((long long)((uint64_t)aA0 | ((uint64_t)aA1 << 32)));
-      const bool ready = (flags & XF_FLAG_V_READY) != 0;
-
-      // ---- lane 1: the scalar weight ; v lanes: four latent coordinates each
-      uint4 out = u;
-      float nn[4] = {0.f, 0.f, 0.f, 0.f}, zz[4] = {0.f, 0.f, 0.f, 0.f};
-      if (q == 0 && SLOTG) { out.z = 0u; out.w = XF_NEG_ZERO_BITS; }  // g = -0.0: "untouched" for the next batch
-      if (q == 1) {
-        float w = __uint_as_float(u.x), nw = __uint_as_float(u.y), zw = __uint_as_float(u.z);
-        if (part & 1) {
-          const float g = SLOTG ? xf_div_rows((float)g_acc, rows) : gw_i;
-          xf_opt_coord(t, g, w, nw, zw);
-        }
-        out.x = __float_as_uint(w); out.y = __float_as_uint(nw); out.z = __float_as_uint(zw);
-        out.w = u.w | XF_FLAG_V_READY;
-      }
-      if (is_v) {
-        float v[4] = {__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w)};
-        nn[0] = __uint_as_float(un.x); nn[1] = __uint_as_float(un.y); nn[2] = __uint_as_float(un.z); nn[3] = __uint_as_float(un.w);
-        zz[0] = __uint_as_float(uz.x); zz[1] = __uint_as_float(uz.y); zz[2] = __uint_as_float(uz.z); zz[3] = __uint_as_float(uz.w);
-        if (!ready) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { v[e] = xf_v_init(t, key, (uint32_t)(4 * jv + e)); nn[e] = 0.f; zz[e] = 0.f; }
-        }
-        float g[4];
-        if (SLOTG) {
-          // gv[k] = Aq - v[k] * L with v as the source pulled it (table.cuh, xf_k_pull_tokens)
-          const float p[4] = {side.x, side.y, side.z, side.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) g[e] = xf_div_rows((float)(accA - (double)(v0_side != nullptr ? p[e] : v[e]) * accL), rows);
-        } else {
-          g[0] = side.x; g[1] = side.y; g[2] = side.z; g[3] = side.w;
-        }
-        if (ftrl) {
-#pragma unroll 1
-          for (int e = 0; e < 4; ++e) xf_ftrl_coord(t, g[e], v[e], nn[e], zz[e]);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) xf_sgd_coord(t, g[e], v[e]);
-        }
-        out = make_uint4(__float_as_uint(v[0]), __float_as_uint(v[1]), __float_as_uint(v[2]), __float_as_uint(v[3]));
-      }
-      // ---- nv / zv back to the lanes that own those bytes
-      uint4 bn, bz;
-      bn.x = __shfl_sync(0xffffffffu, __float_as_uint(nn[0]), back, G); bn.y = __shfl_sync(0xffffffffu, __float_as_uint(nn[1]), back, G);
-      bn.z = __shfl_sync(0xffffffffu, __float_as_uint(nn[2]), back, G); bn.w = __shfl_sync(0xffffffffu, __float_as_uint(nn[3]), back, G);
-      bz.x = __shfl_sync(0xffffffffu, __float_as_uint(zz[0]), back, G); bz.y = __shfl_sync(0xffffffffu, __float_as_uint(zz[1]), back, G);
-      bz.z = __shfl_sync(0xffffffffu, __float_as_uint(zz[2]), back, G); bz.w = __shfl_sync(0xffffffffu, __float_as_uint(zz[3]), back, G);
-      if (is_nv) out = bn;
-      if (is_zv) out = bz;
-      if (q == u_acc && SLOTG) out = make_uint4(0, 0, 0, 0);  // {L, Aq} consumed
-      if (live && q < units) rowu[q] = out;                    // the whole row, one instruction
-      if (SLOTG && live && q == 0 && sv.stamp != nullptr) sv.stamp[s] = sv.now;  // feature eviction
-    }
-  }
-  if (live_total != nullptr) {
-    if (lane == 0 && live_acc) atomicAdd(&s_live, live_acc);
-    __syncthreads();
-    if (threadIdx.x == 0 && s_live) atomicAdd_system(live_total, (unsigned long long)s_live);
-  }
-}
-
-// -------------------------------------------------------------------------------------------------
 // generic pieces: Pull / Push / import / export / growth
 // -------------------------------------------------------------------------------------------------
 // keys -> slots (0xFFFFFFFF = absent / overflow).  Optionally emits w (app-0 Pull, ftrl.h:75-77).  A key it inserts
@@ -610,18 +455,6 @@ static void xf_launch_update_t(const XfTableView& t, const uint32_t* slots, uint
                                cudaStream_t st, const uint32_t* n_dev = nullptr, const uint32_t* rows_dev = nullptr,
                                uint32_t extra_base = 0, uint32_t extra_n = 0, const float* v0_side = nullptr,
                                XfStampView sv = XfStampView{nullptr, 0u}) {
-  // wide variant: whole-row loads / stores by one instruction: fewer requests but only 2 rows in flight per warp
-  // and 90+ registers, slower than the per-coordinate kernel when it was measured; off unless XFLOW_UPDATE_WIDE=1
-  // (A/B measurements)
-  static const bool wide_on = [] { const char* e = getenv("XFLOW_UPDATE_WIDE"); return e && *e == '1'; }();
-  if (wide_on && !t.canon && t.K > 0 && (t.K & 3) == 0 && t.stride <= 512 && (part & 2)) {
-    int G = 1;
-    while (G < (int)(t.stride >> 4)) G <<= 1;
-    const int grid = xf_grid_for(n * (uint64_t)G, 256, 8);
-    xf_k_update_wide<SLOTG><<<grid, 256, 0, st>>>(t, slots, n, G, rows, gw, gv, part, live_total, n_dev, rows_dev,
-                                                   extra_base, extra_n, v0_side, sv);
-    return;
-  }
   const int tps = xf_tps_for(t.K);
   const int grid = xf_grid_for(n * (uint64_t)tps, 256, 8);
 #define XF_UPD_ARGS t, slots, n, tps, rows, gw, gv, part, live_total, n_dev, rows_dev, extra_base, extra_n, v0_side, sv

@@ -345,7 +345,6 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
   // the coalesced inputs of the NEXT iteration (slot, row index, stashed state words) are requested before this
   // iteration's atomics go out.  The first version (one group, nothing ahead) stalled on a chain of four dependent
   // round trips per 32 tokens.
-  const bool have_stash = stash != nullptr;
   uint32_t s_n[2], r_n[2];
   uint4 b_n[2];
 #define XF_PUSH_FETCH(base_)                                                        \
@@ -355,7 +354,7 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
     if (i < n) {                                                                     \
       s_n[u] = __ldcs(slots + i);                                                    \
       r_n[u] = __ldcs(in_rows + i);                                                  \
-      if (have_stash) b_n[u] = __ldcs(stash + (uint64_t)i);                          \
+      b_n[u] = __ldcs(stash + (uint64_t)i);                                          \
     }                                                                                \
   }
   uint32_t base = gwarp * 64;
@@ -363,24 +362,17 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
   for (; base < n; base += nwarps * 64) {
     uint32_t s[2];
     float l[2];
-    uint64_t q1[2], q2[2], q3[2];
+    uint64_t q2[2], q3[2];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       s[u] = s_n[u];
       l[u] = 0.f;
-      q1[u] = 0ull; q2[u] = 0ull; q3[u] = (uint64_t)seq;  // invalid lanes: "open", nothing to do
+      q2[u] = 0ull; q3[u] = (uint64_t)seq;  // invalid lanes: "open", nothing to do
       if (s[u] == XF_NO_SLOT) continue;
       l[u] = __ldcg(rowv + r_n[u]);
-      if (have_stash) {
-        // the row's state as this step's Pull found it (coalesced, streaming) instead of a load of the row
-        q2[u] = (uint64_t)b_n[u].x | ((uint64_t)b_n[u].y << 32);
-        q3[u] = (uint64_t)b_n[u].z | ((uint64_t)b_n[u].w << 32);
-      } else {
-        const XfHead h = xf_load_head(xf_row(t, s[u]));
-        q1[u] = xf_raw_q1(h);
-        q2[u] = xf_raw_q2(h);
-        q3[u] = xf_raw_q3(h);
-      }
+      // the row's state as this step's Pull found it (coalesced, streaming) instead of a load of the row
+      q2[u] = (uint64_t)b_n[u].x | ((uint64_t)b_n[u].y << 32);
+      q3[u] = (uint64_t)b_n[u].z | ((uint64_t)b_n[u].w << 32);
     }
     if (base + nwarps * 64 < n) { XF_PUSH_FETCH(base + nwarps * 64) }
     bool lead[2], issued[2], reload[2];
@@ -403,9 +395,9 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
       }
       issued[u] = false;
       q2n[u] = q2[u]; o2[u] = q2[u]; o3[u] = q3[u];
-      reload[u] = lead[u] && have_stash && (q3[u] & XF_TAG_MASK) == XF_TAG_MASK;  // the Pull saw an imported weight
+      reload[u] = lead[u] && (q3[u] & XF_TAG_MASK) == XF_TAG_MASK;  // the Pull saw an imported weight
       if (lead[u] && !reload[u]) {
-        xf_lazy_fold(t, q1[u], q2[u], q3[u], seq, q2n[u]);
+        xf_lazy_fold(t, 0ull, q2[u], q3[u], seq, q2n[u]);  // no imported weight: bytes 8..15 play no part
         issued[u] = xf_lazy_deposit_issue(xf_row(t, s[u]), q2[u], q3[u], q2n[u], seq, fix[u], o2[u], o3[u]);
       }
     }
@@ -415,7 +407,7 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
       uint8_t* rowp = xf_row(t, s[u]);
       bool stale = false;
       if (!reload[u] &&
-          xf_lazy_deposit_resolve(t, rowp, issued[u], q2[u], q3[u], o2[u], o3[u], seq, fix[u], have_stash ? &stale : nullptr))
+          xf_lazy_deposit_resolve(rowp, issued[u], q2[u], q3[u], o2[u], o3[u], seq, fix[u], &stale))
         ++open_acc;
       if (stale) {
         // An earlier source of this round changed the row since the Pull.  The failed CAS has brought the row's

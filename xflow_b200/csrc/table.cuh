@@ -591,18 +591,18 @@ __device__ __forceinline__ bool xf_lazy_deposit_issue(uint8_t* rowp, uint64_t q2
   xf_cas128(rowp + XF_OFF_STATE, q2, q3, q2_new, ((unsigned long long)fix << 16) | (uint64_t)seq, o2, o3);
   return true;
 }
-// returns true when the issued CAS opened the row; *stale as in xf_lazy_deposit
-__device__ __forceinline__ bool xf_lazy_deposit_resolve(const XfTableView& t, uint8_t* rowp, bool issued, uint64_t q2, uint64_t q3,
-                                                        uint64_t o2, uint64_t o3, uint32_t seq, long long fix, bool* stale) {
-  if (stale) *stale = false;
+// returns true when the issued CAS opened the row.  Its one caller is the sharded owner, which works from the look
+// its Pull stashed: *stale reports a row that moved on to another batch since then (as in xf_lazy_deposit).
+__device__ __forceinline__ bool xf_lazy_deposit_resolve(uint8_t* rowp, bool issued, uint64_t q2, uint64_t q3, uint64_t o2,
+                                                        uint64_t o3, uint32_t seq, long long fix, bool* stale) {
+  *stale = false;
   if (!issued) return false;
   if (o2 == q2 && o3 == q3) return true;
   if ((uint32_t)(o3 & XF_TAG_MASK) == seq) {  // another token of this batch was first
     xf_lazy_add(rowp, fix);
     return false;
   }
-  if (stale) *stale = true;
-  else *t.error = 2;
+  *stale = true;
   return false;
 }
 __device__ __forceinline__ bool xf_lazy_deposit(const XfTableView& t, uint8_t* rowp, uint64_t q2, uint64_t q3, uint64_t q2_new,
