@@ -1,8 +1,10 @@
 """Child process of tests/test_gpu_edges.py, part D: runs the device side of a case under the process-wide setting
 XFLOW_FM_CACHE_LOG2, which the library reads once per process, and writes the results to an npz file for the parent
-test to compare.
+test to compare.  fm_bounds instead checks its cases itself against tests/fm_model.py (test_gpu_fm_step.py) and exits
+non-zero on the first one outside the bounds.
 
     python tests/edge_child.py fm_steps OUT.npz
+    python tests/edge_child.py fm_bounds OUT.npz
 """
 import os
 import sys
@@ -11,7 +13,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-for p in (ROOT, HERE):
+for p in (ROOT, HERE, os.path.join(HERE, "golden")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
@@ -54,6 +56,9 @@ def main():
     out = {}
     if what == "fm_steps":
         fm_steps(out)
+    elif what == "fm_bounds":
+        import test_gpu_fm_step
+        test_gpu_fm_step.cache_setting_cases()
     else:
         raise SystemExit("unknown case " + what)
     np.savez(path, **out)
