@@ -167,7 +167,7 @@ XF_DLL int xf_table_sync(xf_table* t);
  * XF_ADMIT_ALL, predict never inserts: an absent key contributes 0.
  * Single-GPU tables only: refused on canonical tables (canonical_fm = 1), on tables with num_shards > 1, and by
  * xf_trainer_create with a multi-rank comm.  The filter lives in device memory owned by the table (2^log2_cells
- * bytes) and is NOT part of xf_table_save / xf_table_load: a resumed run starts with an empty filter. */
+ * bytes).  It is part of the state image (xf_table_save_state), not of the portable xf_table_save format. */
 enum { XF_ADMIT_ALL = 0, XF_ADMIT_POISSON = 1, XF_ADMIT_BLOOM = 2 };
 typedef struct xf_admission_config {
   int mode;                /* XF_ADMIT_* */
@@ -210,7 +210,8 @@ XF_DLL int xf_table_admission_stats(xf_table* t, uint64_t* batches, uint64_t* re
  * <= 0.5, never above the current capacity; the old and the new table are both allocated while it runs, as in
  * growth.  A sweep that would remove nothing and keep the capacity does nothing.
  * The stamps are one uint32_t per slot of device memory beside the rows (+12.5 % for LR rows, +1.6 % for FM K = 16
- * FTRL rows); they are not part of xf_table_save (a loaded key is an insertion).  A table that has run 2^32 - 1
+ * FTRL rows); they are part of the state image (xf_table_save_state) but not of xf_table_save (a key xf_table_load
+ * loads is an insertion).  A table that has run 2^32 - 1
  * training batches refuses further tracked training steps.  Single-GPU tables only: refused on canonical tables
  * (canonical_fm = 1), on tables with num_shards > 1, and by xf_trainer_create / the step with a multi-rank comm. */
 typedef struct xf_eviction_config {
@@ -225,6 +226,51 @@ XF_DLL int xf_table_set_eviction(xf_table* t, const xf_eviction_config* cfg);
 XF_DLL int xf_table_evict(xf_table* t, uint64_t* evicted);
 /* out[i] = last(keys[i]), or UINT64_MAX for an absent key; never inserts.  XF_ERR_STATE without tracking. */
 XF_DLL int xf_table_last_touch(xf_table* t, const uint64_t* keys, uint64_t n, uint64_t* out);
+
+/* Exact training-state checkpoint of one table (not the portable xf_table_save format).
+ * xf_table_save_state writes an image of everything that decides the table's future: every live row's raw bytes in
+ * its slot, the capacity, the capacity floor and the probing layout, the key count, the training-batch number, the
+ * admission policy, its counters and Bloom filter, the eviction limits and every live key's stamp, the lazy LR
+ * tables' pending-step ring, the config fields that define the rows and their arithmetic, and the caller's `user`
+ * value (the CLI stores the epochs done there).  A table loaded from it is byte-identical to the saved one and trains
+ * on bit for bit as the saved table would have: a run that saves and continues, and a run resumed from the image,
+ * both equal the run that never saved.  Not in the image: the trainers' state (xf_trainer_stats counters, the
+ * negative-sampling policy, which is caller config) and xf_table_set_stream's choice.
+ * Save runs stream-ordered after everything enqueued on the table's stream, waits for it, and changes nothing in the
+ * table.  It writes <path>.tmp and renames it to <path>; on failure no .tmp is left.  Saving the same state twice
+ * gives identical files.
+ * Load needs a table that has never held state: no keys and no training batch (XF_ERR_STATE otherwise).  Its config
+ * must equal the image's field by field (floats bitwise; device and capacity excepted), and so must its row stride,
+ * its lazy or eager row layout (XFLOW_EAGER) and its bucket shift at the image's capacity: XF_ERR_ARG names the first
+ * field that differs.  The table then takes the image's capacity and every row goes back into its saved slot; the
+ * policies, stamps, filter, counters, batch number and capacity floor are the image's (a policy set on the target is
+ * replaced).  A damaged or truncated file, or a file of the other format, is XF_ERR_IO.  On any failure the table
+ * is unchanged.  *user (may be NULL) receives the saved value.
+ * Memory: besides the table, a save or load takes two device and two page-locked staging chunks of at most 64 MiB
+ * each, whatever the table's size; a load holds the old and the new table at once, as growth does.
+ *
+ * File format (little-endian), version 1:
+ *   header, 232 bytes
+ *     0 "XFST"   4 u32 version   8 u64 header bytes (232)   16 u64 capacity   24 u64 capacity floor   32 u64 keys
+ *     40 u32 row stride   44 u32 log2 capacity   48 u32 bucket shift   52 u32 lazy (1) or eager (0) rows
+ *     56 i32 latent_dim   60 i32 optimizer   64 f32 alpha   68 f32 beta   72 f32 lambda1   76 f32 lambda2
+ *     80 f32 learning_rate   84 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   88 u64 seed
+ *     96 i32 shard_index   100 i32 num_shards   104 i32 canonical_fm   108 u32 seq (lazy: the ring's last batch)
+ *     112 u64 training batches   120 u64 rejected tokens   128 u64 admitted keys
+ *     136 i32 admission mode   140 f32 probability   144 u32 threshold   148 u32 log2_cells   152 u32 hashes
+ *     156 u32 eviction tracking (0/1)   160 u64 decay_batches   168 u64 admission seed
+ *     176 u64 max_idle_batches   184 u64 max_keys   192 u64 user   200 u64 chunk slots C
+ *     208 u64 filter bytes F (Bloom: 2^log2_cells, else 0)   216 u64 ring entries R (lazy: seq + 1, else 0)
+ *     224 u64 checksum of bytes [0, 224)
+ *   ring section (R > 0): R u64 (the pending steps' divisors by batch number), u64 checksum
+ *   rows section: capacity / C chunks, chunk i covering slots [i C, (i + 1) C):
+ *     u64 first slot (= i C), u64 live rows n, u64 checksum, u64 0; then n rows of `stride` raw bytes in slot order,
+ *     then n u64 slot | stamp << 32 (stamp 0 without tracking)
+ *   filter section (F > 0): F bytes of cells, u64 checksum
+ * A section's checksum is the sum mod 2^64 of splitmix64(w ^ o) over its 8-byte words w, o = the word's byte offset
+ * in the section's payload; in the rows section o = i << 40 | the offset in chunk i's payload (after its 32 bytes). */
+XF_DLL int xf_table_save_state(xf_table* t, const char* path, uint64_t user);
+XF_DLL int xf_table_load_state(xf_table* t, const char* path, uint64_t* user /* may be NULL */);
 
 /* bucketing rule of ps::Postoffice::GetServerKeyRanges (postoffice.cc:134-143) + DefaultSlicer
  * (kv_app.h:405-460): shard = min(key / floor((2^64-1)/S), S-1).  Pure host function. */

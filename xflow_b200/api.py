@@ -68,6 +68,8 @@ SIGNATURES = {
     "xf_table_touch_decimal_ids": (_i, [_vp, _u64, _u64]),
     "xf_table_save": (_i, [_vp, C.c_char_p]),
     "xf_table_load": (_i, [_vp, C.c_char_p]),
+    "xf_table_save_state": (_i, [_vp, C.c_char_p, _u64]),
+    "xf_table_load_state": (_i, [_vp, C.c_char_p, _vp]),
     "xf_table_set_stream": (_i, [_vp, _vp]),
     "xf_table_sync": (_i, [_vp]),
     "xf_admission_config_default": (_i, [_vp]),
@@ -338,6 +340,16 @@ class Table:
 
     def load(self, path):
         _check(lib().xf_table_load(self.h, path.encode()))
+
+    def save_state(self, path, user=0):
+        """Exact training-state image of the table (xf_table_save_state); `user` is stored with it."""
+        _check(lib().xf_table_save_state(self.h, path.encode(), int(user)))
+
+    def load_state(self, path):
+        """Load an image written by save_state into this table, which must never have held state; returns `user`."""
+        user = C.c_uint64()
+        _check(lib().xf_table_load_state(self.h, path.encode(), C.byref(user)))
+        return user.value
 
     def set_stream(self, cuda_stream):
         _check(lib().xf_table_set_stream(self.h, C.c_void_p(int(cuda_stream)) if cuda_stream else None))

@@ -116,6 +116,17 @@ static uint64_t xf_pow2_at_least(uint64_t x) {
   return p;
 }
 
+// probing buckets = the rows that share one 128-byte line (table.cuh: xf_probe_slot); XFLOW_BUCKET_LOG2
+// overrides (0 = plain linear probing) for A/B measurements
+uint32_t xf_bucket_shift(uint32_t stride, uint32_t log2cap) {
+  uint32_t bs = 0;
+  while ((stride << (bs + 1)) <= 128u) ++bs;
+  const char* be = getenv("XFLOW_BUCKET_LOG2");
+  if (be && *be) bs = (uint32_t)std::min(std::max(atoi(be), 0), 4);
+  if (bs + 4 > log2cap) bs = 0;
+  return bs;
+}
+
 int xf_table::alloc_table(uint64_t capacity) {
   capacity = xf_pow2_at_least(capacity);
   if (capacity > (1ull << 31)) {
@@ -139,14 +150,7 @@ int xf_table::alloc_table(uint64_t capacity) {
   while ((1ull << lg) < capacity) ++lg;
   view.log2cap = lg;
   view.stride = stride;
-  // probing buckets = the rows that share one 128-byte line (table.cuh: xf_probe_slot); XFLOW_BUCKET_LOG2
-  // overrides (0 = plain linear probing) for A/B measurements
-  uint32_t bs = 0;
-  while ((stride << (bs + 1)) <= 128u) ++bs;
-  const char* be = getenv("XFLOW_BUCKET_LOG2");
-  if (be && *be) bs = (uint32_t)std::min(std::max(atoi(be), 0), 4);
-  if (bs + 4 > lg) bs = 0;
-  view.bshift = bs;
+  view.bshift = xf_bucket_shift(stride, lg);
   xf_launch_fill(view, stream);
   ++launches;
   XF_CUDA_TRY(cudaGetLastError());
@@ -742,11 +746,17 @@ XF_DLL int xf_table_load(xf_table* t, const char* path) {
   if (!t || !path) return XF_ERR_ARG;
   FILE* f = fopen(path, "rb");
   if (!f) { xf_set_error("cannot open %s", path); return XF_ERR_IO; }
-  char magic[4];
+  char magic[4] = {0, 0, 0, 0};
   uint64_t n = 0;
   uint32_t K32 = 0, has_nz = 0;
   bool ok = fread(magic, 1, 4, f) == 4 && memcmp(magic, "XFTB", 4) == 0 && fread(&n, 8, 1, f) == 1 &&
             fread(&K32, 4, 1, f) == 1 && fread(&has_nz, 4, 1, f) == 1;
+  if (memcmp(magic, "XFST", 4) == 0) {
+    fclose(f);
+    xf_set_error("%s is a state image written by xf_table_save_state, not a portable checkpoint: load it with "
+                 "xf_table_load_state", path);
+    return XF_ERR_IO;
+  }
   if (!ok || (int)K32 != t->view.K) {
     fclose(f);
     xf_set_error("bad checkpoint %s (K=%u, table K=%d)", path, K32, t->view.K);

@@ -16,6 +16,8 @@ void xf_set_error(const char* fmt, ...);
 int xf_check_host_keys(const uint64_t* keys, uint64_t n, const char* fn);
 // XF_ERR_ARG, naming the row, if any of the n host row weights is NaN, negative or infinite (capi.cu)
 int xf_check_host_weights(const float* weights, uint64_t n, const char* fn);
+// log2 of the slots per probing bucket of a table of 2^log2cap rows of `stride` bytes (capi.cu)
+uint32_t xf_bucket_shift(uint32_t stride, uint32_t log2cap);
 
 #define XF_CUDA_TRY(expr)                                                              \
   do {                                                                                 \
