@@ -18,6 +18,8 @@
  *                                            (src/io/load_data_from_disk.cc:103-210)
  *   5. multi-GPU exchange     xf_comm_*    = KVWorker slicing + Van transport
  *                                            (ps-lite kv_app.h:405-460, postoffice.cc:134-143)
+ *   6. serving model          xf_model_*   = a trained table frozen for prediction only (no reference counterpart:
+ *                                            the reference predicts on its training servers, lr_worker.cc:25-77)
  */
 #ifndef XFLOW_B200_H_
 #define XFLOW_B200_H_
@@ -507,6 +509,91 @@ XF_DLL int xf_comm_create_from_file(xf_comm** out, const char* path, int rank, i
 XF_DLL int xf_comm_allreduce_max(xf_comm* c, uint64_t* inout);
 XF_DLL int xf_comm_destroy(xf_comm* c);
 XF_DLL int xf_comm_barrier(xf_comm* c);
+/* ------------------------------------------------------------------------------------------------
+ * 6. Serving model (csrc/serve.cu).  xf_table_freeze makes an xf_model from a trained table: an immutable, compact,
+ *    device-resident hash table that holds, per key, only what the forward pass reads, with a forward-only predict
+ *    kernel and a file format of its own.  The model shares nothing with the table: the table may train on, be saved
+ *    or destroyed, and a predict on the model never inserts a key.
+ *
+ *    Rows.  LR: {u64 key, f32 w, u32 0} = 16 bytes.  FM of any K: {u64 key, f32 w, f32 st, f32 qt, 12 zero bytes} =
+ *    32 bytes, one aligned sector, with st = sum_k v_k and qt = sum_k v_k^2: the reference's FM forward
+ *    (fm_worker.cc:177-196) reads nothing else of a latent row, and in a frozen model both are constants.  Open
+ *    addressing with the table's hash and bucketised probe sequence; empty slots hold key 2^64 - 1; capacity = the
+ *    smallest power of two >= 2 x keys (load <= 0.5), at least 1024.
+ *
+ *    Freeze waits for everything enqueued on the table's stream and changes nothing in the table (no row, stamp,
+ *    filter cell, batch number or pending step).  It resolves each row as a reader does: a lazy LR row's pending step is
+ *    folded in, an imported weight is honoured, an FM row whose latent block is not materialised gets st, qt of its
+ *    initial values.  The frozen w of a key is, bit for bit, what xf_table_export returns for it, and st, qt are what
+ *    the step kernels' forward pass computes for it; xf_model_predict_* therefore returns, bit for bit, what
+ *    xf_trainer_predict_* returns on the table at the moment of the freeze (with the matching `absent` policy).
+ *
+ *    Absent keys.  XF_ABSENT_DEFAULT: a key the model does not hold reads as the row the table would insert for it
+ *    (w = 0; FM: st, qt of the table's initial latent values, evaluated on the fly: K evaluations per absent token).
+ *    XF_ABSENT_ZERO: it contributes nothing, which is what predict does on a table with an admission policy.
+ *    prune = 1 leaves out every row that reads exactly as an absent key would: w == 0 and (LR, or, under DEFAULT, the
+ *    latent block is not materialised; under ZERO, st == 0 and qt == 0).  Pruning never changes a prediction, and
+ *    keys + pruned_keys == source_keys.  FTRL's L1 term writes exact zeros (ftrl.h:66-74): those are the rows pruned.
+ *
+ *    Refused with XF_ERR_ARG: tables with canonical_fm = 1 (the per-k sums of the canonical FM and the multi-view
+ *    machine do not collapse to st, qt) and tables with num_shards > 1 (one shard's rows are not a model).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct xf_model xf_model;
+enum { XF_ABSENT_DEFAULT = 0, XF_ABSENT_ZERO = 1 };
+typedef struct xf_freeze_config {
+  int absent;            /* XF_ABSENT_*, or -1 = what the table's own predict does: DEFAULT if its admission policy is
+                            XF_ADMIT_ALL, else ZERO */
+  int prune;             /* 1: leave out the rows that read as absent keys (above); 0: keep every key of the table */
+  int device;            /* CUDA ordinal the model lives on; -1 = the table's (another device: built on the table's,
+                            then copied there) */
+} xf_freeze_config;
+/* absent = -1, prune = 1, device = -1 */
+XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg);
+/* cfg == NULL: the defaults.  On failure *out is NULL. */
+XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+XF_DLL int xf_model_destroy(xf_model* m);
+typedef struct xf_model_info {
+  uint64_t keys;         /* keys the model holds */
+  uint64_t capacity;     /* slots */
+  uint64_t bytes;        /* capacity x row_bytes: the model's device memory */
+  uint64_t source_keys;  /* keys of the table when it was frozen */
+  uint64_t pruned_keys;  /* source_keys - keys */
+  uint32_t row_bytes;    /* 16 (LR) or 32 (FM) */
+  int latent_dim, optimizer, absent, fm;
+} xf_model_info;
+XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
+/* Model file "XFSM" (little-endian): a 104-byte header
+ *     0 "XFSM"   4 u32 version (1)   8 u64 header bytes (104)   16 u64 keys   24 u64 capacity   32 u32 row bytes
+ *    36 i32 fm   40 i32 latent_dim   44 i32 optimizer   48 i32 absent   52 i32 resolved v_init (0 constant, 1 counter-
+ *    based normal, 3 zero)   56 f32 the constant   60 u32 0   64 u64 seed   72 u64 source keys   80 u64 pruned keys
+ *    88 u64 rows per chunk (64 MiB / row bytes)   96 u64 checksum of bytes [0, 96)
+ *  then the rows SORTED BY KEY in ceil(keys / rows per chunk) chunks, each {u64 index of its first row, u64 rows,
+ *  u64 checksum, u64 0} followed by its rows.  Checksums are those of the state image above (sum of
+ *  splitmix64(word ^ offset), a chunk's offsets being chunk << 40 | byte offset in its rows).  The file is a function
+ *  of the model's contents, not of where its keys lie: two freezes of one table, and load then save, give identical
+ *  bytes.  Written to <path>.tmp and renamed; the staging is bounded by the chunk size.  xf_model_load rebuilds the
+ *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL. */
+XF_DLL int xf_model_save(xf_model* m, const char* path);
+XF_DLL int xf_model_load(xf_model** out, const char* path, int device);
+/* Forward pass over a CSR batch (row r = keys[row_ptr[r] .. row_ptr[r+1]), row_ptr non-decreasing and <= nnz);
+ * pctr_out[rows].  Rows of any length (none: sigmoid(0)) and rows == 0 are valid; there is no max_rows: the model's
+ * staging grows on demand.  _host refuses key 2^64 - 1 and a malformed row_ptr with XF_ERR_ARG, runs on the model's
+ * own stream and returns when pctr_out is filled; calls on one model are serialised.  _device takes device pointers
+ * on the model's device, is asynchronous on `cuda_stream` (cudaStream_t or NULL), reads nothing on the host and uses
+ * no state of the model but its rows, so any number may be in flight. */
+XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows,
+                                 uint32_t nnz, float* pctr_out);
+XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
+                                   uint32_t nnz, float* d_pctr_out, void* cuda_stream);
+/* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL */
+XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt,
+                           uint8_t* present);
+/* forward pass over rows [row_start, row_end) of a trainer's current ingested block, read from `m` instead of the
+ * trainer's table (same outputs as xf_trainer_predict_ingested; runs on the table's stream).  XF_ERR_ARG if the
+ * trainer's model is not LR / FM as the model is, or if the two live on different devices. */
+XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end,
+                                     float* pctr_out, uint8_t* labels_out);
+
 /* ------------------------------------------------------------------------------------------------
  * 1. Reference C API (src/c_api/c_api.h:26-29), unchanged signatures.
  *    XFCreate builds an LR worker on <train_path>-%05d / <test_path>-%05d (rank from XFLOW_RANK,

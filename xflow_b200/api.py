@@ -15,6 +15,7 @@ MODEL_LR, MODEL_FM, MODEL_FM_CANONICAL, MODEL_MVM = 0, 1, 2, 3
 OPT_FTRL, OPT_SGD = 0, 1
 VINIT_DEFAULT, VINIT_COUNTER, VINIT_ZERO = 0, 1, 3
 ADMIT_ALL, ADMIT_POISSON, ADMIT_BLOOM = 0, 1, 2
+ABSENT_DEFAULT, ABSENT_ZERO = 0, 1
 COMM_ID_BYTES = 128
 
 _lib = None
@@ -38,6 +39,16 @@ class AdmissionConfig(C.Structure):
 
 class EvictionConfig(C.Structure):
     _fields_ = [("max_idle_batches", C.c_uint64), ("max_keys", C.c_uint64)]
+
+
+class FreezeConfig(C.Structure):
+    _fields_ = [("absent", C.c_int), ("prune", C.c_int), ("device", C.c_int)]
+
+
+class ModelInfo(C.Structure):
+    _fields_ = [("keys", C.c_uint64), ("capacity", C.c_uint64), ("bytes", C.c_uint64), ("source_keys", C.c_uint64),
+                ("pruned_keys", C.c_uint64), ("row_bytes", C.c_uint32), ("latent_dim", C.c_int), ("optimizer", C.c_int),
+                ("absent", C.c_int), ("fm", C.c_int)]
 
 
 class TrainerConfig(C.Structure):
@@ -136,6 +147,16 @@ SIGNATURES = {
     "xf_comm_allreduce_max": (_i, [_vp, _vp]),
     "xf_comm_destroy": (_i, [_vp]),
     "xf_comm_barrier": (_i, [_vp]),
+    "xf_freeze_config_default": (_i, [_vp]),
+    "xf_table_freeze": (_i, [_vp, _vp, _vp]),
+    "xf_model_destroy": (_i, [_vp]),
+    "xf_model_get_info": (_i, [_vp, _vp]),
+    "xf_model_save": (_i, [_vp, C.c_char_p]),
+    "xf_model_load": (_i, [_vp, C.c_char_p, _i]),
+    "xf_model_predict_host": (_i, [_vp, _vp, _vp, _u32, _u32, _vp]),
+    "xf_model_predict_device": (_i, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
     "XFCreateEx": (_i, [_vp, C.c_char_p, C.c_char_p, _i, _i, _i, _i]),
@@ -399,6 +420,74 @@ class Table:
         out = np.empty(keys.size, np.uint64)
         _check(lib().xf_table_last_touch(self.h, _p(keys), keys.size, _p(out)))
         return out
+
+
+    def freeze(self, absent=None, prune=True, device=None):
+        """A serving Model of the table as it is now (xf_table_freeze); the table is not changed.  absent: ABSENT_DEFAULT
+        / ABSENT_ZERO, None = what the table's own predict does; device: None = the table's."""
+        cfg = FreezeConfig(-1 if absent is None else absent, 1 if prune else 0, -1 if device is None else device)
+        h = C.c_void_p()
+        _check(lib().xf_table_freeze(self.h, C.byref(cfg), C.byref(h)))
+        return Model(h)
+
+
+class Model:
+    """A frozen, read-only serving model (xf_model_*): made by Table.freeze or Model.load."""
+
+    def __init__(self, handle):
+        self.h = handle
+
+    @classmethod
+    def load(cls, path, device=0):
+        h = C.c_void_p()
+        _check(lib().xf_model_load(C.byref(h), path.encode(), device))
+        return cls(h)
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().xf_model_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def info(self):
+        i = ModelInfo()
+        _check(lib().xf_model_get_info(self.h, C.byref(i)))
+        return {k: getattr(i, k) for k, _ in ModelInfo._fields_}
+
+    def save(self, path):
+        _check(lib().xf_model_save(self.h, path.encode()))
+
+    def predict_host(self, row_ptr, keys):
+        row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
+        keys = np.ascontiguousarray(keys, np.uint64)
+        rows = row_ptr.size - 1
+        out = np.empty(rows, np.float32)
+        _check(lib().xf_model_predict_host(self.h, _p(row_ptr), _p(keys), rows, keys.size, _p(out)))
+        return out
+
+    def predict_device(self, d_row_ptr, d_keys, rows, nnz, d_out, stream=0):
+        """Asynchronous forward pass on device pointers (raw addresses) on the CUDA stream `stream`."""
+        _check(lib().xf_model_predict_device(self.h, _p(d_row_ptr), _p(d_keys), rows, nnz, _p(d_out),
+                                             C.c_void_p(int(stream)) if stream else None))
+
+    def lookup(self, keys):
+        """What the model holds for `keys`: dict of w, st, qt (0 for LR) and present."""
+        keys = np.ascontiguousarray(keys, np.uint64)
+        n = keys.size
+        out = dict(keys=keys, w=np.zeros(n, np.float32), st=np.zeros(n, np.float32), qt=np.zeros(n, np.float32),
+                   present=np.zeros(n, np.uint8))
+        _check(lib().xf_model_lookup(self.h, _p(keys), n, _p(out["w"]), _p(out["st"]), _p(out["qt"]), _p(out["present"])))
+        return out
+
+    def predict_ingested(self, trainer, row_start, row_end):
+        """Trainer.predict_ingested on the trainer's current ingested block, read from this model."""
+        n = row_end - row_start
+        p = np.empty(n, np.float32)
+        lab = np.empty(n, np.uint8)
+        _check(lib().xf_model_predict_ingested(self.h, trainer.h, row_start, row_end, _p(p), _p(lab)))
+        return p, lab
 
 
 class Comm:

@@ -27,7 +27,6 @@
 #include "internal.h"
 
 #define XF_ST_TILE 1024                     // slots per block of the pack kernels
-#define XF_ST_CHUNK_BYTES (64ull << 20)     // staging bytes per chunk: rows + one u64 per row
 #define XF_ST_VERSION 1u
 
 // The file header (little-endian, 232 bytes; the layout is documented in include/xflow_b200.h)
@@ -76,11 +75,7 @@ static_assert(offsetof(XfStateHeader, batches) == 112 && offsetof(XfStateHeader,
               "header layout");
 #define XF_ST_CHUNK_HEAD 32  // {u64 first_slot, u64 live rows, u64 checksum, u64 0}
 
-__host__ __device__ __forceinline__ uint64_t xf_st_hash(uint64_t word, uint64_t off) { return xf_splitmix64(word ^ off); }
-// offsets of a chunk's words: the chunk index above bit 40, the byte offset in the chunk's payload below
-__host__ __device__ __forceinline__ uint64_t xf_st_tag(uint64_t chunk) { return chunk << 40; }
-
-static uint64_t xf_st_host_sum(const void* p, uint64_t bytes, uint64_t off0) {
+uint64_t xf_st_host_sum(const void* p, uint64_t bytes, uint64_t off0) {
   const uint8_t* b = (const uint8_t*)p;
   uint64_t s = 0;
   for (uint64_t i = 0; i + 8 <= bytes; i += 8) {

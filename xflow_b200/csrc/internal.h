@@ -161,6 +161,15 @@ struct xf_trainer {
   size_t prof_used = 0;
 };
 
+// checkpoint.cu: the section checksum of the file formats (XFST state images, XFSM serving models) = the integer sum,
+// mod 2^64, of xf_st_hash(word, offset) over a section's 8-byte words; xf_st_host_sum sums `bytes` of host memory whose
+// first word has offset off0
+#define XF_ST_CHUNK_BYTES (64ull << 20)     // staging bytes per chunk of a file's rows section
+__host__ __device__ __forceinline__ uint64_t xf_st_hash(uint64_t word, uint64_t off) { return xf_splitmix64(word ^ off); }
+// offsets of a chunk's words: the chunk index above bit 40, the byte offset in the chunk's payload below
+__host__ __device__ __forceinline__ uint64_t xf_st_tag(uint64_t chunk) { return chunk << 40; }
+uint64_t xf_st_host_sum(const void* p, uint64_t bytes, uint64_t off0);
+
 // ingest.cu
 int xf_launch_parse(const char* d_text, uint64_t len, XfDevBuf& scratch, uint32_t* d_row_ptr, uint64_t* d_keys,
                     uint8_t* d_labels, uint32_t max_rows, uint32_t max_tok, uint32_t* d_totals, int* d_error,

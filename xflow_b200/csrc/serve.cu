@@ -1,0 +1,721 @@
+// Serving model: a trained table frozen for prediction only (layer 6 of include/xflow_b200.h, which documents the
+// semantics and the XFSM file format).
+//
+// A model row holds what the forward pass reads of a key and nothing else: LR {key, w} in 16 bytes, FM of any K
+// {key, w, st = sum_k v_k, qt = sum_k v_k^2} in one 32-byte sector (fm_worker.cc:177-196 collapses the interaction over
+// k, so a token contributes w, st and qt only, and in a frozen model they are constants).  The model is an
+// open-addressing table of such rows with the training table's hash and probe sequence (xf_probe_slot), described by an
+// XfTableView whose stride is the model's row size, so that the table's device functions serve both.
+//
+//   freeze   xf_k_freeze<COUNT>   one pass counts the rows kept, one inserts them (CAS on the key word); each resolves a
+//                                 row as a reader does: xf_apply_pending for w, xf_fm_token for st, qt
+//   predict  xf_k_serve<FM>       warp per row, two tokens per lane in flight, the mapping and the association of the
+//                                 step kernels' forward pass (step.cu, step_lazy.cu), so the result is theirs bit for bit;
+//                                 no insert, no atomics, no shared memory
+//   file     rows sorted by key (cub radix sort of (key, slot)), gathered a chunk at a time through bounded staging
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+#include <stdio.h>
+#include <string.h>
+
+#include <algorithm>
+#include <cub/cub.cuh>
+#include <mutex>
+#include <string>
+
+#include "internal.h"
+
+#define XF_SM_VERSION 1u
+#define XF_SM_CHUNK_HEAD 32  // {u64 first row, u64 rows, u64 checksum, u64 0}
+
+// The file header (little-endian, 104 bytes; the layout is documented in include/xflow_b200.h)
+struct XfModelHeader {
+  char magic[4];           //   0 "XFSM"
+  uint32_t version;        //   4
+  uint64_t header_bytes;   //   8
+  uint64_t keys;           //  16
+  uint64_t capacity;       //  24
+  uint32_t row_bytes;      //  32
+  int32_t fm;              //  36
+  int32_t latent_dim;      //  40
+  int32_t optimizer;       //  44
+  int32_t absent;          //  48
+  int32_t v_init;          //  52 resolved
+  float v_const;           //  56
+  uint32_t zero;           //  60
+  uint64_t seed;           //  64
+  uint64_t source_keys;    //  72
+  uint64_t pruned_keys;    //  80
+  uint64_t chunk_rows;     //  88
+  uint64_t header_checksum;  // 96 over bytes [0, 96)
+};
+static_assert(sizeof(XfModelHeader) == 104 && offsetof(XfModelHeader, seed) == 64 &&
+                  offsetof(XfModelHeader, header_checksum) == 96,
+              "the documented header is 104 bytes");
+
+struct xf_model {
+  XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source
+  int device = 0;
+  int fm = 0, absent = 0, optimizer = 0;
+  uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
+  cudaStream_t stream = nullptr;
+  // staging of the host entry points, grown on demand; those calls are serialised by the mutex
+  std::mutex mu;
+  XfDevBuf s_row_ptr, s_keys, s_out, s_aux;
+  XfPinBuf h_in, h_out;
+};
+
+// ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
+template <bool FM>
+__device__ __forceinline__ void xf_serve_load(const uint8_t* p, uint64_t& key, float& w, float& st, float& qt) {
+  uint64_t q0, q1, q2 = 0ull, q3 = 0ull;
+  if (FM) {
+    // one sector as two 128-bit loads by the same lane (sm_90 has no 256-bit load), issued back to back
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u64 {%2,%3}, [%4+16];"
+        : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+  } else {
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(q0), "=l"(q1) : "l"(p));
+  }
+  key = q0;
+  w = __uint_as_float((uint32_t)q1);
+  st = __uint_as_float((uint32_t)(q1 >> 32));
+  qt = __uint_as_float((uint32_t)q2);
+}
+
+// Find `key` from its home slot `s`, whose row the caller has loaded into (k, w, st, qt); false: the model does not
+// hold it.  The load is at most 0.5, so a chain ends at an empty slot long before XF_MAX_PROBE.
+template <bool FM>
+__device__ __forceinline__ bool xf_serve_find(const XfTableView& m, uint64_t key, uint64_t k, float& w, float& st, float& qt) {
+  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
+    if (k == key) return true;
+    if (k == XF_EMPTY_KEY) return false;
+    xf_serve_load<FM>(xf_row(m, xf_probe_slot(m, key, i)), k, w, st, qt);
+  }
+  return false;
+}
+
+// one token's terms into the lane's sums, in the order the step kernels add them
+template <bool FM>
+__device__ __forceinline__ void xf_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float w, float st,
+                                               float qt, float& wsum, float& ssum, float& qsum) {
+  if (!xf_serve_find<FM>(m, key, k, w, st, qt)) {
+    if (absent == XF_ABSENT_ZERO) return;
+    // the row the table would insert: w = 0 and, FM, a latent block that is not materialised
+    w = 0.f;
+    if (FM) xf_fm_token<1>(m, 0u, 0u, key, st, qt);
+  }
+  wsum += w;
+  if (FM) { ssum += st; qsum += qt; }
+}
+
+template <bool FM>
+__global__ void __launch_bounds__(256)
+xf_k_serve(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys, int B,
+           float* __restrict__ pctr_out) {
+  const int lane = threadIdx.x & 31;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
+  const int nwarps = gridDim.x * warps_per_block;
+  for (int row = gwarp; row < B; row += nwarps) {
+    const uint32_t beg = __ldg(row_ptr + row);
+    const uint32_t end = __ldg(row_ptr + row + 1);
+    const int chunks = (int)((end - beg + 63u) >> 6);
+    float wsum = 0.f, ssum = 0.f, qsum = 0.f;
+    for (int ch = 0; ch < chunks; ++ch) {
+      const uint32_t j0 = beg + (uint32_t)ch * 64u + (uint32_t)lane;
+      const uint32_t j1 = j0 + 32u;
+      const bool v0 = j0 < end, v1 = j1 < end;
+      const uint64_t k0 = v0 ? __ldcs(keys + j0) : 0ull;  // streaming: do not displace model rows in L2
+      const uint64_t k1 = v1 ? __ldcs(keys + j1) : 0ull;
+      // both first looks are in flight before either is resolved
+      uint64_t a = XF_EMPTY_KEY, b = XF_EMPTY_KEY;
+      float wa = 0.f, sa = 0.f, qa = 0.f, wb = 0.f, sb = 0.f, qb = 0.f;
+      if (v0) xf_serve_load<FM>(xf_row(m, xf_home_slot(m, k0)), a, wa, sa, qa);
+      if (v1) xf_serve_load<FM>(xf_row(m, xf_home_slot(m, k1)), b, wb, sb, qb);
+      if (v0) xf_serve_token<FM>(m, absent, k0, a, wa, sa, qa, wsum, ssum, qsum);
+      if (v1) xf_serve_token<FM>(m, absent, k1, b, wb, sb, qb, wsum, ssum, qsum);
+    }
+    const float wx = xf_warp_sum(wsum);
+    float arg = wx;
+    if (FM) {
+      const float S = xf_warp_sum(ssum);
+      const float Q = xf_warp_sum(qsum);
+      arg = __fadd_rn(wx, __fsub_rn(__fmul_rn(S, S), Q));  // fm_worker.cc:193-196
+    }
+    if (lane == 0) pctr_out[row] = xf_sigmoid(arg);
+  }
+}
+
+static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, float* pctr_out,
+                            cudaStream_t st) {
+  if (rows == 0) return;
+  const int grid = xf_grid_for((uint64_t)rows * 32, 256, 8);
+  if (m->fm) xf_k_serve<true><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
+  else xf_k_serve<false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
+}
+
+// ---- building a model's table
+__global__ void xf_k_model_fill(uint4* base, uint64_t chunks16, uint32_t per_row) {
+  for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < chunks16; c += (uint64_t)gridDim.x * blockDim.x)
+    base[c] = (c % per_row == 0) ? make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u) : make_uint4(0u, 0u, 0u, 0u);
+}
+
+// claim a slot for `key` (unique among the inserted keys) and write its row; a probe overflow or a key met twice sets *error
+__device__ __forceinline__ void xf_model_insert(const XfTableView& m, uint64_t key, float w, float st, float qt, int* error) {
+  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
+    uint8_t* rowp = xf_row(m, xf_probe_slot(m, key, i));
+    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(rowp), (unsigned long long)XF_EMPTY_KEY,
+                                             (unsigned long long)key);
+    if (old == XF_EMPTY_KEY) {
+      if (m.K > 0) {
+        *reinterpret_cast<float2*>(rowp + 8) = make_float2(w, st);
+        *reinterpret_cast<float*>(rowp + 16) = qt;
+      } else {
+        *reinterpret_cast<float*>(rowp + 8) = w;
+      }
+      return;
+    }
+    if (old == key) break;
+  }
+  *error = 1;
+}
+
+// Slot r of the training table as a reader resolves it, and whether the model keeps it.  COUNT: count the rows kept
+// and the live rows; else insert the rows kept into `m`.
+template <bool COUNT, int VEC>
+__global__ void __launch_bounds__(256)
+xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, unsigned long long* __restrict__ counts, int* error) {
+  const uint64_t cap = t.mask + 1;
+  unsigned int kept_n = 0, live_n = 0;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    XfHead h = xf_load_head(xf_row(t, r));
+    if (h.key == XF_EMPTY_KEY) continue;
+    ++live_n;
+    const uint32_t flags = t.lazy ? 0u : h.flags;  // a lazy (LR) row keeps a batch tag there
+    xf_apply_pending(t, h);
+    float st = 0.f, qt = 0.f;
+    if (t.K > 0) xf_fm_token<VEC>(t, (uint32_t)r, flags, h.key, st, qt);
+    bool keep = true;
+    if (prune && h.w == 0.0f)
+      keep = t.K > 0 && (absent == XF_ABSENT_DEFAULT ? (flags & XF_FLAG_V_READY) != 0u : !(st == 0.0f && qt == 0.0f));
+    if (!keep) continue;
+    ++kept_n;
+    if (!COUNT) xf_model_insert(m, h.key, h.w, st, qt, error);
+  }
+  if (COUNT) {
+    kept_n = __reduce_add_sync(0xffffffffu, kept_n);
+    live_n = __reduce_add_sync(0xffffffffu, live_n);
+    if ((threadIdx.x & 31u) == 0u) {
+      if (kept_n) atomicAdd(counts, (unsigned long long)kept_n);
+      if (live_n) atomicAdd(counts + 1, (unsigned long long)live_n);
+    }
+  }
+}
+
+// insert n packed rows (a chunk of a model file) into `m`
+__global__ void xf_k_model_insert_rows(XfTableView m, const uint8_t* __restrict__ rows, uint64_t n, int* error) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* p = rows + i * m.stride;
+    const uint64_t key = *reinterpret_cast<const uint64_t*>(p);
+    const float w = *reinterpret_cast<const float*>(p + 8);
+    float st = 0.f, qt = 0.f;
+    if (m.K > 0) { st = *reinterpret_cast<const float*>(p + 12); qt = *reinterpret_cast<const float*>(p + 16); }
+    xf_model_insert(m, key, w, st, qt, error);
+  }
+}
+
+// every (key, slot) the model holds, in no particular order
+__global__ void xf_k_model_list(XfTableView m, uint64_t* keys_out, uint32_t* slots_out, unsigned long long* count) {
+  const uint64_t cap = m.mask + 1;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = *reinterpret_cast<const uint64_t*>(xf_row(m, r));
+    if (key == XF_EMPTY_KEY) continue;
+    const unsigned long long idx = atomicAdd(count, 1ull);
+    keys_out[idx] = key;
+    slots_out[idx] = (uint32_t)r;
+  }
+}
+
+// out = the rows in slots[0 .. n), packed, 16 bytes per thread and access
+__global__ void xf_k_model_gather(XfTableView m, const uint32_t* __restrict__ slots, uint64_t n, uint4* __restrict__ out) {
+  const uint32_t q = m.stride / 16u;
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n * q; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t i = j / q;
+    out[j] = *reinterpret_cast<const uint4*>(xf_row(m, slots[i]) + 16u * (uint32_t)(j - i * q));
+  }
+}
+
+__global__ void xf_k_model_lookup(XfTableView m, const uint64_t* __restrict__ keys, uint64_t n, float* w_out, float* st_out,
+                                  float* qt_out, uint8_t* present) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = keys[i];
+    uint64_t k;
+    float w, st, qt;
+    bool have;
+    if (m.K > 0) {
+      xf_serve_load<true>(xf_row(m, xf_home_slot(m, key)), k, w, st, qt);
+      have = xf_serve_find<true>(m, key, k, w, st, qt);
+    } else {
+      xf_serve_load<false>(xf_row(m, xf_home_slot(m, key)), k, w, st, qt);
+      have = xf_serve_find<false>(m, key, k, w, st, qt);
+      st = qt = 0.f;
+    }
+    w_out[i] = have ? w : 0.f;
+    st_out[i] = have ? st : 0.f;
+    qt_out[i] = have ? qt : 0.f;
+    present[i] = have ? 1 : 0;
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
+// host side
+// -------------------------------------------------------------------------------------------------
+static uint64_t xf_model_capacity(uint64_t keys) {
+  uint64_t c = 1024;
+  while (c < 2 * keys) c <<= 1;
+  return c;
+}
+
+// the model's table on the current device: `capacity` empty rows
+static int xf_model_alloc(xf_model* m, uint64_t capacity) {
+  if (capacity > (1ull << 32)) {
+    xf_set_error("a serving model of %llu slots exceeds 2^32", (unsigned long long)capacity);
+    return XF_ERR_FULL;
+  }
+  const uint32_t stride = m->fm ? 32u : 16u;
+  uint8_t* base = nullptr;
+  XF_CUDA_TRY(cudaMalloc(&base, capacity * stride));
+  m->view.base = base;
+  m->view.mask = capacity - 1;
+  uint32_t lg = 0;
+  while ((1ull << lg) < capacity) ++lg;
+  m->view.log2cap = lg;
+  m->view.stride = stride;
+  m->view.bshift = xf_bucket_shift(stride, lg);
+  const uint64_t chunks16 = capacity * (stride / 16u);
+  xf_k_model_fill<<<xf_grid_for(chunks16, 256, 16), 256, 0, m->stream>>>(reinterpret_cast<uint4*>(base), chunks16, stride / 16u);
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
+}
+
+static void xf_model_free(xf_model* m) {
+  if (!m) return;
+  cudaSetDevice(m->device);
+  if (m->stream) cudaStreamSynchronize(m->stream);
+  if (m->view.base) cudaFree(m->view.base);
+  m->s_row_ptr.release(); m->s_keys.release(); m->s_out.release(); m->s_aux.release();
+  m->h_in.release(); m->h_out.release();
+  if (m->stream) cudaStreamDestroy(m->stream);
+  delete m;
+}
+
+XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
+  if (!cfg) return XF_ERR_ARG;
+  cfg->absent = -1;
+  cfg->prune = 1;
+  cfg->device = -1;
+  return XF_OK;
+}
+
+// the body of xf_table_freeze: on failure the caller frees `m`
+static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, xf_model* m) {
+  const int src_dev = t->cfg.device;
+  XF_CUDA_TRY(cudaSetDevice(src_dev));
+  XF_TRY(t->check_error());  // waits for everything enqueued on the table's stream
+  m->device = src_dev;
+  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  const XfTableView& tv = t->view;
+  m->fm = tv.K > 0;
+  m->optimizer = tv.opt;
+  m->absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
+  m->view.K = tv.K;
+  m->view.opt = tv.opt;
+  m->view.v_init = tv.v_init;
+  m->view.v_const = tv.v_const;
+  m->view.seed = tv.seed;
+  // the build runs on the model's stream: the table's stream is idle (above) and the host calls on the table are
+  // locked out by the caller, so nothing writes the table while it is read
+  cudaStream_t st = m->stream;
+  unsigned long long* d_counts = nullptr;  // {kept, live, error flag}
+  XF_CUDA_TRY(cudaMalloc(&d_counts, 3 * sizeof(unsigned long long)));
+  struct Free { void* p; ~Free() { cudaFree(p); } } free_counts{d_counts};
+  XF_CUDA_TRY(cudaMemsetAsync(d_counts, 0, 3 * sizeof(unsigned long long), st));
+  int* d_error = reinterpret_cast<int*>(d_counts + 2);
+  const int grid = xf_grid_for(tv.mask + 1, 256, 8);
+  const int prune = cfg.prune ? 1 : 0;
+#define XF_FREEZE_LAUNCH(COUNT)                                                                               \
+  switch (xf_vec_for(tv.K)) {                                                                                 \
+    case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
+    case 2: xf_k_freeze<COUNT, 2><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
+    default: xf_k_freeze<COUNT, 1><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
+  }
+  XF_FREEZE_LAUNCH(true)
+  XF_CUDA_TRY(cudaGetLastError());
+  unsigned long long counts[3] = {0, 0, 0};
+  XF_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  m->keys = counts[0];
+  m->source_keys = counts[1];
+  m->pruned_keys = counts[1] - counts[0];
+  XF_TRY(xf_model_alloc(m, xf_model_capacity(m->keys)));
+  XF_FREEZE_LAUNCH(false)
+#undef XF_FREEZE_LAUNCH
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  if ((int)counts[2] != 0) {
+    xf_set_error("xf_table_freeze: a probe sequence of the model overflowed");
+    return XF_ERR_FULL;
+  }
+  if (cfg.device >= 0 && cfg.device != src_dev) {
+    // the model lives on another device: copy its table there
+    const uint64_t bytes = (m->view.mask + 1) * (uint64_t)m->view.stride;
+    uint8_t* src = m->view.base;
+    XF_CUDA_TRY(cudaStreamDestroy(m->stream));
+    m->stream = nullptr;
+    XF_CUDA_TRY(cudaSetDevice(cfg.device));
+    uint8_t* dst = nullptr;
+    XF_CUDA_TRY(cudaMalloc(&dst, bytes));
+    m->view.base = dst;
+    m->device = cfg.device;
+    const cudaError_t e = cudaMemcpyPeer(dst, cfg.device, src, src_dev, bytes);
+    cudaSetDevice(src_dev);
+    cudaFree(src);
+    XF_CUDA_TRY(e);
+    XF_CUDA_TRY(cudaSetDevice(cfg.device));
+    XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg_in, xf_model** out) {
+  if (out) *out = nullptr;
+  if (!t || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  xf_freeze_config cfg;
+  xf_freeze_config_default(&cfg);
+  if (cfg_in) cfg = *cfg_in;
+  if (cfg.absent < -1 || cfg.absent > XF_ABSENT_ZERO) { xf_set_error("xf_table_freeze: absent = %d is not an XF_ABSENT_* policy", cfg.absent); return XF_ERR_ARG; }
+  if (cfg.device >= xf_device_count()) { xf_set_error("xf_table_freeze: no CUDA device %d", cfg.device); return XF_ERR_ARG; }
+  if (t->cfg.canonical_fm) {
+    xf_set_error("xf_table_freeze: a canonical table (canonical_fm = 1) has no serving model: the per-k sums of the canonical "
+                 "FM and the multi-view machine do not collapse to one pair of sums per key");
+    return XF_ERR_ARG;
+  }
+  if (t->cfg.num_shards > 1) {
+    xf_set_error("xf_table_freeze: the table is shard %d of %d: one shard's rows are not a model", t->cfg.shard_index,
+                 t->cfg.num_shards);
+    return XF_ERR_ARG;
+  }
+  std::lock_guard<std::mutex> host_lock(t->host_mu);
+  xf_model* m = new xf_model;
+  const int rc = xf_freeze_into(t, cfg, m);
+  if (rc != XF_OK) { xf_model_free(m); return rc; }
+  *out = m;
+  return XF_OK;
+}
+
+XF_DLL int xf_model_destroy(xf_model* m) {
+  xf_model_free(m);
+  return XF_OK;
+}
+
+XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out) {
+  if (!m || !out) return XF_ERR_ARG;
+  memset(out, 0, sizeof(*out));
+  out->keys = m->keys;
+  out->capacity = m->view.mask + 1;
+  out->bytes = out->capacity * m->view.stride;
+  out->source_keys = m->source_keys;
+  out->pruned_keys = m->pruned_keys;
+  out->row_bytes = m->view.stride;
+  out->latent_dim = m->view.K;
+  out->optimizer = m->optimizer;
+  out->absent = m->absent;
+  out->fm = m->fm;
+  return XF_OK;
+}
+
+// ---- predict
+// stage `bytes` of pageable host memory into `dev` through the pinned buffer at offset `off` (the model's stream)
+static int xf_model_stage(xf_model* m, XfDevBuf& dev, size_t off, const void* src, size_t bytes) {
+  XF_TRY(dev.ensure(std::max<size_t>(bytes, 16)));
+  if (bytes == 0) return XF_OK;
+  memcpy((uint8_t*)m->h_in.p + off, src, bytes);
+  XF_CUDA_TRY(cudaMemcpyAsync(dev.p, (uint8_t*)m->h_in.p + off, bytes, cudaMemcpyHostToDevice, m->stream));
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, uint32_t nnz,
+                                 float* pctr_out) {
+  if (!m || !row_ptr || (!keys && nnz) || (!pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  for (uint32_t r = 0; r < rows; ++r)
+    if (row_ptr[r] > row_ptr[r + 1]) { xf_set_error("xf_model_predict_host: row_ptr decreases at row %u", r); return XF_ERR_ARG; }
+  if (row_ptr[rows] > nnz) { xf_set_error("xf_model_predict_host: row_ptr ends at %u, past nnz = %u", row_ptr[rows], nnz); return XF_ERR_ARG; }
+  XF_TRY(xf_check_host_keys(keys, nnz, "xf_model_predict_host"));
+  if (rows == 0) return XF_OK;
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  const size_t rp_bytes = ((size_t)rows + 1) * 4, rp_pad = (rp_bytes + 15) & ~(size_t)15, key_bytes = (size_t)nnz * 8;
+  XF_TRY(m->h_in.ensure(rp_pad + key_bytes));
+  XF_TRY(m->h_out.ensure((size_t)rows * 4));
+  XF_TRY(m->s_out.ensure((size_t)rows * 4));
+  XF_TRY(xf_model_stage(m, m->s_row_ptr, 0, row_ptr, rp_bytes));
+  XF_TRY(xf_model_stage(m, m->s_keys, rp_pad, keys, key_bytes));
+  xf_launch_serve(m, m->s_row_ptr.as<uint32_t>(), m->s_keys.as<uint64_t>(), rows, m->s_out.as<float>(), m->stream);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_out.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, m->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
+  memcpy(pctr_out, m->h_out.p, (size_t)rows * 4);
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
+                                   uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
+  if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  xf_launch_serve(m, d_row_ptr, d_keys, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
+                                     uint8_t* labels_out) {
+  if (!m || !tr) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (tr->cfg.model != (m->fm ? XF_MODEL_FM : XF_MODEL_LR)) {
+    xf_set_error("xf_model_predict_ingested: the trainer's model (%d) is not the serving model's (%s)", tr->cfg.model,
+                 m->fm ? "FM" : "LR");
+    return XF_ERR_ARG;
+  }
+  if (tr->table->cfg.device != m->device) {
+    xf_set_error("xf_model_predict_ingested: the trainer's block is on device %d, the model on device %d",
+                 tr->table->cfg.device, m->device);
+    return XF_ERR_ARG;
+  }
+  XF_TRY(xf_ingested_range(tr, row_start, row_end));
+  const uint32_t rows = row_end - row_start;
+  if (rows == 0) return XF_OK;
+  if (!pctr_out) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  xf_trainer::IngestSet& g = tr->ing[tr->ing_cur];
+  cudaStream_t st = tr->table->stream;  // the block's parse is ordered before this stream's work
+  XF_TRY(m->s_out.ensure((size_t)rows * 4));
+  // row_ptr holds absolute token offsets: a slice is a shifted row_ptr
+  xf_launch_serve(m, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(), rows, m->s_out.as<float>(), st);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, m->s_out.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
+  if (labels_out) XF_CUDA_TRY(cudaMemcpyAsync(labels_out, g.labels.as<uint8_t>() + row_start, rows, cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaEventRecord(g.consumed, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  return XF_OK;
+}
+
+XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt, uint8_t* present) {
+  if (!m || (!keys && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup"));
+  if (n == 0) return XF_OK;
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  XF_TRY(m->s_keys.ensure(n * 8));
+  XF_TRY(m->s_aux.ensure(n * 13));  // w[n] st[n] qt[n] present[n]
+  float* d_w = m->s_aux.as<float>();
+  uint8_t* d_present = reinterpret_cast<uint8_t*>(d_w + 3 * n);
+  XF_CUDA_TRY(cudaMemcpyAsync(m->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, m->stream));
+  xf_k_model_lookup<<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w, d_w + n, d_w + 2 * n,
+                                                                  d_present);
+  XF_CUDA_TRY(cudaGetLastError());
+  if (w) XF_CUDA_TRY(cudaMemcpyAsync(w, d_w, n * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (st) XF_CUDA_TRY(cudaMemcpyAsync(st, d_w + n, n * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (qt) XF_CUDA_TRY(cudaMemcpyAsync(qt, d_w + 2 * n, n * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (present) XF_CUDA_TRY(cudaMemcpyAsync(present, d_present, n, cudaMemcpyDeviceToHost, m->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
+  return XF_OK;
+}
+
+// ---- file
+static bool xf_sm_write(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
+static bool xf_sm_read(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
+
+static int xf_sm_save_body(xf_model* m, FILE* f, const char* path) {
+  XfModelHeader h;
+  memset(&h, 0, sizeof(h));
+  memcpy(h.magic, "XFSM", 4);
+  h.version = XF_SM_VERSION;
+  h.header_bytes = sizeof(h);
+  h.keys = m->keys;
+  h.capacity = m->view.mask + 1;
+  h.row_bytes = m->view.stride;
+  h.fm = m->fm;
+  h.latent_dim = m->view.K;
+  h.optimizer = m->optimizer;
+  h.absent = m->absent;
+  h.v_init = m->view.v_init;
+  h.v_const = m->view.v_const;
+  h.seed = m->view.seed;
+  h.source_keys = m->source_keys;
+  h.pruned_keys = m->pruned_keys;
+  h.chunk_rows = XF_ST_CHUNK_BYTES / h.row_bytes;
+  h.header_checksum = xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0);
+  if (!xf_sm_write(f, &h, sizeof(h))) { xf_set_error("write to %s failed", path); return XF_ERR_IO; }
+  const uint64_t n = m->keys;
+  if (n == 0) return XF_OK;
+  // (key, slot) of every row, sorted by key on the device
+  cudaStream_t st = m->stream;
+  XfDevBuf keys_in, keys_out, slots_in, slots_out, tmp, rows, count;
+  struct Release { XfDevBuf* b[7]; ~Release() { for (XfDevBuf* x : b) x->release(); } }
+      rel{{&keys_in, &keys_out, &slots_in, &slots_out, &tmp, &rows, &count}};
+  XF_TRY(keys_in.ensure(n * 8)); XF_TRY(keys_out.ensure(n * 8));
+  XF_TRY(slots_in.ensure(n * 4)); XF_TRY(slots_out.ensure(n * 4));
+  XF_TRY(count.ensure(8));
+  XF_CUDA_TRY(cudaMemsetAsync(count.p, 0, 8, st));
+  xf_k_model_list<<<xf_grid_for(h.capacity, 256, 8), 256, 0, st>>>(m->view, keys_in.as<uint64_t>(), slots_in.as<uint32_t>(),
+                                                                  count.as<unsigned long long>());
+  XF_CUDA_TRY(cudaGetLastError());
+  size_t tb = 0;
+  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys_in.as<uint64_t>(), keys_out.as<uint64_t>(), slots_in.as<uint32_t>(),
+                                              slots_out.as<uint32_t>(), n, 0, 64, st));
+  XF_TRY(tmp.ensure(std::max<size_t>(tb, 16)));
+  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys_in.as<uint64_t>(), keys_out.as<uint64_t>(), slots_in.as<uint32_t>(),
+                                              slots_out.as<uint32_t>(), n, 0, 64, st));
+  // the rows in that order, a chunk at a time: gathered on the device, copied to the pinned buffer, summed and written
+  const uint64_t C = std::min<uint64_t>(h.chunk_rows, n);
+  XF_TRY(rows.ensure(C * h.row_bytes));
+  XF_TRY(m->h_out.ensure(C * h.row_bytes));
+  for (uint64_t first = 0, chunk = 0; first < n; first += h.chunk_rows, ++chunk) {
+    const uint64_t c = std::min<uint64_t>(h.chunk_rows, n - first);
+    xf_k_model_gather<<<xf_grid_for(c * (h.row_bytes / 16u), 256, 8), 256, 0, st>>>(m->view, slots_out.as<uint32_t>() + first, c,
+                                                                                     rows.as<uint4>());
+    XF_CUDA_TRY(cudaGetLastError());
+    XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, rows.p, c * h.row_bytes, cudaMemcpyDeviceToHost, st));
+    XF_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint64_t head[4] = {first, c, xf_st_host_sum(m->h_out.p, c * h.row_bytes, xf_st_tag(chunk)), 0ull};
+    if (!xf_sm_write(f, head, sizeof(head)) || !xf_sm_write(f, m->h_out.p, c * h.row_bytes)) {
+      xf_set_error("write to %s failed", path);
+      return XF_ERR_IO;
+    }
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_save(xf_model* m, const char* path) {
+  if (!m || !path) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  // written under a temporary name and renamed, as xf_table_save does
+  const std::string tmp = std::string(path) + ".tmp";
+  FILE* f = fopen(tmp.c_str(), "wb");
+  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
+  int rc = xf_sm_save_body(m, f, tmp.c_str());
+  if (fclose(f) != 0 && rc == XF_OK) { xf_set_error("write to %s failed", tmp.c_str()); rc = XF_ERR_IO; }
+  if (rc == XF_OK && rename(tmp.c_str(), path) != 0) { xf_set_error("cannot rename %s to %s", tmp.c_str(), path); rc = XF_ERR_IO; }
+  if (rc != XF_OK) remove(tmp.c_str());
+  return rc;
+}
+
+// the header's own consistency (after its checksum): every size derived from it is bounded before it is used
+static bool xf_sm_header_sane(const XfModelHeader& h) {
+  if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) return false;
+  if (h.keys > (1ull << 31) || h.capacity != xf_model_capacity(h.keys) || h.keys + h.pruned_keys != h.source_keys) return false;
+  if (h.absent != XF_ABSENT_DEFAULT && h.absent != XF_ABSENT_ZERO) return false;
+  if (h.optimizer != XF_OPT_FTRL && h.optimizer != XF_OPT_SGD) return false;
+  if (h.v_init != 0 && h.v_init != XF_INIT_COUNTER && h.v_init != XF_INIT_ZERO) return false;
+  return h.chunk_rows == XF_ST_CHUNK_BYTES / h.row_bytes && h.zero == 0;
+}
+
+static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModelHeader& h) {
+  const uint64_t nch = (h.keys + h.chunk_rows - 1) / h.chunk_rows;
+  const uint64_t expect = sizeof(XfModelHeader) + nch * XF_SM_CHUNK_HEAD + h.keys * h.row_bytes;
+  if (fseek(f, 0, SEEK_END) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  const long fsz = ftell(f);
+  if (fsz < 0 || (uint64_t)fsz != expect) {
+    xf_set_error("corrupt or truncated model file %s: %ld bytes, its header announces %llu", path, fsz, (unsigned long long)expect);
+    return XF_ERR_IO;
+  }
+  if (fseek(f, sizeof(XfModelHeader), SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  m->fm = h.fm;
+  m->absent = h.absent;
+  m->optimizer = h.optimizer;
+  m->keys = h.keys;
+  m->source_keys = h.source_keys;
+  m->pruned_keys = h.pruned_keys;
+  m->view.K = h.latent_dim;
+  m->view.opt = h.optimizer;
+  m->view.v_init = h.v_init;
+  m->view.v_const = h.v_const;
+  m->view.seed = h.seed;
+  XF_TRY(xf_model_alloc(m, h.capacity));
+  if (h.keys == 0) { XF_CUDA_TRY(cudaStreamSynchronize(m->stream)); return XF_OK; }
+  const uint64_t C = std::min<uint64_t>(h.chunk_rows, h.keys);
+  XfDevBuf rows, err;
+  struct Release { XfDevBuf* b[2]; ~Release() { for (XfDevBuf* x : b) x->release(); } } rel{{&rows, &err}};
+  XF_TRY(rows.ensure(C * h.row_bytes));
+  XF_TRY(err.ensure(4));
+  XF_TRY(m->h_in.ensure(C * h.row_bytes));
+  XF_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, m->stream));
+  uint64_t prev = 0;
+  for (uint64_t i = 0, first = 0; i < nch; ++i) {
+    const uint64_t c = std::min<uint64_t>(h.chunk_rows, h.keys - first);
+    uint64_t head[4];
+    if (!xf_sm_read(f, head, sizeof(head)) || !xf_sm_read(f, m->h_in.p, c * h.row_bytes)) { xf_set_error("truncated model file %s", path); return XF_ERR_IO; }
+    if (head[0] != first || head[1] != c || head[3] != 0 || head[2] != xf_st_host_sum(m->h_in.p, c * h.row_bytes, xf_st_tag(i))) {
+      xf_set_error("model file %s: chunk %llu of the rows is damaged (checksum mismatch)", path, (unsigned long long)i);
+      return XF_ERR_IO;
+    }
+    // the keys ascend strictly: none twice, none the empty-slot marker but possibly the last
+    for (uint64_t r = 0; r < c; ++r) {
+      uint64_t key;
+      memcpy(&key, (const uint8_t*)m->h_in.p + r * h.row_bytes, 8);
+      if ((first + r > 0 && key <= prev) || key == XF_EMPTY_KEY) {
+        xf_set_error("model file %s: the keys of chunk %llu are not in ascending order", path, (unsigned long long)i);
+        return XF_ERR_IO;
+      }
+      prev = key;
+    }
+    XF_CUDA_TRY(cudaMemcpyAsync(rows.p, m->h_in.p, c * h.row_bytes, cudaMemcpyHostToDevice, m->stream));
+    xf_k_model_insert_rows<<<xf_grid_for(c, 256, 8), 256, 0, m->stream>>>(m->view, rows.as<uint8_t>(), c, err.as<int>());
+    XF_CUDA_TRY(cudaGetLastError());
+    XF_CUDA_TRY(cudaStreamSynchronize(m->stream));  // the pinned buffer is read again for the next chunk
+    first += c;
+  }
+  int e = 0;
+  XF_CUDA_TRY(cudaMemcpy(&e, err.p, 4, cudaMemcpyDeviceToHost));
+  if (e) { xf_set_error("model file %s: a probe sequence of the model overflowed", path); return XF_ERR_IO; }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
+  if (out) *out = nullptr;
+  if (!out || !path) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (device < 0 || device >= xf_device_count()) { xf_set_error("xf_model_load: no CUDA device %d", device); return XF_ERR_CUDA; }
+  FILE* f = fopen(path, "rb");
+  if (!f) { xf_set_error("cannot open %s", path); return XF_ERR_IO; }
+  XfModelHeader h;
+  memset(&h, 0, sizeof(h));
+  const size_t got = fread(&h, 1, sizeof(h), f);
+  int rc = XF_OK;
+  if (got >= 4 && (memcmp(h.magic, "XFTB", 4) == 0 || memcmp(h.magic, "XFST", 4) == 0)) {
+    xf_set_error("%s is a training checkpoint (%.4s), not a serving model: load it into a table and freeze that", path, h.magic);
+    rc = XF_ERR_IO;
+  } else if (got < 4 || memcmp(h.magic, "XFSM", 4) != 0) {
+    xf_set_error("%s is not a serving model (no XFSM magic)", path);
+    rc = XF_ERR_IO;
+  } else if (got != sizeof(h) || h.header_bytes != sizeof(h) || h.version != XF_SM_VERSION) {
+    xf_set_error("model file %s: truncated header or unknown version %u", path, h.version);
+    rc = XF_ERR_IO;
+  } else if (h.header_checksum != xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0) || !xf_sm_header_sane(h)) {
+    xf_set_error("model file %s: the header is damaged (checksum mismatch)", path);
+    rc = XF_ERR_IO;
+  }
+  xf_model* m = nullptr;
+  if (rc == XF_OK) {
+    m = new xf_model;
+    m->device = device;
+    rc = cudaSetDevice(device) == cudaSuccess ? xf_sm_load_body(m, f, path, h) : XF_ERR_CUDA;
+  }
+  fclose(f);
+  if (rc != XF_OK) { xf_model_free(m); return rc; }
+  *out = m;
+  return XF_OK;
+}

@@ -339,6 +339,48 @@ __device__ __forceinline__ void xf_ld8_l1(const float* p, float (&o)[8]) {
   o[6] = __uint_as_float((uint32_t)q3); o[7] = __uint_as_float((uint32_t)(q3 >> 32));
 }
 
+template <int VEC>
+__device__ __forceinline__ void xf_ldv_step(const float* p, float (&o)[VEC]) {
+  // through L1: v does not change during the step kernel (see xf_load_head_l1), hot rows stay SM-local
+  if (VEC == 4) { float4 t = __ldca(reinterpret_cast<const float4*>(p)); o[0] = t.x; o[1 % VEC] = t.y; o[2 % VEC] = t.z; o[3 % VEC] = t.w; }
+  else if (VEC == 2) { float2 t = __ldca(reinterpret_cast<const float2*>(p)); o[0] = t.x; o[1 % VEC] = t.y; }
+  else { o[0] = __ldca(p); }
+}
+// FM: (sum_k v, sum_k v^2) of one token's latent row  (fm_worker.cc:178-192, per-token part).  The step kernels
+// (step.cu) and the freeze of a serving model (serve.cu) both reduce a row through this one function, so that a
+// frozen row holds, bit for bit, what the forward pass computes.
+template <int VEC>
+__device__ __forceinline__ void xf_fm_token(const XfTableView& t, uint32_t slot, uint32_t flags, uint64_t key,
+                                            float& st, float& qt) {
+  const int K = t.K;
+  st = 0.f;
+  qt = 0.f;
+  if ((flags & XF_FLAG_V_READY) && (K & 7) == 0) {
+    // a sector at a time (the row starts 32-byte aligned)
+    const float* vp = reinterpret_cast<const float*>(xf_row(t, slot) + 32);
+    for (int k = 0; k < K; k += 8) {
+      float v[8];
+      xf_ld8_l1(vp + k, v);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { st += v[e]; qt = __fadd_rn(qt, __fmul_rn(v[e], v[e])); }
+    }
+  } else if (flags & XF_FLAG_V_READY) {
+    const float* vp = reinterpret_cast<const float*>(xf_row(t, slot) + 32);
+    for (int k = 0; k < K; k += VEC) {
+      float v[VEC];
+      xf_ldv_step<VEC>(vp + k, v);
+#pragma unroll
+      for (int e = 0; e < VEC; ++e) { st += v[e]; qt = __fadd_rn(qt, __fmul_rn(v[e], v[e])); }
+    }
+  } else {
+    for (int k = 0; k < K; ++k) {
+      const float v = xf_v_init(t, key, (uint32_t)k);
+      st += v;
+      qt = __fadd_rn(qt, __fmul_rn(v, v));
+    }
+  }
+}
+
 // full-sector store of the head
 __device__ __forceinline__ void xf_store_head(uint8_t* row, const XfHead& h) {
   const uint64_t q1 = (uint64_t)__double_as_longlong(h.g);

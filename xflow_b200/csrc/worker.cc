@@ -213,6 +213,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   NegSampleFromEnv(world_);         // and XFLOW_NEG_SAMPLE
   env_path("XFLOW_CHECKPOINT", world_);
   env_path("XFLOW_RESUME", world_);
+  env_path("XFLOW_EXPORT_MODEL", world_);
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -641,6 +642,16 @@ void WorkerBase::train() {
   if (rank == 0) {
     std::cout << model_name() << " AUC: " << std::endl;
     predict(rank, 0);
+    // XFLOW_EXPORT_MODEL = <path>: the trained table frozen into a serving model (xf_table_freeze, the defaults) and
+    // written there; the keys the predict above inserted read as absent keys and are pruned
+    const std::string export_model = env_path("XFLOW_EXPORT_MODEL", 1);
+    if (!export_model.empty()) {
+      xf_model* m = nullptr;
+      must(xf_table_freeze(table_, nullptr, &m), "xf_table_freeze");
+      const int rc = xf_model_save(m, export_model.c_str());
+      xf_model_destroy(m);
+      must(rc, "xf_model_save");
+    }
   } else if (comm_) {
     predict(rank, 0);  // takes part in rank 0's collective forward steps; feeds and prints nothing
   }
