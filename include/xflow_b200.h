@@ -20,6 +20,7 @@
  *                                            (ps-lite kv_app.h:405-460, postoffice.cc:134-143)
  *   6. serving model          xf_model_*   = a trained table frozen for prediction only (no reference counterpart:
  *                                            the reference predicts on its training servers, lr_worker.cc:25-77)
+ *   7. serving model deltas   xf_model_diff / _apply_delta, xf_delta_* = one model carried to the next
  */
 #ifndef XFLOW_B200_H_
 #define XFLOW_B200_H_
@@ -593,6 +594,74 @@ XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float*
  * trainer's model is not LR / FM as the model is, or if the two live on different devices. */
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end,
                                      float* pctr_out, uint8_t* labels_out);
+
+/* ------------------------------------------------------------------------------------------------
+ * 7. Serving model deltas (csrc/delta.cu).  A training run that keeps learning exports models one after another; a
+ *    delta carries one model to the next without shipping and reloading the whole of it.
+ *
+ *    The delta from model A to model B:
+ *      upserts  the rows of B whose key A does not hold, or whose row differs from A's in any byte (a row is 16
+ *               bytes for LR and 32 for FM, padding included), sorted by key;
+ *      deletes  the keys of A that B does not hold, sorted by key;
+ *      header   what XFSM records of B: keys, source_keys and pruned_keys.
+ *    Applying it to A builds a new model whose contents and info are B's, so that xf_model_save of the result is
+ *    byte-identical to xf_model_save(B) and every xf_model_predict_* returns on it, bit for bit, what it returns on B.
+ *
+ *    Fingerprint.  An order-free u64 of a model's contents: the sum mod 2^64 over its rows of h(row), where for the
+ *    row's 8-byte little-endian words w_0 .. w_{n-1} (n = 2 for LR, 4 for FM) h_0 = 0, h_{i+1} = splitmix64(h_i ^ w_i)
+ *    and h(row) = h_n.  The empty model's fingerprint is 0.  A delta records the fingerprint and key count of its base
+ *    and of its result; apply refuses a base whose fingerprint or key count is not the delta's (XF_ERR_STATE), so a
+ *    delta applied to the wrong model never makes a wrong model, and checks the result's after building it.
+ *
+ *    Compatibility.  A and B must agree on what defines how an absent key reads: fm, latent_dim, optimizer, absent,
+ *    the resolved v_init, v_const and seed (else XF_ERR_ARG, naming the field).  Prune may differ: a delta compares
+ *    contents only.
+ *
+ *    A delta lives on a device: that of the models it was diffed from, or the one xf_delta_load names.  Diff and
+ *    apply run on streams of their own and read their models only: neither changes a model, and apply does not use
+ *    the base's host staging or lock it, so the base keeps serving while the next model is built beside it.  The
+ *    caller swaps its pointer to the result and destroys the base afterwards.  Memory: diff takes 24 bytes of scratch
+ *    per key of the larger model (what xf_model_save takes, without its 64 MiB row chunk) besides the delta itself;
+ *    apply holds the base, the delta and the result at once.  On every failure *out is NULL and no model changes.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct xf_delta xf_delta;
+typedef struct xf_delta_info {
+  uint64_t upserts;             /* rows set in the result */
+  uint64_t deletes;             /* keys of the base dropped from the result */
+  uint64_t base_keys, base_fingerprint;
+  uint64_t result_keys, result_fingerprint;
+  uint64_t source_keys, pruned_keys;  /* the result's, as xf_model_info has them */
+  uint64_t file_bytes;          /* the size of the file xf_delta_save writes */
+  uint32_t row_bytes;           /* 16 (LR) or 32 (FM) */
+  int latent_dim;
+} xf_delta_info;
+/* The delta from `base` to `next` (same device, compatible); neither model changes. */
+XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out);
+/* A new model: `base` with the delta applied, on base's device; base is unchanged.  XF_ERR_ARG: the delta is not
+ * compatible with base (the field is named) or lives on another device; XF_ERR_STATE: base's key count or
+ * fingerprint is not the delta's base's; XF_ERR_FULL: the result would exceed 2^32 slots. */
+XF_DLL int xf_model_apply_delta(xf_model* base, const xf_delta* d, xf_model** out);
+XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out);
+/* Delta file "XFSD" (little-endian): a 144-byte header
+ *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm   20 i32 latent_dim   24 i32 optimizer
+ *    28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes   52 u32 0
+ *    56 u64 base keys   64 u64 base fingerprint   72 u64 result keys   80 u64 result source keys
+ *    88 u64 result pruned keys   96 u64 result fingerprint   104 u64 upserts U   112 u64 deletes D
+ *   120 u64 rows per chunk (64 MiB / row bytes)   128 u64 keys per delete chunk (64 MiB / 8)
+ *   136 u64 checksum of bytes [0, 136)
+ *  then the U upsert rows sorted by key in ceil(U / rows per chunk) chunks, then the D delete keys sorted by key in
+ *  ceil(D / keys per chunk) chunks.  Every chunk is {u64 index of its first entry in its section, u64 entries,
+ *  u64 checksum, u64 0} followed by its entries; chunks are numbered through both sections (the first delete chunk
+ *  follows the last upsert chunk) and chunk c's checksum is XFSM's (sum of splitmix64(word ^ (c << 40 | byte offset
+ *  in its entries))).  The file is a function of the two models' contents.  Written to <path>.tmp and renamed; the
+ *  staging is bounded by the chunk size.  xf_delta_load refuses with XF_ERR_IO a truncated or damaged file, another
+ *  format (an XFSM model, an XFST or XFTB checkpoint), and a file whose checksums pass but whose contents break the
+ *  format: keys not strictly ascending in a section, a key both upserted and deleted, key 2^64 - 1, non-zero padding,
+ *  or counts that cannot hold (more upserts than result keys, more deletes than base keys). */
+XF_DLL int xf_delta_save(xf_delta* d, const char* path);
+XF_DLL int xf_delta_load(xf_delta** out, const char* path, int device);
+XF_DLL int xf_delta_get_info(xf_delta* d, xf_delta_info* out);
+XF_DLL int xf_delta_destroy(xf_delta* d);
 
 /* ------------------------------------------------------------------------------------------------
  * 1. Reference C API (src/c_api/c_api.h:26-29), unchanged signatures.

@@ -51,6 +51,13 @@ class ModelInfo(C.Structure):
                 ("absent", C.c_int), ("fm", C.c_int)]
 
 
+class DeltaInfo(C.Structure):
+    _fields_ = [("upserts", C.c_uint64), ("deletes", C.c_uint64), ("base_keys", C.c_uint64),
+                ("base_fingerprint", C.c_uint64), ("result_keys", C.c_uint64), ("result_fingerprint", C.c_uint64),
+                ("source_keys", C.c_uint64), ("pruned_keys", C.c_uint64), ("file_bytes", C.c_uint64),
+                ("row_bytes", C.c_uint32), ("latent_dim", C.c_int)]
+
+
 class TrainerConfig(C.Structure):
     _fields_ = [("model", C.c_int), ("max_rows", C.c_uint32), ("max_nnz", C.c_uint32), ("keep_loss", C.c_int)]
 
@@ -157,6 +164,13 @@ SIGNATURES = {
     "xf_model_predict_device": (_i, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
     "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
+    "xf_model_diff": (_i, [_vp, _vp, _vp]),
+    "xf_model_apply_delta": (_i, [_vp, _vp, _vp]),
+    "xf_model_fingerprint": (_i, [_vp, _vp]),
+    "xf_delta_save": (_i, [_vp, C.c_char_p]),
+    "xf_delta_load": (_i, [_vp, C.c_char_p, _i]),
+    "xf_delta_get_info": (_i, [_vp, _vp]),
+    "xf_delta_destroy": (_i, [_vp]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
     "XFCreateEx": (_i, [_vp, C.c_char_p, C.c_char_p, _i, _i, _i, _i]),
@@ -488,6 +502,53 @@ class Model:
         lab = np.empty(n, np.uint8)
         _check(lib().xf_model_predict_ingested(self.h, trainer.h, row_start, row_end, _p(p), _p(lab)))
         return p, lab
+
+    def fingerprint(self):
+        """The order-free u64 of the model's contents (xf_model_fingerprint)."""
+        f = C.c_uint64()
+        _check(lib().xf_model_fingerprint(self.h, C.byref(f)))
+        return f.value
+
+    def diff(self, next_model):
+        """The Delta that carries this model to `next_model` (xf_model_diff); neither model changes."""
+        h = C.c_void_p()
+        _check(lib().xf_model_diff(self.h, next_model.h, C.byref(h)))
+        return Delta(h)
+
+    def apply(self, delta):
+        """A new Model: this one with `delta` applied (xf_model_apply_delta); this one is not changed."""
+        h = C.c_void_p()
+        _check(lib().xf_model_apply_delta(self.h, delta.h, C.byref(h)))
+        return Model(h)
+
+
+class Delta:
+    """The difference between two serving models (xf_delta_*): made by Model.diff or Delta.load."""
+
+    def __init__(self, handle):
+        self.h = handle
+
+    @classmethod
+    def load(cls, path, device=0):
+        h = C.c_void_p()
+        _check(lib().xf_delta_load(C.byref(h), path.encode(), device))
+        return cls(h)
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().xf_delta_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def info(self):
+        i = DeltaInfo()
+        _check(lib().xf_delta_get_info(self.h, C.byref(i)))
+        return {k: getattr(i, k) for k, _ in DeltaInfo._fields_}
+
+    def save(self, path):
+        _check(lib().xf_delta_save(self.h, path.encode()))
 
 
 class Comm:

@@ -24,7 +24,7 @@
 #include <mutex>
 #include <string>
 
-#include "internal.h"
+#include "serve.cuh"
 
 #define XF_SM_VERSION 1u
 #define XF_SM_CHUNK_HEAD 32  // {u64 first row, u64 rows, u64 checksum, u64 0}
@@ -53,47 +53,6 @@ struct XfModelHeader {
 static_assert(sizeof(XfModelHeader) == 104 && offsetof(XfModelHeader, seed) == 64 &&
                   offsetof(XfModelHeader, header_checksum) == 96,
               "the documented header is 104 bytes");
-
-struct xf_model {
-  XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source
-  int device = 0;
-  int fm = 0, absent = 0, optimizer = 0;
-  uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
-  cudaStream_t stream = nullptr;
-  // staging of the host entry points, grown on demand; those calls are serialised by the mutex
-  std::mutex mu;
-  XfDevBuf s_row_ptr, s_keys, s_out, s_aux;
-  XfPinBuf h_in, h_out;
-};
-
-// ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
-template <bool FM>
-__device__ __forceinline__ void xf_serve_load(const uint8_t* p, uint64_t& key, float& w, float& st, float& qt) {
-  uint64_t q0, q1, q2 = 0ull, q3 = 0ull;
-  if (FM) {
-    // one sector as two 128-bit loads by the same lane (sm_90 has no 256-bit load), issued back to back
-    asm("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u64 {%2,%3}, [%4+16];"
-        : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
-  } else {
-    asm("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(q0), "=l"(q1) : "l"(p));
-  }
-  key = q0;
-  w = __uint_as_float((uint32_t)q1);
-  st = __uint_as_float((uint32_t)(q1 >> 32));
-  qt = __uint_as_float((uint32_t)q2);
-}
-
-// Find `key` from its home slot `s`, whose row the caller has loaded into (k, w, st, qt); false: the model does not
-// hold it.  The load is at most 0.5, so a chain ends at an empty slot long before XF_MAX_PROBE.
-template <bool FM>
-__device__ __forceinline__ bool xf_serve_find(const XfTableView& m, uint64_t key, uint64_t k, float& w, float& st, float& qt) {
-  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
-    if (k == key) return true;
-    if (k == XF_EMPTY_KEY) return false;
-    xf_serve_load<FM>(xf_row(m, xf_probe_slot(m, key, i)), k, w, st, qt);
-  }
-  return false;
-}
 
 // one token's terms into the lane's sums, in the order the step kernels add them
 template <bool FM>
@@ -159,26 +118,6 @@ static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const ui
 __global__ void xf_k_model_fill(uint4* base, uint64_t chunks16, uint32_t per_row) {
   for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < chunks16; c += (uint64_t)gridDim.x * blockDim.x)
     base[c] = (c % per_row == 0) ? make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u) : make_uint4(0u, 0u, 0u, 0u);
-}
-
-// claim a slot for `key` (unique among the inserted keys) and write its row; a probe overflow or a key met twice sets *error
-__device__ __forceinline__ void xf_model_insert(const XfTableView& m, uint64_t key, float w, float st, float qt, int* error) {
-  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
-    uint8_t* rowp = xf_row(m, xf_probe_slot(m, key, i));
-    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(rowp), (unsigned long long)XF_EMPTY_KEY,
-                                             (unsigned long long)key);
-    if (old == XF_EMPTY_KEY) {
-      if (m.K > 0) {
-        *reinterpret_cast<float2*>(rowp + 8) = make_float2(w, st);
-        *reinterpret_cast<float*>(rowp + 16) = qt;
-      } else {
-        *reinterpret_cast<float*>(rowp + 8) = w;
-      }
-      return;
-    }
-    if (old == key) break;
-  }
-  *error = 1;
 }
 
 // Slot r of the training table as a reader resolves it, and whether the model keeps it.  COUNT: count the rows kept
@@ -271,14 +210,8 @@ __global__ void xf_k_model_lookup(XfTableView m, const uint64_t* __restrict__ ke
 // -------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------
-static uint64_t xf_model_capacity(uint64_t keys) {
-  uint64_t c = 1024;
-  while (c < 2 * keys) c <<= 1;
-  return c;
-}
-
 // the model's table on the current device: `capacity` empty rows
-static int xf_model_alloc(xf_model* m, uint64_t capacity) {
+int xf_model_alloc(xf_model* m, uint64_t capacity) {
   if (capacity > (1ull << 32)) {
     xf_set_error("a serving model of %llu slots exceeds 2^32", (unsigned long long)capacity);
     return XF_ERR_FULL;
@@ -299,7 +232,7 @@ static int xf_model_alloc(xf_model* m, uint64_t capacity) {
   return XF_OK;
 }
 
-static void xf_model_free(xf_model* m) {
+void xf_model_free(xf_model* m) {
   if (!m) return;
   cudaSetDevice(m->device);
   if (m->stream) cudaStreamSynchronize(m->stream);
@@ -308,6 +241,50 @@ static void xf_model_free(xf_model* m) {
   m->h_in.release(); m->h_out.release();
   if (m->stream) cudaStreamDestroy(m->stream);
   delete m;
+}
+
+int XfSortedSlots::ensure(uint64_t n) {
+  XF_TRY(keys_in.ensure(std::max<uint64_t>(n, 1) * 8)); XF_TRY(keys_out.ensure(std::max<uint64_t>(n, 1) * 8));
+  XF_TRY(slots_in.ensure(std::max<uint64_t>(n, 1) * 4)); XF_TRY(slots_out.ensure(std::max<uint64_t>(n, 1) * 4));
+  return count.ensure(8);
+}
+
+void XfSortedSlots::release() {
+  keys_in.release(); keys_out.release(); slots_in.release(); slots_out.release(); tmp.release(); count.release();
+}
+
+int xf_sort_slots(XfSortedSlots& s, uint64_t n, cudaStream_t st) {
+  if (n == 0) return XF_OK;
+  size_t tb = 0;
+  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, s.keys_in.as<uint64_t>(), s.keys_out.as<uint64_t>(), s.slots_in.as<uint32_t>(),
+                                              s.slots_out.as<uint32_t>(), n, 0, 64, st));
+  XF_TRY(s.tmp.ensure(std::max<size_t>(tb, 16)));
+  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(s.tmp.p, tb, s.keys_in.as<uint64_t>(), s.keys_out.as<uint64_t>(), s.slots_in.as<uint32_t>(),
+                                              s.slots_out.as<uint32_t>(), n, 0, 64, st));
+  return XF_OK;
+}
+
+int xf_model_list_sorted(const XfTableView& v, uint64_t n, XfSortedSlots& s, cudaStream_t st) {
+  XF_TRY(s.ensure(n));
+  XF_CUDA_TRY(cudaMemsetAsync(s.count.p, 0, 8, st));
+  xf_k_model_list<<<xf_grid_for(v.mask + 1, 256, 8), 256, 0, st>>>(v, s.keys_in.as<uint64_t>(), s.slots_in.as<uint32_t>(),
+                                                                   s.count.as<unsigned long long>());
+  XF_CUDA_TRY(cudaGetLastError());
+  return xf_sort_slots(s, n, st);
+}
+
+int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, void* out, cudaStream_t st) {
+  if (n == 0) return XF_OK;
+  xf_k_model_gather<<<xf_grid_for(n * (v.stride / 16u), 256, 8), 256, 0, st>>>(v, slots, n, reinterpret_cast<uint4*>(out));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
+}
+
+int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st) {
+  if (n == 0) return XF_OK;
+  xf_k_model_insert_rows<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
 }
 
 XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
@@ -562,31 +539,17 @@ static int xf_sm_save_body(xf_model* m, FILE* f, const char* path) {
   if (n == 0) return XF_OK;
   // (key, slot) of every row, sorted by key on the device
   cudaStream_t st = m->stream;
-  XfDevBuf keys_in, keys_out, slots_in, slots_out, tmp, rows, count;
-  struct Release { XfDevBuf* b[7]; ~Release() { for (XfDevBuf* x : b) x->release(); } }
-      rel{{&keys_in, &keys_out, &slots_in, &slots_out, &tmp, &rows, &count}};
-  XF_TRY(keys_in.ensure(n * 8)); XF_TRY(keys_out.ensure(n * 8));
-  XF_TRY(slots_in.ensure(n * 4)); XF_TRY(slots_out.ensure(n * 4));
-  XF_TRY(count.ensure(8));
-  XF_CUDA_TRY(cudaMemsetAsync(count.p, 0, 8, st));
-  xf_k_model_list<<<xf_grid_for(h.capacity, 256, 8), 256, 0, st>>>(m->view, keys_in.as<uint64_t>(), slots_in.as<uint32_t>(),
-                                                                  count.as<unsigned long long>());
-  XF_CUDA_TRY(cudaGetLastError());
-  size_t tb = 0;
-  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys_in.as<uint64_t>(), keys_out.as<uint64_t>(), slots_in.as<uint32_t>(),
-                                              slots_out.as<uint32_t>(), n, 0, 64, st));
-  XF_TRY(tmp.ensure(std::max<size_t>(tb, 16)));
-  XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys_in.as<uint64_t>(), keys_out.as<uint64_t>(), slots_in.as<uint32_t>(),
-                                              slots_out.as<uint32_t>(), n, 0, 64, st));
+  XfSortedSlots sorted;
+  XfDevBuf rows;
+  struct Release { XfSortedSlots* s; XfDevBuf* r; ~Release() { s->release(); r->release(); } } rel{&sorted, &rows};
+  XF_TRY(xf_model_list_sorted(m->view, n, sorted, st));
   // the rows in that order, a chunk at a time: gathered on the device, copied to the pinned buffer, summed and written
   const uint64_t C = std::min<uint64_t>(h.chunk_rows, n);
   XF_TRY(rows.ensure(C * h.row_bytes));
   XF_TRY(m->h_out.ensure(C * h.row_bytes));
   for (uint64_t first = 0, chunk = 0; first < n; first += h.chunk_rows, ++chunk) {
     const uint64_t c = std::min<uint64_t>(h.chunk_rows, n - first);
-    xf_k_model_gather<<<xf_grid_for(c * (h.row_bytes / 16u), 256, 8), 256, 0, st>>>(m->view, slots_out.as<uint32_t>() + first, c,
-                                                                                     rows.as<uint4>());
-    XF_CUDA_TRY(cudaGetLastError());
+    XF_TRY(xf_model_gather(m->view, sorted.slots_out.as<uint32_t>() + first, c, rows.p, st));
     XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, rows.p, c * h.row_bytes, cudaMemcpyDeviceToHost, st));
     XF_CUDA_TRY(cudaStreamSynchronize(st));
     const uint64_t head[4] = {first, c, xf_st_host_sum(m->h_out.p, c * h.row_bytes, xf_st_tag(chunk)), 0ull};
@@ -674,8 +637,7 @@ static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModel
       prev = key;
     }
     XF_CUDA_TRY(cudaMemcpyAsync(rows.p, m->h_in.p, c * h.row_bytes, cudaMemcpyHostToDevice, m->stream));
-    xf_k_model_insert_rows<<<xf_grid_for(c, 256, 8), 256, 0, m->stream>>>(m->view, rows.as<uint8_t>(), c, err.as<int>());
-    XF_CUDA_TRY(cudaGetLastError());
+    XF_TRY(xf_model_insert_rows(m->view, rows.as<uint8_t>(), c, err.as<int>(), m->stream));
     XF_CUDA_TRY(cudaStreamSynchronize(m->stream));  // the pinned buffer is read again for the next chunk
     first += c;
   }

@@ -1,0 +1,107 @@
+// Serving model internals shared by serve.cu (freeze, predict, the XFSM file) and delta.cu (diff, apply, the XFSD file):
+// the model's host structure, the device functions that read and build its rows, and the host steps both use.  The
+// kernels behind the host steps live in serve.cu only.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <mutex>
+
+#include "internal.h"
+
+struct xf_model {
+  XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source
+  int device = 0;
+  int fm = 0, absent = 0, optimizer = 0;
+  uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
+  cudaStream_t stream = nullptr;
+  // staging of the host entry points, grown on demand; those calls are serialised by the mutex
+  std::mutex mu;
+  XfDevBuf s_row_ptr, s_keys, s_out, s_aux;
+  XfPinBuf h_in, h_out;
+};
+
+// ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
+template <bool FM>
+__device__ __forceinline__ void xf_serve_load(const uint8_t* p, uint64_t& key, float& w, float& st, float& qt) {
+  uint64_t q0, q1, q2 = 0ull, q3 = 0ull;
+  if (FM) {
+    // one sector as two 128-bit loads by the same lane (sm_90 has no 256-bit load), issued back to back
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u64 {%2,%3}, [%4+16];"
+        : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
+  } else {
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(q0), "=l"(q1) : "l"(p));
+  }
+  key = q0;
+  w = __uint_as_float((uint32_t)q1);
+  st = __uint_as_float((uint32_t)(q1 >> 32));
+  qt = __uint_as_float((uint32_t)q2);
+}
+
+// Find `key` from its home slot `s`, whose row the caller has loaded into (k, w, st, qt); false: the model does not
+// hold it.  The load is at most 0.5, so a chain ends at an empty slot long before XF_MAX_PROBE.
+template <bool FM>
+__device__ __forceinline__ bool xf_serve_find(const XfTableView& m, uint64_t key, uint64_t k, float& w, float& st, float& qt) {
+  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
+    if (k == key) return true;
+    if (k == XF_EMPTY_KEY) return false;
+    xf_serve_load<FM>(xf_row(m, xf_probe_slot(m, key, i)), k, w, st, qt);
+  }
+  return false;
+}
+
+// Claim a slot for `key` and write its row; a probe overflow sets *error.  KEEP = false: the inserted keys are unique,
+// and a key met twice sets *error.  KEEP = true: a key the model already holds keeps its row (the caller orders the
+// kernels so that the row it holds is complete).
+template <bool KEEP = false>
+__device__ __forceinline__ void xf_model_insert(const XfTableView& m, uint64_t key, float w, float st, float qt, int* error) {
+  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
+    uint8_t* rowp = xf_row(m, xf_probe_slot(m, key, i));
+    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(rowp), (unsigned long long)XF_EMPTY_KEY,
+                                             (unsigned long long)key);
+    if (old == XF_EMPTY_KEY) {
+      if (m.K > 0) {
+        *reinterpret_cast<float2*>(rowp + 8) = make_float2(w, st);
+        *reinterpret_cast<float*>(rowp + 16) = qt;
+      } else {
+        *reinterpret_cast<float*>(rowp + 8) = w;
+      }
+      return;
+    }
+    if (old == key) {
+      if (KEEP) return;
+      break;
+    }
+  }
+  *error = 1;
+}
+
+// slots of a model of `keys` keys: the smallest power of two >= 2 x keys (load <= 0.5), at least 1024
+inline uint64_t xf_model_capacity(uint64_t keys) {
+  uint64_t c = 1024;
+  while (c < 2 * keys) c <<= 1;
+  return c;
+}
+
+// the model's table on the current device: `capacity` empty rows (stride from m->fm), filled on m->stream;
+// XF_ERR_FULL past 2^32 slots
+int xf_model_alloc(xf_model* m, uint64_t capacity);
+// waits for the model's stream and frees everything (m may be NULL)
+void xf_model_free(xf_model* m);
+
+// Rows of a model listed as (key, slot) pairs and sorted by key on the device: the first step of a model file, and of
+// a delta's upserts and deletes.  keys_in / slots_in hold the n pairs in any order; the sort leaves them in keys_out /
+// slots_out.  Device scratch: 24 bytes per pair and cub's temporary storage.
+struct XfSortedSlots {
+  XfDevBuf keys_in, keys_out, slots_in, slots_out, tmp, count;
+  int ensure(uint64_t n);  // room for n pairs and the list kernels' counter
+  void release();
+};
+// list every row of `v` (capacity v.mask + 1) into s and sort; n = the model's keys
+int xf_model_list_sorted(const XfTableView& v, uint64_t n, XfSortedSlots& s, cudaStream_t st);
+// sort the n listed pairs of s by key
+int xf_sort_slots(XfSortedSlots& s, uint64_t n, cudaStream_t st);
+// out = the rows of `v` in slots[0 .. n), packed
+int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, void* out, cudaStream_t st);
+// insert n packed rows (as a model file holds them; keys unique) into `v`; a probe overflow or a key met twice sets *error
+int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st);

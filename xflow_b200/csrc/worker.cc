@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <functional>
 #include <iostream>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 
@@ -177,6 +178,31 @@ static void CheckResumedPolicies(xf_table* t) {
                              "saved with; a resumed run keeps its policies");
 }
 
+// XFLOW_EXPORT_DELTAS = <prefix>: after every epoch the table frozen with the defaults.  The first epoch this process
+// trains writes the whole model, <prefix>-<epochs done>.xfsm; every later epoch writes the delta from the previous
+// epoch's model, <prefix>-<epochs done>.xfsd, and that model is then dropped for the new one.  A server follows the run
+// by loading the first file and applying the others in order.  Single GPU only.
+struct ModelDeleter {
+  void operator()(xf_model* m) const { xf_model_destroy(m); }
+};
+using ModelPtr = std::unique_ptr<xf_model, ModelDeleter>;
+static void ExportEpoch(xf_table* t, const std::string& prefix, uint64_t epochs_done, ModelPtr& prev) {
+  xf_model* m = nullptr;
+  must(xf_table_freeze(t, nullptr, &m), "xf_table_freeze");
+  ModelPtr next(m);
+  const std::string path = prefix + "-" + std::to_string(epochs_done);
+  if (!prev) {
+    must(xf_model_save(m, (path + ".xfsm").c_str()), "xf_model_save");
+  } else {
+    xf_delta* d = nullptr;
+    must(xf_model_diff(prev.get(), m, &d), "xf_model_diff");
+    const int rc = xf_delta_save(d, (path + ".xfsd").c_str());
+    xf_delta_destroy(d);
+    must(rc, "xf_delta_save");
+  }
+  prev = std::move(next);
+}
+
 int MyRank() { return env_int("XFLOW_RANK", env_int("RANK", 0)); }
 int NumWorkers() { return env_int("XFLOW_WORLD", env_int("WORLD_SIZE", 1)); }
 
@@ -214,6 +240,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   env_path("XFLOW_CHECKPOINT", world_);
   env_path("XFLOW_RESUME", world_);
   env_path("XFLOW_EXPORT_MODEL", world_);
+  env_path("XFLOW_EXPORT_DELTAS", world_);
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -446,6 +473,8 @@ void WorkerBase::batch_training() {
   if (host_parse) ensure_trainer(1024, 65536);
   else ensure_trainer_for_block(block_bytes);
   const std::string checkpoint = env_path("XFLOW_CHECKPOINT", 1), resume = env_path("XFLOW_RESUME", 1);
+  const std::string deltas = env_path("XFLOW_EXPORT_DELTAS", 1);
+  ModelPtr exported;  // the model of the last epoch XFLOW_EXPORT_DELTAS wrote
   uint64_t first_epoch = 0;
   if (!resume.empty()) {
     // the image holds the init push's effect: the uninterrupted run made it once, before its first epoch
@@ -487,6 +516,7 @@ void WorkerBase::batch_training() {
     must(xf_trainer_sync(trainer_), "xf_trainer_sync");
     if (!checkpoint.empty())
       must(xf_table_save_state(table_, checkpoint.c_str(), (uint64_t)epoch + 1), "xf_table_save_state");
+    if (!deltas.empty()) ExportEpoch(table_, deltas, (uint64_t)epoch + 1, exported);
     if ((epoch + 1) % 30 == 0) std::cout << "epoch : " << epoch << std::endl;  // :202
   }
   cur_row_ptr_ = nullptr;
