@@ -537,7 +537,30 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *    keys + pruned_keys == source_keys.  FTRL's L1 term writes exact zeros (ftrl.h:66-74): those are the rows pruned.
  *
  *    Refused with XF_ERR_ARG: tables with canonical_fm = 1 (the per-k sums of the canonical FM and the multi-view
- *    machine do not collapse to st, qt) and tables with num_shards > 1 (one shard's rows are not a model).
+ *    machine do not collapse to st, qt: xf_table_freeze_canonical serves them) and tables with num_shards > 1 (one
+ *    shard's rows are not a model).
+ *
+ *    Canonical models.  xf_table_freeze_canonical freezes a table created with canonical_fm = 1 for the textbook FM
+ *    with feature values (XF_MODEL_FM_CANONICAL): its predict is the canonical FM's forward, whichever trainer trained
+ *    the table (the caller states it by calling this function).
+ *      Row: {u64 key, f32 w, u32 0, f32 v[K], zero padding}, 16 + 4K bytes rounded up to 32: K = 4 -> 32, 8 -> 64,
+ *      16 -> 96, 32 -> 160, 64 -> 288, 128 -> 544.  Every row starts on a sector and v starts 16 bytes in, so a
+ *      token's 16-byte piece c of v is one aligned load.  xf_model_info reports fm = 2 and these row bytes.
+ *      Freeze resolves each row as the step kernel reads it: w, and v = the latent block if it is materialised, else
+ *      the initial values of (key, k), evaluated at the freeze.  w and v equal xf_table_export's bit for bit.
+ *      Absent keys: XF_ABSENT_DEFAULT reads an absent key as the row the table would insert (w = 0, v its initial
+ *      values, evaluated on the fly: K per absent token); a canonical table has no admission policy, so absent = -1
+ *      is DEFAULT.  XF_ABSENT_ZERO: an absent key contributes nothing.
+ *      prune = 1 leaves out rows with w == 0 and, under DEFAULT, a latent block that is not materialised; under ZERO,
+ *      every resolved v_k == 0.  Adding +-0 to a float sum that starts at +0 never changes it, so for finite feature
+ *      values pruning never changes a prediction; a NaN or Inf value on a pruned key makes the table's term NaN where
+ *      the model adds nothing.
+ *      xf_model_predict_host_values / _device_values on a canonical model return, bit for bit, what
+ *      xf_trainer_predict_host_values returns on the table at the moment of the freeze (under ZERO: on that table with
+ *      zero rows imported for the query's absent keys).  xf_model_predict_host / _device read every value as 1.
+ *      The XFSM and XFSD files keep version 1 and record fm = 2, latent_dim and these row bytes; a load refuses
+ *      non-zero padding in a canonical row.  Not served: the multi-view machine (XF_MODEL_MVM: its forward needs
+ *      fields), shards.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct xf_model xf_model;
 enum { XF_ABSENT_DEFAULT = 0, XF_ABSENT_ZERO = 1 };
@@ -552,6 +575,9 @@ typedef struct xf_freeze_config {
 XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg);
 /* cfg == NULL: the defaults.  On failure *out is NULL. */
 XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+/* A canonical model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG for tables with
+ * canonical_fm = 0 and tables with num_shards > 1. */
+XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
 XF_DLL int xf_model_destroy(xf_model* m);
 typedef struct xf_model_info {
   uint64_t keys;         /* keys the model holds */
@@ -559,14 +585,14 @@ typedef struct xf_model_info {
   uint64_t bytes;        /* capacity x row_bytes: the model's device memory */
   uint64_t source_keys;  /* keys of the table when it was frozen */
   uint64_t pruned_keys;  /* source_keys - keys */
-  uint32_t row_bytes;    /* 16 (LR) or 32 (FM) */
-  int latent_dim, optimizer, absent, fm;
+  uint32_t row_bytes;    /* 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical) */
+  int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM */
 } xf_model_info;
 XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
 /* Model file "XFSM" (little-endian): a 104-byte header
  *     0 "XFSM"   4 u32 version (1)   8 u64 header bytes (104)   16 u64 keys   24 u64 capacity   32 u32 row bytes
- *    36 i32 fm   40 i32 latent_dim   44 i32 optimizer   48 i32 absent   52 i32 resolved v_init (0 constant, 1 counter-
- *    based normal, 3 zero)   56 f32 the constant   60 u32 0   64 u64 seed   72 u64 source keys   80 u64 pruned keys
+ *    36 i32 fm (0 LR, 1 FM, 2 canonical)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
+ *    52 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   56 f32 the constant   60 u32 0   64 u64 seed   72 u64 source keys   80 u64 pruned keys
  *    88 u64 rows per chunk (64 MiB / row bytes)   96 u64 checksum of bytes [0, 96)
  *  then the rows SORTED BY KEY in ceil(keys / rows per chunk) chunks, each {u64 index of its first row, u64 rows,
  *  u64 checksum, u64 0} followed by its rows.  Checksums are those of the state image above (sum of
@@ -586,12 +612,25 @@ XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uin
                                  uint32_t nnz, float* pctr_out);
 XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream);
-/* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL */
+/* The same with the tokens' feature values vals[nnz] (NULL: all 1; device memory for _device_values), for canonical
+ * models; the contracts are those of _host / _device.  Non-NULL vals on an LR or FM model are XF_ERR_ARG: that model
+ * ignores values. */
+XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
+                                        uint32_t rows, uint32_t nnz, float* pctr_out);
+XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
+                                          const float* d_vals, uint32_t rows, uint32_t nnz, float* d_pctr_out,
+                                          void* cuda_stream);
+/* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL.  On a
+ * canonical model st and qt must be NULL (XF_ERR_ARG): its rows are read with xf_model_lookup_latent. */
 XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt,
                            uint8_t* present);
+/* what a canonical model holds for n host keys: w[n], v[n * K], present[n] (0 for an absent key); any output may be
+ * NULL.  XF_ERR_ARG on an LR or FM model. */
+XF_DLL int xf_model_lookup_latent(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* v, uint8_t* present);
 /* forward pass over rows [row_start, row_end) of a trainer's current ingested block, read from `m` instead of the
  * trainer's table (same outputs as xf_trainer_predict_ingested; runs on the table's stream).  XF_ERR_ARG if the
- * trainer's model is not LR / FM as the model is, or if the two live on different devices. */
+ * trainer's model is not LR / FM as the model is, if the two live on different devices, or for a canonical model
+ * (an ingested text block carries no feature values). */
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end,
                                      float* pctr_out, uint8_t* labels_out);
 
@@ -601,14 +640,16 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
  *
  *    The delta from model A to model B:
  *      upserts  the rows of B whose key A does not hold, or whose row differs from A's in any byte (a row is 16
- *               bytes for LR and 32 for FM, padding included), sorted by key;
+ *               bytes for LR, 32 for FM and 16 + 4K rounded up to 32 for a canonical model, padding included),
+ *               sorted by key;
  *      deletes  the keys of A that B does not hold, sorted by key;
  *      header   what XFSM records of B: keys, source_keys and pruned_keys.
  *    Applying it to A builds a new model whose contents and info are B's, so that xf_model_save of the result is
  *    byte-identical to xf_model_save(B) and every xf_model_predict_* returns on it, bit for bit, what it returns on B.
  *
  *    Fingerprint.  An order-free u64 of a model's contents: the sum mod 2^64 over its rows of h(row), where for the
- *    row's 8-byte little-endian words w_0 .. w_{n-1} (n = 2 for LR, 4 for FM) h_0 = 0, h_{i+1} = splitmix64(h_i ^ w_i)
+ *    row's 8-byte little-endian words w_0 .. w_{n-1} (n = 2 for LR, 4 for FM, row bytes / 8 for a canonical model)
+ *    h_0 = 0, h_{i+1} = splitmix64(h_i ^ w_i)
  *    and h(row) = h_n.  The empty model's fingerprint is 0.  A delta records the fingerprint and key count of its base
  *    and of its result; apply refuses a base whose fingerprint or key count is not the delta's (XF_ERR_STATE), so a
  *    delta applied to the wrong model never makes a wrong model, and checks the result's after building it.
@@ -632,7 +673,7 @@ typedef struct xf_delta_info {
   uint64_t result_keys, result_fingerprint;
   uint64_t source_keys, pruned_keys;  /* the result's, as xf_model_info has them */
   uint64_t file_bytes;          /* the size of the file xf_delta_save writes */
-  uint32_t row_bytes;           /* 16 (LR) or 32 (FM) */
+  uint32_t row_bytes;           /* 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical) */
   int latent_dim;
 } xf_delta_info;
 /* The delta from `base` to `next` (same device, compatible); neither model changes. */
@@ -643,8 +684,9 @@ XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out);
 XF_DLL int xf_model_apply_delta(xf_model* base, const xf_delta* d, xf_model** out);
 XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out);
 /* Delta file "XFSD" (little-endian): a 144-byte header
- *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm   20 i32 latent_dim   24 i32 optimizer
- *    28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes   52 u32 0
+ *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's)   20 i32 latent_dim
+ *    24 i32 optimizer   28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes
+ *    52 u32 0
  *    56 u64 base keys   64 u64 base fingerprint   72 u64 result keys   80 u64 result source keys
  *    88 u64 result pruned keys   96 u64 result fingerprint   104 u64 upserts U   112 u64 deletes D
  *   120 u64 rows per chunk (64 MiB / row bytes)   128 u64 keys per delete chunk (64 MiB / 8)

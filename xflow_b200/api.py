@@ -156,13 +156,17 @@ SIGNATURES = {
     "xf_comm_barrier": (_i, [_vp]),
     "xf_freeze_config_default": (_i, [_vp]),
     "xf_table_freeze": (_i, [_vp, _vp, _vp]),
+    "xf_table_freeze_canonical": (_i, [_vp, _vp, _vp]),
     "xf_model_destroy": (_i, [_vp]),
     "xf_model_get_info": (_i, [_vp, _vp]),
     "xf_model_save": (_i, [_vp, C.c_char_p]),
     "xf_model_load": (_i, [_vp, C.c_char_p, _i]),
     "xf_model_predict_host": (_i, [_vp, _vp, _vp, _u32, _u32, _vp]),
     "xf_model_predict_device": (_i, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "xf_model_predict_host_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp]),
+    "xf_model_predict_device_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "xf_model_lookup_latent": (_i, [_vp, _vp, _u64, _vp, _vp, _vp]),
     "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_diff": (_i, [_vp, _vp, _vp]),
     "xf_model_apply_delta": (_i, [_vp, _vp, _vp]),
@@ -444,6 +448,14 @@ class Table:
         _check(lib().xf_table_freeze(self.h, C.byref(cfg), C.byref(h)))
         return Model(h)
 
+    def freeze_canonical(self, absent=None, prune=True, device=None):
+        """A canonical serving Model of a canonical_fm table (xf_table_freeze_canonical): rows {key, w, v[K]} served
+        with the canonical FM's forward on feature values; arguments as for freeze."""
+        cfg = FreezeConfig(-1 if absent is None else absent, 1 if prune else 0, -1 if device is None else device)
+        h = C.c_void_p()
+        _check(lib().xf_table_freeze_canonical(self.h, C.byref(cfg), C.byref(h)))
+        return Model(h)
+
 
 class Model:
     """A frozen, read-only serving model (xf_model_*): made by Table.freeze or Model.load."""
@@ -473,18 +485,29 @@ class Model:
     def save(self, path):
         _check(lib().xf_model_save(self.h, path.encode()))
 
-    def predict_host(self, row_ptr, keys):
+    def predict_host(self, row_ptr, keys, vals=None):
+        """Forward pass on host CSR arrays; vals: the tokens' feature values (canonical models only; None: all 1)."""
         row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
         keys = np.ascontiguousarray(keys, np.uint64)
         rows = row_ptr.size - 1
         out = np.empty(rows, np.float32)
-        _check(lib().xf_model_predict_host(self.h, _p(row_ptr), _p(keys), rows, keys.size, _p(out)))
+        if vals is None:
+            _check(lib().xf_model_predict_host(self.h, _p(row_ptr), _p(keys), rows, keys.size, _p(out)))
+        else:
+            vals = np.ascontiguousarray(vals, np.float32)
+            if vals.size != keys.size:
+                raise ValueError("one value per token: %d values for %d keys" % (vals.size, keys.size))
+            _check(lib().xf_model_predict_host_values(self.h, _p(row_ptr), _p(keys), _p(vals), rows, keys.size, _p(out)))
         return out
 
-    def predict_device(self, d_row_ptr, d_keys, rows, nnz, d_out, stream=0):
-        """Asynchronous forward pass on device pointers (raw addresses) on the CUDA stream `stream`."""
-        _check(lib().xf_model_predict_device(self.h, _p(d_row_ptr), _p(d_keys), rows, nnz, _p(d_out),
-                                             C.c_void_p(int(stream)) if stream else None))
+    def predict_device(self, d_row_ptr, d_keys, rows, nnz, d_out, stream=0, d_vals=0):
+        """Asynchronous forward pass on device pointers (raw addresses) on the CUDA stream `stream`; d_vals: the tokens'
+        feature values on the device (canonical models only; 0: all 1)."""
+        st = C.c_void_p(int(stream)) if stream else None
+        if d_vals:
+            _check(lib().xf_model_predict_device_values(self.h, _p(d_row_ptr), _p(d_keys), _p(d_vals), rows, nnz, _p(d_out), st))
+        else:
+            _check(lib().xf_model_predict_device(self.h, _p(d_row_ptr), _p(d_keys), rows, nnz, _p(d_out), st))
 
     def lookup(self, keys):
         """What the model holds for `keys`: dict of w, st, qt (0 for LR) and present."""
@@ -493,6 +516,14 @@ class Model:
         out = dict(keys=keys, w=np.zeros(n, np.float32), st=np.zeros(n, np.float32), qt=np.zeros(n, np.float32),
                    present=np.zeros(n, np.uint8))
         _check(lib().xf_model_lookup(self.h, _p(keys), n, _p(out["w"]), _p(out["st"]), _p(out["qt"]), _p(out["present"])))
+        return out
+
+    def lookup_latent(self, keys):
+        """What a canonical model holds for `keys`: dict of w, v [n, K] and present."""
+        keys = np.ascontiguousarray(keys, np.uint64)
+        n, K = keys.size, self.info()["latent_dim"]
+        out = dict(keys=keys, w=np.zeros(n, np.float32), v=np.zeros((n, K), np.float32), present=np.zeros(n, np.uint8))
+        _check(lib().xf_model_lookup_latent(self.h, _p(keys), n, _p(out["w"]), _p(out["v"]), _p(out["present"])))
         return out
 
     def predict_ingested(self, trainer, row_start, row_end):

@@ -11,6 +11,8 @@
 //                base whose key is not deleted (a binary search over the sorted delete keys) and not upserted (the
 //                insert keeps the row it finds); then the result's fingerprint and key count are checked
 //   file         header, upsert rows, delete keys, a chunk at a time through bounded staging
+// Canonical models (rows of 16 + 4K bytes rounded up to 32) take runtime-stride variants of the three passes
+// (xf_k_fingerprint_fmc, xf_k_delta_emit_fmc<DEL>, xf_k_apply_base_fmc) that hash, compare and copy whole rows.
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
@@ -175,6 +177,72 @@ xf_k_delta_emit(XfTableView a, XfTableView b, uint64_t* __restrict__ keys_out, u
   }
 }
 
+// ---- canonical rows (runtime stride): the same three passes over whole rows
+// out[0] += the fingerprint of the rows of `m` (n = stride / 8 words each), out[1] += their number
+__global__ void __launch_bounds__(256) xf_k_fingerprint_fmc(XfTableView m, unsigned long long* out) {
+  const uint64_t cap = m.mask + 1;
+  const uint32_t words = m.stride / 8u;
+  uint64_t sum = 0ull, rows = 0ull;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t* p = reinterpret_cast<const uint64_t*>(xf_row(m, r));
+    if (p[0] == XF_EMPTY_KEY) continue;
+    uint64_t h = 0ull;
+    for (uint32_t i = 0; i < words; ++i) h = xf_splitmix64(h ^ p[i]);
+    sum += h;
+    ++rows;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    sum += xf_shfl_xor_u64(sum, o);
+    rows += xf_shfl_xor_u64(rows, o);
+  }
+  if ((threadIdx.x & 31u) == 0u && rows) {
+    atomicAdd(out, (unsigned long long)sum);
+    atomicAdd(out + 1, (unsigned long long)rows);
+  }
+}
+
+// xf_k_delta_emit for canonical rows: a row differs if any of its bytes 8 .. stride does
+template <bool DEL>
+__global__ void __launch_bounds__(256)
+xf_k_delta_emit_fmc(XfTableView a, XfTableView b, uint64_t* __restrict__ keys_out, uint32_t* __restrict__ slots_out,
+                    unsigned long long* count) {
+  const uint64_t cap = a.mask + 1;
+  const uint32_t lane = threadIdx.x & 31u;
+  for (uint64_t r0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull; r0 < cap; r0 += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t r = r0 + lane;
+    bool emit = false;
+    uint64_t key = XF_EMPTY_KEY;
+    if (r < cap) {
+      const uint8_t* pa = xf_row(a, r);
+      key = __ldg(reinterpret_cast<const unsigned long long*>(pa));
+      if (key != XF_EMPTY_KEY) {
+        const int64_t s = xf_model_find_slot(b, key);
+        emit = s < 0;
+        if (!DEL && s >= 0) {
+          const uint8_t* pb = xf_row(b, (uint64_t)s);
+          uint64_t d = __ldg(reinterpret_cast<const unsigned long long*>(pa + 8)) ^
+                       __ldg(reinterpret_cast<const unsigned long long*>(pb + 8));
+          for (uint32_t o = 16; o < a.stride && d == 0ull; o += 16) {
+            const uint4 x = __ldg(reinterpret_cast<const uint4*>(pa + o)), y = __ldg(reinterpret_cast<const uint4*>(pb + o));
+            d = (uint64_t)((x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w));
+          }
+          emit = d != 0ull;
+        }
+      }
+    }
+    const uint32_t mask = __ballot_sync(0xffffffffu, emit);
+    if (mask == 0u) continue;
+    unsigned long long first = 0ull;
+    if (lane == 0u) first = atomicAdd(count, (unsigned long long)__popc(mask));
+    first = __shfl_sync(0xffffffffu, first, 0);
+    if (emit) {
+      const unsigned long long idx = first + (unsigned long long)__popc(mask & ((1u << lane) - 1u));
+      keys_out[idx] = key;
+      slots_out[idx] = (uint32_t)r;
+    }
+  }
+}
+
 // whether the sorted keys p[0], p[stride], ... p[(n - 1) stride] (the key word of packed rows, or a key array with
 // stride 8) hold `key`
 __device__ __forceinline__ bool xf_sorted_has(const uint8_t* __restrict__ p, uint64_t n, uint32_t stride, uint64_t key) {
@@ -203,6 +271,20 @@ xf_k_apply_base(XfTableView base, XfTableView out, const uint64_t* __restrict__ 
   }
 }
 
+// xf_k_apply_base for canonical rows: whole rows are copied
+__global__ void __launch_bounds__(256)
+xf_k_apply_base_fmc(XfTableView base, XfTableView out, const uint64_t* __restrict__ dels, uint64_t n_del, int* error) {
+  const uint64_t cap = base.mask + 1;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* src = xf_row(base, r);
+    const uint64_t key = __ldg(reinterpret_cast<const unsigned long long*>(src));
+    if (key == XF_EMPTY_KEY) continue;
+    if (n_del && xf_sorted_has(reinterpret_cast<const uint8_t*>(dels), n_del, 8u, key)) continue;
+    uint8_t* p = xf_model_claim<true>(out, key, error);
+    if (p) xf_model_copy_body(out, p, src);
+  }
+}
+
 // *flag = 1 if a delete key is also an upsert key
 __global__ void xf_k_delta_overlap(const uint8_t* __restrict__ rows, uint64_t n_up, uint32_t stride,
                                    const uint64_t* __restrict__ dels, uint64_t n_del, int* flag) {
@@ -216,7 +298,8 @@ __global__ void xf_k_delta_overlap(const uint8_t* __restrict__ rows, uint64_t n_
 // the fingerprint and row count of the rows of `v`, added into d_out[0], d_out[1] on `st`
 static int xf_launch_fingerprint(const XfTableView& v, int fm, unsigned long long* d_out, cudaStream_t st) {
   const int grid = xf_grid_for(v.mask + 1, 256, 8);
-  if (fm) xf_k_fingerprint<true><<<grid, 256, 0, st>>>(v, d_out);
+  if (fm == XF_SERVE_FMC) xf_k_fingerprint_fmc<<<grid, 256, 0, st>>>(v, d_out);
+  else if (fm) xf_k_fingerprint<true><<<grid, 256, 0, st>>>(v, d_out);
   else xf_k_fingerprint<false><<<grid, 256, 0, st>>>(v, d_out);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
@@ -241,7 +324,10 @@ static int xf_delta_list(const XfTableView& a, const XfTableView& b, int fm, boo
   uint64_t* ko = s.keys_in.as<uint64_t>();
   uint32_t* so = s.slots_in.as<uint32_t>();
   unsigned long long* c = s.count.as<unsigned long long>();
-  if (fm) {
+  if (fm == XF_SERVE_FMC) {
+    if (del) xf_k_delta_emit_fmc<true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
+    else xf_k_delta_emit_fmc<false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
+  } else if (fm) {
     if (del) xf_k_delta_emit<true, true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
     else xf_k_delta_emit<true, false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
   } else {
@@ -364,7 +450,8 @@ static int xf_apply_into(xf_model* base, const xf_delta* d, xf_model* m) {
   XF_TRY(xf_model_insert_rows(m->view, static_cast<const uint8_t*>(d->rows.p), h.upserts, d_error, st));
   const int grid = xf_grid_for(base->view.mask + 1, 256, 8);
   const uint64_t* dels = static_cast<const uint64_t*>(d->dels.p);
-  if (m->fm) xf_k_apply_base<true><<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
+  if (m->fm == XF_SERVE_FMC) xf_k_apply_base_fmc<<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
+  else if (m->fm) xf_k_apply_base<true><<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
   else xf_k_apply_base<false><<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
   XF_CUDA_TRY(cudaGetLastError());
   XF_TRY(xf_launch_fingerprint(m->view, m->fm, fp + 2, st));
@@ -495,7 +582,12 @@ XF_DLL int xf_delta_save(xf_delta* d, const char* path) {
 
 // the header's own consistency (after its checksum): every size derived from it is bounded before it is used
 static bool xf_sd_header_sane(const XfDeltaHeader& h) {
-  if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u) || h.zero != 0) return false;
+  if (h.fm == XF_SERVE_FMC) {
+    if (!xf_fmc_latent_ok(h.latent_dim) || h.row_bytes != xf_model_row_bytes(h.fm, h.latent_dim)) return false;
+  } else if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) {
+    return false;
+  }
+  if (h.zero != 0) return false;
   if (h.absent != XF_ABSENT_DEFAULT && h.absent != XF_ABSENT_ZERO) return false;
   if (h.optimizer != XF_OPT_FTRL && h.optimizer != XF_OPT_SGD) return false;
   if (h.v_init != 0 && h.v_init != XF_INIT_COUNTER && h.v_init != XF_INIT_ZERO) return false;
@@ -508,9 +600,10 @@ static bool xf_sd_header_sane(const XfDeltaHeader& h) {
 }
 
 // one section: n entries of `bytes` bytes into device memory `dst`, checked chunk by chunk; rows (bytes > 8) carry
-// their key in the first word and padding after byte `used`
+// their key in the first word and padding after byte `used`, canonical rows (canon_k = K > 0) where
+// xf_fmc_padding_zero says
 static int xf_sd_load_section(xf_delta* d, FILE* f, const char* path, uint8_t* dst, uint64_t n, uint32_t bytes, uint32_t used,
-                              uint64_t per_chunk, uint64_t* chunk, const char* what) {
+                              int canon_k, uint64_t per_chunk, uint64_t* chunk, const char* what) {
   uint64_t prev = 0;
   for (uint64_t first = 0; first < n; first += per_chunk, ++*chunk) {
     const uint64_t c = std::min<uint64_t>(per_chunk, n - first);
@@ -533,7 +626,11 @@ static int xf_sd_load_section(xf_delta* d, FILE* f, const char* path, uint8_t* d
         return XF_ERR_IO;
       }
       prev = key;
-      for (uint32_t b = used; b < bytes; ++b)
+      if (canon_k > 0 && !xf_fmc_padding_zero(p, canon_k, bytes)) {
+        xf_set_error("delta file %s: upsert row %llu has non-zero padding", path, (unsigned long long)(first + r));
+        return XF_ERR_IO;
+      }
+      for (uint32_t b = used; b < bytes && canon_k == 0; ++b)
         if (p[b] != 0) {
           xf_set_error("delta file %s: upsert row %llu has non-zero padding", path, (unsigned long long)(first + r));
           return XF_ERR_IO;
@@ -560,9 +657,9 @@ static int xf_sd_load_body(xf_delta* d, FILE* f, const char* path, const XfDelta
   XF_TRY(d->dels.ensure(std::max<uint64_t>(h.deletes * 8, 16)));
   XF_TRY(d->stage.ensure(std::max<uint64_t>(std::min<uint64_t>(XF_ST_CHUNK_BYTES, std::max(h.upserts * h.row_bytes, h.deletes * 8)), 16)));
   uint64_t chunk = 0;
-  XF_TRY(xf_sd_load_section(d, f, path, d->rows.as<uint8_t>(), h.upserts, h.row_bytes, h.fm ? 20u : 12u, h.chunk_rows, &chunk,
-                            "upsert"));
-  XF_TRY(xf_sd_load_section(d, f, path, d->dels.as<uint8_t>(), h.deletes, 8u, 8u, h.chunk_keys, &chunk, "delete"));
+  XF_TRY(xf_sd_load_section(d, f, path, d->rows.as<uint8_t>(), h.upserts, h.row_bytes, h.fm ? 20u : 12u,
+                            h.fm == XF_SERVE_FMC ? h.latent_dim : 0, h.chunk_rows, &chunk, "upsert"));
+  XF_TRY(xf_sd_load_section(d, f, path, d->dels.as<uint8_t>(), h.deletes, 8u, 8u, 0, h.chunk_keys, &chunk, "delete"));
   if (h.upserts && h.deletes) {
     XfDevBuf flag;
     struct Release { XfDevBuf* b; ~Release() { b->release(); } } rel{&flag};

@@ -13,6 +13,14 @@
 //                                 step kernels' forward pass (step.cu, step_lazy.cu), so the result is theirs bit for bit;
 //                                 no insert, no atomics, no shared memory
 //   file     rows sorted by key (cub radix sort of (key, slot)), gathered a chunk at a time through bounded staging
+//
+// A canonical model (xf_table_freeze_canonical, fm = XF_SERVE_FMC) serves the textbook FM with feature values
+// (step_fmc.cu), whose per-k sums do not collapse: its row is {key, w, 0, v[K]} padded to a multiple of 32 bytes.
+//   freeze   xf_k_freeze_fmc<COUNT>  the same two passes; v is the row's latent block or its initial values
+//   predict  xf_k_serve_fmc<C>       xf_k_step_fmc's mapping (C = K/4 lanes per token), its per-lane order, its
+//                                    reductions and its FMA contraction, spelled out (xf_fmc_add, xf_fmc_arg); the C
+//                                    lanes of a token load the head and their 16-byte piece of the home slot at once;
+//                                    two passes in flight
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
@@ -106,10 +114,121 @@ xf_k_serve(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, cons
   }
 }
 
-static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, float* pctr_out,
-                            cudaStream_t st) {
+// ---- canonical rows {key, w, 0, v[K]}: the forward of xf_k_step_fmc (mode 1) on the model's rows
+// A token's head {key, w} and lane c's latent piece v[4c .. 4c+3] of the row at p, as two non-coherent loads issued
+// back to back (the C lanes of a token load the same head: one request)
+__device__ __forceinline__ void xf_fmc_load(const uint8_t* p, int c, uint64_t& key, float& w, float4& v) {
+  uint64_t q0, q1;
+  asm("ld.global.nc.v2.u64 {%0,%1}, [%6];\n\tld.global.nc.v4.f32 {%2,%3,%4,%5}, [%7];"
+      : "=l"(q0), "=l"(q1), "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+      : "l"(p), "l"(p + 16 + 16 * c));
+  key = q0;
+  w = __uint_as_float((uint32_t)q1);
+}
+
+// The canonical forward's arithmetic, op for op as xf_k_step_fmc's machine code does it.  step_fmc.cu writes it with
+// plain operators and nvcc contracts them into FMAs; which products it fuses is read off its SASS (cuobjdump -sass:
+// the FMUL / FFMA / FADD after the latent load) and spelled out here with explicit rounding, so that this kernel
+// computes the same bits whatever its own instantiation would contract:
+//   a_k = x v_k;  S_k += a_k;  Q += fma(a3, a3, fma(a2, a2, fma(a1, a1, a0 a0)));  wx = fma(w, x, wx)  (lane c == 0)
+//   s2 = fma(S3, S3, fma(S2, S2, fma(S0, S0, S1 S1)))  then the shuffle sums;  arg = fma(0.5, s2 - Q, wx)
+__device__ __forceinline__ void xf_fmc_add(const float4& v, float x, float w, bool lead, float (&S)[4], float& Q, float& wx) {
+  const float a0 = __fmul_rn(v.x, x), a1 = __fmul_rn(v.y, x), a2 = __fmul_rn(v.z, x), a3 = __fmul_rn(v.w, x);
+  S[0] = __fadd_rn(S[0], a0); S[1] = __fadd_rn(S[1], a1); S[2] = __fadd_rn(S[2], a2); S[3] = __fadd_rn(S[3], a3);
+  Q = __fadd_rn(Q, __fmaf_rn(a3, a3, __fmaf_rn(a2, a2, __fmaf_rn(a1, a1, __fmul_rn(a0, a0)))));
+  if (lead) wx = __fmaf_rn(w, x, wx);
+}
+// S_k over the tokens (lanes with the same c), sum_k S_k^2 over the c's, Q and wx over the warp, in xf_k_step_fmc's
+// order; the argument of the sigmoid
+template <int C>
+__device__ __forceinline__ float xf_fmc_arg(float (&S)[4], float Q, float wx) {
+#pragma unroll
+  for (int e = 0; e < 4; ++e)
+#pragma unroll
+    for (int o = C; o < 32; o <<= 1) S[e] = __fadd_rn(S[e], __shfl_xor_sync(0xffffffffu, S[e], o));
+  float s2 = __fmaf_rn(S[3], S[3], __fmaf_rn(S[2], S[2], __fmaf_rn(S[0], S[0], __fmul_rn(S[1], S[1]))));
+#pragma unroll
+  for (int o = 1; o < C; o <<= 1) s2 = __fadd_rn(s2, __shfl_xor_sync(0xffffffffu, s2, o));
+  Q = xf_warp_sum(Q);
+  wx = xf_warp_sum(wx);
+  return __fmaf_rn(0.5f, __fsub_rn(s2, Q), wx);
+}
+
+// one token into the lane's sums: its row found from the home slot the caller loaded (k, w, v), or the absent policy
+__device__ __forceinline__ void xf_fmc_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float w,
+                                                   float4 v, float x, int c, float (&S)[4], float& Q, float& wx) {
+  bool have = false;
+  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
+    if (k == key) { have = true; break; }
+    if (k == XF_EMPTY_KEY) break;
+    xf_fmc_load(xf_row(m, xf_probe_slot(m, key, i)), c, k, w, v);
+  }
+  if (!have) {
+    if (absent == XF_ABSENT_ZERO) return;
+    // the row the table would insert: w = 0 and a latent block that is not materialised
+    w = 0.f;
+    v = make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
+                    xf_v_init(m, key, 4 * c + 3));
+  }
+  xf_fmc_add(v, x, w, c == 0, S, Q, wx);
+}
+
+// One warp per row, C = K/4 lanes per token and T = 32/C tokens per pass, as xf_k_step_fmc; two passes in flight.  A
+// lane adds its tokens in the order of the step kernel's passes, with its arithmetic (xf_fmc_add, xf_fmc_arg), so the
+// result is the table's bit for bit.  No insert, no atomics, no shared memory.
+template <int C>
+__global__ void __launch_bounds__(256)
+xf_k_serve_fmc(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
+               const float* __restrict__ vals, int B, float* __restrict__ pctr_out) {
+  constexpr int T = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const int tg = lane / C;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
+  const int nwarps = gridDim.x * warps_per_block;
+  for (int row = gwarp; row < B; row += nwarps) {
+    const uint32_t beg = __ldg(row_ptr + row);
+    const uint32_t end = __ldg(row_ptr + row + 1);
+    float S[4] = {0.f, 0.f, 0.f, 0.f};
+    float Q = 0.f, wx = 0.f;
+    for (uint32_t j0 = beg; j0 < end; j0 += 2u * T) {
+      const uint32_t ja = j0 + (uint32_t)tg, jb = ja + (uint32_t)T;
+      const bool va = ja < end, vb = jb < end;
+      // streaming: do not displace model rows in L2
+      const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+      const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+      const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+      const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+      // both home rows are in flight before either is resolved
+      uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+      float wa = 0.f, wb = 0.f;
+      float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
+      if (va) xf_fmc_load(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+      if (vb) xf_fmc_load(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+      if (va) xf_fmc_serve_token(m, absent, ka, ra, wa, pa, xa, c, S, Q, wx);
+      if (vb) xf_fmc_serve_token(m, absent, kb, rb, wb, pb, xb, c, S, Q, wx);
+    }
+    const float arg = xf_fmc_arg<C>(S, Q, wx);
+    if (lane == 0) pctr_out[row] = xf_sigmoid(arg);
+  }
+}
+
+static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals, uint32_t rows,
+                            float* pctr_out, cudaStream_t st) {
   if (rows == 0) return;
   const int grid = xf_grid_for((uint64_t)rows * 32, 256, 8);
+  if (m->fm == XF_SERVE_FMC) {
+    switch (m->view.K) {
+      case 4: xf_k_serve_fmc<1><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+      case 8: xf_k_serve_fmc<2><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+      case 16: xf_k_serve_fmc<4><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+      case 32: xf_k_serve_fmc<8><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+      case 64: xf_k_serve_fmc<16><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+      default: xf_k_serve_fmc<32><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    }
+    return;
+  }
   if (m->fm) xf_k_serve<true><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
   else xf_k_serve<false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
 }
@@ -149,6 +268,78 @@ xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, unsigned long l
       if (kept_n) atomicAdd(counts, (unsigned long long)kept_n);
       if (live_n) atomicAdd(counts + 1, (unsigned long long)live_n);
     }
+  }
+}
+
+// latent piece q (coordinates 4q .. 4q+3) of a canonical table's row r as a reader resolves it: the row's block if it is
+// materialised, else the initial values
+__device__ __forceinline__ float4 xf_fmc_piece(const XfTableView& t, uint64_t r, bool ready, uint64_t key, uint32_t q) {
+  if (ready) return __ldcg(reinterpret_cast<const float4*>(xf_row(t, r) + 32) + q);
+  return make_float4(xf_v_init(t, key, 4 * q), xf_v_init(t, key, 4 * q + 1), xf_v_init(t, key, 4 * q + 2),
+                     xf_v_init(t, key, 4 * q + 3));
+}
+
+// xf_k_freeze for a canonical table: the model row is {key, w, 0, v[K]} with v resolved as xf_fmc_piece does.  Prune:
+// w == 0 and, under DEFAULT, a latent block that is not materialised; under ZERO, every resolved v_k == 0.
+template <bool COUNT>
+__global__ void __launch_bounds__(256)
+xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned long long* __restrict__ counts, int* error) {
+  const uint64_t cap = t.mask + 1;
+  const uint32_t pieces = (uint32_t)t.K >> 2;
+  unsigned int kept_n = 0, live_n = 0;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    const XfHead h = xf_load_head(xf_row(t, r));
+    if (h.key == XF_EMPTY_KEY) continue;
+    ++live_n;
+    const bool ready = (h.flags & XF_FLAG_V_READY) != 0u;
+    bool keep = true;
+    if (prune && h.w == 0.0f) {
+      keep = false;
+      if (absent == XF_ABSENT_DEFAULT) keep = ready;
+      else
+        for (uint32_t q = 0; q < pieces && !keep; ++q) {
+          const float4 v = xf_fmc_piece(t, r, ready, h.key, q);
+          keep = v.x != 0.0f || v.y != 0.0f || v.z != 0.0f || v.w != 0.0f;
+        }
+    }
+    if (!keep) continue;
+    ++kept_n;
+    if (COUNT) continue;
+    uint8_t* p = xf_model_claim(m, h.key, error);
+    if (!p) continue;
+    *reinterpret_cast<float*>(p + 8) = h.w;  // bytes 12 .. 15 and the tail stay as the fill left them: zero
+    for (uint32_t q = 0; q < pieces; ++q) reinterpret_cast<float4*>(p + 16)[q] = xf_fmc_piece(t, r, ready, h.key, q);
+  }
+  if (COUNT) {
+    kept_n = __reduce_add_sync(0xffffffffu, kept_n);
+    live_n = __reduce_add_sync(0xffffffffu, live_n);
+    if ((threadIdx.x & 31u) == 0u) {
+      if (kept_n) atomicAdd(counts, (unsigned long long)kept_n);
+      if (live_n) atomicAdd(counts + 1, (unsigned long long)live_n);
+    }
+  }
+}
+
+// insert n packed canonical rows into `m`
+__global__ void xf_k_model_insert_rows_fmc(XfTableView m, const uint8_t* __restrict__ rows, uint64_t n, int* error) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* src = rows + i * m.stride;
+    uint8_t* p = xf_model_claim(m, *reinterpret_cast<const uint64_t*>(src), error);
+    if (p) xf_model_copy_body(m, p, src);
+  }
+}
+
+// what a canonical model holds for keys[0 .. n): w, v[n][K] (either may be nullptr), present
+__global__ void xf_k_model_lookup_fmc(XfTableView m, const uint64_t* __restrict__ keys, uint64_t n, float* w_out, float* v_out,
+                                      uint8_t* present) {
+  const int K = m.K;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const int64_t s = xf_model_find_slot(m, keys[i]);
+    const float* p = s >= 0 ? reinterpret_cast<const float*>(xf_row(m, (uint64_t)s)) : nullptr;
+    if (w_out) w_out[i] = p ? p[2] : 0.f;
+    if (v_out)
+      for (int k = 0; k < K; ++k) v_out[i * K + k] = p ? p[4 + k] : 0.f;
+    present[i] = p ? 1 : 0;
   }
 }
 
@@ -216,7 +407,8 @@ int xf_model_alloc(xf_model* m, uint64_t capacity) {
     xf_set_error("a serving model of %llu slots exceeds 2^32", (unsigned long long)capacity);
     return XF_ERR_FULL;
   }
-  const uint32_t stride = m->fm ? 32u : 16u;
+  const uint32_t stride = xf_model_row_bytes(m->fm, m->view.K);
+  m->view.canon = m->fm == XF_SERVE_FMC ? 1 : 0;
   uint8_t* base = nullptr;
   XF_CUDA_TRY(cudaMalloc(&base, capacity * stride));
   m->view.base = base;
@@ -237,7 +429,7 @@ void xf_model_free(xf_model* m) {
   cudaSetDevice(m->device);
   if (m->stream) cudaStreamSynchronize(m->stream);
   if (m->view.base) cudaFree(m->view.base);
-  m->s_row_ptr.release(); m->s_keys.release(); m->s_out.release(); m->s_aux.release();
+  m->s_row_ptr.release(); m->s_keys.release(); m->s_out.release(); m->s_aux.release(); m->s_vals.release();
   m->h_in.release(); m->h_out.release();
   if (m->stream) cudaStreamDestroy(m->stream);
   delete m;
@@ -282,7 +474,8 @@ int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, voi
 
 int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st) {
   if (n == 0) return XF_OK;
-  xf_k_model_insert_rows<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
+  if (v.canon) xf_k_model_insert_rows_fmc<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
+  else xf_k_model_insert_rows<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }
@@ -295,15 +488,15 @@ XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
   return XF_OK;
 }
 
-// the body of xf_table_freeze: on failure the caller frees `m`
-static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, xf_model* m) {
+// the body of xf_table_freeze (canonical = 0) and xf_table_freeze_canonical: on failure the caller frees `m`
+static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonical, xf_model* m) {
   const int src_dev = t->cfg.device;
   XF_CUDA_TRY(cudaSetDevice(src_dev));
   XF_TRY(t->check_error());  // waits for everything enqueued on the table's stream
   m->device = src_dev;
   XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   const XfTableView& tv = t->view;
-  m->fm = tv.K > 0;
+  m->fm = canonical ? XF_SERVE_FMC : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
   m->optimizer = tv.opt;
   m->absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
   m->view.K = tv.K;
@@ -322,7 +515,8 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, xf_model* m)
   const int grid = xf_grid_for(tv.mask + 1, 256, 8);
   const int prune = cfg.prune ? 1 : 0;
 #define XF_FREEZE_LAUNCH(COUNT)                                                                               \
-  switch (xf_vec_for(tv.K)) {                                                                                 \
+  if (canonical) xf_k_freeze_fmc<COUNT><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
+  else switch (xf_vec_for(tv.K)) {                                                                                 \
     case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
     case 2: xf_k_freeze<COUNT, 2><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
     default: xf_k_freeze<COUNT, 1><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
@@ -342,7 +536,7 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, xf_model* m)
   XF_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaStreamSynchronize(st));
   if ((int)counts[2] != 0) {
-    xf_set_error("xf_table_freeze: a probe sequence of the model overflowed");
+    xf_set_error("%s: a probe sequence of the model overflowed", canonical ? "xf_table_freeze_canonical" : "xf_table_freeze");
     return XF_ERR_FULL;
   }
   if (cfg.device >= 0 && cfg.device != src_dev) {
@@ -366,30 +560,43 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, xf_model* m)
   return XF_OK;
 }
 
-XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg_in, xf_model** out) {
+static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical, xf_model** out) {
+  const char* fn = canonical ? "xf_table_freeze_canonical" : "xf_table_freeze";
   if (out) *out = nullptr;
   if (!t || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
   xf_freeze_config cfg;
   xf_freeze_config_default(&cfg);
   if (cfg_in) cfg = *cfg_in;
-  if (cfg.absent < -1 || cfg.absent > XF_ABSENT_ZERO) { xf_set_error("xf_table_freeze: absent = %d is not an XF_ABSENT_* policy", cfg.absent); return XF_ERR_ARG; }
-  if (cfg.device >= xf_device_count()) { xf_set_error("xf_table_freeze: no CUDA device %d", cfg.device); return XF_ERR_ARG; }
-  if (t->cfg.canonical_fm) {
-    xf_set_error("xf_table_freeze: a canonical table (canonical_fm = 1) has no serving model: the per-k sums of the canonical "
-                 "FM and the multi-view machine do not collapse to one pair of sums per key");
+  if (cfg.absent < -1 || cfg.absent > XF_ABSENT_ZERO) { xf_set_error("%s: absent = %d is not an XF_ABSENT_* policy", fn, cfg.absent); return XF_ERR_ARG; }
+  if (cfg.device >= xf_device_count()) { xf_set_error("%s: no CUDA device %d", fn, cfg.device); return XF_ERR_ARG; }
+  if (!canonical && t->cfg.canonical_fm) {
+    xf_set_error("xf_table_freeze: a canonical table (canonical_fm = 1) has no collapsed serving model: the per-k sums of "
+                 "the canonical FM and the multi-view machine do not collapse to one pair of sums per key; "
+                 "xf_table_freeze_canonical serves it with the canonical FM's forward");
+    return XF_ERR_ARG;
+  }
+  if (canonical && (!t->cfg.canonical_fm || !xf_fmc_latent_ok(t->cfg.latent_dim))) {
+    xf_set_error("xf_table_freeze_canonical: the table is not canonical (canonical_fm = %d, latent_dim = %d): freeze it "
+                 "with xf_table_freeze", t->cfg.canonical_fm, t->cfg.latent_dim);
     return XF_ERR_ARG;
   }
   if (t->cfg.num_shards > 1) {
-    xf_set_error("xf_table_freeze: the table is shard %d of %d: one shard's rows are not a model", t->cfg.shard_index,
+    xf_set_error("%s: the table is shard %d of %d: one shard's rows are not a model", fn, t->cfg.shard_index,
                  t->cfg.num_shards);
     return XF_ERR_ARG;
   }
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   xf_model* m = new xf_model;
-  const int rc = xf_freeze_into(t, cfg, m);
+  const int rc = xf_freeze_into(t, cfg, canonical, m);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
   *out = m;
   return XF_OK;
+}
+
+XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out) { return xf_freeze(t, cfg, false, out); }
+
+XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
+  return xf_freeze(t, cfg, true, out);
 }
 
 XF_DLL int xf_model_destroy(xf_model* m) {
@@ -423,23 +630,37 @@ static int xf_model_stage(xf_model* m, XfDevBuf& dev, size_t off, const void* sr
   return XF_OK;
 }
 
-XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, uint32_t nnz,
-                                 float* pctr_out) {
+// feature values are read by canonical models only: the LR and FM forwards ignore them
+static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
+  if (vals && m->fm != XF_SERVE_FMC) {
+    xf_set_error("%s: an %s model ignores feature values: pass vals = NULL (values need a model frozen with "
+                 "xf_table_freeze_canonical)", fn, m->fm ? "FM" : "LR");
+    return XF_ERR_ARG;
+  }
+  return XF_OK;
+}
+
+static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals, uint32_t rows,
+                           uint32_t nnz, float* pctr_out, const char* fn) {
   if (!m || !row_ptr || (!keys && nnz) || (!pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_check_vals(m, vals, fn));
   for (uint32_t r = 0; r < rows; ++r)
-    if (row_ptr[r] > row_ptr[r + 1]) { xf_set_error("xf_model_predict_host: row_ptr decreases at row %u", r); return XF_ERR_ARG; }
-  if (row_ptr[rows] > nnz) { xf_set_error("xf_model_predict_host: row_ptr ends at %u, past nnz = %u", row_ptr[rows], nnz); return XF_ERR_ARG; }
-  XF_TRY(xf_check_host_keys(keys, nnz, "xf_model_predict_host"));
+    if (row_ptr[r] > row_ptr[r + 1]) { xf_set_error("%s: row_ptr decreases at row %u", fn, r); return XF_ERR_ARG; }
+  if (row_ptr[rows] > nnz) { xf_set_error("%s: row_ptr ends at %u, past nnz = %u", fn, row_ptr[rows], nnz); return XF_ERR_ARG; }
+  XF_TRY(xf_check_host_keys(keys, nnz, fn));
   if (rows == 0) return XF_OK;
   std::lock_guard<std::mutex> lock(m->mu);
   XF_CUDA_TRY(cudaSetDevice(m->device));
   const size_t rp_bytes = ((size_t)rows + 1) * 4, rp_pad = (rp_bytes + 15) & ~(size_t)15, key_bytes = (size_t)nnz * 8;
-  XF_TRY(m->h_in.ensure(rp_pad + key_bytes));
+  const size_t val_bytes = vals ? (size_t)nnz * 4 : 0;
+  XF_TRY(m->h_in.ensure(rp_pad + key_bytes + val_bytes));
   XF_TRY(m->h_out.ensure((size_t)rows * 4));
   XF_TRY(m->s_out.ensure((size_t)rows * 4));
   XF_TRY(xf_model_stage(m, m->s_row_ptr, 0, row_ptr, rp_bytes));
   XF_TRY(xf_model_stage(m, m->s_keys, rp_pad, keys, key_bytes));
-  xf_launch_serve(m, m->s_row_ptr.as<uint32_t>(), m->s_keys.as<uint64_t>(), rows, m->s_out.as<float>(), m->stream);
+  if (vals) XF_TRY(xf_model_stage(m, m->s_vals, rp_pad + key_bytes, vals, val_bytes));
+  xf_launch_serve(m, m->s_row_ptr.as<uint32_t>(), m->s_keys.as<uint64_t>(), vals ? m->s_vals.as<float>() : nullptr, rows,
+                  m->s_out.as<float>(), m->stream);
   XF_CUDA_TRY(cudaGetLastError());
   XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_out.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, m->stream));
   XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
@@ -447,11 +668,31 @@ XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uin
   return XF_OK;
 }
 
+XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, uint32_t nnz,
+                                 float* pctr_out) {
+  return xf_predict_host(m, row_ptr, keys, nullptr, rows, nnz, pctr_out, "xf_model_predict_host");
+}
+
+XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
+                                        uint32_t rows, uint32_t nnz, float* pctr_out) {
+  return xf_predict_host(m, row_ptr, keys, vals, rows, nnz, pctr_out, "xf_model_predict_host_values");
+}
+
 XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
   if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
   XF_CUDA_TRY(cudaSetDevice(m->device));
-  xf_launch_serve(m, d_row_ptr, d_keys, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  xf_launch_serve(m, d_row_ptr, d_keys, nullptr, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, const float* d_vals,
+                                          uint32_t rows, uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
+  if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_check_vals(m, d_vals, "xf_model_predict_device_values"));
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  xf_launch_serve(m, d_row_ptr, d_keys, d_vals, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }
@@ -459,6 +700,11 @@ XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
                                      uint8_t* labels_out) {
   if (!m || !tr) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (m->fm == XF_SERVE_FMC) {
+    xf_set_error("xf_model_predict_ingested: a canonical model reads feature values, which an ingested text block does "
+                 "not carry: use xf_model_predict_host_values / _device_values");
+    return XF_ERR_ARG;
+  }
   if (tr->cfg.model != (m->fm ? XF_MODEL_FM : XF_MODEL_LR)) {
     xf_set_error("xf_model_predict_ingested: the trainer's model (%d) is not the serving model's (%s)", tr->cfg.model,
                  m->fm ? "FM" : "LR");
@@ -479,7 +725,7 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
   cudaStream_t st = tr->table->stream;  // the block's parse is ordered before this stream's work
   XF_TRY(m->s_out.ensure((size_t)rows * 4));
   // row_ptr holds absolute token offsets: a slice is a shifted row_ptr
-  xf_launch_serve(m, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(), rows, m->s_out.as<float>(), st);
+  xf_launch_serve(m, g.row_ptr.as<uint32_t>() + row_start, g.keys.as<uint64_t>(), nullptr, rows, m->s_out.as<float>(), st);
   XF_CUDA_TRY(cudaGetLastError());
   XF_CUDA_TRY(cudaMemcpyAsync(pctr_out, m->s_out.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
   if (labels_out) XF_CUDA_TRY(cudaMemcpyAsync(labels_out, g.labels.as<uint8_t>() + row_start, rows, cudaMemcpyDeviceToHost, st));
@@ -488,8 +734,49 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
   return XF_OK;
 }
 
+// what a canonical model holds for n host keys: w[n], v[n][K], present[n] (any output may be NULL)
+static int xf_lookup_fmc(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* v, uint8_t* present) {
+  if (n == 0) return XF_OK;
+  const uint64_t K = (uint64_t)m->view.K;
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  XF_TRY(m->s_keys.ensure(n * 8));
+  XF_TRY(m->s_aux.ensure(n * (4 * K + 5)));  // v[n][K] w[n] present[n]
+  float* d_v = m->s_aux.as<float>();
+  float* d_w = d_v + n * K;
+  uint8_t* d_present = reinterpret_cast<uint8_t*>(d_w + n);
+  XF_CUDA_TRY(cudaMemcpyAsync(m->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, m->stream));
+  xf_k_model_lookup_fmc<<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w,
+                                                                      v ? d_v : nullptr, d_present);
+  XF_CUDA_TRY(cudaGetLastError());
+  if (w) XF_CUDA_TRY(cudaMemcpyAsync(w, d_w, n * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (v) XF_CUDA_TRY(cudaMemcpyAsync(v, d_v, n * K * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (present) XF_CUDA_TRY(cudaMemcpyAsync(present, d_present, n, cudaMemcpyDeviceToHost, m->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
+  return XF_OK;
+}
+
+XF_DLL int xf_model_lookup_latent(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* v, uint8_t* present) {
+  if (!m || (!keys && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (m->fm != XF_SERVE_FMC) {
+    xf_set_error("xf_model_lookup_latent: an %s model holds no latent rows: use xf_model_lookup", m->fm ? "FM" : "LR");
+    return XF_ERR_ARG;
+  }
+  XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup_latent"));
+  return xf_lookup_fmc(m, keys, n, w, v, present);
+}
+
 XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt, uint8_t* present) {
   if (!m || (!keys && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (m->fm == XF_SERVE_FMC) {
+    if (st || qt) {
+      xf_set_error("xf_model_lookup: a canonical model holds no st, qt: pass NULL, and read its latent rows with "
+                   "xf_model_lookup_latent");
+      return XF_ERR_ARG;
+    }
+    XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup"));
+    return xf_lookup_fmc(m, keys, n, w, nullptr, present);
+  }
   XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup"));
   if (n == 0) return XF_OK;
   std::lock_guard<std::mutex> lock(m->mu);
@@ -578,7 +865,11 @@ XF_DLL int xf_model_save(xf_model* m, const char* path) {
 
 // the header's own consistency (after its checksum): every size derived from it is bounded before it is used
 static bool xf_sm_header_sane(const XfModelHeader& h) {
-  if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) return false;
+  if (h.fm == XF_SERVE_FMC) {
+    if (!xf_fmc_latent_ok(h.latent_dim) || h.row_bytes != xf_model_row_bytes(h.fm, h.latent_dim)) return false;
+  } else if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) {
+    return false;
+  }
   if (h.keys > (1ull << 31) || h.capacity != xf_model_capacity(h.keys) || h.keys + h.pruned_keys != h.source_keys) return false;
   if (h.absent != XF_ABSENT_DEFAULT && h.absent != XF_ABSENT_ZERO) return false;
   if (h.optimizer != XF_OPT_FTRL && h.optimizer != XF_OPT_SGD) return false;
@@ -635,6 +926,10 @@ static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModel
         return XF_ERR_IO;
       }
       prev = key;
+      if (h.fm == XF_SERVE_FMC && !xf_fmc_padding_zero((const uint8_t*)m->h_in.p + r * h.row_bytes, h.latent_dim, h.row_bytes)) {
+        xf_set_error("model file %s: row %llu has non-zero padding", path, (unsigned long long)(first + r));
+        return XF_ERR_IO;
+      }
     }
     XF_CUDA_TRY(cudaMemcpyAsync(rows.p, m->h_in.p, c * h.row_bytes, cudaMemcpyHostToDevice, m->stream));
     XF_TRY(xf_model_insert_rows(m->view, rows.as<uint8_t>(), c, err.as<int>(), m->stream));

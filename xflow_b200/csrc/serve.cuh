@@ -9,17 +9,38 @@
 
 #include "internal.h"
 
+// what a model's rows hold (xf_model::fm, xf_model_info::fm, the files' fm field)
+enum { XF_SERVE_LR = 0, XF_SERVE_FM = 1, XF_SERVE_FMC = 2 };
+
 struct xf_model {
-  XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source
+  XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source;
+                           // canon = 1 for canonical rows
   int device = 0;
-  int fm = 0, absent = 0, optimizer = 0;
+  int fm = 0, absent = 0, optimizer = 0;  // fm: XF_SERVE_*
   uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
   cudaStream_t stream = nullptr;
   // staging of the host entry points, grown on demand; those calls are serialised by the mutex
   std::mutex mu;
-  XfDevBuf s_row_ptr, s_keys, s_out, s_aux;
+  XfDevBuf s_row_ptr, s_keys, s_out, s_aux, s_vals;
   XfPinBuf h_in, h_out;
 };
+
+// Bytes of a model row.  LR {key, w, 0}: 16; FM {key, w, st, qt, 0...}: 32; canonical FM {key, w, 0, v[K], 0...}:
+// 16 + 4K rounded up to 32, so that every row starts on a sector and lane c's piece v[4c .. 4c+3] lies at 16 + 16c.
+__host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K) {
+  if (fm == XF_SERVE_FMC) return (16u + 4u * (uint32_t)K + 31u) & ~31u;
+  return fm ? 32u : 16u;
+}
+// the latent dimensions a canonical model serves: C = K / 4 lanes per token, a power of two <= 32
+inline bool xf_fmc_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 128; }
+// a packed canonical row (K, row_bytes) has zero bytes where the layout has padding: [12, 16) and [16 + 4K, row_bytes)
+inline bool xf_fmc_padding_zero(const uint8_t* p, int K, uint32_t row_bytes) {
+  for (uint32_t b = 12; b < 16; ++b)
+    if (p[b]) return false;
+  for (uint32_t b = 16u + 4u * (uint32_t)K; b < row_bytes; ++b)
+    if (p[b]) return false;
+  return true;
+}
 
 // ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
 template <bool FM>
@@ -76,6 +97,41 @@ __device__ __forceinline__ void xf_model_insert(const XfTableView& m, uint64_t k
   *error = 1;
 }
 
+// ---- canonical rows (runtime stride: any K the model serves)
+// Claim a slot for `key` and return its row, for the caller to write bytes 8 .. stride; nullptr: not claimed.  The
+// error cases and KEEP are xf_model_insert's (a key KEEP finds is nullptr, its row untouched).
+template <bool KEEP = false>
+__device__ __forceinline__ uint8_t* xf_model_claim(const XfTableView& m, uint64_t key, int* error) {
+  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
+    uint8_t* rowp = xf_row(m, xf_probe_slot(m, key, i));
+    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(rowp), (unsigned long long)XF_EMPTY_KEY,
+                                             (unsigned long long)key);
+    if (old == XF_EMPTY_KEY) return rowp;
+    if (old == key) {
+      if (KEEP) return nullptr;
+      break;
+    }
+  }
+  *error = 1;
+  return nullptr;
+}
+// bytes 8 .. stride of the row at `src` into the row at `dst` (16-byte aligned, stride a multiple of 16)
+__device__ __forceinline__ void xf_model_copy_body(const XfTableView& m, uint8_t* dst, const uint8_t* src) {
+  *reinterpret_cast<uint64_t*>(dst + 8) = *reinterpret_cast<const uint64_t*>(src + 8);
+  for (uint32_t o = 16; o < m.stride; o += 16)
+    *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(src + o);
+}
+// the slot that holds `key`, or -1: the key words only, through the non-coherent path
+__device__ __forceinline__ int64_t xf_model_find_slot(const XfTableView& m, uint64_t key) {
+  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
+    const uint64_t s = xf_probe_slot(m, key, i);
+    const uint64_t k = __ldg(reinterpret_cast<const unsigned long long*>(xf_row(m, s)));
+    if (k == key) return (int64_t)s;
+    if (k == XF_EMPTY_KEY) return -1;
+  }
+  return -1;
+}
+
 // slots of a model of `keys` keys: the smallest power of two >= 2 x keys (load <= 0.5), at least 1024
 inline uint64_t xf_model_capacity(uint64_t keys) {
   uint64_t c = 1024;
@@ -83,7 +139,7 @@ inline uint64_t xf_model_capacity(uint64_t keys) {
   return c;
 }
 
-// the model's table on the current device: `capacity` empty rows (stride from m->fm), filled on m->stream;
+// the model's table on the current device: `capacity` empty rows (stride from m->fm, m->view.K), filled on m->stream;
 // XF_ERR_FULL past 2^32 slots
 int xf_model_alloc(xf_model* m, uint64_t capacity);
 // waits for the model's stream and frees everything (m may be NULL)
@@ -103,5 +159,6 @@ int xf_model_list_sorted(const XfTableView& v, uint64_t n, XfSortedSlots& s, cud
 int xf_sort_slots(XfSortedSlots& s, uint64_t n, cudaStream_t st);
 // out = the rows of `v` in slots[0 .. n), packed
 int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, void* out, cudaStream_t st);
-// insert n packed rows (as a model file holds them; keys unique) into `v`; a probe overflow or a key met twice sets *error
+// insert n packed rows (as a model file holds them; keys unique) into `v` (canonical rows if v.canon); a probe overflow
+// or a key met twice sets *error
 int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st);
