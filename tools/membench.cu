@@ -14,6 +14,17 @@
 // fetch granularity 32, 64 and 128 B (to within 1 %), in G rows/s: read 21.9, read pair 30.4-30.7 (1.40x),
 // CAS.128 only 12.0, load + CAS.128 10.3-10.4, read pair + CAS.128 10.3-10.5.  A paired look costs fewer requests
 // than a one-lane one, but a row that is also CAS'd is bound by the atomic.
+//   look, then CAS.128 after D MB (klag)  a lane-pair look at a row, and the CAS.128 on that row only after every
+//               thread of the grid has made `lag` more looks: D = the lines those looks bring into L2
+// On one H100 80GB HBM3 (SXM, power limit 700 W, SM clock 1980 MHz read after the run), 8 GiB table, 2 CTAs of 256
+// per SM (67 584 threads), 32 M rows per launch, best of 3; look alone 31.2 G rows/s; "CAS" = per-row time over the
+// look alone:
+//   D (MB of 128-B lines)   0      8.2    16.5   24.8   33.0   49.5   66.0
+//   G rows/s                12.34  11.06  9.51   8.89   8.76   8.74   8.73
+//   CAS, ps per row         49.0   58.4   73.1   80.4   82.0   82.3   82.5
+// At 32-B fetch granularity the CAS costs 81.9 ps already at 4 rounds (270 k other looks: 8.2 MB of sectors, but
+// 33 MB of 128-B lines) and 84.1 at 31 rounds: L2 room is counted in lines, so a finer fetch makes none.  The more
+// other lines were looked at since a row's look, the less often its CAS finds the line; past about 25 MB, almost never.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -151,6 +162,35 @@ __global__ void __launch_bounds__(256) k(uint8_t* base, uint64_t mask, uint64_t 
   if (acc == 0x123456789ull) *sink = acc;
 }
 
+// A lane-pair look at a row, then a CAS.128 on that row after `lag` more rounds of looks by every thread of the grid:
+// between a row's look and its CAS the GPU makes lag x (grid threads) other random looks, and D = that x the L2 fetch
+// granularity (the bytes those looks fetch).  The CAS compares against the newest look, so it waits for it (as the
+// step kernel's CAS waits for the row's looks); on the zeroed table both rows are almost always untouched and it
+// succeeds.  The last `lag` rounds look past n (fill and drain: at most 7 % more looks in the sweep below).
+__global__ void __launch_bounds__(256) klag(uint8_t* base, uint64_t mask, uint64_t n, uint64_t seed, uint32_t tag, int lag,
+                                            uint64_t* sink) {
+  const uint64_t T = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const uint64_t K = (n + T - 1) / T;
+  uint64_t acc = 0;
+  for (uint64_t k = 0; k < K + (uint64_t)lag; ++k) {
+    const uint64_t i = t + k * T;
+    uint64_t a, b, c, d;
+    ld256_pair(base + ((mix(seed + i) & mask) << 5), a, b, c, d);
+    acc += a ^ b;
+    if (k >= (uint64_t)lag && i - (uint64_t)lag * T < n) {
+      uint8_t* p = base + ((mix(seed + i - (uint64_t)lag * T) & mask) << 5);
+      uint64_t o0, o1;
+      const uint64_t n0 = c + 1, n1 = (d & 0xFFFFFFFFull) | ((uint64_t)tag << 32);
+      asm volatile("{\n .reg .b128 cmp, swp, old;\n mov.b128 cmp, {%2, %3};\n mov.b128 swp, {%4, %5};\n"
+                   " atom.global.cas.b128 old, [%6], cmp, swp;\n mov.b128 {%0, %1}, old;\n}"
+                   : "=l"(o0), "=l"(o1) : "l"(c), "l"(d), "l"(n0), "l"(n1), "l"(p + 16) : "memory");
+      acc += o0 ^ o1;
+    }
+  }
+  if (acc == 0x123456789ull) *sink = acc;
+}
+
 // V: 0 read 4 lanes x 4 x uint4 | 1 read 16 lanes x uint4 | 2 rmw 4 lanes | 3 rmw 16 lanes
 template <int V>
 __global__ void __launch_bounds__(256) krow(uint8_t* base, uint64_t mask, uint64_t n, uint64_t seed, uint64_t* sink) {
@@ -255,6 +295,39 @@ int main(int argc, char** argv) {
       printf("  prefetch.global.L2 check (2 M rows = 64 MB): cold read %.1f us, prefetch kernel %.1f us, read after prefetch %.1f us\n",
              cold * 1e3, pf * 1e3, warm * 1e3);
     }
+  }
+  // look, then CAS.128 on the same row after D MB of other looks (klag): does the CAS find the row's line in L2?
+  {
+    const uint64_t nl = 32000000;  // rows per launch: about 470 rounds of the 2-CTA-per-SM grid, 12 % of the table
+    const int bps = 2;
+    const uint64_t T = (uint64_t)g_sms * bps * 256;
+    const int dmb[] = {0, 8, 16, 24, 32, 48, 64};
+    for (int fetch = 128; fetch >= 32; fetch /= 4) {
+      cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, fetch);
+      const float look = run<M_READ_PAIR>("", base, nsect, nl, sink, bps, 31, false);
+      printf("look, then CAS.128 after D MB of other looks: L2 fetch granularity %d B, %llu threads, %llu rows per launch,"
+             " look alone %.2f G rows/s\n", fetch, (unsigned long long)T, (unsigned long long)nl, (double)nl / (look * 1e-3) / 1e9);
+      for (int di = 0; di < (int)(sizeof(dmb) / sizeof(dmb[0])); ++di) {
+        const int lag = (int)((double)dmb[di] * 1048576.0 / ((double)T * fetch) + 0.5);
+        float best = 1e30f;
+        for (int r = 0; r < 3; ++r) {
+          cudaEvent_t e0, e1;
+          cudaEventCreate(&e0); cudaEventCreate(&e1);
+          cudaMemset(base, 0, nsect * 32);  // every CAS finds the zeros it compares against, as on the first launch
+          cudaEventRecord(e0);
+          klag<<<g_sms * bps, 256>>>(base, nsect - 1, nl, 4242 + 1000 * r + 100 * di + fetch, 9 + r, lag, sink);
+          cudaEventRecord(e1);
+          cudaEventSynchronize(e1);
+          float ms; cudaEventElapsedTime(&ms, e0, e1);
+          if (ms < best) best = ms;
+        }
+        const double rate = (double)nl / (best * 1e-3) / 1e9;
+        printf("  D %5.1f MB (lag %2d rounds)  %8.1f us  %6.2f G rows/s  CAS after the look %5.1f ps per row\n",
+               (double)lag * T * fetch / 1048576.0, lag, best * 1e3, rate, 1e3 / rate - (double)look * 1e9 / nl);
+      }
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) printf("CUDA error: %s\n", cudaGetErrorString(e));
   }
   // 256-byte rows (the FM k=16 FTRL row): per-thread pieces vs one cooperative instruction per row
   {

@@ -633,8 +633,9 @@ __device__ __forceinline__ bool xf_lazy_deposit_issue(uint8_t* rowp, uint64_t q2
   xf_cas128(rowp + XF_OFF_STATE, q2, q3, q2_new, ((unsigned long long)fix << 16) | (uint64_t)seq, o2, o3);
   return true;
 }
-// returns true when the issued CAS opened the row.  Its one caller is the sharded owner, which works from the look
-// its Pull stashed: *stale reports a row that moved on to another batch since then (as in xf_lazy_deposit).
+// returns true when the issued CAS opened the row.  *stale reports a row that moved on to another batch since the
+// caller's look (as in xf_lazy_deposit): the sharded owner, which works from the look its Pull stashed, looks again;
+// for the lazy step kernel, whose look is from this batch, it is an error.
 __device__ __forceinline__ bool xf_lazy_deposit_resolve(uint8_t* rowp, bool issued, uint64_t q2, uint64_t q3, uint64_t o2,
                                                         uint64_t o3, uint32_t seq, long long fix, bool* stale) {
   *stale = false;
