@@ -538,7 +538,7 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *
  *    Refused with XF_ERR_ARG: tables with canonical_fm = 1 (the per-k sums of the canonical FM and the multi-view
  *    machine do not collapse to st, qt: xf_table_freeze_canonical serves them) and tables with num_shards > 1 (one
- *    shard's rows are not a model).
+ *    shard's rows are not a model: xf_table_freeze_part and xf_model_merge, below, serve them).
  *
  *    Canonical models.  xf_table_freeze_canonical freezes a table created with canonical_fm = 1 for the textbook FM
  *    with feature values (XF_MODEL_FM_CANONICAL): its predict is the canonical FM's forward, whichever trainer trained
@@ -561,6 +561,22 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *      The XFSM and XFSD files keep version 1 and record fm = 2, latent_dim and these row bytes; a load refuses
  *      non-zero padding in a canonical row.  Not served: the multi-view machine (XF_MODEL_MVM: its forward needs
  *      fields), shards.
+ *
+ *    Sharded tables: parts and merge.  A run sharded over S GPUs holds shard s of the key space in table s
+ *    (num_shards = S; shard s owns [s width, (s + 1) width) with width = floor((2^64 - 1) / S), the last shard up to
+ *    2^64 - 2, as xf_shard_of).  xf_table_freeze_part freezes one LR or FM table of any num_shards (1 included) into
+ *    a part: an xf_model whose rows are exactly those xf_table_freeze would make of the same table (the same
+ *    resolution, prune rule and absent policy; the table does not change) and which records shard_index and
+ *    num_shards.  xf_model_merge(parts of shards 0 .. S-1) builds the whole model: its contents, info and file are
+ *    those of xf_table_freeze applied to one unsharded table that holds the union of the shards' rows, so its
+ *    xf_model_save file is byte-identical to that freeze's, its predictions equal that model's bit for bit, and its
+ *    fingerprint is the sum mod 2^64 of the parts' fingerprints.  A part serves xf_model_get_info (its shard's keys,
+ *    source_keys, pruned_keys), xf_model_lookup, xf_model_fingerprint and xf_model_save (an XFSP file, below); it is
+ *    not a model: xf_model_predict_* (every variant), xf_model_diff and xf_model_apply_delta refuse it with
+ *    XF_ERR_STATE.  Memory of a merge: the parts, the result, and on the result's device one staging buffer of at
+ *    most 64 MiB for the slots of parts on other devices (peer copies, a chunk at a time).  The merge only reads the
+ *    parts.  Not provided: a model served sharded across GPUs, a merge over the comm's peer mappings without files
+ *    or staging, and deltas made from parts without merging them.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct xf_model xf_model;
 enum { XF_ABSENT_DEFAULT = 0, XF_ABSENT_ZERO = 1 };
@@ -578,6 +594,17 @@ XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** 
 /* A canonical model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG for tables with
  * canonical_fm = 0 and tables with num_shards > 1. */
 XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+/* A part of a table of any num_shards (above); the same config and defaults.  XF_ERR_ARG for canonical tables (they
+ * are never sharded); XF_ERR_STATE, naming their count, if the table holds keys outside its shard's range (a Pull,
+ * Push or import can put them there). */
+XF_DLL int xf_table_freeze_part(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+/* the shard a part holds; XF_ERR_STATE for a whole model */
+XF_DLL int xf_model_part_info(xf_model* m, int* shard_index, int* num_shards);
+/* The whole model of parts[0 .. n) on `device` (-1: parts[0]'s).  The parts must be shards 0 .. n-1 of one n-way
+ * split, each once, and agree on fm, latent_dim, optimizer, absent, the resolved v_init, v_const and seed (prune may
+ * differ): else XF_ERR_ARG, naming what is wrong.  XF_ERR_FULL past 2^32 slots or on a probe overflow.  No part
+ * changes; on failure *out is NULL. */
+XF_DLL int xf_model_merge(xf_model* const* parts, int n, int device, xf_model** out);
 XF_DLL int xf_model_destroy(xf_model* m);
 typedef struct xf_model_info {
   uint64_t keys;         /* keys the model holds */
@@ -599,7 +626,13 @@ XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
  *  splitmix64(word ^ offset), a chunk's offsets being chunk << 40 | byte offset in its rows).  The file is a function
  *  of the model's contents, not of where its keys lie: two freezes of one table, and load then save, give identical
  *  bytes.  Written to <path>.tmp and renamed; the staging is bounded by the chunk size.  xf_model_load rebuilds the
- *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL. */
+ *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL.
+ * Part file "XFSP" (xf_model_save of a part): XFSM's layout with a 112-byte header
+ *     0 "XFSP"   4 u32 version (1)   8 u64 header bytes (112)   16 .. 95 as XFSM's (the part's keys, capacity,
+ *    source and pruned keys; fm 0 or 1)   96 i32 shard_index   100 i32 num_shards   104 u64 checksum of bytes [0, 104)
+ *  then the part's rows sorted by key in XFSM's chunks.  xf_model_load reads either magic and returns a part for
+ *  XFSP; it also refuses (XF_ERR_IO) a part file whose keys do not ascend strictly, whose keys leave the shard's range,
+ *  or whose shard_index is not below num_shards.  xf_delta_load refuses both. */
 XF_DLL int xf_model_save(xf_model* m, const char* path);
 XF_DLL int xf_model_load(xf_model** out, const char* path, int device);
 /* Forward pass over a CSR batch (row r = keys[row_ptr[r] .. row_ptr[r+1]), row_ptr non-decreasing and <= nnz);

@@ -157,6 +157,9 @@ SIGNATURES = {
     "xf_freeze_config_default": (_i, [_vp]),
     "xf_table_freeze": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_canonical": (_i, [_vp, _vp, _vp]),
+    "xf_table_freeze_part": (_i, [_vp, _vp, _vp]),
+    "xf_model_part_info": (_i, [_vp, _vp, _vp]),
+    "xf_model_merge": (_i, [_vp, _i, _i, _vp]),
     "xf_model_destroy": (_i, [_vp]),
     "xf_model_get_info": (_i, [_vp, _vp]),
     "xf_model_save": (_i, [_vp, C.c_char_p]),
@@ -456,18 +459,42 @@ class Table:
         _check(lib().xf_table_freeze_canonical(self.h, C.byref(cfg), C.byref(h)))
         return Model(h)
 
+    def freeze_part(self, absent=None, prune=True, device=None):
+        """The part of a shard table (xf_table_freeze_part): the rows freeze would make of it, tagged with its shard;
+        Model.merge of every shard's part is the whole model.  Arguments as for freeze."""
+        cfg = FreezeConfig(-1 if absent is None else absent, 1 if prune else 0, -1 if device is None else device)
+        h = C.c_void_p()
+        _check(lib().xf_table_freeze_part(self.h, C.byref(cfg), C.byref(h)))
+        return Model(h)
+
 
 class Model:
-    """A frozen, read-only serving model (xf_model_*): made by Table.freeze or Model.load."""
+    """A frozen, read-only serving model (xf_model_*): made by Table.freeze, Model.merge or Model.load; or a part of
+    one (Table.freeze_part, Model.load of an XFSP file)."""
 
     def __init__(self, handle):
         self.h = handle
 
     @classmethod
     def load(cls, path, device=0):
+        """The model (XFSM file) or part (XFSP file) at `path`."""
         h = C.c_void_p()
         _check(lib().xf_model_load(C.byref(h), path.encode(), device))
         return cls(h)
+
+    @classmethod
+    def merge(cls, parts, device=-1):
+        """The whole model of the parts of shards 0 .. n-1 (xf_model_merge), on `device` (-1: parts[0]'s)."""
+        arr = (C.c_void_p * max(len(parts), 1))(*[p.h.value for p in parts])
+        h = C.c_void_p()
+        _check(lib().xf_model_merge(arr, len(parts), device, C.byref(h)))
+        return cls(h)
+
+    def part_info(self):
+        """(shard_index, num_shards) of a part; XflowError for a whole model."""
+        s, n = C.c_int(), C.c_int()
+        _check(lib().xf_model_part_info(self.h, C.byref(s), C.byref(n)))
+        return s.value, n.value
 
     def close(self):
         if getattr(self, "h", None):

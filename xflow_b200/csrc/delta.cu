@@ -68,28 +68,9 @@ struct xf_delta {
   XfPinBuf stage;
 };
 
-// what defines how an absent key reads: the fields two models (or a model and a delta) must agree on
-struct XfCompat {
-  int fm, latent_dim, optimizer, absent, v_init;
-  float v_const;
-  uint64_t seed;
-};
-static XfCompat xf_compat_of(const xf_model* m) {
-  return XfCompat{m->fm, m->view.K, m->optimizer, m->absent, m->view.v_init, m->view.v_const, m->view.seed};
-}
+// the delta's side of the compatibility check (serve.cuh: XfCompat)
 static XfCompat xf_compat_of(const XfDeltaHeader& h) {
   return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed};
-}
-// the first field that differs, or nullptr
-static const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
-  if (a.fm != b.fm) return "fm";
-  if (a.latent_dim != b.latent_dim) return "latent_dim";
-  if (a.optimizer != b.optimizer) return "optimizer";
-  if (a.absent != b.absent) return "absent";
-  if (a.v_init != b.v_init) return "v_init";
-  if (memcmp(&a.v_const, &b.v_const, sizeof(float)) != 0) return "v_const";
-  if (a.seed != b.seed) return "seed";
-  return nullptr;
 }
 
 static uint64_t xf_sd_chunks(uint64_t n, uint64_t per_chunk) { return (n + per_chunk - 1) / per_chunk; }
@@ -391,6 +372,8 @@ static int xf_diff_into(xf_model* base, xf_model* next, xf_delta* d) {
 XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out) {
   if (out) *out = nullptr;
   if (!base || !next || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(base, "xf_model_diff"));
+  XF_TRY(xf_refuse_part(next, "xf_model_diff"));
   if (const char* f = xf_compat_diff(xf_compat_of(base), xf_compat_of(next))) {
     xf_set_error("xf_model_diff: the models differ in %s: a delta carries contents only, not how an absent key reads", f);
     return XF_ERR_ARG;
@@ -474,6 +457,7 @@ static int xf_apply_into(xf_model* base, const xf_delta* d, xf_model* m) {
 XF_DLL int xf_model_apply_delta(xf_model* base, const xf_delta* d, xf_model** out) {
   if (out) *out = nullptr;
   if (!base || !d || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(base, "xf_model_apply_delta"));
   if (const char* f = xf_compat_diff(xf_compat_of(base), xf_compat_of(d->h))) {
     xf_set_error("xf_model_apply_delta: the model and the delta differ in %s", f);
     return XF_ERR_ARG;
@@ -686,8 +670,8 @@ XF_DLL int xf_delta_load(xf_delta** out, const char* path, int device) {
   memset(&h, 0, sizeof(h));
   const size_t got = fread(&h, 1, sizeof(h), f);
   int rc = XF_OK;
-  if (got >= 4 && memcmp(h.magic, "XFSM", 4) == 0) {
-    xf_set_error("%s is a serving model (XFSM), not a delta: load it with xf_model_load", path);
+  if (got >= 4 && (memcmp(h.magic, "XFSM", 4) == 0 || memcmp(h.magic, "XFSP", 4) == 0)) {
+    xf_set_error("%s is a serving model (%.4s), not a delta: load it with xf_model_load", path, h.magic);
     rc = XF_ERR_IO;
   } else if (got >= 4 && (memcmp(h.magic, "XFTB", 4) == 0 || memcmp(h.magic, "XFST", 4) == 0)) {
     xf_set_error("%s is a training checkpoint (%.4s), not a delta", path, h.magic);

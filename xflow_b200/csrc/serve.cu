@@ -14,6 +14,11 @@
 //                                 no insert, no atomics, no shared memory
 //   file     rows sorted by key (cub radix sort of (key, slot)), gathered a chunk at a time through bounded staging
 //
+// A part (xf_table_freeze_part) is what xf_k_freeze makes of one shard table, whose counting pass also counts the keys
+// outside the shard's range; its file is XFSP.  xf_model_merge makes the whole model of S parts:
+//   merge    xf_k_merge<FM>        a grid-stride walk over a part's slots in place (or a 64 MiB chunk of them peer-copied
+//                                  from another device), each live row inserted with xf_model_insert
+//
 // A canonical model (xf_table_freeze_canonical, fm = XF_SERVE_FMC) serves the textbook FM with feature values
 // (step_fmc.cu), whose per-k sums do not collapse: its row is {key, w, 0, v[K]} padded to a multiple of 32 bytes.
 //   freeze   xf_k_freeze_fmc<COUNT>  the same two passes; v is the row's latent block or its initial values
@@ -31,6 +36,7 @@
 #include <cub/cub.cuh>
 #include <mutex>
 #include <string>
+#include <vector>
 
 #include "serve.cuh"
 
@@ -61,6 +67,16 @@ struct XfModelHeader {
 static_assert(sizeof(XfModelHeader) == 104 && offsetof(XfModelHeader, seed) == 64 &&
                   offsetof(XfModelHeader, header_checksum) == 96,
               "the documented header is 104 bytes");
+
+// A part file "XFSP" (112 bytes): XFSM's header with its own magic, bytes [0, 96) as XFSM's, then the shard
+struct XfPartHeader {
+  uint8_t model[96];         //   0 XFSM's fields up to chunk_rows, magic "XFSP", header_bytes 112
+  int32_t shard_index;       //  96
+  int32_t num_shards;        // 100
+  uint64_t header_checksum;  // 104 over bytes [0, 104)
+};
+static_assert(sizeof(XfPartHeader) == 112 && offsetof(XfPartHeader, header_checksum) == 104,
+              "the documented part header is 112 bytes");
 
 // one token's terms into the lane's sums, in the order the step kernels add them
 template <bool FM>
@@ -239,17 +255,19 @@ __global__ void xf_k_model_fill(uint4* base, uint64_t chunks16, uint32_t per_row
     base[c] = (c % per_row == 0) ? make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u) : make_uint4(0u, 0u, 0u, 0u);
 }
 
-// Slot r of the training table as a reader resolves it, and whether the model keeps it.  COUNT: count the rows kept
-// and the live rows; else insert the rows kept into `m`.
+// Slot r of the training table as a reader resolves it, and whether the model keeps it.  COUNT: count the rows kept,
+// the live rows and the live keys outside [lo, hi] (counts[3]: a part's foreign keys); else insert the rows kept into `m`.
 template <bool COUNT, int VEC>
 __global__ void __launch_bounds__(256)
-xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, unsigned long long* __restrict__ counts, int* error) {
+xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, uint64_t lo, uint64_t hi,
+            unsigned long long* __restrict__ counts, int* error) {
   const uint64_t cap = t.mask + 1;
-  unsigned int kept_n = 0, live_n = 0;
+  unsigned int kept_n = 0, live_n = 0, foreign_n = 0;
   for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
     XfHead h = xf_load_head(xf_row(t, r));
     if (h.key == XF_EMPTY_KEY) continue;
     ++live_n;
+    if (COUNT && (h.key < lo || h.key > hi)) ++foreign_n;
     const uint32_t flags = t.lazy ? 0u : h.flags;  // a lazy (LR) row keeps a batch tag there
     xf_apply_pending(t, h);
     float st = 0.f, qt = 0.f;
@@ -264,9 +282,11 @@ xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, unsigned long l
   if (COUNT) {
     kept_n = __reduce_add_sync(0xffffffffu, kept_n);
     live_n = __reduce_add_sync(0xffffffffu, live_n);
+    foreign_n = __reduce_add_sync(0xffffffffu, foreign_n);
     if ((threadIdx.x & 31u) == 0u) {
       if (kept_n) atomicAdd(counts, (unsigned long long)kept_n);
       if (live_n) atomicAdd(counts + 1, (unsigned long long)live_n);
+      if (foreign_n) atomicAdd(counts + 3, (unsigned long long)foreign_n);
     }
   }
 }
@@ -351,6 +371,19 @@ __global__ void xf_k_model_insert_rows(XfTableView m, const uint8_t* __restrict_
     const float w = *reinterpret_cast<const float*>(p + 8);
     float st = 0.f, qt = 0.f;
     if (m.K > 0) { st = *reinterpret_cast<const float*>(p + 12); qt = *reinterpret_cast<const float*>(p + 16); }
+    xf_model_insert(m, key, w, st, qt, error);
+  }
+}
+
+// merge: the live rows among n slots of a part (its own slot array, or a chunk of it staged on this device) into `m`
+template <bool FM>
+__global__ void __launch_bounds__(256)
+xf_k_merge(const uint8_t* __restrict__ slots, uint64_t n, XfTableView m, int* error) {
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t key;
+    float w, st, qt;
+    xf_serve_load<FM>(slots + r * m.stride, key, w, st, qt);
+    if (key == XF_EMPTY_KEY) continue;
     xf_model_insert(m, key, w, st, qt, error);
   }
 }
@@ -488,8 +521,9 @@ XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
   return XF_OK;
 }
 
-// the body of xf_table_freeze (canonical = 0) and xf_table_freeze_canonical: on failure the caller frees `m`
-static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonical, xf_model* m) {
+// the body of xf_table_freeze (canonical = 0), xf_table_freeze_canonical and xf_table_freeze_part (part): on failure
+// the caller frees `m`
+static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonical, bool part, xf_model* m, const char* fn) {
   const int src_dev = t->cfg.device;
   XF_CUDA_TRY(cudaSetDevice(src_dev));
   XF_TRY(t->check_error());  // waits for everything enqueued on the table's stream
@@ -507,25 +541,37 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   // the build runs on the model's stream: the table's stream is idle (above) and the host calls on the table are
   // locked out by the caller, so nothing writes the table while it is read
   cudaStream_t st = m->stream;
-  unsigned long long* d_counts = nullptr;  // {kept, live, error flag}
-  XF_CUDA_TRY(cudaMalloc(&d_counts, 3 * sizeof(unsigned long long)));
+  unsigned long long* d_counts = nullptr;  // {kept, live, error flag, foreign}
+  XF_CUDA_TRY(cudaMalloc(&d_counts, 4 * sizeof(unsigned long long)));
   struct Free { void* p; ~Free() { cudaFree(p); } } free_counts{d_counts};
-  XF_CUDA_TRY(cudaMemsetAsync(d_counts, 0, 3 * sizeof(unsigned long long), st));
+  XF_CUDA_TRY(cudaMemsetAsync(d_counts, 0, 4 * sizeof(unsigned long long), st));
   int* d_error = reinterpret_cast<int*>(d_counts + 2);
   const int grid = xf_grid_for(tv.mask + 1, 256, 8);
   const int prune = cfg.prune ? 1 : 0;
-#define XF_FREEZE_LAUNCH(COUNT)                                                                               \
-  if (canonical) xf_k_freeze_fmc<COUNT><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
-  else switch (xf_vec_for(tv.K)) {                                                                                 \
-    case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
-    case 2: xf_k_freeze<COUNT, 2><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
-    default: xf_k_freeze<COUNT, 1><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); break; \
+  // the keys the table owns: a part refuses others; a whole table (num_shards == 1) owns every key
+  uint64_t lo = 0, hi = 0;
+  xf_shard_range(t->cfg.shard_index, t->cfg.num_shards, &lo, &hi);
+#define XF_FREEZE_LAUNCH(COUNT)                                                                                       \
+  if (canonical) xf_k_freeze_fmc<COUNT><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error);         \
+  else switch (xf_vec_for(tv.K)) {                                                                                         \
+    case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
+    case 2: xf_k_freeze<COUNT, 2><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
+    default: xf_k_freeze<COUNT, 1><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
   }
   XF_FREEZE_LAUNCH(true)
   XF_CUDA_TRY(cudaGetLastError());
-  unsigned long long counts[3] = {0, 0, 0};
+  unsigned long long counts[4] = {0, 0, 0, 0};
   XF_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaStreamSynchronize(st));
+  if (part && counts[3] != 0) {
+    xf_set_error("%s: the table is shard %d of %d and holds %llu keys outside its range (pulled, pushed or imported "
+                 "there): a part holds its own range only", fn, t->cfg.shard_index, t->cfg.num_shards, counts[3]);
+    return XF_ERR_STATE;
+  }
+  if (part) {
+    m->shard_index = t->cfg.shard_index;
+    m->num_shards = t->cfg.num_shards;
+  }
   m->keys = counts[0];
   m->source_keys = counts[1];
   m->pruned_keys = counts[1] - counts[0];
@@ -536,7 +582,7 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   XF_CUDA_TRY(cudaMemcpyAsync(counts, d_counts, sizeof(counts), cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaStreamSynchronize(st));
   if ((int)counts[2] != 0) {
-    xf_set_error("%s: a probe sequence of the model overflowed", canonical ? "xf_table_freeze_canonical" : "xf_table_freeze");
+    xf_set_error("%s: a probe sequence of the model overflowed", fn);
     return XF_ERR_FULL;
   }
   if (cfg.device >= 0 && cfg.device != src_dev) {
@@ -560,8 +606,8 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   return XF_OK;
 }
 
-static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical, xf_model** out) {
-  const char* fn = canonical ? "xf_table_freeze_canonical" : "xf_table_freeze";
+static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical, bool part, xf_model** out) {
+  const char* fn = part ? "xf_table_freeze_part" : canonical ? "xf_table_freeze_canonical" : "xf_table_freeze";
   if (out) *out = nullptr;
   if (!t || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
   xf_freeze_config cfg;
@@ -569,7 +615,12 @@ static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical
   if (cfg_in) cfg = *cfg_in;
   if (cfg.absent < -1 || cfg.absent > XF_ABSENT_ZERO) { xf_set_error("%s: absent = %d is not an XF_ABSENT_* policy", fn, cfg.absent); return XF_ERR_ARG; }
   if (cfg.device >= xf_device_count()) { xf_set_error("%s: no CUDA device %d", fn, cfg.device); return XF_ERR_ARG; }
-  if (!canonical && t->cfg.canonical_fm) {
+  if (part && t->cfg.canonical_fm) {
+    xf_set_error("xf_table_freeze_part: a canonical table (canonical_fm = 1) is never sharded: freeze it whole with "
+                 "xf_table_freeze_canonical");
+    return XF_ERR_ARG;
+  }
+  if (!canonical && !part && t->cfg.canonical_fm) {
     xf_set_error("xf_table_freeze: a canonical table (canonical_fm = 1) has no collapsed serving model: the per-k sums of "
                  "the canonical FM and the multi-view machine do not collapse to one pair of sums per key; "
                  "xf_table_freeze_canonical serves it with the canonical FM's forward");
@@ -580,23 +631,40 @@ static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical
                  "with xf_table_freeze", t->cfg.canonical_fm, t->cfg.latent_dim);
     return XF_ERR_ARG;
   }
-  if (t->cfg.num_shards > 1) {
-    xf_set_error("%s: the table is shard %d of %d: one shard's rows are not a model", fn, t->cfg.shard_index,
-                 t->cfg.num_shards);
+  if (!part && t->cfg.num_shards > 1) {
+    xf_set_error("%s: the table is shard %d of %d: one shard's rows are not a model (freeze every shard with "
+                 "xf_table_freeze_part and merge the parts with xf_model_merge)", fn, t->cfg.shard_index, t->cfg.num_shards);
     return XF_ERR_ARG;
   }
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   xf_model* m = new xf_model;
-  const int rc = xf_freeze_into(t, cfg, canonical, m);
+  const int rc = xf_freeze_into(t, cfg, canonical, part, m, fn);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
   *out = m;
   return XF_OK;
 }
 
-XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out) { return xf_freeze(t, cfg, false, out); }
+XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
+  return xf_freeze(t, cfg, false, false, out);
+}
 
 XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
-  return xf_freeze(t, cfg, true, out);
+  return xf_freeze(t, cfg, true, false, out);
+}
+
+XF_DLL int xf_table_freeze_part(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
+  return xf_freeze(t, cfg, false, true, out);
+}
+
+XF_DLL int xf_model_part_info(xf_model* m, int* shard_index, int* num_shards) {
+  if (!m) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (m->num_shards == 0) {
+    xf_set_error("xf_model_part_info: the model is whole, not a part");
+    return XF_ERR_STATE;
+  }
+  if (shard_index) *shard_index = m->shard_index;
+  if (num_shards) *num_shards = m->num_shards;
+  return XF_OK;
 }
 
 XF_DLL int xf_model_destroy(xf_model* m) {
@@ -643,6 +711,7 @@ static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
 static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals, uint32_t rows,
                            uint32_t nnz, float* pctr_out, const char* fn) {
   if (!m || !row_ptr || (!keys && nnz) || (!pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(m, fn));
   XF_TRY(xf_check_vals(m, vals, fn));
   for (uint32_t r = 0; r < rows; ++r)
     if (row_ptr[r] > row_ptr[r + 1]) { xf_set_error("%s: row_ptr decreases at row %u", fn, r); return XF_ERR_ARG; }
@@ -681,6 +750,7 @@ XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, co
 XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
   if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(m, "xf_model_predict_device"));
   XF_CUDA_TRY(cudaSetDevice(m->device));
   xf_launch_serve(m, d_row_ptr, d_keys, nullptr, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
   XF_CUDA_TRY(cudaGetLastError());
@@ -690,6 +760,7 @@ XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const
 XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, const float* d_vals,
                                           uint32_t rows, uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
   if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(m, "xf_model_predict_device_values"));
   XF_TRY(xf_check_vals(m, d_vals, "xf_model_predict_device_values"));
   XF_CUDA_TRY(cudaSetDevice(m->device));
   xf_launch_serve(m, d_row_ptr, d_keys, d_vals, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
@@ -700,6 +771,7 @@ XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
                                      uint8_t* labels_out) {
   if (!m || !tr) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  XF_TRY(xf_refuse_part(m, "xf_model_predict_ingested"));
   if (m->fm == XF_SERVE_FMC) {
     xf_set_error("xf_model_predict_ingested: a canonical model reads feature values, which an ingested text block does "
                  "not carry: use xf_model_predict_host_values / _device_values");
@@ -820,8 +892,22 @@ static int xf_sm_save_body(xf_model* m, FILE* f, const char* path) {
   h.source_keys = m->source_keys;
   h.pruned_keys = m->pruned_keys;
   h.chunk_rows = XF_ST_CHUNK_BYTES / h.row_bytes;
-  h.header_checksum = xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0);
-  if (!xf_sm_write(f, &h, sizeof(h))) { xf_set_error("write to %s failed", path); return XF_ERR_IO; }
+  bool wrote;
+  if (m->num_shards) {
+    // a part: XFSP, XFSM's fields and then the shard
+    XfPartHeader p;
+    memcpy(h.magic, "XFSP", 4);
+    h.header_bytes = sizeof(XfPartHeader);
+    memcpy(p.model, &h, sizeof(p.model));
+    p.shard_index = m->shard_index;
+    p.num_shards = m->num_shards;
+    p.header_checksum = xf_st_host_sum(&p, offsetof(XfPartHeader, header_checksum), 0);
+    wrote = xf_sm_write(f, &p, sizeof(p));
+  } else {
+    h.header_checksum = xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0);
+    wrote = xf_sm_write(f, &h, sizeof(h));
+  }
+  if (!wrote) { xf_set_error("write to %s failed", path); return XF_ERR_IO; }
   const uint64_t n = m->keys;
   if (n == 0) return XF_OK;
   // (key, slot) of every row, sorted by key on the device
@@ -877,16 +963,20 @@ static bool xf_sm_header_sane(const XfModelHeader& h) {
   return h.chunk_rows == XF_ST_CHUNK_BYTES / h.row_bytes && h.zero == 0;
 }
 
-static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModelHeader& h) {
+// the rows of an XFSM or XFSP file (header of `header_bytes`) into `m`; m->shard_index, num_shards are set: a part's
+// keys must lie in its shard's range
+static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModelHeader& h, uint64_t header_bytes) {
+  uint64_t lo = 0, hi = 0;
+  xf_shard_range(m->shard_index, m->num_shards, &lo, &hi);
   const uint64_t nch = (h.keys + h.chunk_rows - 1) / h.chunk_rows;
-  const uint64_t expect = sizeof(XfModelHeader) + nch * XF_SM_CHUNK_HEAD + h.keys * h.row_bytes;
+  const uint64_t expect = header_bytes + nch * XF_SM_CHUNK_HEAD + h.keys * h.row_bytes;
   if (fseek(f, 0, SEEK_END) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
   const long fsz = ftell(f);
   if (fsz < 0 || (uint64_t)fsz != expect) {
     xf_set_error("corrupt or truncated model file %s: %ld bytes, its header announces %llu", path, fsz, (unsigned long long)expect);
     return XF_ERR_IO;
   }
-  if (fseek(f, sizeof(XfModelHeader), SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  if (fseek(f, (long)header_bytes, SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
   XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   m->fm = h.fm;
   m->absent = h.absent;
@@ -926,6 +1016,11 @@ static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModel
         return XF_ERR_IO;
       }
       prev = key;
+      if (key < lo || key > hi) {
+        xf_set_error("model file %s: key %016llx of row %llu lies outside shard %d of %d", path, (unsigned long long)key,
+                     (unsigned long long)(first + r), m->shard_index, m->num_shards);
+        return XF_ERR_IO;
+      }
       if (h.fm == XF_SERVE_FMC && !xf_fmc_padding_zero((const uint8_t*)m->h_in.p + r * h.row_bytes, h.latent_dim, h.row_bytes)) {
         xf_set_error("model file %s: row %llu has non-zero padding", path, (unsigned long long)(first + r));
         return XF_ERR_IO;
@@ -948,30 +1043,147 @@ XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
   if (device < 0 || device >= xf_device_count()) { xf_set_error("xf_model_load: no CUDA device %d", device); return XF_ERR_CUDA; }
   FILE* f = fopen(path, "rb");
   if (!f) { xf_set_error("cannot open %s", path); return XF_ERR_IO; }
+  XfPartHeader p;  // an XFSP header; an XFSM one is its first 104 bytes
+  memset(&p, 0, sizeof(p));
+  const size_t got = fread(&p, 1, sizeof(p), f);
   XfModelHeader h;
-  memset(&h, 0, sizeof(h));
-  const size_t got = fread(&h, 1, sizeof(h), f);
+  memcpy(&h, &p, sizeof(h));
+  const bool part = got >= 4 && memcmp(h.magic, "XFSP", 4) == 0;
+  const size_t hbytes = part ? sizeof(XfPartHeader) : sizeof(XfModelHeader);
   int rc = XF_OK;
   if (got >= 4 && (memcmp(h.magic, "XFTB", 4) == 0 || memcmp(h.magic, "XFST", 4) == 0)) {
     xf_set_error("%s is a training checkpoint (%.4s), not a serving model: load it into a table and freeze that", path, h.magic);
     rc = XF_ERR_IO;
-  } else if (got < 4 || memcmp(h.magic, "XFSM", 4) != 0) {
-    xf_set_error("%s is not a serving model (no XFSM magic)", path);
+  } else if (got < 4 || (memcmp(h.magic, "XFSM", 4) != 0 && !part)) {
+    xf_set_error("%s is not a serving model (no XFSM or XFSP magic)", path);
     rc = XF_ERR_IO;
-  } else if (got != sizeof(h) || h.header_bytes != sizeof(h) || h.version != XF_SM_VERSION) {
+  } else if (got < hbytes || h.header_bytes != hbytes || h.version != XF_SM_VERSION) {
     xf_set_error("model file %s: truncated header or unknown version %u", path, h.version);
     rc = XF_ERR_IO;
-  } else if (h.header_checksum != xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0) || !xf_sm_header_sane(h)) {
+  } else if (!part && (h.header_checksum != xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0) ||
+                       !xf_sm_header_sane(h))) {
     xf_set_error("model file %s: the header is damaged (checksum mismatch)", path);
+    rc = XF_ERR_IO;
+  } else if (part && (p.header_checksum != xf_st_host_sum(&p, offsetof(XfPartHeader, header_checksum), 0) ||
+                      !xf_sm_header_sane(h) || h.fm == XF_SERVE_FMC)) {
+    xf_set_error("model part file %s: the header is damaged (checksum mismatch)", path);
+    rc = XF_ERR_IO;
+  } else if (part && (p.num_shards < 1 || p.shard_index < 0 || p.shard_index >= p.num_shards)) {
+    xf_set_error("model part file %s: shard %d of %d does not exist", path, p.shard_index, p.num_shards);
     rc = XF_ERR_IO;
   }
   xf_model* m = nullptr;
   if (rc == XF_OK) {
     m = new xf_model;
     m->device = device;
-    rc = cudaSetDevice(device) == cudaSuccess ? xf_sm_load_body(m, f, path, h) : XF_ERR_CUDA;
+    if (part) {
+      m->shard_index = p.shard_index;
+      m->num_shards = p.num_shards;
+    }
+    rc = cudaSetDevice(device) == cudaSuccess ? xf_sm_load_body(m, f, path, h, hbytes) : XF_ERR_CUDA;
   }
   fclose(f);
+  if (rc != XF_OK) { xf_model_free(m); return rc; }
+  *out = m;
+  return XF_OK;
+}
+
+// ---- merge
+// the body of xf_model_merge (the parts checked): on failure the caller frees `m`
+static int xf_merge_into(xf_model* const* parts, int n, int device, xf_model* m) {
+  const xf_model* p0 = parts[0];
+  m->device = device;
+  XF_CUDA_TRY(cudaSetDevice(device));
+  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  cudaStream_t st = m->stream;
+  m->fm = p0->fm;
+  m->absent = p0->absent;
+  m->optimizer = p0->optimizer;
+  m->view.K = p0->view.K;
+  m->view.opt = p0->view.opt;
+  m->view.v_init = p0->view.v_init;
+  m->view.v_const = p0->view.v_const;
+  m->view.seed = p0->view.seed;
+  for (int i = 0; i < n; ++i) {
+    m->keys += parts[i]->keys;
+    m->source_keys += parts[i]->source_keys;
+    m->pruned_keys += parts[i]->pruned_keys;
+  }
+  if (m->keys > (1ull << 31)) {
+    xf_set_error("xf_model_merge: a serving model of %llu keys exceeds 2^32 slots", (unsigned long long)m->keys);
+    return XF_ERR_FULL;
+  }
+  XF_TRY(xf_model_alloc(m, xf_model_capacity(m->keys)));
+  XfDevBuf err, stage;
+  struct Release { XfDevBuf* b[2]; ~Release() { for (XfDevBuf* x : b) x->release(); } } rel{{&err, &stage}};
+  XF_TRY(err.ensure(4));
+  XF_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, st));
+  const uint32_t stride = m->view.stride;
+  auto launch = [&](const uint8_t* slots, uint64_t c) -> int {
+    if (m->fm) xf_k_merge<true><<<xf_grid_for(c, 256, 8), 256, 0, st>>>(slots, c, m->view, err.as<int>());
+    else xf_k_merge<false><<<xf_grid_for(c, 256, 8), 256, 0, st>>>(slots, c, m->view, err.as<int>());
+    XF_CUDA_TRY(cudaGetLastError());
+    return XF_OK;
+  };
+  for (int i = 0; i < n; ++i) {
+    const xf_model* q = parts[i];
+    const uint64_t slots = q->view.mask + 1;
+    if (q->device == device) {  // read in place
+      XF_TRY(launch(q->view.base, slots));
+      continue;
+    }
+    // another device: its slots come over by peer copy, 64 MiB at a time, into one staging buffer that the stream's
+    // order hands from each chunk's kernel to the next chunk's copy
+    const uint64_t per = XF_ST_CHUNK_BYTES / stride;
+    XF_TRY(stage.ensure(std::min(per, slots) * stride));
+    for (uint64_t first = 0; first < slots; first += per) {
+      const uint64_t c = std::min(per, slots - first);
+      XF_CUDA_TRY(cudaMemcpyPeerAsync(stage.p, device, q->view.base + first * stride, q->device, c * stride, st));
+      XF_TRY(launch(stage.as<uint8_t>(), c));
+    }
+  }
+  int e = 0;
+  XF_CUDA_TRY(cudaMemcpyAsync(&e, err.p, 4, cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  if (e) {
+    xf_set_error("xf_model_merge: a probe sequence of the model overflowed");
+    return XF_ERR_FULL;
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_merge(xf_model* const* parts, int n, int device, xf_model** out) {
+  if (out) *out = nullptr;
+  if (!out || (!parts && n > 0)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (n < 1) { xf_set_error("xf_model_merge: %d parts: a merge takes every part of one split", n); return XF_ERR_ARG; }
+  std::vector<int> seen((size_t)n, -1);
+  for (int i = 0; i < n; ++i) {
+    const xf_model* q = parts[i];
+    if (!q) { xf_set_error("null argument: parts[%d]", i); return XF_ERR_ARG; }
+    if (q->num_shards == 0) {
+      xf_set_error("xf_model_merge: parts[%d] is a whole model, not a part (xf_table_freeze_part makes parts)", i);
+      return XF_ERR_ARG;
+    }
+    if (q->num_shards != n) {
+      xf_set_error("xf_model_merge: parts[%d] is shard %d of a %d-way split, but %d parts were passed: a merge takes "
+                   "every part of one split, each once", i, q->shard_index, q->num_shards, n);
+      return XF_ERR_ARG;
+    }
+    if (seen[(size_t)q->shard_index] >= 0) {
+      xf_set_error("xf_model_merge: shard %d is passed twice (parts[%d] and parts[%d]), so another shard is missing",
+                   q->shard_index, seen[(size_t)q->shard_index], i);
+      return XF_ERR_ARG;
+    }
+    seen[(size_t)q->shard_index] = i;
+    if (const char* f = xf_compat_diff(xf_compat_of(parts[0]), xf_compat_of(q))) {
+      xf_set_error("xf_model_merge: parts[0] and parts[%d] differ in %s: the parts of one model read absent keys alike", i, f);
+      return XF_ERR_ARG;
+    }
+  }
+  const int target = device < 0 ? parts[0]->device : device;
+  if (target >= xf_device_count()) { xf_set_error("xf_model_merge: no CUDA device %d", target); return XF_ERR_ARG; }
+  xf_model* m = new xf_model;
+  const int rc = xf_merge_into(parts, n, target, m);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
   *out = m;
   return XF_OK;

@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include <mutex>
 
@@ -17,6 +18,7 @@ struct xf_model {
                            // canon = 1 for canonical rows
   int device = 0;
   int fm = 0, absent = 0, optimizer = 0;  // fm: XF_SERVE_*
+  int shard_index = 0, num_shards = 0;    // a part (xf_table_freeze_part): shard_index of num_shards >= 1; 0: a whole model
   uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
   cudaStream_t stream = nullptr;
   // staging of the host entry points, grown on demand; those calls are serialised by the mutex
@@ -24,6 +26,43 @@ struct xf_model {
   XfDevBuf s_row_ptr, s_keys, s_out, s_aux, s_vals;
   XfPinBuf h_in, h_out;
 };
+
+// the keys shard s of S owns (xf_shard_of, postoffice.cc:134-143): [s width, (s + 1) width) with width =
+// floor((2^64 - 1) / S); the last shard runs to 2^64 - 2.  *lo and *hi are inclusive.
+inline void xf_shard_range(int s, int S, uint64_t* lo, uint64_t* hi) {
+  const uint64_t width = 0xFFFFFFFFFFFFFFFFull / (uint64_t)(S > 1 ? S : 1);
+  *lo = (uint64_t)s * width;
+  *hi = s + 1 >= S ? 0xFFFFFFFFFFFFFFFEull : (uint64_t)(s + 1) * width - 1ull;
+}
+
+// XF_ERR_STATE for a part passed where a whole model is needed (predict, diff, apply)
+inline int xf_refuse_part(const xf_model* m, const char* fn) {
+  if (m->num_shards == 0) return XF_OK;
+  xf_set_error("%s: the model is a part (shard %d of %d), not a model: merge the parts with xf_model_merge", fn,
+               m->shard_index, m->num_shards);
+  return XF_ERR_STATE;
+}
+
+// what defines how an absent key reads: the fields two models (a model and a delta, the parts of a merge) must agree on
+struct XfCompat {
+  int fm, latent_dim, optimizer, absent, v_init;
+  float v_const;
+  uint64_t seed;
+};
+inline XfCompat xf_compat_of(const xf_model* m) {
+  return XfCompat{m->fm, m->view.K, m->optimizer, m->absent, m->view.v_init, m->view.v_const, m->view.seed};
+}
+// the first field that differs, or nullptr
+inline const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
+  if (a.fm != b.fm) return "fm";
+  if (a.latent_dim != b.latent_dim) return "latent_dim";
+  if (a.optimizer != b.optimizer) return "optimizer";
+  if (a.absent != b.absent) return "absent";
+  if (a.v_init != b.v_init) return "v_init";
+  if (memcmp(&a.v_const, &b.v_const, sizeof(float)) != 0) return "v_const";
+  if (a.seed != b.seed) return "seed";
+  return nullptr;
+}
 
 // Bytes of a model row.  LR {key, w, 0}: 16; FM {key, w, st, qt, 0...}: 32; canonical FM {key, w, 0, v[K], 0...}:
 // 16 + 4K rounded up to 32, so that every row starts on a sector and lane c's piece v[4c .. 4c+3] lies at 16 + 16c.

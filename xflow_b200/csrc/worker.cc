@@ -12,6 +12,8 @@
 #include <memory>
 #include <mutex>
 #include <stdexcept>
+#include <string>
+#include <vector>
 
 #include "../../include/xflow/xflow.h"
 
@@ -203,6 +205,37 @@ static void ExportEpoch(xf_table* t, const std::string& prefix, uint64_t epochs_
   prev = std::move(next);
 }
 
+// XFLOW_EXPORT_SHARDED_MODEL = <path>: the serving model of a run of any world size.  Every rank freezes its shard of
+// the table into a part (xf_table_freeze_part, the defaults) and writes <path>.part-<rank>-of-<world>.xfsp; after a
+// barrier rank 0 loads the parts onto its device, merges them (xf_model_merge) and writes <path>, the file
+// XFLOW_EXPORT_MODEL would write for the same rows in one table.  Rank 0 removes the part files once <path> is in
+// place; on a failure they stay and the run fails.  The ranks share a filesystem, as for XFLOW_COMM_FILE.
+static std::string PartPath(const std::string& path, int rank, int world) {
+  return path + ".part-" + std::to_string(rank) + "-of-" + std::to_string(world) + ".xfsp";
+}
+static void ExportShardedModel(xf_table* t, xf_comm* comm, const std::string& path, int rank, int world, int device) {
+  xf_model* part = nullptr;
+  must(xf_table_freeze_part(t, nullptr, &part), "xf_table_freeze_part");
+  const int rc = xf_model_save(part, PartPath(path, rank, world).c_str());
+  xf_model_destroy(part);
+  must(rc, "xf_model_save");
+  if (comm) must(xf_comm_barrier(comm), "xf_comm_barrier");
+  if (rank != 0) return;
+  std::vector<ModelPtr> parts;
+  std::vector<xf_model*> raw;
+  for (int r = 0; r < world; ++r) {
+    xf_model* m = nullptr;
+    must(xf_model_load(&m, PartPath(path, r, world).c_str(), device), "xf_model_load");
+    parts.emplace_back(m);
+    raw.push_back(m);
+  }
+  xf_model* whole = nullptr;
+  must(xf_model_merge(raw.data(), world, device, &whole), "xf_model_merge");
+  ModelPtr merged(whole);
+  must(xf_model_save(whole, path.c_str()), "xf_model_save");
+  for (int r = 0; r < world; ++r) remove(PartPath(path, r, world).c_str());
+}
+
 int MyRank() { return env_int("XFLOW_RANK", env_int("RANK", 0)); }
 int NumWorkers() { return env_int("XFLOW_WORLD", env_int("WORLD_SIZE", 1)); }
 
@@ -241,6 +274,8 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   env_path("XFLOW_RESUME", world_);
   env_path("XFLOW_EXPORT_MODEL", world_);
   env_path("XFLOW_EXPORT_DELTAS", world_);
+  if (!env_path("XFLOW_EXPORT_MODEL", 1).empty() && !env_path("XFLOW_EXPORT_SHARDED_MODEL", 1).empty())
+    throw std::runtime_error("XFLOW_EXPORT_MODEL and XFLOW_EXPORT_SHARDED_MODEL write the same model: set one of them");
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_server) g_server = this;
@@ -684,6 +719,11 @@ void WorkerBase::train() {
     }
   } else if (comm_) {
     predict(rank, 0);  // takes part in rank 0's collective forward steps; feeds and prints nothing
+  }
+  const std::string sharded = env_path("XFLOW_EXPORT_SHARDED_MODEL", 1);
+  if (!sharded.empty()) {
+    Server* s = Server::Get();
+    ExportShardedModel(table_, comm_, sharded, rank, s->world(), s->device());
   }
   std::cout << "train end......" << std::endl;
 }
