@@ -626,7 +626,9 @@ XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
  *  splitmix64(word ^ offset), a chunk's offsets being chunk << 40 | byte offset in its rows).  The file is a function
  *  of the model's contents, not of where its keys lie: two freezes of one table, and load then save, give identical
  *  bytes.  Written to <path>.tmp and renamed; the staging is bounded by the chunk size.  xf_model_load rebuilds the
- *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL.
+ *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL, and so is
+ *  a file whose checksums pass but whose keys do not ascend strictly below 2^64 - 1 or whose rows have a non-zero
+ *  padding byte (LR bytes 12 .. 15, FM 20 .. 31, canonical 12 .. 15 and 16 + 4K .. row bytes).
  * Part file "XFSP" (xf_model_save of a part): XFSM's layout with a 112-byte header
  *     0 "XFSP"   4 u32 version (1)   8 u64 header bytes (112)   16 .. 95 as XFSM's (the part's keys, capacity,
  *    source and pruned keys; fm 0 or 1)   96 i32 shard_index   100 i32 num_shards   104 u64 checksum of bytes [0, 104)

@@ -100,7 +100,8 @@ def build_file(rows, latent_dim, optimizer, absent, v_init, v_const, seed, sourc
 
 
 def parse_file(data):
-    """(header dict, rows) of an XFSM file; ValueError if it is not one, is truncated, or a checksum fails."""
+    """(header dict, rows) of an XFSM file; ValueError if it is not one, is truncated, a checksum fails, or a row's
+    padding is not zero."""
     if len(data) < HEADER.size or data[:4] != b"XFSM":
         raise ValueError("not an XFSM file")
     h = dict(zip(FIELDS, HEADER.unpack(data[:HEADER.size])))
@@ -126,4 +127,6 @@ def parse_file(data):
     rows = np.concatenate(parts) if parts else np.zeros(0, dt)
     if np.any(np.diff(rows["key"].astype(object)) <= 0):
         raise ValueError("keys not ascending")
+    if rows.size and np.any(np.ascontiguousarray(rows["pad"]) != 0):
+        raise ValueError("non-zero padding")
     return h, rows

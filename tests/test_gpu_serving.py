@@ -339,6 +339,15 @@ def test_damaged_and_foreign_files_are_refused(frozen, tmp_path):
         x = bytearray(data)
         x[pos] ^= 0x04
         refused(bytes(x))
+    # checksums that pass over a row whose padding is not zero (LR bytes 12 .. 15, FM 20 .. 31)
+    row_bytes = struct.unpack_from("<I", data, 32)[0]
+    assert len(data) == 104 + 32 + struct.unpack_from("<Q", data, 16)[0] * row_bytes  # one chunk
+    x = bytearray(data)
+    x[104 + 32 + row_bytes - 1] = 1
+    struct.pack_into("<Q", x, 104 + 16, M.section_sum(bytes(x[104 + 32:]), 0))
+    open(bad, "wb").write(bytes(x))
+    with pytest.raises(api.XflowError, match=ERR_IO + ".*padding"):
+        api.Model.load(bad)
     xftb, xfst = str(tmp_path / "xftb"), str(tmp_path / "xfst")
     t.save(xftb)
     t.save_state(xfst)

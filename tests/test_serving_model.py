@@ -90,6 +90,11 @@ def test_file_round_trip_and_layout(fm):
     for cut in (0, 50, 104, 120, len(data) - 1):
         with pytest.raises(ValueError):
             M.parse_file(data[:cut])
+    # a dirty padding byte is refused even when the checksums are right
+    dirty = rows.copy()
+    dirty["pad"][2] = 1 if dirty["pad"].ndim == 1 else [0, 1, 0]
+    with pytest.raises(ValueError, match="padding"):
+        M.parse_file(M.build_file(dirty, 8 if fm else 0, 0, M.ABSENT_ZERO, 1, 0.0, 11, 10))
 
 
 def test_empty_model_file():

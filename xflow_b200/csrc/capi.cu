@@ -8,7 +8,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <string>
 
 #include "internal.h"
 
@@ -686,25 +685,20 @@ XF_DLL int xf_table_save(xf_table* t, const char* path) {
                          K ? nv.data() : nullptr, K ? zv.data() : nullptr, present.data()));
   // written under a temporary name and renamed: a reader never sees a half-written checkpoint, and a
   // short write (ENOSPC ...) is an error, not a silently truncated file
-  const std::string tmp = std::string(path) + ".tmp";
-  FILE* f = fopen(tmp.c_str(), "wb");
-  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
-  uint32_t K32 = (uint32_t)K;
-  bool ok = fwrite("XFTB", 1, 4, f) == 4 && fwrite(&n, 8, 1, f) == 1 && fwrite(&K32, 4, 1, f) == 1 && fwrite(&has_nz, 4, 1, f) == 1;
-  auto put = [&](const void* p, size_t sz, size_t cnt) { if (ok && cnt) ok = fwrite(p, sz, cnt, f) == cnt; };
-  put(keys.data(), 8, n);
-  put(w.data(), 4, n);
-  if (has_nz) { put(nw.data(), 4, n); put(zw.data(), 4, n); }
-  put(v.data(), 4, n * K);
-  if (has_nz) { put(nv.data(), 4, n * K); put(zv.data(), 4, n * K); }
-  put(present.data(), 1, n);
-  if (fclose(f) != 0) ok = false;
-  if (!ok || rename(tmp.c_str(), path) != 0) {
-    remove(tmp.c_str());
-    xf_set_error("write to %s failed", path);
+  return xf_save_atomic(path, [&](FILE* f, const char* name) {
+    uint32_t K32 = (uint32_t)K;
+    bool ok = fwrite("XFTB", 1, 4, f) == 4 && fwrite(&n, 8, 1, f) == 1 && fwrite(&K32, 4, 1, f) == 1 && fwrite(&has_nz, 4, 1, f) == 1;
+    auto put = [&](const void* p, size_t sz, size_t cnt) { if (ok && cnt) ok = fwrite(p, sz, cnt, f) == cnt; };
+    put(keys.data(), 8, n);
+    put(w.data(), 4, n);
+    if (has_nz) { put(nw.data(), 4, n); put(zw.data(), 4, n); }
+    put(v.data(), 4, n * K);
+    if (has_nz) { put(nv.data(), 4, n * K); put(zv.data(), 4, n * K); }
+    put(present.data(), 1, n);
+    if (ok) return XF_OK;
+    xf_set_error("write to %s failed", name);
     return XF_ERR_IO;
-  }
-  return XF_OK;
+  });
 }
 
 // text model dump (SURVEY.md section 8f-3; the reference has none): one line per key, sorted by key,
@@ -749,14 +743,13 @@ XF_DLL int xf_table_load(xf_table* t, const char* path) {
   char magic[4] = {0, 0, 0, 0};
   uint64_t n = 0;
   uint32_t K32 = 0, has_nz = 0;
-  bool ok = fread(magic, 1, 4, f) == 4 && memcmp(magic, "XFTB", 4) == 0 && fread(&n, 8, 1, f) == 1 &&
-            fread(&K32, 4, 1, f) == 1 && fread(&has_nz, 4, 1, f) == 1;
-  if (memcmp(magic, "XFST", 4) == 0) {
+  const size_t got = fread(magic, 1, 4, f);
+  if (xf_refuse_foreign(magic, got, path, "XFTB") != XF_OK) {
     fclose(f);
-    xf_set_error("%s is a state image written by xf_table_save_state, not a portable checkpoint: load it with "
-                 "xf_table_load_state", path);
     return XF_ERR_IO;
   }
+  bool ok = got == 4 && memcmp(magic, "XFTB", 4) == 0 && fread(&n, 8, 1, f) == 1 && fread(&K32, 4, 1, f) == 1 &&
+            fread(&has_nz, 4, 1, f) == 1;
   if (!ok || (int)K32 != t->view.K) {
     fclose(f);
     xf_set_error("bad checkpoint %s (K=%u, table K=%d)", path, K32, t->view.K);

@@ -86,6 +86,41 @@ uint64_t xf_st_host_sum(const void* p, uint64_t bytes, uint64_t off0) {
   return s;
 }
 
+int xf_save_atomic(const char* path, const std::function<int(FILE* f, const char* name)>& body) {
+  const std::string tmp = std::string(path) + ".tmp";
+  FILE* f = fopen(tmp.c_str(), "wb");
+  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
+  int rc = body(f, tmp.c_str());
+  if (fclose(f) != 0 && rc == XF_OK) { xf_set_error("write to %s failed", tmp.c_str()); rc = XF_ERR_IO; }
+  if (rc == XF_OK && rename(tmp.c_str(), path) != 0) { xf_set_error("cannot rename %s to %s", tmp.c_str(), path); rc = XF_ERR_IO; }
+  if (rc != XF_OK) remove(tmp.c_str());
+  return rc;
+}
+
+// the project's file formats: what each is, the call that writes it and the call that loads it
+static const struct { char magic[5]; const char *kind, *save, *load; } xf_file_formats[] = {
+    {"XFTB", "portable training checkpoint", "xf_table_save", "xf_table_load"},
+    {"XFST", "training state checkpoint", "xf_table_save_state", "xf_table_load_state"},
+    {"XFSM", "serving model", "xf_model_save", "xf_model_load"},
+    {"XFSP", "serving model part", "xf_model_save", "xf_model_load"},
+    {"XFSD", "serving model delta", "xf_delta_save", "xf_delta_load"},
+};
+
+int xf_refuse_foreign(const void* head, size_t got, const char* path, const char* own) {
+  if (got < 4) return XF_OK;
+  for (size_t o = 0; own[o]; o += 4)
+    if (memcmp(head, own + o, 4) == 0) return XF_OK;
+  const char* own_kind = "";
+  for (const auto& x : xf_file_formats)
+    if (memcmp(x.magic, own, 4) == 0) own_kind = x.kind;
+  for (const auto& x : xf_file_formats)
+    if (memcmp(head, x.magic, 4) == 0) {
+      xf_set_error("%s is a %s written by %s (%s), not a %s: load it with %s", path, x.kind, x.save, x.magic, own_kind, x.load);
+      return XF_ERR_IO;
+    }
+  return XF_OK;
+}
+
 __device__ __forceinline__ unsigned long long xf_st_warp_sum(unsigned long long v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -427,15 +462,7 @@ XF_DLL int xf_table_save_state(xf_table* t, const char* path, uint64_t user) {
   h.filter_bytes = (t->admit.mode == XF_ADMIT_BLOOM && t->d_filter) ? (1ull << t->admit.log2_cells) : 0ull;
   h.ring_entries = t->view.lazy ? (uint64_t)t->seq + 1 : 0ull;
   h.header_checksum = xf_st_host_sum(&h, offsetof(XfStateHeader, header_checksum), 0);
-  // written under a temporary name and renamed, as xf_table_save does
-  const std::string tmp = std::string(path) + ".tmp";
-  FILE* f = fopen(tmp.c_str(), "wb");
-  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
-  int rc = xf_st_save_body(t, h, f, tmp.c_str());
-  if (fclose(f) != 0 && rc == XF_OK) { xf_set_error("write to %s failed", tmp.c_str()); rc = XF_ERR_IO; }
-  if (rc == XF_OK && rename(tmp.c_str(), path) != 0) { xf_set_error("cannot rename %s to %s", tmp.c_str(), path); rc = XF_ERR_IO; }
-  if (rc != XF_OK) remove(tmp.c_str());
-  return rc;
+  return xf_save_atomic(path, [&](FILE* f, const char* name) { return xf_st_save_body(t, h, f, name); });
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -626,8 +653,7 @@ XF_DLL int xf_table_load_state(xf_table* t, const char* path, uint64_t* user) {
   memset(&h, 0, sizeof(h));
   const size_t got = fread(&h, 1, sizeof(h), f);
   int rc = XF_OK;
-  if (got >= 4 && memcmp(h.magic, "XFTB", 4) == 0) {
-    xf_set_error("%s is a portable checkpoint written by xf_table_save, not a state image: load it with xf_table_load", path);
+  if (xf_refuse_foreign(h.magic, got, path, "XFST") != XF_OK) {
     rc = XF_ERR_IO;
   } else if (got < 4 || memcmp(h.magic, "XFST", 4) != 0) {
     xf_set_error("%s is not a state image (no XFST magic)", path);

@@ -1,18 +1,17 @@
 // Serving model deltas: carry one frozen model to the next (layer 7 of include/xflow_b200.h, which documents the
 // semantics and the XFSD file format).
 //
-//   fingerprint  xf_k_fingerprint<FM>     one pass over a model's slots: each row's splitmix64 chain, a warp sum, one
-//                                         atomic per warp for the sum and one for the row count
-//   diff         xf_k_delta_emit<FM, DEL>  one pass over next's slots probing base (the upserts), one over base's slots
-//                                         probing next (the deletes), through xf_serve_load / xf_serve_find; a warp-
-//                                         aggregated atomic cursor; then the (key, slot) pairs are sorted by key as a
-//                                         model file's are, and the upsert rows gathered from next
-//   apply        the upserts inserted into a new model sized for the result; xf_k_apply_base<FM> inserts every row of
-//                base whose key is not deleted (a binary search over the sorted delete keys) and not upserted (the
-//                insert keeps the row it finds); then the result's fingerprint and key count are checked
-//   file         header, upsert rows, delete keys, a chunk at a time through bounded staging
-// Canonical models (rows of 16 + 4K bytes rounded up to 32) take runtime-stride variants of the three passes
-// (xf_k_fingerprint_fmc, xf_k_delta_emit_fmc<DEL>, xf_k_apply_base_fmc) that hash, compare and copy whole rows.
+//   fingerprint  xf_k_fingerprint        one pass over a model's slots: each row's splitmix64 chain, a warp sum, one
+//                                        atomic per warp for the sum and one for the row count
+//   diff         xf_k_delta_emit<DEL>    one pass over next's slots probing base (the upserts), one over base's slots
+//                                        probing next (the deletes), through xf_model_find_slot; a warp-aggregated
+//                                        atomic cursor; then the (key, slot) pairs are sorted by key as a model file's
+//                                        are, and the upsert rows gathered from next
+//   apply        the upserts inserted into a new model sized for the result; xf_k_apply_base puts every row of base
+//                whose key is not deleted (a binary search over the sorted delete keys) and not upserted (the claim
+//                keeps the row it finds); then the result's fingerprint and key count are checked
+//   file         header, upsert rows, delete keys: the chunked sections of serve.cu (xf_chunks_save, xf_chunks_load)
+// Every pass hashes, compares or copies whole rows at the model's stride, so one kernel serves LR, FM and canonical rows.
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
@@ -21,12 +20,10 @@
 
 #include <algorithm>
 #include <mutex>
-#include <string>
 
 #include "serve.cuh"
 
 #define XF_SD_VERSION 1u
-#define XF_SD_CHUNK_HEAD 32  // {u64 first entry, u64 entries, u64 checksum, u64 0}
 
 // The file header (little-endian, 144 bytes; the layout is documented in include/xflow_b200.h)
 struct XfDeltaHeader {
@@ -73,10 +70,8 @@ static XfCompat xf_compat_of(const XfDeltaHeader& h) {
   return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed};
 }
 
-static uint64_t xf_sd_chunks(uint64_t n, uint64_t per_chunk) { return (n + per_chunk - 1) / per_chunk; }
 static uint64_t xf_sd_file_bytes(const XfDeltaHeader& h) {
-  return sizeof(XfDeltaHeader) + (xf_sd_chunks(h.upserts, h.chunk_rows) + xf_sd_chunks(h.deletes, h.chunk_keys)) * XF_SD_CHUNK_HEAD +
-         h.upserts * h.row_bytes + h.deletes * 8;
+  return sizeof(XfDeltaHeader) + xf_section_bytes(h.upserts, h.row_bytes, h.chunk_rows) + xf_section_bytes(h.deletes, 8u, h.chunk_keys);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -88,17 +83,18 @@ __device__ __forceinline__ uint64_t xf_shfl_xor_u64(uint64_t v, int lane_mask) {
   return (uint64_t)hi << 32 | lo;
 }
 
-// out[0] += the fingerprint of the rows of `m`, out[1] += their number
-template <bool FM>
+// out[0] += the fingerprint of the rows of `m`, out[1] += their number.  A row's fingerprint chains its stride / 8 words
+// through splitmix64 (h_0 = 0, h_{i+1} = splitmix64(h_i ^ word_i)), two words per 16-byte load.
 __global__ void __launch_bounds__(256) xf_k_fingerprint(XfTableView m, unsigned long long* out) {
   const uint64_t cap = m.mask + 1;
   uint64_t sum = 0ull, rows = 0ull;
   for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
-    const ulonglong2 a = *reinterpret_cast<const ulonglong2*>(xf_row(m, r));
+    const uint8_t* p = xf_row(m, r);
+    const ulonglong2 a = *reinterpret_cast<const ulonglong2*>(p);
     if (a.x == XF_EMPTY_KEY) continue;
-    uint64_t h = xf_splitmix64(a.y ^ xf_splitmix64(a.x));  // h_0 = 0: h_1 = splitmix64(w_0)
-    if (FM) {
-      const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(xf_row(m, r) + 16);
+    uint64_t h = xf_splitmix64(a.y ^ xf_splitmix64(a.x));
+    for (uint32_t o = 16; o < m.stride; o += 16) {
+      const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(p + o);
       h = xf_splitmix64(xf_splitmix64(h ^ b.x) ^ b.y);
     }
     sum += h;
@@ -108,87 +104,22 @@ __global__ void __launch_bounds__(256) xf_k_fingerprint(XfTableView m, unsigned 
     sum += xf_shfl_xor_u64(sum, o);
     rows += xf_shfl_xor_u64(rows, o);
   }
-  if ((threadIdx.x & 31u) == 0u) {
-    if (rows) {
-      atomicAdd(out, (unsigned long long)sum);  // wraps mod 2^64: the fingerprint is that sum
-      atomicAdd(out + 1, (unsigned long long)rows);
-    }
+  if ((threadIdx.x & 31u) == 0u && rows) {
+    atomicAdd(out, (unsigned long long)sum);  // wraps mod 2^64: the fingerprint is that sum
+    atomicAdd(out + 1, (unsigned long long)rows);
   }
 }
 
-// The rows of `a` that `b` does not hold and, DEL = false, also those `b` holds with other contents, as (key, slot of
+// The rows of `a` that `b` does not hold and, DEL = false, also those `b` holds with other bytes, as (key, slot of
 // `a`) pairs at an atomic cursor.  diff(base, next): upserts = emit<false>(next, base), deletes = emit<true>(base, next).
-// A row's bytes are compared through w, st (LR: the padding word) and qt: the rest of a model row is padding, which
-// every model keeps at zero (the fill writes it, no insert touches it).
-template <bool FM, bool DEL>
+// Whole rows are compared, 16 bytes per load: the padding is zero in every model (xf_model_padding_zero).
+template <bool DEL>
 __global__ void __launch_bounds__(256)
 xf_k_delta_emit(XfTableView a, XfTableView b, uint64_t* __restrict__ keys_out, uint32_t* __restrict__ slots_out,
                 unsigned long long* count) {
   const uint64_t cap = a.mask + 1;
   const uint32_t lane = threadIdx.x & 31u;
   // a warp walks 32 consecutive slots per iteration (cap and the stride are multiples of 32: the loop is warp-uniform)
-  for (uint64_t r0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull; r0 < cap; r0 += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t r = r0 + lane;
-    bool emit = false;
-    uint64_t key = XF_EMPTY_KEY;
-    if (r < cap) {
-      float w, st, qt;
-      xf_serve_load<FM>(xf_row(a, r), key, w, st, qt);
-      if (key != XF_EMPTY_KEY) {
-        uint64_t k;
-        float bw, bst, bqt;
-        xf_serve_load<FM>(xf_row(b, xf_home_slot(b, key)), k, bw, bst, bqt);
-        const bool have = xf_serve_find<FM>(b, key, k, bw, bst, bqt);
-        emit = !have;
-        if (!DEL && have)
-          emit = ((__float_as_uint(w) ^ __float_as_uint(bw)) | (__float_as_uint(st) ^ __float_as_uint(bst)) |
-                  (FM ? (__float_as_uint(qt) ^ __float_as_uint(bqt)) : 0u)) != 0u;
-      }
-    }
-    const uint32_t mask = __ballot_sync(0xffffffffu, emit);
-    if (mask == 0u) continue;
-    unsigned long long first = 0ull;
-    if (lane == 0u) first = atomicAdd(count, (unsigned long long)__popc(mask));
-    first = __shfl_sync(0xffffffffu, first, 0);
-    if (emit) {
-      const unsigned long long idx = first + (unsigned long long)__popc(mask & ((1u << lane) - 1u));
-      keys_out[idx] = key;
-      slots_out[idx] = (uint32_t)r;
-    }
-  }
-}
-
-// ---- canonical rows (runtime stride): the same three passes over whole rows
-// out[0] += the fingerprint of the rows of `m` (n = stride / 8 words each), out[1] += their number
-__global__ void __launch_bounds__(256) xf_k_fingerprint_fmc(XfTableView m, unsigned long long* out) {
-  const uint64_t cap = m.mask + 1;
-  const uint32_t words = m.stride / 8u;
-  uint64_t sum = 0ull, rows = 0ull;
-  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t* p = reinterpret_cast<const uint64_t*>(xf_row(m, r));
-    if (p[0] == XF_EMPTY_KEY) continue;
-    uint64_t h = 0ull;
-    for (uint32_t i = 0; i < words; ++i) h = xf_splitmix64(h ^ p[i]);
-    sum += h;
-    ++rows;
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    sum += xf_shfl_xor_u64(sum, o);
-    rows += xf_shfl_xor_u64(rows, o);
-  }
-  if ((threadIdx.x & 31u) == 0u && rows) {
-    atomicAdd(out, (unsigned long long)sum);
-    atomicAdd(out + 1, (unsigned long long)rows);
-  }
-}
-
-// xf_k_delta_emit for canonical rows: a row differs if any of its bytes 8 .. stride does
-template <bool DEL>
-__global__ void __launch_bounds__(256)
-xf_k_delta_emit_fmc(XfTableView a, XfTableView b, uint64_t* __restrict__ keys_out, uint32_t* __restrict__ slots_out,
-                    unsigned long long* count) {
-  const uint64_t cap = a.mask + 1;
-  const uint32_t lane = threadIdx.x & 31u;
   for (uint64_t r0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull; r0 < cap; r0 += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t r = r0 + lane;
     bool emit = false;
@@ -201,13 +132,10 @@ xf_k_delta_emit_fmc(XfTableView a, XfTableView b, uint64_t* __restrict__ keys_ou
         emit = s < 0;
         if (!DEL && s >= 0) {
           const uint8_t* pb = xf_row(b, (uint64_t)s);
-          uint64_t d = __ldg(reinterpret_cast<const unsigned long long*>(pa + 8)) ^
-                       __ldg(reinterpret_cast<const unsigned long long*>(pb + 8));
-          for (uint32_t o = 16; o < a.stride && d == 0ull; o += 16) {
+          for (uint32_t o = 0; o < a.stride && !emit; o += 16) {
             const uint4 x = __ldg(reinterpret_cast<const uint4*>(pa + o)), y = __ldg(reinterpret_cast<const uint4*>(pb + o));
-            d = (uint64_t)((x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w));
+            emit = ((x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w)) != 0u;
           }
-          emit = d != 0ull;
         }
       }
     }
@@ -238,31 +166,15 @@ __device__ __forceinline__ bool xf_sorted_has(const uint8_t* __restrict__ p, uin
 }
 
 // every row of `base` whose key is not in dels[0 .. n_del) into `out`, keeping a row `out` already holds (an upsert)
-template <bool FM>
 __global__ void __launch_bounds__(256)
 xf_k_apply_base(XfTableView base, XfTableView out, const uint64_t* __restrict__ dels, uint64_t n_del, int* error) {
   const uint64_t cap = base.mask + 1;
   for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
-    uint64_t key;
-    float w, st, qt;
-    xf_serve_load<FM>(xf_row(base, r), key, w, st, qt);
-    if (key == XF_EMPTY_KEY) continue;
-    if (n_del && xf_sorted_has(reinterpret_cast<const uint8_t*>(dels), n_del, 8u, key)) continue;
-    xf_model_insert<true>(out, key, w, st, qt, error);
-  }
-}
-
-// xf_k_apply_base for canonical rows: whole rows are copied
-__global__ void __launch_bounds__(256)
-xf_k_apply_base_fmc(XfTableView base, XfTableView out, const uint64_t* __restrict__ dels, uint64_t n_del, int* error) {
-  const uint64_t cap = base.mask + 1;
-  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t* src = xf_row(base, r);
-    const uint64_t key = __ldg(reinterpret_cast<const unsigned long long*>(src));
-    if (key == XF_EMPTY_KEY) continue;
-    if (n_del && xf_sorted_has(reinterpret_cast<const uint8_t*>(dels), n_del, 8u, key)) continue;
-    uint8_t* p = xf_model_claim<true>(out, key, error);
-    if (p) xf_model_copy_body(out, p, src);
+    const ulonglong2 head = __ldg(reinterpret_cast<const ulonglong2*>(src));
+    if (head.x == XF_EMPTY_KEY) continue;
+    if (n_del && xf_sorted_has(reinterpret_cast<const uint8_t*>(dels), n_del, 8u, head.x)) continue;
+    xf_model_put_row<true>(out, src, head, error);
   }
 }
 
@@ -277,11 +189,8 @@ __global__ void xf_k_delta_overlap(const uint8_t* __restrict__ rows, uint64_t n_
 // host side
 // -------------------------------------------------------------------------------------------------
 // the fingerprint and row count of the rows of `v`, added into d_out[0], d_out[1] on `st`
-static int xf_launch_fingerprint(const XfTableView& v, int fm, unsigned long long* d_out, cudaStream_t st) {
-  const int grid = xf_grid_for(v.mask + 1, 256, 8);
-  if (fm == XF_SERVE_FMC) xf_k_fingerprint_fmc<<<grid, 256, 0, st>>>(v, d_out);
-  else if (fm) xf_k_fingerprint<true><<<grid, 256, 0, st>>>(v, d_out);
-  else xf_k_fingerprint<false><<<grid, 256, 0, st>>>(v, d_out);
+static int xf_launch_fingerprint(const XfTableView& v, unsigned long long* d_out, cudaStream_t st) {
+  xf_k_fingerprint<<<xf_grid_for(v.mask + 1, 256, 8), 256, 0, st>>>(v, d_out);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }
@@ -298,23 +207,15 @@ static void xf_delta_free(xf_delta* d) {
 }
 
 // the pairs emit<DEL>(a, b) lists, sorted by key; returns their number in *n
-static int xf_delta_list(const XfTableView& a, const XfTableView& b, int fm, bool del, XfSortedSlots& s, uint64_t* n,
+static int xf_delta_list(const XfTableView& a, const XfTableView& b, bool del, XfSortedSlots& s, uint64_t* n,
                          cudaStream_t st) {
   XF_CUDA_TRY(cudaMemsetAsync(s.count.p, 0, 8, st));
   const int grid = xf_grid_for(a.mask + 1, 256, 8);
   uint64_t* ko = s.keys_in.as<uint64_t>();
   uint32_t* so = s.slots_in.as<uint32_t>();
   unsigned long long* c = s.count.as<unsigned long long>();
-  if (fm == XF_SERVE_FMC) {
-    if (del) xf_k_delta_emit_fmc<true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-    else xf_k_delta_emit_fmc<false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-  } else if (fm) {
-    if (del) xf_k_delta_emit<true, true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-    else xf_k_delta_emit<true, false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-  } else {
-    if (del) xf_k_delta_emit<false, true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-    else xf_k_delta_emit<false, false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
-  }
+  if (del) xf_k_delta_emit<true><<<grid, 256, 0, st>>>(a, b, ko, so, c);
+  else xf_k_delta_emit<false><<<grid, 256, 0, st>>>(a, b, ko, so, c);
   XF_CUDA_TRY(cudaGetLastError());
   unsigned long long got = 0;
   XF_CUDA_TRY(cudaMemcpyAsync(&got, c, 8, cudaMemcpyDeviceToHost, st));
@@ -345,15 +246,15 @@ static int xf_diff_into(xf_model* base, xf_model* next, xf_delta* d) {
   struct Release { XfDevBuf* f; XfSortedSlots* s; ~Release() { f->release(); s->release(); } } rel{&fp, &s};
   XF_TRY(fp.ensure(32));
   XF_CUDA_TRY(cudaMemsetAsync(fp.p, 0, 32, st));
-  XF_TRY(xf_launch_fingerprint(base->view, base->fm, fp.as<unsigned long long>(), st));
-  XF_TRY(xf_launch_fingerprint(next->view, next->fm, fp.as<unsigned long long>() + 2, st));
+  XF_TRY(xf_launch_fingerprint(base->view, fp.as<unsigned long long>(), st));
+  XF_TRY(xf_launch_fingerprint(next->view, fp.as<unsigned long long>() + 2, st));
   XF_TRY(s.ensure(std::max(base->keys, next->keys)));
   // upserts: next's rows that base lacks or holds otherwise, gathered from next in key order
-  XF_TRY(xf_delta_list(next->view, base->view, h.fm, false, s, &h.upserts, st));
+  XF_TRY(xf_delta_list(next->view, base->view, false, s, &h.upserts, st));
   XF_TRY(d->rows.ensure(std::max<uint64_t>(h.upserts * h.row_bytes, 16)));
   XF_TRY(xf_model_gather(next->view, s.slots_out.as<uint32_t>(), h.upserts, d->rows.p, st));
   // deletes: base's keys that next lacks
-  XF_TRY(xf_delta_list(base->view, next->view, h.fm, true, s, &h.deletes, st));
+  XF_TRY(xf_delta_list(base->view, next->view, true, s, &h.deletes, st));
   XF_TRY(d->dels.ensure(std::max<uint64_t>(h.deletes * 8, 16)));
   if (h.deletes) XF_CUDA_TRY(cudaMemcpyAsync(d->dels.p, s.keys_out.p, h.deletes * 8, cudaMemcpyDeviceToDevice, st));
   unsigned long long f[4] = {0, 0, 0, 0};
@@ -392,18 +293,8 @@ XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out) {
 // the body of xf_model_apply_delta: on failure the caller frees `m`
 static int xf_apply_into(xf_model* base, const xf_delta* d, xf_model* m) {
   const XfDeltaHeader& h = d->h;
-  m->device = base->device;
-  XF_CUDA_TRY(cudaSetDevice(m->device));
-  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  XF_TRY(xf_model_init(m, base->device, xf_compat_of(base)));
   cudaStream_t st = m->stream;
-  m->fm = base->fm;
-  m->absent = base->absent;
-  m->optimizer = base->optimizer;
-  m->view.K = base->view.K;
-  m->view.opt = base->view.opt;
-  m->view.v_init = base->view.v_init;
-  m->view.v_const = base->view.v_const;
-  m->view.seed = base->view.seed;
   m->keys = h.result_keys;
   m->source_keys = h.source_keys;
   m->pruned_keys = h.pruned_keys;
@@ -414,7 +305,7 @@ static int xf_apply_into(xf_model* base, const xf_delta* d, xf_model* m) {
   unsigned long long* fp = aux.as<unsigned long long>();
   int* d_error = reinterpret_cast<int*>(fp + 4);
   XF_CUDA_TRY(cudaMemsetAsync(aux.p, 0, 40, st));
-  XF_TRY(xf_launch_fingerprint(base->view, base->fm, fp, st));
+  XF_TRY(xf_launch_fingerprint(base->view, fp, st));
   unsigned long long f[4] = {0, 0, 0, 0};
   XF_CUDA_TRY(cudaMemcpyAsync(f, fp, 16, cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaStreamSynchronize(st));
@@ -424,20 +315,14 @@ static int xf_apply_into(xf_model* base, const xf_delta* d, xf_model* m) {
                  (unsigned long long)h.base_keys);
     return XF_ERR_STATE;
   }
-  if (h.result_keys > (1ull << 31)) {
-    xf_set_error("xf_model_apply_delta: a serving model of %llu keys exceeds 2^32 slots", (unsigned long long)h.result_keys);
-    return XF_ERR_FULL;
-  }
   XF_TRY(xf_model_alloc(m, xf_model_capacity(h.result_keys)));
   // 1. the upserts; 2. base's rows that are neither deleted nor upserted; 3. the result's fingerprint
   XF_TRY(xf_model_insert_rows(m->view, static_cast<const uint8_t*>(d->rows.p), h.upserts, d_error, st));
   const int grid = xf_grid_for(base->view.mask + 1, 256, 8);
   const uint64_t* dels = static_cast<const uint64_t*>(d->dels.p);
-  if (m->fm == XF_SERVE_FMC) xf_k_apply_base_fmc<<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
-  else if (m->fm) xf_k_apply_base<true><<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
-  else xf_k_apply_base<false><<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
+  xf_k_apply_base<<<grid, 256, 0, st>>>(base->view, m->view, dels, h.deletes, d_error);
   XF_CUDA_TRY(cudaGetLastError());
-  XF_TRY(xf_launch_fingerprint(m->view, m->fm, fp + 2, st));
+  XF_TRY(xf_launch_fingerprint(m->view, fp + 2, st));
   int e = 0;
   XF_CUDA_TRY(cudaMemcpyAsync(f, fp, sizeof(f), cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaMemcpyAsync(&e, d_error, 4, cudaMemcpyDeviceToHost, st));
@@ -484,7 +369,7 @@ XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out) {
   XF_CUDA_TRY(cudaSetDevice(m->device));
   XF_TRY(m->s_aux.ensure(16));
   XF_CUDA_TRY(cudaMemsetAsync(m->s_aux.p, 0, 16, m->stream));
-  XF_TRY(xf_launch_fingerprint(m->view, m->fm, m->s_aux.as<unsigned long long>(), m->stream));
+  XF_TRY(xf_launch_fingerprint(m->view, m->s_aux.as<unsigned long long>(), m->stream));
   unsigned long long f[2] = {0, 0};
   XF_CUDA_TRY(cudaMemcpyAsync(f, m->s_aux.p, sizeof(f), cudaMemcpyDeviceToHost, m->stream));
   XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
@@ -516,65 +401,37 @@ XF_DLL int xf_delta_destroy(xf_delta* d) {
 }
 
 // ---- file
-static bool xf_sd_write(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
-static bool xf_sd_read(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
-
-// one section of n entries of `bytes` bytes from device memory `src`, chunk numbers from *chunk on
-static int xf_sd_save_section(xf_delta* d, FILE* f, const char* path, const uint8_t* src, uint64_t n, uint32_t bytes,
-                              uint64_t per_chunk, uint64_t* chunk) {
-  for (uint64_t first = 0; first < n; first += per_chunk, ++*chunk) {
-    const uint64_t c = std::min<uint64_t>(per_chunk, n - first);
-    XF_CUDA_TRY(cudaMemcpyAsync(d->stage.p, src + first * bytes, c * bytes, cudaMemcpyDeviceToHost, d->stream));
-    XF_CUDA_TRY(cudaStreamSynchronize(d->stream));
-    const uint64_t head[4] = {first, c, xf_st_host_sum(d->stage.p, c * bytes, xf_st_tag(*chunk)), 0ull};
-    if (!xf_sd_write(f, head, sizeof(head)) || !xf_sd_write(f, d->stage.p, c * bytes)) {
-      xf_set_error("write to %s failed", path);
-      return XF_ERR_IO;
-    }
-  }
-  return XF_OK;
-}
-
-static int xf_sd_save_body(xf_delta* d, FILE* f, const char* path) {
+static int xf_sd_save_body(xf_delta* d, FILE* f, const char* name) {
   XfDeltaHeader h = d->h;
   memcpy(h.magic, "XFSD", 4);
   h.version = XF_SD_VERSION;
   h.header_bytes = sizeof(h);
   h.zero = 0;
   h.header_checksum = xf_st_host_sum(&h, offsetof(XfDeltaHeader, header_checksum), 0);
-  if (!xf_sd_write(f, &h, sizeof(h))) { xf_set_error("write to %s failed", path); return XF_ERR_IO; }
-  XF_TRY(d->stage.ensure(std::max<uint64_t>(std::min<uint64_t>(XF_ST_CHUNK_BYTES, std::max(h.upserts * h.row_bytes, h.deletes * 8)), 16)));
+  if (fwrite(&h, 1, sizeof(h), f) != sizeof(h)) { xf_set_error("write to %s failed", name); return XF_ERR_IO; }
   uint64_t chunk = 0;
-  XF_TRY(xf_sd_save_section(d, f, path, d->rows.as<uint8_t>(), h.upserts, h.row_bytes, h.chunk_rows, &chunk));
-  return xf_sd_save_section(d, f, path, d->dels.as<uint8_t>(), h.deletes, 8u, h.chunk_keys, &chunk);
+  XF_TRY(xf_chunks_save(f, name, h.upserts, h.row_bytes, h.chunk_rows, &chunk, d->stage, d->stream,
+                        [&](uint64_t first, uint64_t, const void** dev) {
+                          *dev = d->rows.as<uint8_t>() + first * h.row_bytes;
+                          return XF_OK;
+                        }));
+  return xf_chunks_save(f, name, h.deletes, 8u, h.chunk_keys, &chunk, d->stage, d->stream,
+                        [&](uint64_t first, uint64_t, const void** dev) {
+                          *dev = d->dels.as<uint64_t>() + first;
+                          return XF_OK;
+                        });
 }
 
 XF_DLL int xf_delta_save(xf_delta* d, const char* path) {
   if (!d || !path) { xf_set_error("null argument"); return XF_ERR_ARG; }
   std::lock_guard<std::mutex> lock(d->mu);
   XF_CUDA_TRY(cudaSetDevice(d->device));
-  // written under a temporary name and renamed, as xf_model_save does
-  const std::string tmp = std::string(path) + ".tmp";
-  FILE* f = fopen(tmp.c_str(), "wb");
-  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
-  int rc = xf_sd_save_body(d, f, tmp.c_str());
-  if (fclose(f) != 0 && rc == XF_OK) { xf_set_error("write to %s failed", tmp.c_str()); rc = XF_ERR_IO; }
-  if (rc == XF_OK && rename(tmp.c_str(), path) != 0) { xf_set_error("cannot rename %s to %s", tmp.c_str(), path); rc = XF_ERR_IO; }
-  if (rc != XF_OK) remove(tmp.c_str());
-  return rc;
+  return xf_save_atomic(path, [&](FILE* f, const char* name) { return xf_sd_save_body(d, f, name); });
 }
 
 // the header's own consistency (after its checksum): every size derived from it is bounded before it is used
 static bool xf_sd_header_sane(const XfDeltaHeader& h) {
-  if (h.fm == XF_SERVE_FMC) {
-    if (!xf_fmc_latent_ok(h.latent_dim) || h.row_bytes != xf_model_row_bytes(h.fm, h.latent_dim)) return false;
-  } else if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) {
-    return false;
-  }
-  if (h.zero != 0) return false;
-  if (h.absent != XF_ABSENT_DEFAULT && h.absent != XF_ABSENT_ZERO) return false;
-  if (h.optimizer != XF_OPT_FTRL && h.optimizer != XF_OPT_SGD) return false;
-  if (h.v_init != 0 && h.v_init != XF_INIT_COUNTER && h.v_init != XF_INIT_ZERO) return false;
+  if (!xf_compat_sane(xf_compat_of(h), h.row_bytes) || h.zero != 0) return false;
   if (h.chunk_rows != XF_ST_CHUNK_BYTES / h.row_bytes || h.chunk_keys != XF_ST_CHUNK_BYTES / 8) return false;
   // a model holds at most 2^31 keys; a result past that is refused by apply (XF_ERR_FULL), not by the file
   if (h.base_keys > (1ull << 31) || h.result_keys > (1ull << 62) || h.source_keys < h.result_keys ||
@@ -583,67 +440,25 @@ static bool xf_sd_header_sane(const XfDeltaHeader& h) {
   return h.upserts <= h.result_keys && h.upserts <= (1ull << 31) && h.deletes <= h.base_keys;
 }
 
-// one section: n entries of `bytes` bytes into device memory `dst`, checked chunk by chunk; rows (bytes > 8) carry
-// their key in the first word and padding after byte `used`, canonical rows (canon_k = K > 0) where
-// xf_fmc_padding_zero says
-static int xf_sd_load_section(xf_delta* d, FILE* f, const char* path, uint8_t* dst, uint64_t n, uint32_t bytes, uint32_t used,
-                              int canon_k, uint64_t per_chunk, uint64_t* chunk, const char* what) {
-  uint64_t prev = 0;
-  for (uint64_t first = 0; first < n; first += per_chunk, ++*chunk) {
-    const uint64_t c = std::min<uint64_t>(per_chunk, n - first);
-    uint64_t head[4];
-    if (!xf_sd_read(f, head, sizeof(head)) || !xf_sd_read(f, d->stage.p, c * bytes)) {
-      xf_set_error("truncated delta file %s", path);
-      return XF_ERR_IO;
-    }
-    if (head[0] != first || head[1] != c || head[3] != 0 || head[2] != xf_st_host_sum(d->stage.p, c * bytes, xf_st_tag(*chunk))) {
-      xf_set_error("delta file %s: chunk %llu is damaged (checksum mismatch)", path, (unsigned long long)*chunk);
-      return XF_ERR_IO;
-    }
-    const uint8_t* p = d->stage.as<uint8_t>();
-    for (uint64_t r = 0; r < c; ++r, p += bytes) {
-      uint64_t key;
-      memcpy(&key, p, 8);
-      if ((first + r > 0 && key <= prev) || key == XF_EMPTY_KEY) {
-        xf_set_error("delta file %s: the %s keys are not strictly ascending below 2^64 - 1 (entry %llu)", path, what,
-                     (unsigned long long)(first + r));
-        return XF_ERR_IO;
-      }
-      prev = key;
-      if (canon_k > 0 && !xf_fmc_padding_zero(p, canon_k, bytes)) {
-        xf_set_error("delta file %s: upsert row %llu has non-zero padding", path, (unsigned long long)(first + r));
-        return XF_ERR_IO;
-      }
-      for (uint32_t b = used; b < bytes && canon_k == 0; ++b)
-        if (p[b] != 0) {
-          xf_set_error("delta file %s: upsert row %llu has non-zero padding", path, (unsigned long long)(first + r));
-          return XF_ERR_IO;
-        }
-    }
-    XF_CUDA_TRY(cudaMemcpyAsync(dst + first * bytes, d->stage.p, c * bytes, cudaMemcpyHostToDevice, d->stream));
-    XF_CUDA_TRY(cudaStreamSynchronize(d->stream));  // the pinned buffer is read again for the next chunk
-  }
-  return XF_OK;
-}
-
 static int xf_sd_load_body(xf_delta* d, FILE* f, const char* path, const XfDeltaHeader& h) {
-  const uint64_t expect = xf_sd_file_bytes(h);
-  if (fseek(f, 0, SEEK_END) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
-  const long fsz = ftell(f);
-  if (fsz < 0 || (uint64_t)fsz != expect) {
-    xf_set_error("corrupt or truncated delta file %s: %ld bytes, its header announces %llu", path, fsz, (unsigned long long)expect);
-    return XF_ERR_IO;
-  }
-  if (fseek(f, sizeof(XfDeltaHeader), SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  XF_TRY(xf_file_size_check(f, path, "delta file", xf_sd_file_bytes(h), sizeof(XfDeltaHeader)));
   d->h = h;
   XF_CUDA_TRY(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
   XF_TRY(d->rows.ensure(std::max<uint64_t>(h.upserts * h.row_bytes, 16)));
   XF_TRY(d->dels.ensure(std::max<uint64_t>(h.deletes * 8, 16)));
-  XF_TRY(d->stage.ensure(std::max<uint64_t>(std::min<uint64_t>(XF_ST_CHUNK_BYTES, std::max(h.upserts * h.row_bytes, h.deletes * 8)), 16)));
+  // each section into its device buffer as it is
+  auto into = [&](XfDevBuf& dst, uint32_t bytes) {
+    return [&dst, bytes, d](uint64_t first, uint64_t c, const void* host) {
+      XF_CUDA_TRY(cudaMemcpyAsync(dst.as<uint8_t>() + first * bytes, host, c * bytes, cudaMemcpyHostToDevice, d->stream));
+      return XF_OK;
+    };
+  };
   uint64_t chunk = 0;
-  XF_TRY(xf_sd_load_section(d, f, path, d->rows.as<uint8_t>(), h.upserts, h.row_bytes, h.fm ? 20u : 12u,
-                            h.fm == XF_SERVE_FMC ? h.latent_dim : 0, h.chunk_rows, &chunk, "upsert"));
-  XF_TRY(xf_sd_load_section(d, f, path, d->dels.as<uint8_t>(), h.deletes, 8u, 8u, 0, h.chunk_keys, &chunk, "delete"));
+  XF_TRY(xf_chunks_load(f, path, h.upserts, h.row_bytes, h.chunk_rows, &chunk,
+                        XfChunkCheck{"delta file", "upsert", h.fm, h.latent_dim, 0, 0}, d->stage, d->stream,
+                        into(d->rows, h.row_bytes)));
+  XF_TRY(xf_chunks_load(f, path, h.deletes, 8u, h.chunk_keys, &chunk, XfChunkCheck{"delta file", "delete", -1, 0, 0, 0},
+                        d->stage, d->stream, into(d->dels, 8u)));
   if (h.upserts && h.deletes) {
     XfDevBuf flag;
     struct Release { XfDevBuf* b; ~Release() { b->release(); } } rel{&flag};
@@ -670,11 +485,7 @@ XF_DLL int xf_delta_load(xf_delta** out, const char* path, int device) {
   memset(&h, 0, sizeof(h));
   const size_t got = fread(&h, 1, sizeof(h), f);
   int rc = XF_OK;
-  if (got >= 4 && (memcmp(h.magic, "XFSM", 4) == 0 || memcmp(h.magic, "XFSP", 4) == 0)) {
-    xf_set_error("%s is a serving model (%.4s), not a delta: load it with xf_model_load", path, h.magic);
-    rc = XF_ERR_IO;
-  } else if (got >= 4 && (memcmp(h.magic, "XFTB", 4) == 0 || memcmp(h.magic, "XFST", 4) == 0)) {
-    xf_set_error("%s is a training checkpoint (%.4s), not a delta", path, h.magic);
+  if (xf_refuse_foreign(h.magic, got, path, "XFSD") != XF_OK) {
     rc = XF_ERR_IO;
   } else if (got < 4 || memcmp(h.magic, "XFSD", 4) != 0) {
     xf_set_error("%s is not a serving model delta (no XFSD magic)", path);

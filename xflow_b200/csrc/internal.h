@@ -2,7 +2,9 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -169,6 +171,14 @@ __host__ __device__ __forceinline__ uint64_t xf_st_hash(uint64_t word, uint64_t 
 // offsets of a chunk's words: the chunk index above bit 40, the byte offset in the chunk's payload below
 __host__ __device__ __forceinline__ uint64_t xf_st_tag(uint64_t chunk) { return chunk << 40; }
 uint64_t xf_st_host_sum(const void* p, uint64_t bytes, uint64_t off0);
+// Write a file so that a reader never sees it half written: body(f, name) writes `path`.tmp (named `name` in its
+// errors), which is then closed and renamed to `path`.  On any failure the temporary file is removed and the error
+// returned; a short write or a failed close or rename is XF_ERR_IO.
+int xf_save_atomic(const char* path, const std::function<int(FILE* f, const char* name)>& body);
+// XF_ERR_IO, naming the format and the call that loads it, if the `got` bytes at `head` begin with the magic of one of
+// the project's file formats (XFTB, XFST, XFSM, XFSP, XFSD) that is not among `own`, the caller's magics (4 characters
+// each, the first naming what the caller loads); XF_OK otherwise
+int xf_refuse_foreign(const void* head, size_t got, const char* path, const char* own);
 
 // ingest.cu
 int xf_launch_parse(const char* d_text, uint64_t len, XfDevBuf& scratch, uint32_t* d_row_ptr, uint64_t* d_keys,

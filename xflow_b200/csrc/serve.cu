@@ -12,12 +12,17 @@
 //   predict  xf_k_serve<FM>       warp per row, two tokens per lane in flight, the mapping and the association of the
 //                                 step kernels' forward pass (step.cu, step_lazy.cu), so the result is theirs bit for bit;
 //                                 no insert, no atomics, no shared memory
-//   file     rows sorted by key (cub radix sort of (key, slot)), gathered a chunk at a time through bounded staging
+//   file     rows sorted by key (cub radix sort of (key, slot)), gathered a chunk at a time through bounded staging;
+//            xf_chunks_save / xf_chunks_load write and check the chunked sections of XFSM, XFSP and XFSD;
+//            load: xf_k_model_insert_rows
+//
+// Outside freeze, predict and lookup a row is {key, body}: the other passes (here xf_k_model_insert_rows and xf_k_merge,
+// in delta.cu fingerprint, diff and apply) copy, compare or hash bytes [8, stride) whole, one kernel for every row kind.
 //
 // A part (xf_table_freeze_part) is what xf_k_freeze makes of one shard table, whose counting pass also counts the keys
 // outside the shard's range; its file is XFSP.  xf_model_merge makes the whole model of S parts:
-//   merge    xf_k_merge<FM>        a grid-stride walk over a part's slots in place (or a 64 MiB chunk of them peer-copied
-//                                  from another device), each live row inserted with xf_model_insert
+//   merge    xf_k_merge            a grid-stride walk over a part's slots in place (or a 64 MiB chunk of them peer-copied
+//                                  from another device), each live row put whole with xf_model_put_row
 //
 // A canonical model (xf_table_freeze_canonical, fm = XF_SERVE_FMC) serves the textbook FM with feature values
 // (step_fmc.cu), whose per-k sums do not collapse: its row is {key, w, 0, v[K]} padded to a multiple of 32 bytes.
@@ -35,13 +40,11 @@
 #include <algorithm>
 #include <cub/cub.cuh>
 #include <mutex>
-#include <string>
 #include <vector>
 
 #include "serve.cuh"
 
 #define XF_SM_VERSION 1u
-#define XF_SM_CHUNK_HEAD 32  // {u64 first row, u64 rows, u64 checksum, u64 0}
 
 // The file header (little-endian, 104 bytes; the layout is documented in include/xflow_b200.h)
 struct XfModelHeader {
@@ -277,7 +280,16 @@ xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, uint64_t lo, ui
       keep = t.K > 0 && (absent == XF_ABSENT_DEFAULT ? (flags & XF_FLAG_V_READY) != 0u : !(st == 0.0f && qt == 0.0f));
     if (!keep) continue;
     ++kept_n;
-    if (!COUNT) xf_model_insert(m, h.key, h.w, st, qt, error);
+    if (COUNT) continue;
+    uint8_t* p = xf_model_claim(m, h.key, error);
+    if (!p) continue;
+    // the fields only: the padding stays as the fill left it, zero
+    if (t.K > 0) {
+      *reinterpret_cast<float2*>(p + 8) = make_float2(h.w, st);
+      *reinterpret_cast<float*>(p + 16) = qt;
+    } else {
+      *reinterpret_cast<float*>(p + 8) = h.w;
+    }
   }
   if (COUNT) {
     kept_n = __reduce_add_sync(0xffffffffu, kept_n);
@@ -340,15 +352,6 @@ xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned lo
   }
 }
 
-// insert n packed canonical rows into `m`
-__global__ void xf_k_model_insert_rows_fmc(XfTableView m, const uint8_t* __restrict__ rows, uint64_t n, int* error) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint8_t* src = rows + i * m.stride;
-    uint8_t* p = xf_model_claim(m, *reinterpret_cast<const uint64_t*>(src), error);
-    if (p) xf_model_copy_body(m, p, src);
-  }
-}
-
 // what a canonical model holds for keys[0 .. n): w, v[n][K] (either may be nullptr), present
 __global__ void xf_k_model_lookup_fmc(XfTableView m, const uint64_t* __restrict__ keys, uint64_t n, float* w_out, float* v_out,
                                       uint8_t* present) {
@@ -363,28 +366,23 @@ __global__ void xf_k_model_lookup_fmc(XfTableView m, const uint64_t* __restrict_
   }
 }
 
-// insert n packed rows (a chunk of a model file) into `m`
-__global__ void xf_k_model_insert_rows(XfTableView m, const uint8_t* __restrict__ rows, uint64_t n, int* error) {
+// insert n packed rows (a chunk of a model file, or a delta's upserts) into `m`
+__global__ void __launch_bounds__(256)
+xf_k_model_insert_rows(XfTableView m, const uint8_t* __restrict__ rows, uint64_t n, int* error) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint8_t* p = rows + i * m.stride;
-    const uint64_t key = *reinterpret_cast<const uint64_t*>(p);
-    const float w = *reinterpret_cast<const float*>(p + 8);
-    float st = 0.f, qt = 0.f;
-    if (m.K > 0) { st = *reinterpret_cast<const float*>(p + 12); qt = *reinterpret_cast<const float*>(p + 16); }
-    xf_model_insert(m, key, w, st, qt, error);
+    const uint8_t* src = rows + i * m.stride;
+    xf_model_put_row(m, src, __ldg(reinterpret_cast<const ulonglong2*>(src)), error);
   }
 }
 
 // merge: the live rows among n slots of a part (its own slot array, or a chunk of it staged on this device) into `m`
-template <bool FM>
 __global__ void __launch_bounds__(256)
 xf_k_merge(const uint8_t* __restrict__ slots, uint64_t n, XfTableView m, int* error) {
   for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
-    uint64_t key;
-    float w, st, qt;
-    xf_serve_load<FM>(slots + r * m.stride, key, w, st, qt);
-    if (key == XF_EMPTY_KEY) continue;
-    xf_model_insert(m, key, w, st, qt, error);
+    const uint8_t* src = slots + r * m.stride;
+    const ulonglong2 head = __ldg(reinterpret_cast<const ulonglong2*>(src));
+    if (head.x == XF_EMPTY_KEY) continue;
+    xf_model_put_row(m, src, head, error);
   }
 }
 
@@ -457,6 +455,21 @@ int xf_model_alloc(xf_model* m, uint64_t capacity) {
   return XF_OK;
 }
 
+int xf_model_init(xf_model* m, int device, const XfCompat& c) {
+  m->device = device;
+  XF_CUDA_TRY(cudaSetDevice(device));
+  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  m->fm = c.fm;
+  m->absent = c.absent;
+  m->optimizer = c.optimizer;
+  m->view.K = c.latent_dim;
+  m->view.opt = c.optimizer;
+  m->view.v_init = c.v_init;
+  m->view.v_const = c.v_const;
+  m->view.seed = c.seed;
+  return XF_OK;
+}
+
 void xf_model_free(xf_model* m) {
   if (!m) return;
   cudaSetDevice(m->device);
@@ -507,8 +520,7 @@ int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, voi
 
 int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st) {
   if (n == 0) return XF_OK;
-  if (v.canon) xf_k_model_insert_rows_fmc<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
-  else xf_k_model_insert_rows<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
+  xf_k_model_insert_rows<<<xf_grid_for(n, 256, 8), 256, 0, st>>>(v, rows, n, error);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }
@@ -527,17 +539,10 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   const int src_dev = t->cfg.device;
   XF_CUDA_TRY(cudaSetDevice(src_dev));
   XF_TRY(t->check_error());  // waits for everything enqueued on the table's stream
-  m->device = src_dev;
-  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   const XfTableView& tv = t->view;
-  m->fm = canonical ? XF_SERVE_FMC : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
-  m->optimizer = tv.opt;
-  m->absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
-  m->view.K = tv.K;
-  m->view.opt = tv.opt;
-  m->view.v_init = tv.v_init;
-  m->view.v_const = tv.v_const;
-  m->view.seed = tv.seed;
+  const int fm = canonical ? XF_SERVE_FMC : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
+  const int absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
+  XF_TRY(xf_model_init(m, src_dev, XfCompat{fm, tv.K, tv.opt, absent, tv.v_init, tv.v_const, tv.seed}));
   // the build runs on the model's stream: the table's stream is idle (above) and the host calls on the table are
   // locked out by the caller, so nothing writes the table while it is read
   cudaStream_t st = m->stream;
@@ -870,10 +875,100 @@ XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float*
 }
 
 // ---- file
-static bool xf_sm_write(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
-static bool xf_sm_read(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
+static bool xf_write(FILE* f, const void* p, size_t n) { return n == 0 || fwrite(p, 1, n, f) == n; }
+static bool xf_read(FILE* f, void* p, size_t n) { return n == 0 || fread(p, 1, n, f) == n; }
 
-static int xf_sm_save_body(xf_model* m, FILE* f, const char* path) {
+int xf_chunks_save(FILE* f, const char* name, uint64_t n, uint32_t bytes, uint64_t per_chunk, uint64_t* chunk, XfPinBuf& pin,
+                   cudaStream_t st, const std::function<int(uint64_t first, uint64_t c, const void** dev)>& src) {
+  if (n == 0) return XF_OK;
+  XF_TRY(pin.ensure(std::min(per_chunk, n) * bytes));
+  for (uint64_t first = 0; first < n; first += per_chunk, ++*chunk) {
+    const uint64_t c = std::min(per_chunk, n - first);
+    const void* dev = nullptr;
+    XF_TRY(src(first, c, &dev));
+    XF_CUDA_TRY(cudaMemcpyAsync(pin.p, dev, c * bytes, cudaMemcpyDeviceToHost, st));
+    XF_CUDA_TRY(cudaStreamSynchronize(st));
+    const uint64_t head[4] = {first, c, xf_st_host_sum(pin.p, c * bytes, xf_st_tag(*chunk)), 0ull};
+    if (!xf_write(f, head, sizeof(head)) || !xf_write(f, pin.p, c * bytes)) {
+      xf_set_error("write to %s failed", name);
+      return XF_ERR_IO;
+    }
+  }
+  return XF_OK;
+}
+
+int xf_chunks_load(FILE* f, const char* path, uint64_t n, uint32_t bytes, uint64_t per_chunk, uint64_t* chunk,
+                   const XfChunkCheck& check, XfPinBuf& pin, cudaStream_t st,
+                   const std::function<int(uint64_t first, uint64_t c, const void* host)>& sink) {
+  if (n == 0) return XF_OK;
+  XF_TRY(pin.ensure(std::min(per_chunk, n) * bytes));
+  uint64_t lo = 0, hi = 0, prev = 0;
+  xf_shard_range(check.shard_index, check.num_shards, &lo, &hi);
+  for (uint64_t first = 0; first < n; first += per_chunk, ++*chunk) {
+    const uint64_t c = std::min(per_chunk, n - first);
+    uint64_t head[4];
+    if (!xf_read(f, head, sizeof(head)) || !xf_read(f, pin.p, c * bytes)) {
+      xf_set_error("truncated %s %s", check.file, path);
+      return XF_ERR_IO;
+    }
+    if (head[0] != first || head[1] != c || head[3] != 0 || head[2] != xf_st_host_sum(pin.p, c * bytes, xf_st_tag(*chunk))) {
+      xf_set_error("%s %s: chunk %llu is damaged (checksum mismatch)", check.file, path, (unsigned long long)*chunk);
+      return XF_ERR_IO;
+    }
+    const uint8_t* p = pin.as<uint8_t>();
+    for (uint64_t r = first; r < first + c; ++r, p += bytes) {
+      uint64_t key;
+      memcpy(&key, p, 8);
+      if ((r > 0 && key <= prev) || key == XF_EMPTY_KEY) {
+        xf_set_error("%s %s: the %s keys are not strictly ascending below 2^64 - 1 (entry %llu)", check.file, path, check.what,
+                     (unsigned long long)r);
+        return XF_ERR_IO;
+      }
+      prev = key;
+      if (key < lo || key > hi) {
+        xf_set_error("%s %s: key %016llx of %s %llu lies outside shard %d of %d", check.file, path, (unsigned long long)key,
+                     check.what, (unsigned long long)r, check.shard_index, check.num_shards);
+        return XF_ERR_IO;
+      }
+      if (check.fm >= 0 && !xf_model_padding_zero(p, check.fm, check.K, bytes)) {
+        xf_set_error("%s %s: %s %llu has non-zero padding", check.file, path, check.what, (unsigned long long)r);
+        return XF_ERR_IO;
+      }
+    }
+    XF_TRY(sink(first, c, pin.p));
+    XF_CUDA_TRY(cudaStreamSynchronize(st));  // the pinned buffer is read again for the next chunk
+  }
+  return XF_OK;
+}
+
+int xf_file_size_check(FILE* f, const char* path, const char* file, uint64_t expect, uint64_t header_bytes) {
+  if (fseek(f, 0, SEEK_END) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  const long fsz = ftell(f);
+  if (fsz < 0 || (uint64_t)fsz != expect) {
+    xf_set_error("corrupt or truncated %s %s: %ld bytes, its header announces %llu", file, path, fsz, (unsigned long long)expect);
+    return XF_ERR_IO;
+  }
+  if (fseek(f, (long)header_bytes, SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
+  return XF_OK;
+}
+
+bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
+  if (c.fm == XF_SERVE_FMC) {
+    if (!xf_fmc_latent_ok(c.latent_dim) || row_bytes != xf_model_row_bytes(c.fm, c.latent_dim)) return false;
+  } else if (c.fm != (c.latent_dim > 0 ? 1 : 0) || c.latent_dim < 0 || row_bytes != (c.fm ? 32u : 16u)) {
+    return false;
+  }
+  if (c.absent != XF_ABSENT_DEFAULT && c.absent != XF_ABSENT_ZERO) return false;
+  if (c.optimizer != XF_OPT_FTRL && c.optimizer != XF_OPT_SGD) return false;
+  return c.v_init == 0 || c.v_init == XF_INIT_COUNTER || c.v_init == XF_INIT_ZERO;
+}
+
+// the model header's side of the compatibility check (serve.cuh: XfCompat)
+static XfCompat xf_compat_of(const XfModelHeader& h) {
+  return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed};
+}
+
+static int xf_sm_save_body(xf_model* m, FILE* f, const char* name) {
   XfModelHeader h;
   memset(&h, 0, sizeof(h));
   memcpy(h.magic, "XFSM", 4);
@@ -902,135 +997,66 @@ static int xf_sm_save_body(xf_model* m, FILE* f, const char* path) {
     p.shard_index = m->shard_index;
     p.num_shards = m->num_shards;
     p.header_checksum = xf_st_host_sum(&p, offsetof(XfPartHeader, header_checksum), 0);
-    wrote = xf_sm_write(f, &p, sizeof(p));
+    wrote = xf_write(f, &p, sizeof(p));
   } else {
     h.header_checksum = xf_st_host_sum(&h, offsetof(XfModelHeader, header_checksum), 0);
-    wrote = xf_sm_write(f, &h, sizeof(h));
+    wrote = xf_write(f, &h, sizeof(h));
   }
-  if (!wrote) { xf_set_error("write to %s failed", path); return XF_ERR_IO; }
+  if (!wrote) { xf_set_error("write to %s failed", name); return XF_ERR_IO; }
   const uint64_t n = m->keys;
   if (n == 0) return XF_OK;
-  // (key, slot) of every row, sorted by key on the device
+  // (key, slot) of every row, sorted by key on the device; then the rows in that order, a chunk at a time gathered
   cudaStream_t st = m->stream;
   XfSortedSlots sorted;
   XfDevBuf rows;
   struct Release { XfSortedSlots* s; XfDevBuf* r; ~Release() { s->release(); r->release(); } } rel{&sorted, &rows};
   XF_TRY(xf_model_list_sorted(m->view, n, sorted, st));
-  // the rows in that order, a chunk at a time: gathered on the device, copied to the pinned buffer, summed and written
-  const uint64_t C = std::min<uint64_t>(h.chunk_rows, n);
-  XF_TRY(rows.ensure(C * h.row_bytes));
-  XF_TRY(m->h_out.ensure(C * h.row_bytes));
-  for (uint64_t first = 0, chunk = 0; first < n; first += h.chunk_rows, ++chunk) {
-    const uint64_t c = std::min<uint64_t>(h.chunk_rows, n - first);
-    XF_TRY(xf_model_gather(m->view, sorted.slots_out.as<uint32_t>() + first, c, rows.p, st));
-    XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, rows.p, c * h.row_bytes, cudaMemcpyDeviceToHost, st));
-    XF_CUDA_TRY(cudaStreamSynchronize(st));
-    const uint64_t head[4] = {first, c, xf_st_host_sum(m->h_out.p, c * h.row_bytes, xf_st_tag(chunk)), 0ull};
-    if (!xf_sm_write(f, head, sizeof(head)) || !xf_sm_write(f, m->h_out.p, c * h.row_bytes)) {
-      xf_set_error("write to %s failed", path);
-      return XF_ERR_IO;
-    }
-  }
-  return XF_OK;
+  XF_TRY(rows.ensure(std::min<uint64_t>(h.chunk_rows, n) * h.row_bytes));
+  uint64_t chunk = 0;
+  return xf_chunks_save(f, name, n, h.row_bytes, h.chunk_rows, &chunk, m->h_out, st,
+                        [&](uint64_t first, uint64_t c, const void** dev) {
+                          *dev = rows.p;
+                          return xf_model_gather(m->view, sorted.slots_out.as<uint32_t>() + first, c, rows.p, st);
+                        });
 }
 
 XF_DLL int xf_model_save(xf_model* m, const char* path) {
   if (!m || !path) { xf_set_error("null argument"); return XF_ERR_ARG; }
   std::lock_guard<std::mutex> lock(m->mu);
   XF_CUDA_TRY(cudaSetDevice(m->device));
-  // written under a temporary name and renamed, as xf_table_save does
-  const std::string tmp = std::string(path) + ".tmp";
-  FILE* f = fopen(tmp.c_str(), "wb");
-  if (!f) { xf_set_error("cannot open %s for writing", tmp.c_str()); return XF_ERR_IO; }
-  int rc = xf_sm_save_body(m, f, tmp.c_str());
-  if (fclose(f) != 0 && rc == XF_OK) { xf_set_error("write to %s failed", tmp.c_str()); rc = XF_ERR_IO; }
-  if (rc == XF_OK && rename(tmp.c_str(), path) != 0) { xf_set_error("cannot rename %s to %s", tmp.c_str(), path); rc = XF_ERR_IO; }
-  if (rc != XF_OK) remove(tmp.c_str());
-  return rc;
+  return xf_save_atomic(path, [&](FILE* f, const char* name) { return xf_sm_save_body(m, f, name); });
 }
 
 // the header's own consistency (after its checksum): every size derived from it is bounded before it is used
 static bool xf_sm_header_sane(const XfModelHeader& h) {
-  if (h.fm == XF_SERVE_FMC) {
-    if (!xf_fmc_latent_ok(h.latent_dim) || h.row_bytes != xf_model_row_bytes(h.fm, h.latent_dim)) return false;
-  } else if (h.fm != (h.latent_dim > 0 ? 1 : 0) || h.latent_dim < 0 || h.row_bytes != (h.fm ? 32u : 16u)) {
-    return false;
-  }
+  if (!xf_compat_sane(xf_compat_of(h), h.row_bytes)) return false;
   if (h.keys > (1ull << 31) || h.capacity != xf_model_capacity(h.keys) || h.keys + h.pruned_keys != h.source_keys) return false;
-  if (h.absent != XF_ABSENT_DEFAULT && h.absent != XF_ABSENT_ZERO) return false;
-  if (h.optimizer != XF_OPT_FTRL && h.optimizer != XF_OPT_SGD) return false;
-  if (h.v_init != 0 && h.v_init != XF_INIT_COUNTER && h.v_init != XF_INIT_ZERO) return false;
   return h.chunk_rows == XF_ST_CHUNK_BYTES / h.row_bytes && h.zero == 0;
 }
 
-// the rows of an XFSM or XFSP file (header of `header_bytes`) into `m`; m->shard_index, num_shards are set: a part's
-// keys must lie in its shard's range
-static int xf_sm_load_body(xf_model* m, FILE* f, const char* path, const XfModelHeader& h, uint64_t header_bytes) {
-  uint64_t lo = 0, hi = 0;
-  xf_shard_range(m->shard_index, m->num_shards, &lo, &hi);
-  const uint64_t nch = (h.keys + h.chunk_rows - 1) / h.chunk_rows;
-  const uint64_t expect = header_bytes + nch * XF_SM_CHUNK_HEAD + h.keys * h.row_bytes;
-  if (fseek(f, 0, SEEK_END) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
-  const long fsz = ftell(f);
-  if (fsz < 0 || (uint64_t)fsz != expect) {
-    xf_set_error("corrupt or truncated model file %s: %ld bytes, its header announces %llu", path, fsz, (unsigned long long)expect);
-    return XF_ERR_IO;
-  }
-  if (fseek(f, (long)header_bytes, SEEK_SET) != 0) { xf_set_error("cannot read %s", path); return XF_ERR_IO; }
-  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
-  m->fm = h.fm;
-  m->absent = h.absent;
-  m->optimizer = h.optimizer;
+// the rows of an XFSM or XFSP file (header of `header_bytes`) into `m` on `device`; m->shard_index, num_shards are set:
+// a part's keys must lie in its shard's range
+static int xf_sm_load_body(xf_model* m, int device, FILE* f, const char* path, const XfModelHeader& h, uint64_t header_bytes) {
+  XF_TRY(xf_model_init(m, device, xf_compat_of(h)));
+  XF_TRY(xf_file_size_check(f, path, "model file", header_bytes + xf_section_bytes(h.keys, h.row_bytes, h.chunk_rows),
+                            header_bytes));
   m->keys = h.keys;
   m->source_keys = h.source_keys;
   m->pruned_keys = h.pruned_keys;
-  m->view.K = h.latent_dim;
-  m->view.opt = h.optimizer;
-  m->view.v_init = h.v_init;
-  m->view.v_const = h.v_const;
-  m->view.seed = h.seed;
   XF_TRY(xf_model_alloc(m, h.capacity));
   if (h.keys == 0) { XF_CUDA_TRY(cudaStreamSynchronize(m->stream)); return XF_OK; }
-  const uint64_t C = std::min<uint64_t>(h.chunk_rows, h.keys);
   XfDevBuf rows, err;
   struct Release { XfDevBuf* b[2]; ~Release() { for (XfDevBuf* x : b) x->release(); } } rel{{&rows, &err}};
-  XF_TRY(rows.ensure(C * h.row_bytes));
+  XF_TRY(rows.ensure(std::min<uint64_t>(h.chunk_rows, h.keys) * h.row_bytes));
   XF_TRY(err.ensure(4));
-  XF_TRY(m->h_in.ensure(C * h.row_bytes));
   XF_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, m->stream));
-  uint64_t prev = 0;
-  for (uint64_t i = 0, first = 0; i < nch; ++i) {
-    const uint64_t c = std::min<uint64_t>(h.chunk_rows, h.keys - first);
-    uint64_t head[4];
-    if (!xf_sm_read(f, head, sizeof(head)) || !xf_sm_read(f, m->h_in.p, c * h.row_bytes)) { xf_set_error("truncated model file %s", path); return XF_ERR_IO; }
-    if (head[0] != first || head[1] != c || head[3] != 0 || head[2] != xf_st_host_sum(m->h_in.p, c * h.row_bytes, xf_st_tag(i))) {
-      xf_set_error("model file %s: chunk %llu of the rows is damaged (checksum mismatch)", path, (unsigned long long)i);
-      return XF_ERR_IO;
-    }
-    // the keys ascend strictly: none twice, none the empty-slot marker but possibly the last
-    for (uint64_t r = 0; r < c; ++r) {
-      uint64_t key;
-      memcpy(&key, (const uint8_t*)m->h_in.p + r * h.row_bytes, 8);
-      if ((first + r > 0 && key <= prev) || key == XF_EMPTY_KEY) {
-        xf_set_error("model file %s: the keys of chunk %llu are not in ascending order", path, (unsigned long long)i);
-        return XF_ERR_IO;
-      }
-      prev = key;
-      if (key < lo || key > hi) {
-        xf_set_error("model file %s: key %016llx of row %llu lies outside shard %d of %d", path, (unsigned long long)key,
-                     (unsigned long long)(first + r), m->shard_index, m->num_shards);
-        return XF_ERR_IO;
-      }
-      if (h.fm == XF_SERVE_FMC && !xf_fmc_padding_zero((const uint8_t*)m->h_in.p + r * h.row_bytes, h.latent_dim, h.row_bytes)) {
-        xf_set_error("model file %s: row %llu has non-zero padding", path, (unsigned long long)(first + r));
-        return XF_ERR_IO;
-      }
-    }
-    XF_CUDA_TRY(cudaMemcpyAsync(rows.p, m->h_in.p, c * h.row_bytes, cudaMemcpyHostToDevice, m->stream));
-    XF_TRY(xf_model_insert_rows(m->view, rows.as<uint8_t>(), c, err.as<int>(), m->stream));
-    XF_CUDA_TRY(cudaStreamSynchronize(m->stream));  // the pinned buffer is read again for the next chunk
-    first += c;
-  }
+  XfChunkCheck check{"model file", "row", h.fm, h.latent_dim, m->shard_index, m->num_shards};
+  uint64_t chunk = 0;
+  XF_TRY(xf_chunks_load(f, path, h.keys, h.row_bytes, h.chunk_rows, &chunk, check, m->h_in, m->stream,
+                        [&](uint64_t, uint64_t c, const void* host) -> int {
+                          XF_CUDA_TRY(cudaMemcpyAsync(rows.p, host, c * h.row_bytes, cudaMemcpyHostToDevice, m->stream));
+                          return xf_model_insert_rows(m->view, rows.as<uint8_t>(), c, err.as<int>(), m->stream);
+                        }));
   int e = 0;
   XF_CUDA_TRY(cudaMemcpy(&e, err.p, 4, cudaMemcpyDeviceToHost));
   if (e) { xf_set_error("model file %s: a probe sequence of the model overflowed", path); return XF_ERR_IO; }
@@ -1051,8 +1077,7 @@ XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
   const bool part = got >= 4 && memcmp(h.magic, "XFSP", 4) == 0;
   const size_t hbytes = part ? sizeof(XfPartHeader) : sizeof(XfModelHeader);
   int rc = XF_OK;
-  if (got >= 4 && (memcmp(h.magic, "XFTB", 4) == 0 || memcmp(h.magic, "XFST", 4) == 0)) {
-    xf_set_error("%s is a training checkpoint (%.4s), not a serving model: load it into a table and freeze that", path, h.magic);
+  if (xf_refuse_foreign(h.magic, got, path, "XFSMXFSP") != XF_OK) {
     rc = XF_ERR_IO;
   } else if (got < 4 || (memcmp(h.magic, "XFSM", 4) != 0 && !part)) {
     xf_set_error("%s is not a serving model (no XFSM or XFSP magic)", path);
@@ -1075,12 +1100,11 @@ XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
   xf_model* m = nullptr;
   if (rc == XF_OK) {
     m = new xf_model;
-    m->device = device;
     if (part) {
       m->shard_index = p.shard_index;
       m->num_shards = p.num_shards;
     }
-    rc = cudaSetDevice(device) == cudaSuccess ? xf_sm_load_body(m, f, path, h, hbytes) : XF_ERR_CUDA;
+    rc = xf_sm_load_body(m, device, f, path, h, hbytes);
   }
   fclose(f);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
@@ -1091,27 +1115,12 @@ XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
 // ---- merge
 // the body of xf_model_merge (the parts checked): on failure the caller frees `m`
 static int xf_merge_into(xf_model* const* parts, int n, int device, xf_model* m) {
-  const xf_model* p0 = parts[0];
-  m->device = device;
-  XF_CUDA_TRY(cudaSetDevice(device));
-  XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+  XF_TRY(xf_model_init(m, device, xf_compat_of(parts[0])));
   cudaStream_t st = m->stream;
-  m->fm = p0->fm;
-  m->absent = p0->absent;
-  m->optimizer = p0->optimizer;
-  m->view.K = p0->view.K;
-  m->view.opt = p0->view.opt;
-  m->view.v_init = p0->view.v_init;
-  m->view.v_const = p0->view.v_const;
-  m->view.seed = p0->view.seed;
   for (int i = 0; i < n; ++i) {
     m->keys += parts[i]->keys;
     m->source_keys += parts[i]->source_keys;
     m->pruned_keys += parts[i]->pruned_keys;
-  }
-  if (m->keys > (1ull << 31)) {
-    xf_set_error("xf_model_merge: a serving model of %llu keys exceeds 2^32 slots", (unsigned long long)m->keys);
-    return XF_ERR_FULL;
   }
   XF_TRY(xf_model_alloc(m, xf_model_capacity(m->keys)));
   XfDevBuf err, stage;
@@ -1120,8 +1129,7 @@ static int xf_merge_into(xf_model* const* parts, int n, int device, xf_model* m)
   XF_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, st));
   const uint32_t stride = m->view.stride;
   auto launch = [&](const uint8_t* slots, uint64_t c) -> int {
-    if (m->fm) xf_k_merge<true><<<xf_grid_for(c, 256, 8), 256, 0, st>>>(slots, c, m->view, err.as<int>());
-    else xf_k_merge<false><<<xf_grid_for(c, 256, 8), 256, 0, st>>>(slots, c, m->view, err.as<int>());
+    xf_k_merge<<<xf_grid_for(c, 256, 8), 256, 0, st>>>(slots, c, m->view, err.as<int>());
     XF_CUDA_TRY(cudaGetLastError());
     return XF_OK;
   };

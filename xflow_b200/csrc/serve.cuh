@@ -1,6 +1,6 @@
 // Serving model internals shared by serve.cu (freeze, predict, the XFSM file) and delta.cu (diff, apply, the XFSD file):
-// the model's host structure, the device functions that read and build its rows, and the host steps both use.  The
-// kernels behind the host steps live in serve.cu only.
+// the model's host structure, the device functions that read and build its rows, the host steps both use and the
+// chunked sections of their files.  The kernels behind the host steps live in serve.cu only.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -72,13 +72,20 @@ __host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K) {
 }
 // the latent dimensions a canonical model serves: C = K / 4 lanes per token, a power of two <= 32
 inline bool xf_fmc_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 128; }
-// a packed canonical row (K, row_bytes) has zero bytes where the layout has padding: [12, 16) and [16 + 4K, row_bytes)
-inline bool xf_fmc_padding_zero(const uint8_t* p, int K, uint32_t row_bytes) {
-  for (uint32_t b = 12; b < 16; ++b)
-    if (p[b]) return false;
-  for (uint32_t b = 16u + 4u * (uint32_t)K; b < row_bytes; ++b)
-    if (p[b]) return false;
-  return true;
+// A packed row of a model (fm, K, row_bytes) has zero bytes where its layout has padding: LR [12, 16), FM [20, 32),
+// canonical [12, 16) and [16 + 4K, row_bytes).  Every model in memory keeps them zero (the fill writes them, freeze
+// writes fields only, the other passes copy whole rows), so that whole rows compare and hash as their fields do.
+// Checked a word at a time: the 4-byte word after w (LR, canonical) or qt (FM), then 8-byte words to the row's end.
+inline bool xf_model_padding_zero(const uint8_t* p, int fm, int K, uint32_t row_bytes) {
+  uint32_t w4;
+  memcpy(&w4, p + (fm == XF_SERVE_FM ? 20 : 12), 4);
+  uint64_t any = w4;
+  for (uint32_t b = fm == XF_SERVE_FMC ? 16u + 4u * (uint32_t)K : fm == XF_SERVE_FM ? 24u : 16u; b < row_bytes; b += 8) {
+    uint64_t x;
+    memcpy(&x, p + b, 8);
+    any |= x;
+  }
+  return any == 0;
 }
 
 // ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
@@ -110,35 +117,11 @@ __device__ __forceinline__ bool xf_serve_find(const XfTableView& m, uint64_t key
   return false;
 }
 
-// Claim a slot for `key` and write its row; a probe overflow sets *error.  KEEP = false: the inserted keys are unique,
-// and a key met twice sets *error.  KEEP = true: a key the model already holds keeps its row (the caller orders the
-// kernels so that the row it holds is complete).
-template <bool KEEP = false>
-__device__ __forceinline__ void xf_model_insert(const XfTableView& m, uint64_t key, float w, float st, float qt, int* error) {
-  for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
-    uint8_t* rowp = xf_row(m, xf_probe_slot(m, key, i));
-    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(rowp), (unsigned long long)XF_EMPTY_KEY,
-                                             (unsigned long long)key);
-    if (old == XF_EMPTY_KEY) {
-      if (m.K > 0) {
-        *reinterpret_cast<float2*>(rowp + 8) = make_float2(w, st);
-        *reinterpret_cast<float*>(rowp + 16) = qt;
-      } else {
-        *reinterpret_cast<float*>(rowp + 8) = w;
-      }
-      return;
-    }
-    if (old == key) {
-      if (KEEP) return;
-      break;
-    }
-  }
-  *error = 1;
-}
-
-// ---- canonical rows (runtime stride: any K the model serves)
-// Claim a slot for `key` and return its row, for the caller to write bytes 8 .. stride; nullptr: not claimed.  The
-// error cases and KEEP are xf_model_insert's (a key KEEP finds is nullptr, its row untouched).
+// ---- whole rows: bytes [8, stride) are opaque outside freeze, predict and lookup
+// Claim a slot for `key` and return its row, for the caller to write bytes 8 .. stride; nullptr: not claimed.  A probe
+// overflow sets *error.  KEEP = false: the inserted keys are unique, and a key met twice sets *error.  KEEP = true: a
+// key the model already holds keeps its row, untouched (the caller orders the kernels so that the row it holds is
+// complete).
 template <bool KEEP = false>
 __device__ __forceinline__ uint8_t* xf_model_claim(const XfTableView& m, uint64_t key, int* error) {
   for (uint32_t i = 0; i < XF_MAX_PROBE; ++i) {
@@ -154,10 +137,18 @@ __device__ __forceinline__ uint8_t* xf_model_claim(const XfTableView& m, uint64_
   *error = 1;
   return nullptr;
 }
-// bytes 8 .. stride of the row at `src` into the row at `dst` (16-byte aligned, stride a multiple of 16)
-__device__ __forceinline__ void xf_model_copy_body(const XfTableView& m, uint8_t* dst, const uint8_t* src) {
-  *reinterpret_cast<uint64_t*>(dst + 8) = *reinterpret_cast<const uint64_t*>(src + 8);
-  for (uint32_t o = 16; o < m.stride; o += 16)
+// The row at `src` into the model `m`: `head` is its first 16 bytes {key, word 8}, which the caller has loaded to read
+// the key; bytes 16 .. stride follow 16 bytes per access.  Bytes 16 .. 31 (all of an FM row's rest) are loaded before
+// the claim, so that their latency overlaps the CAS's.  The claim is xf_model_claim<KEEP>'s.
+template <bool KEEP = false>
+__device__ __forceinline__ void xf_model_put_row(const XfTableView& m, const uint8_t* src, ulonglong2 head, int* error) {
+  const bool wide = m.stride > 16u;
+  const uint4 second = wide ? *reinterpret_cast<const uint4*>(src + 16) : make_uint4(0u, 0u, 0u, 0u);
+  uint8_t* dst = xf_model_claim<KEEP>(m, head.x, error);
+  if (!dst) return;
+  *reinterpret_cast<unsigned long long*>(dst + 8) = head.y;
+  if (wide) *reinterpret_cast<uint4*>(dst + 16) = second;
+  for (uint32_t o = 32; o < m.stride; o += 16)
     *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(src + o);
 }
 // the slot that holds `key`, or -1: the key words only, through the non-coherent path
@@ -171,13 +162,15 @@ __device__ __forceinline__ int64_t xf_model_find_slot(const XfTableView& m, uint
   return -1;
 }
 
-// slots of a model of `keys` keys: the smallest power of two >= 2 x keys (load <= 0.5), at least 1024
+// slots of a model of `keys` keys: the smallest power of two >= 2 x keys (load <= 0.5), at least 1024; keys <= 2^62
 inline uint64_t xf_model_capacity(uint64_t keys) {
   uint64_t c = 1024;
   while (c < 2 * keys) c <<= 1;
   return c;
 }
 
+// a new model on `device`, which is made current: its stream, and the fields XfCompat describes
+int xf_model_init(xf_model* m, int device, const XfCompat& c);
 // the model's table on the current device: `capacity` empty rows (stride from m->fm, m->view.K), filled on m->stream;
 // XF_ERR_FULL past 2^32 slots
 int xf_model_alloc(xf_model* m, uint64_t capacity);
@@ -198,6 +191,40 @@ int xf_model_list_sorted(const XfTableView& v, uint64_t n, XfSortedSlots& s, cud
 int xf_sort_slots(XfSortedSlots& s, uint64_t n, cudaStream_t st);
 // out = the rows of `v` in slots[0 .. n), packed
 int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, void* out, cudaStream_t st);
-// insert n packed rows (as a model file holds them; keys unique) into `v` (canonical rows if v.canon); a probe overflow
-// or a key met twice sets *error
+// insert n packed rows (as a model file holds them; keys unique) into `v`; a probe overflow or a key met twice sets
+// *error
 int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st);
+
+// ---- the files' chunked sections (XFSM and XFSP rows, XFSD upserts and delete keys)
+// A section of n entries of `bytes` bytes is a sequence of chunks of per_chunk entries (the last may be shorter), each a
+// head {u64 first entry, u64 entries, u64 checksum, u64 0} and its entries.  The checksum is xf_st_host_sum over the
+// entries, their offsets tagged with the chunk's index in the file (xf_st_tag), which runs on from section to section.
+#define XF_CHUNK_HEAD 32
+// the section's bytes in the file
+inline uint64_t xf_section_bytes(uint64_t n, uint32_t bytes, uint64_t per_chunk) {
+  return (n + per_chunk - 1) / per_chunk * XF_CHUNK_HEAD + n * bytes;
+}
+// Write a section, chunk indices from *chunk on (advanced past it).  src(first, c, &dev) makes entries [first, first + c)
+// ready at device address dev on `st`; each chunk is staged through `pin`, summed and written.
+int xf_chunks_save(FILE* f, const char* name, uint64_t n, uint32_t bytes, uint64_t per_chunk, uint64_t* chunk, XfPinBuf& pin,
+                   cudaStream_t st, const std::function<int(uint64_t first, uint64_t c, const void** dev)>& src);
+// What a section's entries must satisfy besides their checksums: each begins with a key, and the keys ascend strictly,
+// stay below 2^64 - 1 and lie in shard shard_index of num_shards (xf_shard_range; 0 of 0: any key); entries that are
+// rows (fm >= 0: XF_SERVE_*, of latent_dim K) have zero padding (xf_model_padding_zero).  file and what name the file
+// and the entries in the errors.
+struct XfChunkCheck {
+  const char* file;
+  const char* what;
+  int fm, K;
+  int shard_index, num_shards;
+};
+// Read a section written by xf_chunks_save and check it chunk by chunk (XF_ERR_IO at the first fault), staged through
+// `pin`; sink(first, c, host) takes each verified chunk, and `st` is synchronised before the next one is read into `pin`.
+int xf_chunks_load(FILE* f, const char* path, uint64_t n, uint32_t bytes, uint64_t per_chunk, uint64_t* chunk,
+                   const XfChunkCheck& check, XfPinBuf& pin, cudaStream_t st,
+                   const std::function<int(uint64_t first, uint64_t c, const void* host)>& sink);
+// XF_ERR_IO unless the file is `expect` bytes long, as its header announces; leaves it positioned at `header_bytes`
+int xf_file_size_check(FILE* f, const char* path, const char* file, uint64_t expect, uint64_t header_bytes);
+// the fields a model's and a delta's header share: a row kind with its latent_dim and row_bytes, and a known absent
+// policy, optimizer and v_init
+bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes);
