@@ -577,9 +577,28 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *    most 64 MiB for the slots of parts on other devices (peer copies, a chunk at a time).  The merge only reads the
  *    parts.  Not provided: a model served sharded across GPUs, a merge over the comm's peer mappings without files
  *    or staging, and deltas made from parts without merging them.
+ *
+ *    Precision.  Every model has a precision for its latent fields.  XF_PRECISION_F32 is what freeze, merge, load and
+ *    apply make of F32 inputs.  xf_model_convert makes an XF_PRECISION_F16 model of an FM or canonical one: w stays
+ *    float32, and only the latent fields (FM st and qt; canonical every v_k) become IEEE binary16, rounded to nearest
+ *    even (subnormals included).  Every row still starts with its u64 key, and padding stays zero:
+ *      kind        F32                                                   F16
+ *      LR          {key, f32 w, u32 0} 16 bytes                          refused: nothing to narrow
+ *      FM          {key, f32 w, f32 st, f32 qt, 12 zero bytes} 32        {key, f32 w, f16 st, f16 qt} 16, no padding
+ *      canonical   {key, f32 w, u32 0, f32 v[K], 0...} 16 + 4K           {key, f32 w, u32 0, f16 v[K], 0...} 16 + 2K
+ *                  rounded up to 32                                      rounded up to 32: K = 4 -> 32, 8 -> 32,
+ *                                                                        16 -> 64, 32 -> 96, 64 -> 160, 128 -> 288
+ *    In an F16 canonical row a token's piece c of v (v[4c .. 4c+3]) is one aligned 8-byte load at byte 16 + 8c.  Every
+ *    xf_model_predict_* on an F16 model returns, bit for bit, what it returns on the F32 model whose latent fields are
+ *    replaced by their binary16 values: the kernels widen each field after the load and then run the F32 model's
+ *    arithmetic in its order.  Absent keys under XF_ABSENT_DEFAULT read as before, evaluated in float32 on the fly:
+ *    only stored rows are narrowed.  xf_model_lookup (st, qt) and xf_model_lookup_latent (v) return the widened
+ *    binary16 values.  The files, deltas and merges of F16 models work as for F32 ones; two models of different
+ *    precisions cannot be diffed, applied or merged.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct xf_model xf_model;
 enum { XF_ABSENT_DEFAULT = 0, XF_ABSENT_ZERO = 1 };
+enum { XF_PRECISION_F32 = 0, XF_PRECISION_F16 = 1 };  /* of a model's latent fields (above) */
 typedef struct xf_freeze_config {
   int absent;            /* XF_ABSENT_*, or -1 = what the table's own predict does: DEFAULT if its admission policy is
                             XF_ADMIT_ALL, else ZERO */
@@ -601,10 +620,18 @@ XF_DLL int xf_table_freeze_part(xf_table* t, const xf_freeze_config* cfg, xf_mod
 /* the shard a part holds; XF_ERR_STATE for a whole model */
 XF_DLL int xf_model_part_info(xf_model* m, int* shard_index, int* num_shards);
 /* The whole model of parts[0 .. n) on `device` (-1: parts[0]'s).  The parts must be shards 0 .. n-1 of one n-way
- * split, each once, and agree on fm, latent_dim, optimizer, absent, the resolved v_init, v_const and seed (prune may
- * differ): else XF_ERR_ARG, naming what is wrong.  XF_ERR_FULL past 2^32 slots or on a probe overflow.  No part
+ * split, each once, and agree on fm, latent_dim, precision, optimizer, absent, the resolved v_init, v_const and seed
+ * (prune may differ): else XF_ERR_ARG, naming what is wrong.  XF_ERR_FULL past 2^32 slots or on a probe overflow.  No part
  * changes; on failure *out is NULL. */
 XF_DLL int xf_model_merge(xf_model* const* parts, int n, int device, xf_model** out);
+/* A new model on m's device, m with its latent fields at `precision` (XF_PRECISION_*); m is unchanged.  F32 -> F16
+ * rounds each latent field to nearest even, F16 -> F32 widens it exactly, and converting to m's own precision copies
+ * m.  The result holds exactly m's keys (conversion never prunes), and its keys, source_keys, pruned_keys, absent,
+ * optimizer, v_init and seed are m's; a part converts to a part of the same shard.  Runs on a stream of its own and
+ * reads m only.  Refused, with *out NULL and m unchanged: XF_ERR_ARG for an LR model or an unknown precision;
+ * XF_ERR_STATE if a field is finite in float32 and not in binary16 (|x| >= 65520), naming how many such fields there
+ * are and the smallest key that holds one (conversion never saturates).  A NaN field stays NaN. */
+XF_DLL int xf_model_convert(xf_model* m, int precision, xf_model** out);
 XF_DLL int xf_model_destroy(xf_model* m);
 typedef struct xf_model_info {
   uint64_t keys;         /* keys the model holds */
@@ -612,14 +639,18 @@ typedef struct xf_model_info {
   uint64_t bytes;        /* capacity x row_bytes: the model's device memory */
   uint64_t source_keys;  /* keys of the table when it was frozen */
   uint64_t pruned_keys;  /* source_keys - keys */
-  uint32_t row_bytes;    /* 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical) */
+  uint32_t row_bytes;    /* F32: 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical); F16: 16 (FM), 16 + 2K
+                            rounded up to 32 (canonical) */
   int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM */
+  int precision;         /* XF_PRECISION_* of the latent fields */
 } xf_model_info;
 XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
 /* Model file "XFSM" (little-endian): a 104-byte header
  *     0 "XFSM"   4 u32 version (1)   8 u64 header bytes (104)   16 u64 keys   24 u64 capacity   32 u32 row bytes
  *    36 i32 fm (0 LR, 1 FM, 2 canonical)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
- *    52 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   56 f32 the constant   60 u32 0   64 u64 seed   72 u64 source keys   80 u64 pruned keys
+ *    52 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   56 f32 the constant
+ *    60 u32 precision (0 F32, 1 F16; the word was reserved as 0, so every F32 file is unchanged)   64 u64 seed
+ *    72 u64 source keys   80 u64 pruned keys
  *    88 u64 rows per chunk (64 MiB / row bytes)   96 u64 checksum of bytes [0, 96)
  *  then the rows SORTED BY KEY in ceil(keys / rows per chunk) chunks, each {u64 index of its first row, u64 rows,
  *  u64 checksum, u64 0} followed by its rows.  Checksums are those of the state image above (sum of
@@ -628,7 +659,9 @@ XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
  *  bytes.  Written to <path>.tmp and renamed; the staging is bounded by the chunk size.  xf_model_load rebuilds the
  *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL, and so is
  *  a file whose checksums pass but whose keys do not ascend strictly below 2^64 - 1 or whose rows have a non-zero
- *  padding byte (LR bytes 12 .. 15, FM 20 .. 31, canonical 12 .. 15 and 16 + 4K .. row bytes).
+ *  padding byte (LR bytes 12 .. 15, FM 20 .. 31 at F32 and none at F16, canonical 12 .. 15 and 16 + 4K .. row bytes at
+ *  F32 or 16 + 2K .. row bytes at F16), and a header whose precision is not 0 or 1 or whose row bytes are not those of
+ *  its fm, latent_dim and precision (an F16 LR model included).
  * Part file "XFSP" (xf_model_save of a part): XFSM's layout with a 112-byte header
  *     0 "XFSP"   4 u32 version (1)   8 u64 header bytes (112)   16 .. 95 as XFSM's (the part's keys, capacity,
  *    source and pruned keys; fm 0 or 1)   96 i32 shard_index   100 i32 num_shards   104 u64 checksum of bytes [0, 104)
@@ -690,8 +723,9 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
  *    delta applied to the wrong model never makes a wrong model, and checks the result's after building it.
  *
  *    Compatibility.  A and B must agree on what defines how an absent key reads: fm, latent_dim, optimizer, absent,
- *    the resolved v_init, v_const and seed (else XF_ERR_ARG, naming the field).  Prune may differ: a delta compares
- *    contents only.
+ *    the resolved v_init, v_const and seed, and on their rows' precision (else XF_ERR_ARG, naming the field).  Prune
+ *    may differ: a delta compares contents only.  A delta between F16 models carries F16 rows and records the
+ *    precision; convert both models first to carry an F32 chain to F16.
  *
  *    A delta lives on a device: that of the models it was diffed from, or the one xf_delta_load names.  Diff and
  *    apply run on streams of their own and read their models only: neither changes a model, and apply does not use
@@ -708,8 +742,9 @@ typedef struct xf_delta_info {
   uint64_t result_keys, result_fingerprint;
   uint64_t source_keys, pruned_keys;  /* the result's, as xf_model_info has them */
   uint64_t file_bytes;          /* the size of the file xf_delta_save writes */
-  uint32_t row_bytes;           /* 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical) */
+  uint32_t row_bytes;           /* as xf_model_info has them */
   int latent_dim;
+  int precision;                /* XF_PRECISION_* of the models it carries */
 } xf_delta_info;
 /* The delta from `base` to `next` (same device, compatible); neither model changes. */
 XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out);
@@ -721,7 +756,7 @@ XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out);
 /* Delta file "XFSD" (little-endian): a 144-byte header
  *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's)   20 i32 latent_dim
  *    24 i32 optimizer   28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes
- *    52 u32 0
+ *    52 u32 precision (as XFSM's; reserved as 0 before, so every F32 file is unchanged)
  *    56 u64 base keys   64 u64 base fingerprint   72 u64 result keys   80 u64 result source keys
  *    88 u64 result pruned keys   96 u64 result fingerprint   104 u64 upserts U   112 u64 deletes D
  *   120 u64 rows per chunk (64 MiB / row bytes)   128 u64 keys per delete chunk (64 MiB / 8)

@@ -16,6 +16,7 @@ OPT_FTRL, OPT_SGD = 0, 1
 VINIT_DEFAULT, VINIT_COUNTER, VINIT_ZERO = 0, 1, 3
 ADMIT_ALL, ADMIT_POISSON, ADMIT_BLOOM = 0, 1, 2
 ABSENT_DEFAULT, ABSENT_ZERO = 0, 1
+PRECISION_F32, PRECISION_F16 = 0, 1
 COMM_ID_BYTES = 128
 
 _lib = None
@@ -48,14 +49,14 @@ class FreezeConfig(C.Structure):
 class ModelInfo(C.Structure):
     _fields_ = [("keys", C.c_uint64), ("capacity", C.c_uint64), ("bytes", C.c_uint64), ("source_keys", C.c_uint64),
                 ("pruned_keys", C.c_uint64), ("row_bytes", C.c_uint32), ("latent_dim", C.c_int), ("optimizer", C.c_int),
-                ("absent", C.c_int), ("fm", C.c_int)]
+                ("absent", C.c_int), ("fm", C.c_int), ("precision", C.c_int)]
 
 
 class DeltaInfo(C.Structure):
     _fields_ = [("upserts", C.c_uint64), ("deletes", C.c_uint64), ("base_keys", C.c_uint64),
                 ("base_fingerprint", C.c_uint64), ("result_keys", C.c_uint64), ("result_fingerprint", C.c_uint64),
                 ("source_keys", C.c_uint64), ("pruned_keys", C.c_uint64), ("file_bytes", C.c_uint64),
-                ("row_bytes", C.c_uint32), ("latent_dim", C.c_int)]
+                ("row_bytes", C.c_uint32), ("latent_dim", C.c_int), ("precision", C.c_int)]
 
 
 class TrainerConfig(C.Structure):
@@ -160,6 +161,7 @@ SIGNATURES = {
     "xf_table_freeze_part": (_i, [_vp, _vp, _vp]),
     "xf_model_part_info": (_i, [_vp, _vp, _vp]),
     "xf_model_merge": (_i, [_vp, _i, _i, _vp]),
+    "xf_model_convert": (_i, [_vp, _i, _vp]),
     "xf_model_destroy": (_i, [_vp]),
     "xf_model_get_info": (_i, [_vp, _vp]),
     "xf_model_save": (_i, [_vp, C.c_char_p]),
@@ -489,6 +491,13 @@ class Model:
         h = C.c_void_p()
         _check(lib().xf_model_merge(arr, len(parts), device, C.byref(h)))
         return cls(h)
+
+    def convert(self, precision):
+        """A new Model (or part): this one with its latent fields at `precision`, PRECISION_F32 or PRECISION_F16
+        (xf_model_convert); this one is not changed."""
+        h = C.c_void_p()
+        _check(lib().xf_model_convert(self.h, precision, C.byref(h)))
+        return Model(h)
 
     def part_info(self):
         """(shard_index, num_shards) of a part; XflowError for a whole model."""

@@ -38,7 +38,7 @@ struct XfDeltaHeader {
   float v_const;                // 36
   uint64_t seed;                // 40
   uint32_t row_bytes;           // 48
-  uint32_t zero;                // 52
+  uint32_t precision;           // 52 XF_PRECISION_* (reserved as 0 before F16 models)
   uint64_t base_keys;           // 56
   uint64_t base_fingerprint;    // 64
   uint64_t result_keys;         // 72
@@ -67,7 +67,7 @@ struct xf_delta {
 
 // the delta's side of the compatibility check (serve.cuh: XfCompat)
 static XfCompat xf_compat_of(const XfDeltaHeader& h) {
-  return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed};
+  return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed, (int)h.precision};
 }
 
 static uint64_t xf_sd_file_bytes(const XfDeltaHeader& h) {
@@ -232,7 +232,7 @@ static int xf_diff_into(xf_model* base, xf_model* next, xf_delta* d) {
   XfDeltaHeader& h = d->h;
   const XfCompat c = xf_compat_of(next);
   h.fm = c.fm; h.latent_dim = c.latent_dim; h.optimizer = c.optimizer; h.absent = c.absent; h.v_init = c.v_init;
-  h.v_const = c.v_const; h.seed = c.seed;
+  h.v_const = c.v_const; h.seed = c.seed; h.precision = (uint32_t)c.precision;
   h.row_bytes = next->view.stride;
   h.base_keys = base->keys;
   h.result_keys = next->keys;
@@ -392,6 +392,7 @@ XF_DLL int xf_delta_get_info(xf_delta* d, xf_delta_info* out) {
   out->file_bytes = xf_sd_file_bytes(h);
   out->row_bytes = h.row_bytes;
   out->latent_dim = h.latent_dim;
+  out->precision = (int)h.precision;
   return XF_OK;
 }
 
@@ -406,7 +407,6 @@ static int xf_sd_save_body(xf_delta* d, FILE* f, const char* name) {
   memcpy(h.magic, "XFSD", 4);
   h.version = XF_SD_VERSION;
   h.header_bytes = sizeof(h);
-  h.zero = 0;
   h.header_checksum = xf_st_host_sum(&h, offsetof(XfDeltaHeader, header_checksum), 0);
   if (fwrite(&h, 1, sizeof(h), f) != sizeof(h)) { xf_set_error("write to %s failed", name); return XF_ERR_IO; }
   uint64_t chunk = 0;
@@ -431,7 +431,7 @@ XF_DLL int xf_delta_save(xf_delta* d, const char* path) {
 
 // the header's own consistency (after its checksum): every size derived from it is bounded before it is used
 static bool xf_sd_header_sane(const XfDeltaHeader& h) {
-  if (!xf_compat_sane(xf_compat_of(h), h.row_bytes) || h.zero != 0) return false;
+  if (!xf_compat_sane(xf_compat_of(h), h.row_bytes)) return false;
   if (h.chunk_rows != XF_ST_CHUNK_BYTES / h.row_bytes || h.chunk_keys != XF_ST_CHUNK_BYTES / 8) return false;
   // a model holds at most 2^31 keys; a result past that is refused by apply (XF_ERR_FULL), not by the file
   if (h.base_keys > (1ull << 31) || h.result_keys > (1ull << 62) || h.source_keys < h.result_keys ||
@@ -455,9 +455,9 @@ static int xf_sd_load_body(xf_delta* d, FILE* f, const char* path, const XfDelta
   };
   uint64_t chunk = 0;
   XF_TRY(xf_chunks_load(f, path, h.upserts, h.row_bytes, h.chunk_rows, &chunk,
-                        XfChunkCheck{"delta file", "upsert", h.fm, h.latent_dim, 0, 0}, d->stage, d->stream,
+                        XfChunkCheck{"delta file", "upsert", h.fm, h.latent_dim, (int)h.precision, 0, 0}, d->stage, d->stream,
                         into(d->rows, h.row_bytes)));
-  XF_TRY(xf_chunks_load(f, path, h.deletes, 8u, h.chunk_keys, &chunk, XfChunkCheck{"delta file", "delete", -1, 0, 0, 0},
+  XF_TRY(xf_chunks_load(f, path, h.deletes, 8u, h.chunk_keys, &chunk, XfChunkCheck{"delta file", "delete", -1, 0, 0, 0, 0},
                         d->stage, d->stream, into(d->dels, 8u)));
   if (h.upserts && h.deletes) {
     XfDevBuf flag;

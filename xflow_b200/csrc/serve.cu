@@ -31,6 +31,12 @@
 //                                    reductions and its FMA contraction, spelled out (xf_fmc_add, xf_fmc_arg); the C
 //                                    lanes of a token load the head and their 16-byte piece of the home slot at once;
 //                                    two passes in flight
+//
+// An F16 model (xf_model_convert) holds its latent fields in binary16: FM {key, w, st, qt} in 16 bytes, canonical
+// {key, w, 0, v[K]} with 2-byte v.  Its predict and lookup kernels are the F32 ones' H = true instantiations, which widen
+// each field right after the load and then run the F32 arithmetic unchanged.
+//   convert  xf_k_model_convert<FMC, TO_HALF>  a grid-stride walk over the source's slots as xf_k_merge's; each live row
+//                                              converted and put into the result with xf_model_claim
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
@@ -60,7 +66,7 @@ struct XfModelHeader {
   int32_t absent;          //  48
   int32_t v_init;          //  52 resolved
   float v_const;           //  56
-  uint32_t zero;           //  60
+  uint32_t precision;      //  60 XF_PRECISION_* (reserved as 0 before F16 models)
   uint64_t seed;           //  64
   uint64_t source_keys;    //  72
   uint64_t pruned_keys;    //  80
@@ -82,10 +88,10 @@ static_assert(sizeof(XfPartHeader) == 112 && offsetof(XfPartHeader, header_check
               "the documented part header is 112 bytes");
 
 // one token's terms into the lane's sums, in the order the step kernels add them
-template <bool FM>
+template <bool FM, bool H>
 __device__ __forceinline__ void xf_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float w, float st,
                                                float qt, float& wsum, float& ssum, float& qsum) {
-  if (!xf_serve_find<FM>(m, key, k, w, st, qt)) {
+  if (!xf_serve_find<FM, H>(m, key, k, w, st, qt)) {
     if (absent == XF_ABSENT_ZERO) return;
     // the row the table would insert: w = 0 and, FM, a latent block that is not materialised
     w = 0.f;
@@ -95,7 +101,7 @@ __device__ __forceinline__ void xf_serve_token(const XfTableView& m, int absent,
   if (FM) { ssum += st; qsum += qt; }
 }
 
-template <bool FM>
+template <bool FM, bool H>
 __global__ void __launch_bounds__(256)
 xf_k_serve(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys, int B,
            float* __restrict__ pctr_out) {
@@ -117,10 +123,10 @@ xf_k_serve(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, cons
       // both first looks are in flight before either is resolved
       uint64_t a = XF_EMPTY_KEY, b = XF_EMPTY_KEY;
       float wa = 0.f, sa = 0.f, qa = 0.f, wb = 0.f, sb = 0.f, qb = 0.f;
-      if (v0) xf_serve_load<FM>(xf_row(m, xf_home_slot(m, k0)), a, wa, sa, qa);
-      if (v1) xf_serve_load<FM>(xf_row(m, xf_home_slot(m, k1)), b, wb, sb, qb);
-      if (v0) xf_serve_token<FM>(m, absent, k0, a, wa, sa, qa, wsum, ssum, qsum);
-      if (v1) xf_serve_token<FM>(m, absent, k1, b, wb, sb, qb, wsum, ssum, qsum);
+      if (v0) xf_serve_load<FM, H>(xf_row(m, xf_home_slot(m, k0)), a, wa, sa, qa);
+      if (v1) xf_serve_load<FM, H>(xf_row(m, xf_home_slot(m, k1)), b, wb, sb, qb);
+      if (v0) xf_serve_token<FM, H>(m, absent, k0, a, wa, sa, qa, wsum, ssum, qsum);
+      if (v1) xf_serve_token<FM, H>(m, absent, k1, b, wb, sb, qb, wsum, ssum, qsum);
     }
     const float wx = xf_warp_sum(wsum);
     float arg = wx;
@@ -135,12 +141,22 @@ xf_k_serve(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, cons
 
 // ---- canonical rows {key, w, 0, v[K]}: the forward of xf_k_step_fmc (mode 1) on the model's rows
 // A token's head {key, w} and lane c's latent piece v[4c .. 4c+3] of the row at p, as two non-coherent loads issued
-// back to back (the C lanes of a token load the same head: one request)
+// back to back (the C lanes of a token load the same head: one request).  H: the piece is four binary16 values, one
+// 8-byte load at 16 + 8c, widened after it.
+template <bool H>
 __device__ __forceinline__ void xf_fmc_load(const uint8_t* p, int c, uint64_t& key, float& w, float4& v) {
   uint64_t q0, q1;
-  asm("ld.global.nc.v2.u64 {%0,%1}, [%6];\n\tld.global.nc.v4.f32 {%2,%3,%4,%5}, [%7];"
-      : "=l"(q0), "=l"(q1), "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-      : "l"(p), "l"(p + 16 + 16 * c));
+  if (H) {
+    uint32_t h0, h1;
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u32 {%2,%3}, [%5];"
+        : "=l"(q0), "=l"(q1), "=r"(h0), "=r"(h1)
+        : "l"(p), "l"(p + 16 + 8 * c));
+    v = make_float4(xf_h2f(h0), xf_h2f(h0 >> 16), xf_h2f(h1), xf_h2f(h1 >> 16));
+  } else {
+    asm("ld.global.nc.v2.u64 {%0,%1}, [%6];\n\tld.global.nc.v4.f32 {%2,%3,%4,%5}, [%7];"
+        : "=l"(q0), "=l"(q1), "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+        : "l"(p), "l"(p + 16 + 16 * c));
+  }
   key = q0;
   w = __uint_as_float((uint32_t)q1);
 }
@@ -174,13 +190,14 @@ __device__ __forceinline__ float xf_fmc_arg(float (&S)[4], float Q, float wx) {
 }
 
 // one token into the lane's sums: its row found from the home slot the caller loaded (k, w, v), or the absent policy
+template <bool H>
 __device__ __forceinline__ void xf_fmc_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float w,
                                                    float4 v, float x, int c, float (&S)[4], float& Q, float& wx) {
   bool have = false;
   for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
     if (k == key) { have = true; break; }
     if (k == XF_EMPTY_KEY) break;
-    xf_fmc_load(xf_row(m, xf_probe_slot(m, key, i)), c, k, w, v);
+    xf_fmc_load<H>(xf_row(m, xf_probe_slot(m, key, i)), c, k, w, v);
   }
   if (!have) {
     if (absent == XF_ABSENT_ZERO) return;
@@ -195,7 +212,7 @@ __device__ __forceinline__ void xf_fmc_serve_token(const XfTableView& m, int abs
 // One warp per row, C = K/4 lanes per token and T = 32/C tokens per pass, as xf_k_step_fmc; two passes in flight.  A
 // lane adds its tokens in the order of the step kernel's passes, with its arithmetic (xf_fmc_add, xf_fmc_arg), so the
 // result is the table's bit for bit.  No insert, no atomics, no shared memory.
-template <int C>
+template <int C, bool H>
 __global__ void __launch_bounds__(256)
 xf_k_serve_fmc(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
                const float* __restrict__ vals, int B, float* __restrict__ pctr_out) {
@@ -223,13 +240,26 @@ xf_k_serve_fmc(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, 
       uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
       float wa = 0.f, wb = 0.f;
       float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
-      if (va) xf_fmc_load(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
-      if (vb) xf_fmc_load(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
-      if (va) xf_fmc_serve_token(m, absent, ka, ra, wa, pa, xa, c, S, Q, wx);
-      if (vb) xf_fmc_serve_token(m, absent, kb, rb, wb, pb, xb, c, S, Q, wx);
+      if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+      if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+      if (va) xf_fmc_serve_token<H>(m, absent, ka, ra, wa, pa, xa, c, S, Q, wx);
+      if (vb) xf_fmc_serve_token<H>(m, absent, kb, rb, wb, pb, xb, c, S, Q, wx);
     }
     const float arg = xf_fmc_arg<C>(S, Q, wx);
     if (lane == 0) pctr_out[row] = xf_sigmoid(arg);
+  }
+}
+
+template <bool H>
+static void xf_launch_serve_fmc(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
+                                uint32_t rows, float* pctr_out, int grid, cudaStream_t st) {
+  switch (m->view.K) {
+    case 4: xf_k_serve_fmc<1, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    case 8: xf_k_serve_fmc<2, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    case 16: xf_k_serve_fmc<4, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    case 32: xf_k_serve_fmc<8, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    case 64: xf_k_serve_fmc<16, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+    default: xf_k_serve_fmc<32, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
   }
 }
 
@@ -237,19 +267,15 @@ static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const ui
                             float* pctr_out, cudaStream_t st) {
   if (rows == 0) return;
   const int grid = xf_grid_for((uint64_t)rows * 32, 256, 8);
+  const bool half = m->precision == XF_PRECISION_F16;
   if (m->fm == XF_SERVE_FMC) {
-    switch (m->view.K) {
-      case 4: xf_k_serve_fmc<1><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-      case 8: xf_k_serve_fmc<2><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-      case 16: xf_k_serve_fmc<4><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-      case 32: xf_k_serve_fmc<8><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-      case 64: xf_k_serve_fmc<16><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-      default: xf_k_serve_fmc<32><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
-    }
+    if (half) xf_launch_serve_fmc<true>(m, row_ptr, keys, vals, rows, pctr_out, grid, st);
+    else xf_launch_serve_fmc<false>(m, row_ptr, keys, vals, rows, pctr_out, grid, st);
     return;
   }
-  if (m->fm) xf_k_serve<true><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
-  else xf_k_serve<false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
+  if (m->fm && half) xf_k_serve<true, true><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
+  else if (m->fm) xf_k_serve<true, false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
+  else xf_k_serve<false, false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
 }
 
 // ---- building a model's table
@@ -352,16 +378,18 @@ xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned lo
   }
 }
 
-// what a canonical model holds for keys[0 .. n): w, v[n][K] (either may be nullptr), present
+// what a canonical model holds for keys[0 .. n): w, v[n][K] (either may be nullptr; H: v widened from binary16), present
+template <bool H>
 __global__ void xf_k_model_lookup_fmc(XfTableView m, const uint64_t* __restrict__ keys, uint64_t n, float* w_out, float* v_out,
                                       uint8_t* present) {
   const int K = m.K;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const int64_t s = xf_model_find_slot(m, keys[i]);
-    const float* p = s >= 0 ? reinterpret_cast<const float*>(xf_row(m, (uint64_t)s)) : nullptr;
-    if (w_out) w_out[i] = p ? p[2] : 0.f;
+    const uint8_t* p = s >= 0 ? xf_row(m, (uint64_t)s) : nullptr;
+    if (w_out) w_out[i] = p ? reinterpret_cast<const float*>(p)[2] : 0.f;
     if (v_out)
-      for (int k = 0; k < K; ++k) v_out[i * K + k] = p ? p[4 + k] : 0.f;
+      for (int k = 0; k < K; ++k)
+        v_out[i * K + k] = !p ? 0.f : H ? xf_h2f(reinterpret_cast<const uint16_t*>(p + 16)[k]) : reinterpret_cast<const float*>(p + 16)[k];
     present[i] = p ? 1 : 0;
   }
 }
@@ -386,6 +414,69 @@ xf_k_merge(const uint8_t* __restrict__ slots, uint64_t n, XfTableView m, int* er
   }
 }
 
+// A latent field at the result's precision: binary16 bits rounded to nearest even (TO_HALF), or the float32 value of
+// binary16 bits.  *over counts a field finite in float32 and not in binary16 (|x| >= 65520); NaN stays NaN.
+__device__ __forceinline__ uint32_t xf_to_half(float x, uint32_t& over) {
+  const __half h = __float2half_rn(x);
+  over += (isfinite(x) && __hisinf(h)) ? 1u : 0u;
+  return (uint32_t)__half_as_ushort(h);
+}
+
+// convert: the live rows of a model's slots into `m`, its latent fields converted (TO_HALF: F32 -> F16, else F16 ->
+// F32); w and the key are copied, the result's padding stays as the fill left it, zero.  An FM row is built in registers
+// before the claim.  A canonical row (up to 544 bytes) is converted a piece v[4q .. 4q+3] at a time after the claim, as
+// xf_model_put_row copies the rest of a row.  overflow[0] += the fields that do not fit binary16, overflow[1] = the
+// smallest key that holds one.
+template <bool FMC, bool TO_HALF>
+__global__ void __launch_bounds__(256)
+xf_k_model_convert(XfTableView src, XfTableView m, unsigned long long* overflow, int* error) {
+  const uint64_t cap = src.mask + 1;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < cap; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint8_t* p = xf_row(src, r);
+    const ulonglong2 head = __ldg(reinterpret_cast<const ulonglong2*>(p));
+    if (head.x == XF_EMPTY_KEY) continue;
+    uint32_t over = 0;
+    if (!FMC) {
+      // F32 {key, w, st | qt, 0...}: head.y = w | st << 32, qt at 16; F16 {key, w | st << 32 | qt << 48}
+      uint64_t body;
+      float qt = 0.f;
+      if (TO_HALF) {
+        const float st = __uint_as_float((uint32_t)(head.y >> 32));
+        qt = __ldg(reinterpret_cast<const float*>(p + 16));
+        body = (head.y & 0xFFFFFFFFull) | (uint64_t)xf_to_half(st, over) << 32 | (uint64_t)xf_to_half(qt, over) << 48;
+      } else {
+        body = (head.y & 0xFFFFFFFFull) | (uint64_t)__float_as_uint(xf_h2f((uint32_t)(head.y >> 32))) << 32;
+        qt = xf_h2f((uint32_t)(head.y >> 48));
+      }
+      uint8_t* dst = xf_model_claim(m, head.x, error);
+      if (dst) {
+        *reinterpret_cast<unsigned long long*>(dst + 8) = body;
+        if (!TO_HALF) *reinterpret_cast<float*>(dst + 16) = qt;
+      }
+    } else {
+      uint8_t* dst = xf_model_claim(m, head.x, error);
+      if (dst) {
+        *reinterpret_cast<unsigned long long*>(dst + 8) = head.y;  // w and the zero word
+        const uint32_t pieces = (uint32_t)src.K >> 2;
+        for (uint32_t q = 0; q < pieces; ++q) {
+          if (TO_HALF) {
+            const float4 v = __ldg(reinterpret_cast<const float4*>(p + 16) + q);
+            reinterpret_cast<uint2*>(dst + 16)[q] = make_uint2(xf_to_half(v.x, over) | xf_to_half(v.y, over) << 16,
+                                                               xf_to_half(v.z, over) | xf_to_half(v.w, over) << 16);
+          } else {
+            const uint2 h = __ldg(reinterpret_cast<const uint2*>(p + 16) + q);
+            reinterpret_cast<float4*>(dst + 16)[q] = make_float4(xf_h2f(h.x), xf_h2f(h.x >> 16), xf_h2f(h.y), xf_h2f(h.y >> 16));
+          }
+        }
+      }
+    }
+    if (TO_HALF && over) {
+      atomicAdd(overflow, (unsigned long long)over);
+      atomicMin(overflow + 1, (unsigned long long)head.x);
+    }
+  }
+}
+
 // every (key, slot) the model holds, in no particular order
 __global__ void xf_k_model_list(XfTableView m, uint64_t* keys_out, uint32_t* slots_out, unsigned long long* count) {
   const uint64_t cap = m.mask + 1;
@@ -407,6 +498,7 @@ __global__ void xf_k_model_gather(XfTableView m, const uint32_t* __restrict__ sl
   }
 }
 
+template <bool H>
 __global__ void xf_k_model_lookup(XfTableView m, const uint64_t* __restrict__ keys, uint64_t n, float* w_out, float* st_out,
                                   float* qt_out, uint8_t* present) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
@@ -415,8 +507,8 @@ __global__ void xf_k_model_lookup(XfTableView m, const uint64_t* __restrict__ ke
     float w, st, qt;
     bool have;
     if (m.K > 0) {
-      xf_serve_load<true>(xf_row(m, xf_home_slot(m, key)), k, w, st, qt);
-      have = xf_serve_find<true>(m, key, k, w, st, qt);
+      xf_serve_load<true, H>(xf_row(m, xf_home_slot(m, key)), k, w, st, qt);
+      have = xf_serve_find<true, H>(m, key, k, w, st, qt);
     } else {
       xf_serve_load<false>(xf_row(m, xf_home_slot(m, key)), k, w, st, qt);
       have = xf_serve_find<false>(m, key, k, w, st, qt);
@@ -438,7 +530,7 @@ int xf_model_alloc(xf_model* m, uint64_t capacity) {
     xf_set_error("a serving model of %llu slots exceeds 2^32", (unsigned long long)capacity);
     return XF_ERR_FULL;
   }
-  const uint32_t stride = xf_model_row_bytes(m->fm, m->view.K);
+  const uint32_t stride = xf_model_row_bytes(m->fm, m->view.K, m->precision);
   m->view.canon = m->fm == XF_SERVE_FMC ? 1 : 0;
   uint8_t* base = nullptr;
   XF_CUDA_TRY(cudaMalloc(&base, capacity * stride));
@@ -460,6 +552,7 @@ int xf_model_init(xf_model* m, int device, const XfCompat& c) {
   XF_CUDA_TRY(cudaSetDevice(device));
   XF_CUDA_TRY(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   m->fm = c.fm;
+  m->precision = c.precision;
   m->absent = c.absent;
   m->optimizer = c.optimizer;
   m->view.K = c.latent_dim;
@@ -542,7 +635,8 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   const XfTableView& tv = t->view;
   const int fm = canonical ? XF_SERVE_FMC : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
   const int absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
-  XF_TRY(xf_model_init(m, src_dev, XfCompat{fm, tv.K, tv.opt, absent, tv.v_init, tv.v_const, tv.seed}));
+  XF_TRY(xf_model_init(m, src_dev, XfCompat{fm, tv.K, tv.opt, absent, tv.v_init, tv.v_const, tv.seed,
+                                                   XF_PRECISION_F32}));
   // the build runs on the model's stream: the table's stream is idle (above) and the host calls on the table are
   // locked out by the caller, so nothing writes the table while it is read
   cudaStream_t st = m->stream;
@@ -690,6 +784,7 @@ XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out) {
   out->optimizer = m->optimizer;
   out->absent = m->absent;
   out->fm = m->fm;
+  out->precision = m->precision;
   return XF_OK;
 }
 
@@ -823,8 +918,12 @@ static int xf_lookup_fmc(xf_model* m, const uint64_t* keys, uint64_t n, float* w
   float* d_w = d_v + n * K;
   uint8_t* d_present = reinterpret_cast<uint8_t*>(d_w + n);
   XF_CUDA_TRY(cudaMemcpyAsync(m->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, m->stream));
-  xf_k_model_lookup_fmc<<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w,
-                                                                      v ? d_v : nullptr, d_present);
+  if (m->precision == XF_PRECISION_F16)
+    xf_k_model_lookup_fmc<true><<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w,
+                                                                              v ? d_v : nullptr, d_present);
+  else
+    xf_k_model_lookup_fmc<false><<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w,
+                                                                               v ? d_v : nullptr, d_present);
   XF_CUDA_TRY(cudaGetLastError());
   if (w) XF_CUDA_TRY(cudaMemcpyAsync(w, d_w, n * 4, cudaMemcpyDeviceToHost, m->stream));
   if (v) XF_CUDA_TRY(cudaMemcpyAsync(v, d_v, n * K * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -863,8 +962,12 @@ XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float*
   float* d_w = m->s_aux.as<float>();
   uint8_t* d_present = reinterpret_cast<uint8_t*>(d_w + 3 * n);
   XF_CUDA_TRY(cudaMemcpyAsync(m->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, m->stream));
-  xf_k_model_lookup<<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w, d_w + n, d_w + 2 * n,
-                                                                  d_present);
+  if (m->precision == XF_PRECISION_F16)
+    xf_k_model_lookup<true><<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w, d_w + n,
+                                                                          d_w + 2 * n, d_present);
+  else
+    xf_k_model_lookup<false><<<xf_grid_for(n, 256, 8), 256, 0, m->stream>>>(m->view, m->s_keys.as<uint64_t>(), n, d_w, d_w + n,
+                                                                           d_w + 2 * n, d_present);
   XF_CUDA_TRY(cudaGetLastError());
   if (w) XF_CUDA_TRY(cudaMemcpyAsync(w, d_w, n * 4, cudaMemcpyDeviceToHost, m->stream));
   if (st) XF_CUDA_TRY(cudaMemcpyAsync(st, d_w + n, n * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -930,7 +1033,7 @@ int xf_chunks_load(FILE* f, const char* path, uint64_t n, uint32_t bytes, uint64
                      check.what, (unsigned long long)r, check.shard_index, check.num_shards);
         return XF_ERR_IO;
       }
-      if (check.fm >= 0 && !xf_model_padding_zero(p, check.fm, check.K, bytes)) {
+      if (check.fm >= 0 && !xf_model_padding_zero(p, check.fm, check.K, check.precision, bytes)) {
         xf_set_error("%s %s: %s %llu has non-zero padding", check.file, path, check.what, (unsigned long long)r);
         return XF_ERR_IO;
       }
@@ -953,11 +1056,13 @@ int xf_file_size_check(FILE* f, const char* path, const char* file, uint64_t exp
 }
 
 bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
+  if (c.precision != XF_PRECISION_F32 && c.precision != XF_PRECISION_F16) return false;
   if (c.fm == XF_SERVE_FMC) {
-    if (!xf_fmc_latent_ok(c.latent_dim) || row_bytes != xf_model_row_bytes(c.fm, c.latent_dim)) return false;
-  } else if (c.fm != (c.latent_dim > 0 ? 1 : 0) || c.latent_dim < 0 || row_bytes != (c.fm ? 32u : 16u)) {
+    if (!xf_fmc_latent_ok(c.latent_dim)) return false;
+  } else if (c.fm != (c.latent_dim > 0 ? 1 : 0) || c.latent_dim < 0 || (c.fm == XF_SERVE_LR && c.precision != XF_PRECISION_F32)) {
     return false;
   }
+  if (row_bytes != xf_model_row_bytes(c.fm, c.latent_dim, c.precision)) return false;
   if (c.absent != XF_ABSENT_DEFAULT && c.absent != XF_ABSENT_ZERO) return false;
   if (c.optimizer != XF_OPT_FTRL && c.optimizer != XF_OPT_SGD) return false;
   return c.v_init == 0 || c.v_init == XF_INIT_COUNTER || c.v_init == XF_INIT_ZERO;
@@ -965,7 +1070,7 @@ bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
 
 // the model header's side of the compatibility check (serve.cuh: XfCompat)
 static XfCompat xf_compat_of(const XfModelHeader& h) {
-  return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed};
+  return XfCompat{h.fm, h.latent_dim, h.optimizer, h.absent, h.v_init, h.v_const, h.seed, (int)h.precision};
 }
 
 static int xf_sm_save_body(xf_model* m, FILE* f, const char* name) {
@@ -983,6 +1088,7 @@ static int xf_sm_save_body(xf_model* m, FILE* f, const char* name) {
   h.absent = m->absent;
   h.v_init = m->view.v_init;
   h.v_const = m->view.v_const;
+  h.precision = (uint32_t)m->precision;
   h.seed = m->view.seed;
   h.source_keys = m->source_keys;
   h.pruned_keys = m->pruned_keys;
@@ -1031,7 +1137,7 @@ XF_DLL int xf_model_save(xf_model* m, const char* path) {
 static bool xf_sm_header_sane(const XfModelHeader& h) {
   if (!xf_compat_sane(xf_compat_of(h), h.row_bytes)) return false;
   if (h.keys > (1ull << 31) || h.capacity != xf_model_capacity(h.keys) || h.keys + h.pruned_keys != h.source_keys) return false;
-  return h.chunk_rows == XF_ST_CHUNK_BYTES / h.row_bytes && h.zero == 0;
+  return h.chunk_rows == XF_ST_CHUNK_BYTES / h.row_bytes;
 }
 
 // the rows of an XFSM or XFSP file (header of `header_bytes`) into `m` on `device`; m->shard_index, num_shards are set:
@@ -1050,7 +1156,7 @@ static int xf_sm_load_body(xf_model* m, int device, FILE* f, const char* path, c
   XF_TRY(rows.ensure(std::min<uint64_t>(h.chunk_rows, h.keys) * h.row_bytes));
   XF_TRY(err.ensure(4));
   XF_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, m->stream));
-  XfChunkCheck check{"model file", "row", h.fm, h.latent_dim, m->shard_index, m->num_shards};
+  XfChunkCheck check{"model file", "row", h.fm, h.latent_dim, (int)h.precision, m->shard_index, m->num_shards};
   uint64_t chunk = 0;
   XF_TRY(xf_chunks_load(f, path, h.keys, h.row_bytes, h.chunk_rows, &chunk, check, m->h_in, m->stream,
                         [&](uint64_t, uint64_t c, const void* host) -> int {
@@ -1194,5 +1300,76 @@ XF_DLL int xf_model_merge(xf_model* const* parts, int n, int device, xf_model** 
   const int rc = xf_merge_into(parts, n, target, m);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
   *out = m;
+  return XF_OK;
+}
+
+// ---- convert
+// the body of xf_model_convert: on failure the caller frees `out`
+static int xf_convert_into(xf_model* m, int precision, xf_model* out) {
+  XfCompat c = xf_compat_of(m);
+  c.precision = precision;
+  XF_TRY(xf_model_init(out, m->device, c));
+  out->keys = m->keys;
+  out->source_keys = m->source_keys;
+  out->pruned_keys = m->pruned_keys;
+  out->shard_index = m->shard_index;
+  out->num_shards = m->num_shards;
+  cudaStream_t st = out->stream;
+  XF_TRY(xf_model_alloc(out, m->view.mask + 1));
+  if (precision == m->precision) {
+    // a copy: the same rows at the same stride and capacity, so the same slots
+    XF_CUDA_TRY(cudaMemcpyAsync(out->view.base, m->view.base, (m->view.mask + 1) * (uint64_t)m->view.stride,
+                                cudaMemcpyDeviceToDevice, st));
+    XF_CUDA_TRY(cudaStreamSynchronize(st));
+    return XF_OK;
+  }
+  XfDevBuf aux;  // {overflowing fields, their smallest key, probe error}
+  struct Release { XfDevBuf* a; ~Release() { a->release(); } } rel{&aux};
+  XF_TRY(aux.ensure(24));
+  unsigned long long* d_over = aux.as<unsigned long long>();
+  int* d_error = reinterpret_cast<int*>(d_over + 2);
+  XF_CUDA_TRY(cudaMemsetAsync(d_over, 0, 8, st));
+  XF_CUDA_TRY(cudaMemsetAsync(d_over + 1, 0xFF, 8, st));
+  XF_CUDA_TRY(cudaMemsetAsync(d_error, 0, 4, st));
+  const int grid = xf_grid_for(m->view.mask + 1, 256, 8);
+  const bool to_half = precision == XF_PRECISION_F16;
+  if (m->fm == XF_SERVE_FMC) {
+    if (to_half) xf_k_model_convert<true, true><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
+    else xf_k_model_convert<true, false><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
+  } else {
+    if (to_half) xf_k_model_convert<false, true><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
+    else xf_k_model_convert<false, false><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
+  }
+  XF_CUDA_TRY(cudaGetLastError());
+  unsigned long long h[3] = {0, 0, 0};
+  XF_CUDA_TRY(cudaMemcpyAsync(h, d_over, 24, cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  if ((int)h[2] != 0) {
+    xf_set_error("xf_model_convert: a probe sequence of the model overflowed");
+    return XF_ERR_FULL;
+  }
+  if (h[0] != 0) {
+    xf_set_error("xf_model_convert: %llu latent fields are finite in float32 but not in binary16 (|x| >= 65520), the "
+                 "smallest key that holds one is %llu (%016llx): conversion never saturates", h[0], h[1], h[1]);
+    return XF_ERR_STATE;
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_convert(xf_model* m, int precision, xf_model** out) {
+  if (out) *out = nullptr;
+  if (!m || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
+  if (precision != XF_PRECISION_F32 && precision != XF_PRECISION_F16) {
+    xf_set_error("xf_model_convert: precision = %d is not an XF_PRECISION_* value", precision);
+    return XF_ERR_ARG;
+  }
+  if (m->fm == XF_SERVE_LR) {
+    xf_set_error("xf_model_convert: an LR model has no latent fields to narrow (its row is a key and w in 16 bytes)");
+    return XF_ERR_ARG;
+  }
+  xf_model* c = new xf_model;
+  const int rc = xf_convert_into(m, precision, c);
+  if (rc != XF_OK) { xf_model_free(c); return rc; }
+  *out = c;
   return XF_OK;
 }

@@ -2,6 +2,7 @@
 // the model's host structure, the device functions that read and build its rows, the host steps both use and the
 // chunked sections of their files.  The kernels behind the host steps live in serve.cu only.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -18,6 +19,7 @@ struct xf_model {
                            // canon = 1 for canonical rows
   int device = 0;
   int fm = 0, absent = 0, optimizer = 0;  // fm: XF_SERVE_*
+  int precision = XF_PRECISION_F32;       // of the latent fields (FM st, qt; canonical v): XF_PRECISION_*
   int shard_index = 0, num_shards = 0;    // a part (xf_table_freeze_part): shard_index of num_shards >= 1; 0: a whole model
   uint64_t keys = 0, source_keys = 0, pruned_keys = 0;
   cudaStream_t stream = nullptr;
@@ -44,18 +46,21 @@ inline int xf_refuse_part(const xf_model* m, const char* fn) {
 }
 
 // what defines how an absent key reads: the fields two models (a model and a delta, the parts of a merge) must agree on
+// (and on the layout of their rows: precision)
 struct XfCompat {
   int fm, latent_dim, optimizer, absent, v_init;
   float v_const;
   uint64_t seed;
+  int precision;
 };
 inline XfCompat xf_compat_of(const xf_model* m) {
-  return XfCompat{m->fm, m->view.K, m->optimizer, m->absent, m->view.v_init, m->view.v_const, m->view.seed};
+  return XfCompat{m->fm, m->view.K, m->optimizer, m->absent, m->view.v_init, m->view.v_const, m->view.seed, m->precision};
 }
 // the first field that differs, or nullptr
 inline const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
   if (a.fm != b.fm) return "fm";
   if (a.latent_dim != b.latent_dim) return "latent_dim";
+  if (a.precision != b.precision) return "precision";
   if (a.optimizer != b.optimizer) return "optimizer";
   if (a.absent != b.absent) return "absent";
   if (a.v_init != b.v_init) return "v_init";
@@ -64,35 +69,45 @@ inline const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
   return nullptr;
 }
 
-// Bytes of a model row.  LR {key, w, 0}: 16; FM {key, w, st, qt, 0...}: 32; canonical FM {key, w, 0, v[K], 0...}:
+// Bytes of a model row.  F32: LR {key, w, 0}: 16; FM {key, w, st, qt, 0...}: 32; canonical FM {key, w, 0, v[K], 0...}:
 // 16 + 4K rounded up to 32, so that every row starts on a sector and lane c's piece v[4c .. 4c+3] lies at 16 + 16c.
-__host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K) {
-  if (fm == XF_SERVE_FMC) return (16u + 4u * (uint32_t)K + 31u) & ~31u;
-  return fm ? 32u : 16u;
+// F16 (FM and canonical only; w stays float32): FM {key, w, st, qt}: 16, no padding; canonical {key, w, 0, v[K], 0...}:
+// 16 + 2K rounded up to 32, lane c's piece at 16 + 8c.
+__host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K, int precision) {
+  const uint32_t vb = precision == XF_PRECISION_F16 ? 2u : 4u;
+  if (fm == XF_SERVE_FMC) return (16u + vb * (uint32_t)K + 31u) & ~31u;
+  if (fm == XF_SERVE_FM) return precision == XF_PRECISION_F16 ? 16u : 32u;
+  return 16u;
 }
 // the latent dimensions a canonical model serves: C = K / 4 lanes per token, a power of two <= 32
 inline bool xf_fmc_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 128; }
-// A packed row of a model (fm, K, row_bytes) has zero bytes where its layout has padding: LR [12, 16), FM [20, 32),
-// canonical [12, 16) and [16 + 4K, row_bytes).  Every model in memory keeps them zero (the fill writes them, freeze
-// writes fields only, the other passes copy whole rows), so that whole rows compare and hash as their fields do.
-// Checked a word at a time: the 4-byte word after w (LR, canonical) or qt (FM), then 8-byte words to the row's end.
-inline bool xf_model_padding_zero(const uint8_t* p, int fm, int K, uint32_t row_bytes) {
+// A packed row of a model (fm, K, precision, row_bytes) has zero bytes where its layout has padding: LR [12, 16); FM
+// [20, 32) at F32, none at F16; canonical [12, 16) and [16 + 4K, row_bytes) at F32, [16 + 2K, row_bytes) at F16.  Every
+// model in memory keeps them zero (the fill writes them, freeze and convert write fields only, the other passes copy
+// whole rows), so that whole rows compare and hash as their fields do.  Checked a word at a time: the 4-byte word after
+// w (LR, canonical) or qt (FM), then 8-byte words to the row's end.
+inline bool xf_model_padding_zero(const uint8_t* p, int fm, int K, int precision, uint32_t row_bytes) {
+  if (fm == XF_SERVE_FM && precision == XF_PRECISION_F16) return true;
+  const uint32_t vb = precision == XF_PRECISION_F16 ? 2u : 4u;
   uint32_t w4;
   memcpy(&w4, p + (fm == XF_SERVE_FM ? 20 : 12), 4);
   uint64_t any = w4;
-  for (uint32_t b = fm == XF_SERVE_FMC ? 16u + 4u * (uint32_t)K : fm == XF_SERVE_FM ? 24u : 16u; b < row_bytes; b += 8) {
+  for (uint32_t b = fm == XF_SERVE_FMC ? 16u + vb * (uint32_t)K : fm == XF_SERVE_FM ? 24u : 16u; b < row_bytes; b += 8) {
     uint64_t x;
     memcpy(&x, p + b, 8);
     any |= x;
   }
   return any == 0;
 }
+// a binary16 field's bits (the low 16 of x) widened to float32, exactly
+__device__ __forceinline__ float xf_h2f(uint32_t x) { return __half2float(__ushort_as_half((unsigned short)(x & 0xFFFFu))); }
 
 // ---- model rows: read-only for the lifetime of every kernel that looks keys up, hence the non-coherent path
-template <bool FM>
+// H: an F16 FM row {key, w, st, qt} of 16 bytes, one load as for LR, its fields widened after the load
+template <bool FM, bool H = false>
 __device__ __forceinline__ void xf_serve_load(const uint8_t* p, uint64_t& key, float& w, float& st, float& qt) {
   uint64_t q0, q1, q2 = 0ull, q3 = 0ull;
-  if (FM) {
+  if (FM && !H) {
     // one sector as two 128-bit loads by the same lane (sm_90 has no 256-bit load), issued back to back
     asm("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\tld.global.nc.v2.u64 {%2,%3}, [%4+16];"
         : "=l"(q0), "=l"(q1), "=l"(q2), "=l"(q3) : "l"(p));
@@ -101,18 +116,23 @@ __device__ __forceinline__ void xf_serve_load(const uint8_t* p, uint64_t& key, f
   }
   key = q0;
   w = __uint_as_float((uint32_t)q1);
-  st = __uint_as_float((uint32_t)(q1 >> 32));
-  qt = __uint_as_float((uint32_t)q2);
+  if (H) {
+    st = xf_h2f((uint32_t)(q1 >> 32));
+    qt = xf_h2f((uint32_t)(q1 >> 48));
+  } else {
+    st = __uint_as_float((uint32_t)(q1 >> 32));
+    qt = __uint_as_float((uint32_t)q2);
+  }
 }
 
 // Find `key` from its home slot `s`, whose row the caller has loaded into (k, w, st, qt); false: the model does not
 // hold it.  The load is at most 0.5, so a chain ends at an empty slot long before XF_MAX_PROBE.
-template <bool FM>
+template <bool FM, bool H = false>
 __device__ __forceinline__ bool xf_serve_find(const XfTableView& m, uint64_t key, uint64_t k, float& w, float& st, float& qt) {
   for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
     if (k == key) return true;
     if (k == XF_EMPTY_KEY) return false;
-    xf_serve_load<FM>(xf_row(m, xf_probe_slot(m, key, i)), k, w, st, qt);
+    xf_serve_load<FM, H>(xf_row(m, xf_probe_slot(m, key, i)), k, w, st, qt);
   }
   return false;
 }
@@ -169,9 +189,10 @@ inline uint64_t xf_model_capacity(uint64_t keys) {
   return c;
 }
 
-// a new model on `device`, which is made current: its stream, and the fields XfCompat describes
+// a new model on `device`, which is made current: its stream, and the fields XfCompat describes (precision included)
 int xf_model_init(xf_model* m, int device, const XfCompat& c);
-// the model's table on the current device: `capacity` empty rows (stride from m->fm, m->view.K), filled on m->stream;
+// the model's table on the current device: `capacity` empty rows (stride from m->fm, m->view.K, m->precision), filled on
+// m->stream;
 // XF_ERR_FULL past 2^32 slots
 int xf_model_alloc(xf_model* m, uint64_t capacity);
 // waits for the model's stream and frees everything (m may be NULL)
@@ -210,12 +231,12 @@ int xf_chunks_save(FILE* f, const char* name, uint64_t n, uint32_t bytes, uint64
                    cudaStream_t st, const std::function<int(uint64_t first, uint64_t c, const void** dev)>& src);
 // What a section's entries must satisfy besides their checksums: each begins with a key, and the keys ascend strictly,
 // stay below 2^64 - 1 and lie in shard shard_index of num_shards (xf_shard_range; 0 of 0: any key); entries that are
-// rows (fm >= 0: XF_SERVE_*, of latent_dim K) have zero padding (xf_model_padding_zero).  file and what name the file
-// and the entries in the errors.
+// rows (fm >= 0: XF_SERVE_*, of latent_dim K and precision) have zero padding (xf_model_padding_zero).  file and what
+// name the file and the entries in the errors.
 struct XfChunkCheck {
   const char* file;
   const char* what;
-  int fm, K;
+  int fm, K, precision;
   int shard_index, num_shards;
 };
 // Read a section written by xf_chunks_save and check it chunk by chunk (XF_ERR_IO at the first fault), staged through
@@ -225,6 +246,6 @@ int xf_chunks_load(FILE* f, const char* path, uint64_t n, uint32_t bytes, uint64
                    const std::function<int(uint64_t first, uint64_t c, const void* host)>& sink);
 // XF_ERR_IO unless the file is `expect` bytes long, as its header announces; leaves it positioned at `header_bytes`
 int xf_file_size_check(FILE* f, const char* path, const char* file, uint64_t expect, uint64_t header_bytes);
-// the fields a model's and a delta's header share: a row kind with its latent_dim and row_bytes, and a known absent
-// policy, optimizer and v_init
+// the fields a model's and a delta's header share: a row kind with its latent_dim, precision (F16: FM and canonical
+// only) and row_bytes, and a known absent policy, optimizer and v_init
 bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes);

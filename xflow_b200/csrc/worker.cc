@@ -180,6 +180,26 @@ static void CheckResumedPolicies(xf_table* t) {
                              "saved with; a resumed run keeps its policies");
 }
 
+// XFLOW_EXPORT_PRECISION = f32 | f16 (default f32): the precision of the latent fields of every model the run exports
+// (XFLOW_EXPORT_MODEL, XFLOW_EXPORT_DELTAS, XFLOW_EXPORT_SHARDED_MODEL).  With f16 each frozen model or part is
+// converted (xf_model_convert) before it is written or diffed.  An LR model has no latent fields: f16 is refused.
+static int ExportPrecision() {
+  const char* v = getenv("XFLOW_EXPORT_PRECISION");
+  if (!v || !*v || strcmp(v, "f32") == 0) return XF_PRECISION_F32;
+  if (strcmp(v, "f16") == 0) return XF_PRECISION_F16;
+  throw std::runtime_error(std::string("XFLOW_EXPORT_PRECISION = '") + v + "' is not f32 or f16");
+}
+// the frozen model m at the export precision (m itself at f32; else m is destroyed and its conversion returned)
+static xf_model* AtExportPrecision(xf_model* m) {
+  const int precision = ExportPrecision();
+  if (precision == XF_PRECISION_F32) return m;
+  xf_model* c = nullptr;
+  const int rc = xf_model_convert(m, precision, &c);
+  xf_model_destroy(m);
+  must(rc, "xf_model_convert");
+  return c;
+}
+
 // XFLOW_EXPORT_DELTAS = <prefix>: after every epoch the table frozen with the defaults.  The first epoch this process
 // trains writes the whole model, <prefix>-<epochs done>.xfsm; every later epoch writes the delta from the previous
 // epoch's model, <prefix>-<epochs done>.xfsd, and that model is then dropped for the new one.  A server follows the run
@@ -191,6 +211,7 @@ using ModelPtr = std::unique_ptr<xf_model, ModelDeleter>;
 static void ExportEpoch(xf_table* t, const std::string& prefix, uint64_t epochs_done, ModelPtr& prev) {
   xf_model* m = nullptr;
   must(xf_table_freeze(t, nullptr, &m), "xf_table_freeze");
+  m = AtExportPrecision(m);
   ModelPtr next(m);
   const std::string path = prefix + "-" + std::to_string(epochs_done);
   if (!prev) {
@@ -216,6 +237,7 @@ static std::string PartPath(const std::string& path, int rank, int world) {
 static void ExportShardedModel(xf_table* t, xf_comm* comm, const std::string& path, int rank, int world, int device) {
   xf_model* part = nullptr;
   must(xf_table_freeze_part(t, nullptr, &part), "xf_table_freeze_part");
+  part = AtExportPrecision(part);
   const int rc = xf_model_save(part, PartPath(path, rank, world).c_str());
   xf_model_destroy(part);
   must(rc, "xf_model_save");
@@ -274,6 +296,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   env_path("XFLOW_RESUME", world_);
   env_path("XFLOW_EXPORT_MODEL", world_);
   env_path("XFLOW_EXPORT_DELTAS", world_);
+  ExportPrecision();  // a malformed XFLOW_EXPORT_PRECISION fails here
   if (!env_path("XFLOW_EXPORT_MODEL", 1).empty() && !env_path("XFLOW_EXPORT_SHARDED_MODEL", 1).empty())
     throw std::runtime_error("XFLOW_EXPORT_MODEL and XFLOW_EXPORT_SHARDED_MODEL write the same model: set one of them");
   if (world_ > 1) must(xf_comm_create_from_file(&comm_, CommFile().c_str(), rank_, world_, device_), "xf_comm_create_from_file");
@@ -358,6 +381,9 @@ WorkerBase::WorkerBase(const char* train_file, const char* test_file, int model)
   if (core_num < 1) core_num = 1;
   block_size = env_int("XFLOW_BLOCK_MB", 2);
   test_block_size = (model == XF_MODEL_LR) ? 4 : 2;
+  if (model == XF_MODEL_LR && ExportPrecision() != XF_PRECISION_F32)
+    throw std::runtime_error("XFLOW_EXPORT_PRECISION = f16: an LR model has no latent fields to narrow (its rows stay "
+                             "16 bytes); unset it or set it to f32");
   Server* s = Server::Get();
   table_ = (model == XF_MODEL_LR) ? s->table_lr() : s->table_fm();
   comm_ = s->comm();
@@ -713,6 +739,7 @@ void WorkerBase::train() {
     if (!export_model.empty()) {
       xf_model* m = nullptr;
       must(xf_table_freeze(table_, nullptr, &m), "xf_table_freeze");
+      m = AtExportPrecision(m);
       const int rc = xf_model_save(m, export_model.c_str());
       xf_model_destroy(m);
       must(rc, "xf_model_save");
