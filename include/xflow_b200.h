@@ -537,7 +537,7 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *    keys + pruned_keys == source_keys.  FTRL's L1 term writes exact zeros (ftrl.h:66-74): those are the rows pruned.
  *
  *    Refused with XF_ERR_ARG: tables with canonical_fm = 1 (the per-k sums of the canonical FM and the multi-view
- *    machine do not collapse to st, qt: xf_table_freeze_canonical serves them) and tables with num_shards > 1 (one
+ *    machine do not collapse to st, qt: xf_table_freeze_canonical and xf_table_freeze_mvm serve them) and tables with num_shards > 1 (one
  *    shard's rows are not a model: xf_table_freeze_part and xf_model_merge, below, serve them).
  *
  *    Canonical models.  xf_table_freeze_canonical freezes a table created with canonical_fm = 1 for the textbook FM
@@ -559,8 +559,43 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *      xf_trainer_predict_host_values returns on the table at the moment of the freeze (under ZERO: on that table with
  *      zero rows imported for the query's absent keys).  xf_model_predict_host / _device read every value as 1.
  *      The XFSM and XFSD files keep version 1 and record fm = 2, latent_dim and these row bytes; a load refuses
- *      non-zero padding in a canonical row.  Not served: the multi-view machine (XF_MODEL_MVM: its forward needs
- *      fields), shards.
+ *      non-zero padding in a canonical row.  Not served: shards.
+ *
+ *    Multi-view machine models.  xf_table_freeze_mvm freezes a table created with canonical_fm = 1 for the multi-view
+ *    machine (XF_MODEL_MVM, which trains such tables): its predict is the machine's forward on the tokens' field ids
+ *    and feature values, served by xf_model_predict_host_fields / _device_fields only.
+ *      Row: {u64 key, u64 0, f32 v[K], zero padding}: the canonical row with w = 0, the same bytes (K = 4 -> 32, 8 -> 64,
+ *      16 -> 96, 32 -> 160; F16 as the canonical table below), piece c of v at the same place.  The machine has no
+ *      linear term, so the row holds no w: bytes 8 .. 15 are zero.  K is 4, 8, 16 or 32, the latent dimensions the
+ *      machine trains.  xf_model_info reports fm = 3 and these row bytes.
+ *      Freeze resolves v as xf_table_freeze_canonical does (v equals xf_table_export's bit for bit) and ignores w;
+ *      absent = -1 is DEFAULT.  Refused with XF_ERR_ARG: tables with canonical_fm = 0, a latent_dim outside
+ *      {4, 8, 16, 32}, num_shards > 1.
+ *      Absent keys: XF_ABSENT_DEFAULT reads an absent key as the row the table would insert (v its initial values,
+ *      evaluated on the fly), which is what the table's own predict sees after inserting it.  XF_ABSENT_ZERO reads it
+ *      as a row of zeros: its field is present and it adds 0 x, as the table does with zero rows imported for the
+ *      query's absent keys.  ZERO does not skip the token: in a product over fields, a skipped token would remove its
+ *      field from the product, a different model, and pruning would then change predictions.
+ *      prune = 1 leaves out the rows that read exactly as an absent key does: under DEFAULT a latent block that is
+ *      not materialised, under ZERO every resolved v_k == +-0; w plays no part.  A field's sum starts at +0 and
+ *      round-to-nearest adds never make it -0, so a term of +0 and one of -0 leave it alike, and 0 x is the same NaN
+ *      for either sign when x is NaN or Inf: pruning never changes a prediction, NaN and Inf values included.
+ *      Forward, row r with tokens j = row_ptr[r] .. row_ptr[r+1] - 1 in that order, f_j = fields[j] & 31,
+ *      x_j = vals[j] (1 when vals is NULL) and v_j the token's row as the absent policy reads it:
+ *          S[f][k] = +0;  for j in order: S[f_j][k] = S[f_j][k] + (v_jk * x_j)   (round to nearest, no FMA, no flush)
+ *          P_k = 1;  for the fields f present in the row, ascending: P_k = P_k * S[f][k]   (k < K; no tokens: P_k = 0)
+ *          y = the sum of P_0 .. P_K-1 and zeros for k >= K over 32 lanes by xor 16, 8, 4, 2, 1;  pctr = sigmoid(y)
+ *      This is xf_trainer_predict_host_fields's forward (step_mvm.cu) with its same-field adds in token order.  That
+ *      kernel adds a pass's same-field terms with shared-memory atomics (a pass: T = 128 / K consecutive tokens from
+ *      the row's first), whose order among contending lanes the hardware picks, and token order is one of those
+ *      orders.  So the model returns, bit for bit, what the table's predict returns at the moment of the freeze (under
+ *      ZERO: with zero rows imported for the absent keys) on every row where no field has more than two tokens (0 + a
+ *      + b is commutative) or no pass holds two tokens of one field.  On other rows the table's own result is not
+ *      reproducible, and the model's is the order above, the same bits on every call and every entry point.
+ *      The XFSM and XFSD files keep version 1 and record fm = 3, latent_dim and these row bytes; a load refuses a
+ *      non-zero byte 8 .. 15 or padding byte.  Diff, apply and convert serve these models as canonical ones (a
+ *      canonical model and a multi-view machine's differ in fm and are never diffed or applied to one another);
+ *      merge does not apply (canonical tables are never sharded).
  *
  *    Sharded tables: parts and merge.  A run sharded over S GPUs holds shard s of the key space in table s
  *    (num_shards = S; shard s owns [s width, (s + 1) width) with width = floor((2^64 - 1) / S), the last shard up to
@@ -579,8 +614,9 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *    or staging, and deltas made from parts without merging them.
  *
  *    Precision.  Every model has a precision for its latent fields.  XF_PRECISION_F32 is what freeze, merge, load and
- *    apply make of F32 inputs.  xf_model_convert makes an XF_PRECISION_F16 model of an FM or canonical one: w stays
- *    float32, and only the latent fields (FM st and qt; canonical every v_k) become IEEE binary16, rounded to nearest
+ *    apply make of F32 inputs.  xf_model_convert makes an XF_PRECISION_F16 model of an FM, canonical or multi-view
+ *    machine's one: w stays float32, and only the latent fields (FM st and qt; canonical and multi-view machine every
+ *    v_k) become IEEE binary16, rounded to nearest
  *    even (subnormals included).  Every row still starts with its u64 key, and padding stays zero:
  *      kind        F32                                                   F16
  *      LR          {key, f32 w, u32 0} 16 bytes                          refused: nothing to narrow
@@ -613,6 +649,9 @@ XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** 
 /* A canonical model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG for tables with
  * canonical_fm = 0 and tables with num_shards > 1. */
 XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+/* A multi-view machine's model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG,
+ * naming the reason, for tables with canonical_fm = 0, a latent_dim outside {4, 8, 16, 32} and num_shards > 1. */
+XF_DLL int xf_table_freeze_mvm(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
 /* A part of a table of any num_shards (above); the same config and defaults.  XF_ERR_ARG for canonical tables (they
  * are never sharded); XF_ERR_STATE, naming their count, if the table holds keys outside its shard's range (a Pull,
  * Push or import can put them there). */
@@ -639,15 +678,15 @@ typedef struct xf_model_info {
   uint64_t bytes;        /* capacity x row_bytes: the model's device memory */
   uint64_t source_keys;  /* keys of the table when it was frozen */
   uint64_t pruned_keys;  /* source_keys - keys */
-  uint32_t row_bytes;    /* F32: 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical); F16: 16 (FM), 16 + 2K
-                            rounded up to 32 (canonical) */
-  int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM */
+  uint32_t row_bytes;    /* F32: 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical, multi-view machine); F16: 16
+                            (FM), 16 + 2K rounded up to 32 (canonical, multi-view machine) */
+  int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM, 3 multi-view machine */
   int precision;         /* XF_PRECISION_* of the latent fields */
 } xf_model_info;
 XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
 /* Model file "XFSM" (little-endian): a 104-byte header
  *     0 "XFSM"   4 u32 version (1)   8 u64 header bytes (104)   16 u64 keys   24 u64 capacity   32 u32 row bytes
- *    36 i32 fm (0 LR, 1 FM, 2 canonical)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
+ *    36 i32 fm (0 LR, 1 FM, 2 canonical, 3 multi-view machine)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
  *    52 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   56 f32 the constant
  *    60 u32 precision (0 F32, 1 F16; the word was reserved as 0, so every F32 file is unchanged)   64 u64 seed
  *    72 u64 source keys   80 u64 pruned keys
@@ -660,7 +699,7 @@ XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
  *  device table from the rows; a truncated, damaged or other-format file is XF_ERR_IO and leaves *out NULL, and so is
  *  a file whose checksums pass but whose keys do not ascend strictly below 2^64 - 1 or whose rows have a non-zero
  *  padding byte (LR bytes 12 .. 15, FM 20 .. 31 at F32 and none at F16, canonical 12 .. 15 and 16 + 4K .. row bytes at
- *  F32 or 16 + 2K .. row bytes at F16), and a header whose precision is not 0 or 1 or whose row bytes are not those of
+ *  F32 or 16 + 2K .. row bytes at F16, multi-view machine as canonical and 8 .. 11 too), and a header whose precision is not 0 or 1 or whose row bytes are not those of
  *  its fm, latent_dim and precision (an F16 LR model included).
  * Part file "XFSP" (xf_model_save of a part): XFSM's layout with a 112-byte header
  *     0 "XFSP"   4 u32 version (1)   8 u64 header bytes (112)   16 .. 95 as XFSM's (the part's keys, capacity,
@@ -682,18 +721,30 @@ XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream);
 /* The same with the tokens' feature values vals[nnz] (NULL: all 1; device memory for _device_values), for canonical
  * models; the contracts are those of _host / _device.  Non-NULL vals on an LR or FM model are XF_ERR_ARG: that model
- * ignores values. */
+ * ignores values.  These four and xf_model_predict_ingested refuse a multi-view machine's model (XF_ERR_ARG): it
+ * reads field ids. */
 XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
                                         uint32_t rows, uint32_t nnz, float* pctr_out);
 XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                           const float* d_vals, uint32_t rows, uint32_t nnz, float* d_pctr_out,
                                           void* cuda_stream);
+/* The forward of a multi-view machine's model (above) with the tokens' field ids fields[nnz] and feature values
+ * vals[nnz] (NULL: all 1); the contracts are those of _host_values / _device_values.  _host refuses a field id of 32 or
+ * more with XF_ERR_ARG, naming the token and the id; on the device the ids are the caller's contract, and the kernel
+ * reads fields[j] & 31 as the step kernel does.  NULL fields with nnz > 0 are XF_ERR_ARG.  XF_ERR_ARG on an LR, FM or
+ * canonical model: they read no field ids. */
+XF_DLL int xf_model_predict_host_fields(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
+                                        const float* vals, uint32_t rows, uint32_t nnz, float* pctr_out);
+XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
+                                          const uint8_t* d_fields, const float* d_vals, uint32_t rows, uint32_t nnz,
+                                          float* d_pctr_out, void* cuda_stream);
 /* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL.  On a
- * canonical model st and qt must be NULL (XF_ERR_ARG): its rows are read with xf_model_lookup_latent. */
+ * canonical or multi-view machine's model st and qt must be NULL (XF_ERR_ARG): its rows are read with
+ * xf_model_lookup_latent. */
 XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt,
                            uint8_t* present);
 /* what a canonical model holds for n host keys: w[n], v[n * K], present[n] (0 for an absent key); any output may be
- * NULL.  XF_ERR_ARG on an LR or FM model. */
+ * NULL.  On a multi-view machine's model w is 0: its row holds no linear term.  XF_ERR_ARG on an LR or FM model. */
 XF_DLL int xf_model_lookup_latent(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* v, uint8_t* present);
 /* forward pass over rows [row_start, row_end) of a trainer's current ingested block, read from `m` instead of the
  * trainer's table (same outputs as xf_trainer_predict_ingested; runs on the table's stream).  XF_ERR_ARG if the
@@ -708,7 +759,8 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
  *
  *    The delta from model A to model B:
  *      upserts  the rows of B whose key A does not hold, or whose row differs from A's in any byte (a row is 16
- *               bytes for LR, 32 for FM and 16 + 4K rounded up to 32 for a canonical model, padding included),
+ *               bytes for LR, 32 for FM and 16 + 4K rounded up to 32 for a canonical or multi-view machine's
+ *               model, padding included),
  *               sorted by key;
  *      deletes  the keys of A that B does not hold, sorted by key;
  *      header   what XFSM records of B: keys, source_keys and pruned_keys.
@@ -716,7 +768,7 @@ XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_s
  *    byte-identical to xf_model_save(B) and every xf_model_predict_* returns on it, bit for bit, what it returns on B.
  *
  *    Fingerprint.  An order-free u64 of a model's contents: the sum mod 2^64 over its rows of h(row), where for the
- *    row's 8-byte little-endian words w_0 .. w_{n-1} (n = 2 for LR, 4 for FM, row bytes / 8 for a canonical model)
+ *    row's 8-byte little-endian words w_0 .. w_{n-1} (n = 2 for LR, 4 for FM, row bytes / 8 for a canonical or multi-view machine's model)
  *    h_0 = 0, h_{i+1} = splitmix64(h_i ^ w_i)
  *    and h(row) = h_n.  The empty model's fingerprint is 0.  A delta records the fingerprint and key count of its base
  *    and of its result; apply refuses a base whose fingerprint or key count is not the delta's (XF_ERR_STATE), so a
@@ -754,7 +806,7 @@ XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out);
 XF_DLL int xf_model_apply_delta(xf_model* base, const xf_delta* d, xf_model** out);
 XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out);
 /* Delta file "XFSD" (little-endian): a 144-byte header
- *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's)   20 i32 latent_dim
+ *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's: 0, 1, 2 or 3)   20 i32 latent_dim
  *    24 i32 optimizer   28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes
  *    52 u32 precision (as XFSM's; reserved as 0 before, so every F32 file is unchanged)
  *    56 u64 base keys   64 u64 base fingerprint   72 u64 result keys   80 u64 result source keys

@@ -158,6 +158,7 @@ SIGNATURES = {
     "xf_freeze_config_default": (_i, [_vp]),
     "xf_table_freeze": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_canonical": (_i, [_vp, _vp, _vp]),
+    "xf_table_freeze_mvm": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_part": (_i, [_vp, _vp, _vp]),
     "xf_model_part_info": (_i, [_vp, _vp, _vp]),
     "xf_model_merge": (_i, [_vp, _i, _i, _vp]),
@@ -170,6 +171,8 @@ SIGNATURES = {
     "xf_model_predict_device": (_i, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_predict_host_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "xf_model_predict_device_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "xf_model_predict_host_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
+    "xf_model_predict_device_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
     "xf_model_lookup_latent": (_i, [_vp, _vp, _u64, _vp, _vp, _vp]),
     "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
@@ -461,6 +464,15 @@ class Table:
         _check(lib().xf_table_freeze_canonical(self.h, C.byref(cfg), C.byref(h)))
         return Model(h)
 
+    def freeze_mvm(self, absent=None, prune=True, device=None):
+        """A multi-view machine's serving Model of a canonical_fm table (xf_table_freeze_mvm): rows {key, 0, v[K]}
+        served with the machine's forward on field ids and feature values (Model.predict_*_fields); arguments as for
+        freeze."""
+        cfg = FreezeConfig(-1 if absent is None else absent, 1 if prune else 0, -1 if device is None else device)
+        h = C.c_void_p()
+        _check(lib().xf_table_freeze_mvm(self.h, C.byref(cfg), C.byref(h)))
+        return Model(h)
+
     def freeze_part(self, absent=None, prune=True, device=None):
         """The part of a shard table (xf_table_freeze_part): the rows freeze would make of it, tagged with its shard;
         Model.merge of every shard's part is the whole model.  Arguments as for freeze."""
@@ -545,6 +557,31 @@ class Model:
         else:
             _check(lib().xf_model_predict_device(self.h, _p(d_row_ptr), _p(d_keys), rows, nnz, _p(d_out), st))
 
+    def predict_host_fields(self, row_ptr, keys, fields, vals=None):
+        """Forward pass of a multi-view machine's model on host CSR arrays with the tokens' field ids (< 32) and
+        feature values (None: all 1)."""
+        row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
+        keys = np.ascontiguousarray(keys, np.uint64)
+        fields = np.ascontiguousarray(fields, np.uint8)
+        if fields.size != keys.size:
+            raise ValueError("one field id per token: %d field ids for %d keys" % (fields.size, keys.size))
+        if vals is not None:
+            vals = np.ascontiguousarray(vals, np.float32)
+            if vals.size != keys.size:
+                raise ValueError("one value per token: %d values for %d keys" % (vals.size, keys.size))
+        rows = row_ptr.size - 1
+        out = np.empty(rows, np.float32)
+        _check(lib().xf_model_predict_host_fields(self.h, _p(row_ptr), _p(keys), _p(fields), _p(vals), rows, keys.size,
+                                                  _p(out)))
+        return out
+
+    def predict_device_fields(self, d_row_ptr, d_keys, d_fields, rows, nnz, d_out, stream=0, d_vals=0):
+        """Asynchronous forward pass of a multi-view machine's model on device pointers (raw addresses) on the CUDA
+        stream `stream`: d_fields the tokens' u8 field ids, d_vals their feature values (0: all 1)."""
+        st = C.c_void_p(int(stream)) if stream else None
+        _check(lib().xf_model_predict_device_fields(self.h, _p(d_row_ptr), _p(d_keys), _p(d_fields),
+                                                    _p(d_vals) if d_vals else None, rows, nnz, _p(d_out), st))
+
     def lookup(self, keys):
         """What the model holds for `keys`: dict of w, st, qt (0 for LR) and present."""
         keys = np.ascontiguousarray(keys, np.uint64)
@@ -555,7 +592,8 @@ class Model:
         return out
 
     def lookup_latent(self, keys):
-        """What a canonical model holds for `keys`: dict of w, v [n, K] and present."""
+        """What a canonical or multi-view machine's model holds for `keys`: dict of w (0 for the latter), v [n, K]
+        and present."""
         keys = np.ascontiguousarray(keys, np.uint64)
         n, K = keys.size, self.info()["latent_dim"]
         out = dict(keys=keys, w=np.zeros(n, np.float32), v=np.zeros((n, K), np.float32), present=np.zeros(n, np.uint8))

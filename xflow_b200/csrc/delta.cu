@@ -11,7 +11,7 @@
 //                whose key is not deleted (a binary search over the sorted delete keys) and not upserted (the claim
 //                keeps the row it finds); then the result's fingerprint and key count are checked
 //   file         header, upsert rows, delete keys: the chunked sections of serve.cu (xf_chunks_save, xf_chunks_load)
-// Every pass hashes, compares or copies whole rows at the model's stride, so one kernel serves LR, FM and canonical rows.
+// Every pass hashes, compares or copies whole rows at the model's stride, so one kernel serves every row kind.
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>

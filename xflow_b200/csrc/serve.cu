@@ -32,6 +32,13 @@
 //                                    lanes of a token load the head and their 16-byte piece of the home slot at once;
 //                                    two passes in flight
 //
+// A multi-view machine's model (xf_table_freeze_mvm, fm = XF_SERVE_MVM) serves step_mvm.cu's forward on field ids and
+// feature values: its row is the canonical one with w = 0, {key, 0, v[K]} (the machine has no linear term).
+//   freeze   xf_k_freeze_fmc<COUNT, true>  v resolved as for a canonical model, w neither written nor pruned on
+//   predict  xf_k_serve_mvm<C>             xf_k_serve_fmc's mapping, loads and probe; the per-(field, k) sums in shared
+//                                          memory, added in token order without atomics: a pass's tokens of one field
+//                                          are ranked with __match_any_sync and added a rank per round
+//
 // An F16 model (xf_model_convert) holds its latent fields in binary16: FM {key, w, st, qt} in 16 bytes, canonical
 // {key, w, 0, v[K]} with 2-byte v.  Its predict and lookup kernels are the F32 ones' H = true instantiations, which widen
 // each field right after the load and then run the F32 arithmetic unchanged.
@@ -189,17 +196,22 @@ __device__ __forceinline__ float xf_fmc_arg(float (&S)[4], float Q, float wx) {
   return __fmaf_rn(0.5f, __fsub_rn(s2, Q), wx);
 }
 
+// Find `key` from its home slot, whose row the caller has loaded into (k, w, v); false: the model does not hold it
+template <bool H>
+__device__ __forceinline__ bool xf_fmc_find(const XfTableView& m, uint64_t key, uint64_t k, float& w, float4& v, int c) {
+  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
+    if (k == key) return true;
+    if (k == XF_EMPTY_KEY) return false;
+    xf_fmc_load<H>(xf_row(m, xf_probe_slot(m, key, i)), c, k, w, v);
+  }
+  return false;
+}
+
 // one token into the lane's sums: its row found from the home slot the caller loaded (k, w, v), or the absent policy
 template <bool H>
 __device__ __forceinline__ void xf_fmc_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float w,
                                                    float4 v, float x, int c, float (&S)[4], float& Q, float& wx) {
-  bool have = false;
-  for (uint32_t i = 1; i <= XF_MAX_PROBE; ++i) {
-    if (k == key) { have = true; break; }
-    if (k == XF_EMPTY_KEY) break;
-    xf_fmc_load<H>(xf_row(m, xf_probe_slot(m, key, i)), c, k, w, v);
-  }
-  if (!have) {
+  if (!xf_fmc_find<H>(m, key, k, w, v, c)) {
     if (absent == XF_ABSENT_ZERO) return;
     // the row the table would insert: w = 0 and a latent block that is not materialised
     w = 0.f;
@@ -260,6 +272,117 @@ static void xf_launch_serve_fmc(const xf_model* m, const uint32_t* row_ptr, cons
     case 32: xf_k_serve_fmc<8, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
     case 64: xf_k_serve_fmc<16, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
     default: xf_k_serve_fmc<32, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, vals, (int)rows, pctr_out); break;
+  }
+}
+
+// ---- multi-view machine rows {key, 0, v[K]}: the forward of xf_k_step_mvm (mode 1) with its same-field adds in token
+// order
+// A token's latent piece v[4c .. 4c+3]: its row found from the home slot the caller loaded (k, v), or the absent
+// policy's row (DEFAULT: the initial values; ZERO: zeros)
+template <bool H>
+__device__ __forceinline__ float4 xf_mvm_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float4 v,
+                                                     int c) {
+  float w;
+  if (xf_fmc_find<H>(m, key, k, w, v, c)) return v;
+  if (absent == XF_ABSENT_ZERO) return make_float4(0.f, 0.f, 0.f, 0.f);
+  return make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
+                     xf_v_init(m, key, 4 * c + 3));
+}
+
+// One pass's tokens into the warp's sums S[f][k]: lane (token, c) adds v[4c .. 4c+3] x into S[f][4c .. 4c+3] with one
+// float4 read-modify-write.  The pass's tokens of one field are ranked in token order (lanes with the same (f, c), lower
+// lanes holding earlier tokens) and added a rank per round, __syncwarp between rounds, so each S[f][k] takes its terms
+// in token order and no two lanes touch one entry in a round.  A pass without two tokens of one field is one round.
+template <int K>
+__device__ __forceinline__ void xf_mvm_add(float (*S)[K], bool live, uint32_t f, int c, float4 v, float x) {
+  const unsigned lane = threadIdx.x & 31u;
+  const unsigned peers = __match_any_sync(0xffffffffu, live ? (f << 5 | (unsigned)c) : 0xFFFFFFFFu);
+  const unsigned rank = __popc(peers & ((1u << lane) - 1u));
+  const unsigned rounds = __reduce_max_sync(0xffffffffu, live ? rank + 1u : 0u);
+  const float4 a = make_float4(__fmul_rn(v.x, x), __fmul_rn(v.y, x), __fmul_rn(v.z, x), __fmul_rn(v.w, x));
+  float4* s = reinterpret_cast<float4*>(&S[f][4 * c]);
+  for (unsigned r = 0; r < rounds; ++r) {
+    if (live && rank == r) {
+      float4 t = *s;
+      t.x = __fadd_rn(t.x, a.x); t.y = __fadd_rn(t.y, a.y); t.z = __fadd_rn(t.z, a.z); t.w = __fadd_rn(t.w, a.w);
+      *s = t;
+    }
+    __syncwarp();
+  }
+}
+
+// One warp per row, C = K/4 lanes per token and T = 32/C tokens per pass, two passes in flight, as xf_k_serve_fmc; the
+// per-(field, k) sums of the row in shared memory, XF_MVM_FIELDS x K floats per warp as xf_k_step_mvm's.  Every token
+// makes its field present (under ZERO an absent key is a row of zeros: it adds 0 x).  Lane k < K forms P_k over the
+// present fields in ascending order and clears their sums for the warp's next row; y is the warp sum of the P_k, as in
+// the step kernel.  No insert, no atomics.
+template <int C, bool H>
+__global__ void __launch_bounds__(256)
+xf_k_serve_mvm(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
+               const uint8_t* __restrict__ fields, const float* __restrict__ vals, int B, float* __restrict__ pctr_out) {
+  constexpr int K = 4 * C;
+  constexpr int T = 32 / C;
+  __shared__ __align__(16) float s_sum[8][XF_MVM_FIELDS][K];  // K x 128 bytes per warp, at most 4 KB
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const int tg = lane / C;
+  const int wib = threadIdx.x >> 5;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + wib;
+  const int nwarps = gridDim.x * warps_per_block;
+  float (*S)[K] = s_sum[wib];
+  if (lane < K)
+    for (int f = 0; f < XF_MVM_FIELDS; ++f) S[f][lane] = 0.f;
+  __syncwarp();
+  for (int row = gwarp; row < B; row += nwarps) {
+    const uint32_t beg = __ldg(row_ptr + row);
+    const uint32_t end = __ldg(row_ptr + row + 1);
+    unsigned present = 0u;
+    for (uint32_t j0 = beg; j0 < end; j0 += 2u * T) {
+      const uint32_t ja = j0 + (uint32_t)tg, jb = ja + (uint32_t)T;
+      const bool va = ja < end, vb = jb < end;
+      // streaming: do not displace model rows in L2
+      const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+      const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+      const uint32_t fa = va ? (uint32_t)__ldcs(fields + ja) & (XF_MVM_FIELDS - 1) : 0u;
+      const uint32_t fb = vb ? (uint32_t)__ldcs(fields + jb) & (XF_MVM_FIELDS - 1) : 0u;
+      const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+      const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+      // both home rows are in flight before either is resolved
+      uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+      float wa, wb;  // a multi-view machine's row holds no w
+      float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
+      if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+      if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+      if (va) pa = xf_mvm_serve_token<H>(m, absent, ka, ra, pa, c);
+      if (vb) pb = xf_mvm_serve_token<H>(m, absent, kb, rb, pb, c);
+      present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
+      xf_mvm_add<K>(S, va, fa, c, pa, xa);  // pass a, then pass b
+      xf_mvm_add<K>(S, vb, fb, c, pb, xb);
+    }
+    present = __reduce_or_sync(0xffffffffu, present);
+    float P = 0.f;
+    if (lane < K && present) {
+      P = 1.f;
+      for (unsigned q = present; q; q &= q - 1) P = __fmul_rn(P, S[__ffs(q) - 1][lane]);
+      for (unsigned q = present; q; q &= q - 1) S[__ffs(q) - 1][lane] = 0.f;
+    }
+    __syncwarp();  // the sums are clear before the warp's next row adds to them
+    const float y = xf_warp_sum(P);
+    if (lane == 0) pctr_out[row] = xf_sigmoid(y);
+  }
+}
+
+template <bool H>
+static void xf_launch_serve_mvm(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
+                                const float* vals, uint32_t rows, float* pctr_out, cudaStream_t st) {
+  if (rows == 0) return;
+  const int grid = xf_grid_for((uint64_t)rows * 32, 256, 8);
+  switch (m->view.K) {
+    case 4: xf_k_serve_mvm<1, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, (int)rows, pctr_out); break;
+    case 8: xf_k_serve_mvm<2, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, (int)rows, pctr_out); break;
+    case 16: xf_k_serve_mvm<4, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, (int)rows, pctr_out); break;
+    default: xf_k_serve_mvm<8, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, (int)rows, pctr_out); break;
   }
 }
 
@@ -338,8 +461,9 @@ __device__ __forceinline__ float4 xf_fmc_piece(const XfTableView& t, uint64_t r,
 }
 
 // xf_k_freeze for a canonical table: the model row is {key, w, 0, v[K]} with v resolved as xf_fmc_piece does.  Prune:
-// w == 0 and, under DEFAULT, a latent block that is not materialised; under ZERO, every resolved v_k == 0.
-template <bool COUNT>
+// w == 0 and, under DEFAULT, a latent block that is not materialised; under ZERO, every resolved v_k == 0.  MVM: the
+// multi-view machine's row {key, 0, v[K]}: w is neither written nor part of the prune rule.
+template <bool COUNT, bool MVM>
 __global__ void __launch_bounds__(256)
 xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned long long* __restrict__ counts, int* error) {
   const uint64_t cap = t.mask + 1;
@@ -351,7 +475,7 @@ xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned lo
     ++live_n;
     const bool ready = (h.flags & XF_FLAG_V_READY) != 0u;
     bool keep = true;
-    if (prune && h.w == 0.0f) {
+    if (prune && (MVM || h.w == 0.0f)) {
       keep = false;
       if (absent == XF_ABSENT_DEFAULT) keep = ready;
       else
@@ -365,7 +489,7 @@ xf_k_freeze_fmc(XfTableView t, XfTableView m, int absent, int prune, unsigned lo
     if (COUNT) continue;
     uint8_t* p = xf_model_claim(m, h.key, error);
     if (!p) continue;
-    *reinterpret_cast<float*>(p + 8) = h.w;  // bytes 12 .. 15 and the tail stay as the fill left them: zero
+    if (!MVM) *reinterpret_cast<float*>(p + 8) = h.w;  // bytes 12 .. 15 (MVM: 8 .. 15) and the tail stay as the fill left them: zero
     for (uint32_t q = 0; q < pieces; ++q) reinterpret_cast<float4*>(p + 16)[q] = xf_fmc_piece(t, r, ready, h.key, q);
   }
   if (COUNT) {
@@ -531,7 +655,7 @@ int xf_model_alloc(xf_model* m, uint64_t capacity) {
     return XF_ERR_FULL;
   }
   const uint32_t stride = xf_model_row_bytes(m->fm, m->view.K, m->precision);
-  m->view.canon = m->fm == XF_SERVE_FMC ? 1 : 0;
+  m->view.canon = xf_serve_latent_rows(m->fm) ? 1 : 0;
   uint8_t* base = nullptr;
   XF_CUDA_TRY(cudaMalloc(&base, capacity * stride));
   m->view.base = base;
@@ -568,7 +692,7 @@ void xf_model_free(xf_model* m) {
   cudaSetDevice(m->device);
   if (m->stream) cudaStreamSynchronize(m->stream);
   if (m->view.base) cudaFree(m->view.base);
-  m->s_row_ptr.release(); m->s_keys.release(); m->s_out.release(); m->s_aux.release(); m->s_vals.release();
+  m->s_row_ptr.release(); m->s_keys.release(); m->s_out.release(); m->s_aux.release(); m->s_vals.release(); m->s_fields.release();
   m->h_in.release(); m->h_out.release();
   if (m->stream) cudaStreamDestroy(m->stream);
   delete m;
@@ -626,14 +750,14 @@ XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
   return XF_OK;
 }
 
-// the body of xf_table_freeze (canonical = 0), xf_table_freeze_canonical and xf_table_freeze_part (part): on failure
-// the caller frees `m`
-static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonical, bool part, xf_model* m, const char* fn) {
+// the body of xf_table_freeze (latent = XF_SERVE_LR), xf_table_freeze_canonical (XF_SERVE_FMC), xf_table_freeze_mvm
+// (XF_SERVE_MVM) and xf_table_freeze_part (part): on failure the caller frees `m`
+static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, int latent, bool part, xf_model* m, const char* fn) {
   const int src_dev = t->cfg.device;
   XF_CUDA_TRY(cudaSetDevice(src_dev));
   XF_TRY(t->check_error());  // waits for everything enqueued on the table's stream
   const XfTableView& tv = t->view;
-  const int fm = canonical ? XF_SERVE_FMC : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
+  const int fm = latent != XF_SERVE_LR ? latent : (tv.K > 0 ? XF_SERVE_FM : XF_SERVE_LR);
   const int absent = cfg.absent >= 0 ? cfg.absent : (t->admit.mode == XF_ADMIT_ALL ? XF_ABSENT_DEFAULT : XF_ABSENT_ZERO);
   XF_TRY(xf_model_init(m, src_dev, XfCompat{fm, tv.K, tv.opt, absent, tv.v_init, tv.v_const, tv.seed,
                                                    XF_PRECISION_F32}));
@@ -651,7 +775,8 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   uint64_t lo = 0, hi = 0;
   xf_shard_range(t->cfg.shard_index, t->cfg.num_shards, &lo, &hi);
 #define XF_FREEZE_LAUNCH(COUNT)                                                                                       \
-  if (canonical) xf_k_freeze_fmc<COUNT><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error);         \
+  if (fm == XF_SERVE_FMC) xf_k_freeze_fmc<COUNT, false><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
+  else if (fm == XF_SERVE_MVM) xf_k_freeze_fmc<COUNT, true><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
   else switch (xf_vec_for(tv.K)) {                                                                                         \
     case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
     case 2: xf_k_freeze<COUNT, 2><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
@@ -705,8 +830,10 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, bool canonic
   return XF_OK;
 }
 
-static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical, bool part, xf_model** out) {
-  const char* fn = part ? "xf_table_freeze_part" : canonical ? "xf_table_freeze_canonical" : "xf_table_freeze";
+static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, int latent, bool part, xf_model** out) {
+  const bool canonical = latent == XF_SERVE_FMC, mvm = latent == XF_SERVE_MVM;
+  const char* fn = part ? "xf_table_freeze_part" : canonical ? "xf_table_freeze_canonical" : mvm ? "xf_table_freeze_mvm"
+                                                                                                 : "xf_table_freeze";
   if (out) *out = nullptr;
   if (!t || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
   xf_freeze_config cfg;
@@ -719,10 +846,20 @@ static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical
                  "xf_table_freeze_canonical");
     return XF_ERR_ARG;
   }
-  if (!canonical && !part && t->cfg.canonical_fm) {
+  if (latent == XF_SERVE_LR && !part && t->cfg.canonical_fm) {
     xf_set_error("xf_table_freeze: a canonical table (canonical_fm = 1) has no collapsed serving model: the per-k sums of "
                  "the canonical FM and the multi-view machine do not collapse to one pair of sums per key; "
                  "xf_table_freeze_canonical serves it with the canonical FM's forward");
+    return XF_ERR_ARG;
+  }
+  if (mvm && !t->cfg.canonical_fm) {
+    xf_set_error("xf_table_freeze_mvm: the table is not canonical (canonical_fm = 0): the multi-view machine trains "
+                 "canonical tables only");
+    return XF_ERR_ARG;
+  }
+  if (mvm && !xf_mvm_latent_ok(t->cfg.latent_dim)) {
+    xf_set_error("xf_table_freeze_mvm: latent_dim = %d: the multi-view machine serves K = 4, 8, 16 or 32",
+                 t->cfg.latent_dim);
     return XF_ERR_ARG;
   }
   if (canonical && (!t->cfg.canonical_fm || !xf_fmc_latent_ok(t->cfg.latent_dim))) {
@@ -737,22 +874,26 @@ static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, bool canonical
   }
   std::lock_guard<std::mutex> host_lock(t->host_mu);
   xf_model* m = new xf_model;
-  const int rc = xf_freeze_into(t, cfg, canonical, part, m, fn);
+  const int rc = xf_freeze_into(t, cfg, latent, part, m, fn);
   if (rc != XF_OK) { xf_model_free(m); return rc; }
   *out = m;
   return XF_OK;
 }
 
 XF_DLL int xf_table_freeze(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
-  return xf_freeze(t, cfg, false, false, out);
+  return xf_freeze(t, cfg, XF_SERVE_LR, false, out);
 }
 
 XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
-  return xf_freeze(t, cfg, true, false, out);
+  return xf_freeze(t, cfg, XF_SERVE_FMC, false, out);
+}
+
+XF_DLL int xf_table_freeze_mvm(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
+  return xf_freeze(t, cfg, XF_SERVE_MVM, false, out);
 }
 
 XF_DLL int xf_table_freeze_part(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
-  return xf_freeze(t, cfg, false, true, out);
+  return xf_freeze(t, cfg, XF_SERVE_LR, true, out);
 }
 
 XF_DLL int xf_model_part_info(xf_model* m, int* shard_index, int* num_shards) {
@@ -798,9 +939,9 @@ static int xf_model_stage(xf_model* m, XfDevBuf& dev, size_t off, const void* sr
   return XF_OK;
 }
 
-// feature values are read by canonical models only: the LR and FM forwards ignore them
+// feature values are read by canonical and multi-view machine models only: the LR and FM forwards ignore them
 static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
-  if (vals && m->fm != XF_SERVE_FMC) {
+  if (vals && !xf_serve_latent_rows(m->fm)) {
     xf_set_error("%s: an %s model ignores feature values: pass vals = NULL (values need a model frozen with "
                  "xf_table_freeze_canonical)", fn, m->fm ? "FM" : "LR");
     return XF_ERR_ARG;
@@ -808,28 +949,65 @@ static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
   return XF_OK;
 }
 
-static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals, uint32_t rows,
-                           uint32_t nnz, float* pctr_out, const char* fn) {
-  if (!m || !row_ptr || (!keys && nnz) || (!pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
+// field ids are read by multi-view machine models, and those read nothing without them: the _fields entry points serve
+// them only, and every other entry point refuses them
+static int xf_check_fields_kind(const xf_model* m, bool with_fields, const char* fn) {
+  if (m->fm == XF_SERVE_MVM && !with_fields) {
+    xf_set_error("%s: a multi-view machine's model reads the tokens' field ids: use xf_model_predict_host_fields or "
+                 "xf_model_predict_device_fields", fn);
+    return XF_ERR_ARG;
+  }
+  if (m->fm != XF_SERVE_MVM && with_fields) {
+    static const char* const kind[] = {"LR", "FM", "canonical"};
+    xf_set_error("%s: an %s model reads no field ids: field ids need a model frozen with xf_table_freeze_mvm", fn,
+                 kind[m->fm]);
+    return XF_ERR_ARG;
+  }
+  return XF_OK;
+}
+
+// the forward of any model on device arrays (fields: a multi-view machine's, which reads nothing else)
+static void xf_launch_predict(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
+                              const float* vals, uint32_t rows, float* pctr_out, cudaStream_t st) {
+  if (m->fm != XF_SERVE_MVM) xf_launch_serve(m, row_ptr, keys, vals, rows, pctr_out, st);
+  else if (m->precision == XF_PRECISION_F16) xf_launch_serve_mvm<true>(m, row_ptr, keys, fields, vals, rows, pctr_out, st);
+  else xf_launch_serve_mvm<false>(m, row_ptr, keys, fields, vals, rows, pctr_out, st);
+}
+
+static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields, const float* vals,
+                           uint32_t rows, uint32_t nnz, float* pctr_out, bool with_fields, const char* fn) {
+  if (!m || !row_ptr || (!keys && nnz) || (!pctr_out && rows) || (with_fields && !fields && nnz)) {
+    xf_set_error("null argument");
+    return XF_ERR_ARG;
+  }
   XF_TRY(xf_refuse_part(m, fn));
+  XF_TRY(xf_check_fields_kind(m, with_fields, fn));
   XF_TRY(xf_check_vals(m, vals, fn));
   for (uint32_t r = 0; r < rows; ++r)
     if (row_ptr[r] > row_ptr[r + 1]) { xf_set_error("%s: row_ptr decreases at row %u", fn, r); return XF_ERR_ARG; }
   if (row_ptr[rows] > nnz) { xf_set_error("%s: row_ptr ends at %u, past nnz = %u", fn, row_ptr[rows], nnz); return XF_ERR_ARG; }
   XF_TRY(xf_check_host_keys(keys, nnz, fn));
+  if (with_fields)
+    for (uint32_t j = 0; j < nnz; ++j)
+      if (fields[j] >= XF_MVM_FIELDS) {
+        xf_set_error("%s: field id %u of token %u: a multi-view machine takes field ids below %d", fn, (unsigned)fields[j], j,
+                     XF_MVM_FIELDS);
+        return XF_ERR_ARG;
+      }
   if (rows == 0) return XF_OK;
   std::lock_guard<std::mutex> lock(m->mu);
   XF_CUDA_TRY(cudaSetDevice(m->device));
   const size_t rp_bytes = ((size_t)rows + 1) * 4, rp_pad = (rp_bytes + 15) & ~(size_t)15, key_bytes = (size_t)nnz * 8;
-  const size_t val_bytes = vals ? (size_t)nnz * 4 : 0;
-  XF_TRY(m->h_in.ensure(rp_pad + key_bytes + val_bytes));
+  const size_t val_bytes = vals ? (size_t)nnz * 4 : 0, field_bytes = with_fields ? (size_t)nnz : 0;
+  XF_TRY(m->h_in.ensure(rp_pad + key_bytes + val_bytes + field_bytes));
   XF_TRY(m->h_out.ensure((size_t)rows * 4));
   XF_TRY(m->s_out.ensure((size_t)rows * 4));
   XF_TRY(xf_model_stage(m, m->s_row_ptr, 0, row_ptr, rp_bytes));
   XF_TRY(xf_model_stage(m, m->s_keys, rp_pad, keys, key_bytes));
   if (vals) XF_TRY(xf_model_stage(m, m->s_vals, rp_pad + key_bytes, vals, val_bytes));
-  xf_launch_serve(m, m->s_row_ptr.as<uint32_t>(), m->s_keys.as<uint64_t>(), vals ? m->s_vals.as<float>() : nullptr, rows,
-                  m->s_out.as<float>(), m->stream);
+  if (with_fields) XF_TRY(xf_model_stage(m, m->s_fields, rp_pad + key_bytes + val_bytes, fields, field_bytes));
+  xf_launch_predict(m, m->s_row_ptr.as<uint32_t>(), m->s_keys.as<uint64_t>(), with_fields ? m->s_fields.as<uint8_t>() : nullptr,
+                    vals ? m->s_vals.as<float>() : nullptr, rows, m->s_out.as<float>(), m->stream);
   XF_CUDA_TRY(cudaGetLastError());
   XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_out.p, (size_t)rows * 4, cudaMemcpyDeviceToHost, m->stream));
   XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
@@ -839,39 +1017,59 @@ static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t*
 
 XF_DLL int xf_model_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, uint32_t rows, uint32_t nnz,
                                  float* pctr_out) {
-  return xf_predict_host(m, row_ptr, keys, nullptr, rows, nnz, pctr_out, "xf_model_predict_host");
+  return xf_predict_host(m, row_ptr, keys, nullptr, nullptr, rows, nnz, pctr_out, false, "xf_model_predict_host");
 }
 
 XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
                                         uint32_t rows, uint32_t nnz, float* pctr_out) {
-  return xf_predict_host(m, row_ptr, keys, vals, rows, nnz, pctr_out, "xf_model_predict_host_values");
+  return xf_predict_host(m, row_ptr, keys, nullptr, vals, rows, nnz, pctr_out, false, "xf_model_predict_host_values");
+}
+
+XF_DLL int xf_model_predict_host_fields(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
+                                        const float* vals, uint32_t rows, uint32_t nnz, float* pctr_out) {
+  return xf_predict_host(m, row_ptr, keys, fields, vals, rows, nnz, pctr_out, true, "xf_model_predict_host_fields");
+}
+
+static int xf_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, const uint8_t* d_fields,
+                             const float* d_vals, uint32_t rows, uint32_t nnz, float* d_pctr_out, void* cuda_stream,
+                             bool with_fields, const char* fn) {
+  if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows) || (with_fields && !d_fields && nnz)) {
+    xf_set_error("null argument");
+    return XF_ERR_ARG;
+  }
+  XF_TRY(xf_refuse_part(m, fn));
+  XF_TRY(xf_check_fields_kind(m, with_fields, fn));
+  XF_TRY(xf_check_vals(m, d_vals, fn));
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  xf_launch_predict(m, d_row_ptr, d_keys, d_fields, d_vals, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
 }
 
 XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, uint32_t rows,
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
-  if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
-  XF_TRY(xf_refuse_part(m, "xf_model_predict_device"));
-  XF_CUDA_TRY(cudaSetDevice(m->device));
-  xf_launch_serve(m, d_row_ptr, d_keys, nullptr, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
-  XF_CUDA_TRY(cudaGetLastError());
-  return XF_OK;
+  return xf_predict_device(m, d_row_ptr, d_keys, nullptr, nullptr, rows, nnz, d_pctr_out, cuda_stream, false,
+                           "xf_model_predict_device");
 }
 
 XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys, const float* d_vals,
                                           uint32_t rows, uint32_t nnz, float* d_pctr_out, void* cuda_stream) {
-  if (!m || !d_row_ptr || (!d_keys && nnz) || (!d_pctr_out && rows)) { xf_set_error("null argument"); return XF_ERR_ARG; }
-  XF_TRY(xf_refuse_part(m, "xf_model_predict_device_values"));
-  XF_TRY(xf_check_vals(m, d_vals, "xf_model_predict_device_values"));
-  XF_CUDA_TRY(cudaSetDevice(m->device));
-  xf_launch_serve(m, d_row_ptr, d_keys, d_vals, rows, d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
-  XF_CUDA_TRY(cudaGetLastError());
-  return XF_OK;
+  return xf_predict_device(m, d_row_ptr, d_keys, nullptr, d_vals, rows, nnz, d_pctr_out, cuda_stream, false,
+                           "xf_model_predict_device_values");
+}
+
+XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
+                                          const uint8_t* d_fields, const float* d_vals, uint32_t rows, uint32_t nnz,
+                                          float* d_pctr_out, void* cuda_stream) {
+  return xf_predict_device(m, d_row_ptr, d_keys, d_fields, d_vals, rows, nnz, d_pctr_out, cuda_stream, true,
+                           "xf_model_predict_device_fields");
 }
 
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
                                      uint8_t* labels_out) {
   if (!m || !tr) { xf_set_error("null argument"); return XF_ERR_ARG; }
   XF_TRY(xf_refuse_part(m, "xf_model_predict_ingested"));
+  XF_TRY(xf_check_fields_kind(m, false, "xf_model_predict_ingested"));
   if (m->fm == XF_SERVE_FMC) {
     xf_set_error("xf_model_predict_ingested: a canonical model reads feature values, which an ingested text block does "
                  "not carry: use xf_model_predict_host_values / _device_values");
@@ -934,7 +1132,7 @@ static int xf_lookup_fmc(xf_model* m, const uint64_t* keys, uint64_t n, float* w
 
 XF_DLL int xf_model_lookup_latent(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* v, uint8_t* present) {
   if (!m || (!keys && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
-  if (m->fm != XF_SERVE_FMC) {
+  if (!xf_serve_latent_rows(m->fm)) {
     xf_set_error("xf_model_lookup_latent: an %s model holds no latent rows: use xf_model_lookup", m->fm ? "FM" : "LR");
     return XF_ERR_ARG;
   }
@@ -944,10 +1142,10 @@ XF_DLL int xf_model_lookup_latent(xf_model* m, const uint64_t* keys, uint64_t n,
 
 XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float* w, float* st, float* qt, uint8_t* present) {
   if (!m || (!keys && n)) { xf_set_error("null argument"); return XF_ERR_ARG; }
-  if (m->fm == XF_SERVE_FMC) {
+  if (xf_serve_latent_rows(m->fm)) {
     if (st || qt) {
-      xf_set_error("xf_model_lookup: a canonical model holds no st, qt: pass NULL, and read its latent rows with "
-                   "xf_model_lookup_latent");
+      xf_set_error("xf_model_lookup: a %s model holds no st, qt: pass NULL, and read its latent rows with "
+                   "xf_model_lookup_latent", m->fm == XF_SERVE_MVM ? "multi-view machine's" : "canonical");
       return XF_ERR_ARG;
     }
     XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup"));
@@ -1059,6 +1257,8 @@ bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
   if (c.precision != XF_PRECISION_F32 && c.precision != XF_PRECISION_F16) return false;
   if (c.fm == XF_SERVE_FMC) {
     if (!xf_fmc_latent_ok(c.latent_dim)) return false;
+  } else if (c.fm == XF_SERVE_MVM) {
+    if (!xf_mvm_latent_ok(c.latent_dim)) return false;
   } else if (c.fm != (c.latent_dim > 0 ? 1 : 0) || c.latent_dim < 0 || (c.fm == XF_SERVE_LR && c.precision != XF_PRECISION_F32)) {
     return false;
   }
@@ -1196,7 +1396,7 @@ XF_DLL int xf_model_load(xf_model** out, const char* path, int device) {
     xf_set_error("model file %s: the header is damaged (checksum mismatch)", path);
     rc = XF_ERR_IO;
   } else if (part && (p.header_checksum != xf_st_host_sum(&p, offsetof(XfPartHeader, header_checksum), 0) ||
-                      !xf_sm_header_sane(h) || h.fm == XF_SERVE_FMC)) {
+                      !xf_sm_header_sane(h) || xf_serve_latent_rows(h.fm))) {
     xf_set_error("model part file %s: the header is damaged (checksum mismatch)", path);
     rc = XF_ERR_IO;
   } else if (part && (p.num_shards < 1 || p.shard_index < 0 || p.shard_index >= p.num_shards)) {
@@ -1333,7 +1533,7 @@ static int xf_convert_into(xf_model* m, int precision, xf_model* out) {
   XF_CUDA_TRY(cudaMemsetAsync(d_error, 0, 4, st));
   const int grid = xf_grid_for(m->view.mask + 1, 256, 8);
   const bool to_half = precision == XF_PRECISION_F16;
-  if (m->fm == XF_SERVE_FMC) {
+  if (xf_serve_latent_rows(m->fm)) {  // a multi-view machine's zero word is copied as a canonical row's w
     if (to_half) xf_k_model_convert<true, true><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
     else xf_k_model_convert<true, false><<<grid, 256, 0, st>>>(m->view, out->view, d_over, d_error);
   } else {

@@ -12,7 +12,9 @@
 #include "internal.h"
 
 // what a model's rows hold (xf_model::fm, xf_model_info::fm, the files' fm field)
-enum { XF_SERVE_LR = 0, XF_SERVE_FM = 1, XF_SERVE_FMC = 2 };
+enum { XF_SERVE_LR = 0, XF_SERVE_FM = 1, XF_SERVE_FMC = 2, XF_SERVE_MVM = 3 };
+// rows {key, word 8, v[K], 0...}: the canonical FM's (word 8: w) and the multi-view machine's (word 8: 0, no linear term)
+__host__ __device__ inline bool xf_serve_latent_rows(int fm) { return fm == XF_SERVE_FMC || fm == XF_SERVE_MVM; }
 
 struct xf_model {
   XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source;
@@ -25,7 +27,7 @@ struct xf_model {
   cudaStream_t stream = nullptr;
   // staging of the host entry points, grown on demand; those calls are serialised by the mutex
   std::mutex mu;
-  XfDevBuf s_row_ptr, s_keys, s_out, s_aux, s_vals;
+  XfDevBuf s_row_ptr, s_keys, s_out, s_aux, s_vals, s_fields;
   XfPinBuf h_in, h_out;
 };
 
@@ -72,27 +74,35 @@ inline const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
 // Bytes of a model row.  F32: LR {key, w, 0}: 16; FM {key, w, st, qt, 0...}: 32; canonical FM {key, w, 0, v[K], 0...}:
 // 16 + 4K rounded up to 32, so that every row starts on a sector and lane c's piece v[4c .. 4c+3] lies at 16 + 16c.
 // F16 (FM and canonical only; w stays float32): FM {key, w, st, qt}: 16, no padding; canonical {key, w, 0, v[K], 0...}:
-// 16 + 2K rounded up to 32, lane c's piece at 16 + 8c.
+// 16 + 2K rounded up to 32, lane c's piece at 16 + 8c.  A multi-view machine's row {key, u64 0, v[K], 0...} is the
+// canonical one with w = 0.
 __host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K, int precision) {
   const uint32_t vb = precision == XF_PRECISION_F16 ? 2u : 4u;
-  if (fm == XF_SERVE_FMC) return (16u + vb * (uint32_t)K + 31u) & ~31u;
+  if (xf_serve_latent_rows(fm)) return (16u + vb * (uint32_t)K + 31u) & ~31u;
   if (fm == XF_SERVE_FM) return precision == XF_PRECISION_F16 ? 16u : 32u;
   return 16u;
 }
 // the latent dimensions a canonical model serves: C = K / 4 lanes per token, a power of two <= 32
 inline bool xf_fmc_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32 || K == 64 || K == 128; }
+// those a multi-view machine's model serves: the ones its trainer takes (step_mvm.cu, XF_MVM_K_MAX)
+inline bool xf_mvm_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32; }
 // A packed row of a model (fm, K, precision, row_bytes) has zero bytes where its layout has padding: LR [12, 16); FM
-// [20, 32) at F32, none at F16; canonical [12, 16) and [16 + 4K, row_bytes) at F32, [16 + 2K, row_bytes) at F16.  Every
-// model in memory keeps them zero (the fill writes them, freeze and convert write fields only, the other passes copy
-// whole rows), so that whole rows compare and hash as their fields do.  Checked a word at a time: the 4-byte word after
-// w (LR, canonical) or qt (FM), then 8-byte words to the row's end.
+// [20, 32) at F32, none at F16; canonical [12, 16) and [16 + 4K, row_bytes) at F32, [16 + 2K, row_bytes) at F16; a
+// multi-view machine's as the canonical one's, and [8, 12) too.  Every model in memory keeps them zero (the fill writes
+// them, freeze and convert write fields only, the other passes copy whole rows), so that whole rows compare and hash as
+// their fields do.  Checked a word at a time: the 4-byte word after w (LR, canonical; for a multi-view machine's row
+// the word of w too) or qt (FM), then 8-byte words to the row's end.
 inline bool xf_model_padding_zero(const uint8_t* p, int fm, int K, int precision, uint32_t row_bytes) {
   if (fm == XF_SERVE_FM && precision == XF_PRECISION_F16) return true;
   const uint32_t vb = precision == XF_PRECISION_F16 ? 2u : 4u;
   uint32_t w4;
   memcpy(&w4, p + (fm == XF_SERVE_FM ? 20 : 12), 4);
   uint64_t any = w4;
-  for (uint32_t b = fm == XF_SERVE_FMC ? 16u + vb * (uint32_t)K : fm == XF_SERVE_FM ? 24u : 16u; b < row_bytes; b += 8) {
+  if (fm == XF_SERVE_MVM) {
+    memcpy(&w4, p + 8, 4);
+    any |= w4;
+  }
+  for (uint32_t b = xf_serve_latent_rows(fm) ? 16u + vb * (uint32_t)K : fm == XF_SERVE_FM ? 24u : 16u; b < row_bytes; b += 8) {
     uint64_t x;
     memcpy(&x, p + b, 8);
     any |= x;
