@@ -25,6 +25,10 @@
 // At 32-B fetch granularity the CAS costs 81.9 ps already at 4 rounds (270 k other looks: 8.2 MB of sectors, but
 // 33 MB of 128-B lines) and 84.1 at 31 rounds: L2 room is counted in lines, so a finer fetch makes none.  The more
 // other lines were looked at since a row's look, the less often its CAS finds the line; past about 25 MB, almost never.
+//   look, then CAS.128 after one round  the same at 4 CTAs of 256 per SM (135 168 threads), lag 0 and 1 round: what
+//               the lazy LR step's row groups see, one token per thread, depositing one round of looks after the look
+// Same card (700 W, 1980 MHz), 128-B fetch, look alone 31.5 G rows/s: 51.4 ps per row at lag 0, 75.2 at lag 1 (D = 16.5
+// MB: one round at 1 024 threads per SM brings in as many lines as two rounds at 512).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -238,6 +242,24 @@ static float run(const char* name, uint8_t* base, uint64_t nsect, uint64_t n, ui
   return best;
 }
 
+// best of 3 launches of klag, each on the zeroed table (every CAS finds the zeros it compares against, as on the first
+// launch)
+static float run_lag(uint8_t* base, uint64_t nsect, uint64_t nl, int bps, int lag, uint64_t seed0, uint64_t* sink) {
+  float best = 1e30f;
+  for (int r = 0; r < 3; ++r) {
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    cudaMemset(base, 0, nsect * 32);
+    cudaEventRecord(e0);
+    klag<<<g_sms * bps, 256>>>(base, nsect - 1, nl, seed0 + 1000 * r, 9 + r, lag, sink);
+    cudaEventRecord(e1);
+    cudaEventSynchronize(e1);
+    float ms; cudaEventElapsedTime(&ms, e0, e1);
+    if (ms < best) best = ms;
+  }
+  return best;
+}
+
 int main(int argc, char** argv) {
   uint64_t mb = argc > 1 ? strtoull(argv[1], 0, 10) : 8192;
   double acc_m = argc > 2 ? atof(argv[2]) : 6.5;
@@ -309,22 +331,30 @@ int main(int argc, char** argv) {
              " look alone %.2f G rows/s\n", fetch, (unsigned long long)T, (unsigned long long)nl, (double)nl / (look * 1e-3) / 1e9);
       for (int di = 0; di < (int)(sizeof(dmb) / sizeof(dmb[0])); ++di) {
         const int lag = (int)((double)dmb[di] * 1048576.0 / ((double)T * fetch) + 0.5);
-        float best = 1e30f;
-        for (int r = 0; r < 3; ++r) {
-          cudaEvent_t e0, e1;
-          cudaEventCreate(&e0); cudaEventCreate(&e1);
-          cudaMemset(base, 0, nsect * 32);  // every CAS finds the zeros it compares against, as on the first launch
-          cudaEventRecord(e0);
-          klag<<<g_sms * bps, 256>>>(base, nsect - 1, nl, 4242 + 1000 * r + 100 * di + fetch, 9 + r, lag, sink);
-          cudaEventRecord(e1);
-          cudaEventSynchronize(e1);
-          float ms; cudaEventElapsedTime(&ms, e0, e1);
-          if (ms < best) best = ms;
-        }
+        const float best = run_lag(base, nsect, nl, bps, lag, 4242 + 100 * di + fetch, sink);
         const double rate = (double)nl / (best * 1e-3) / 1e9;
         printf("  D %5.1f MB (lag %2d rounds)  %8.1f us  %6.2f G rows/s  CAS after the look %5.1f ps per row\n",
                (double)lag * T * fetch / 1048576.0, lag, best * 1e3, rate, 1e3 / rate - (double)look * 1e9 / nl);
       }
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) printf("CUDA error: %s\n", cudaGetErrorString(e));
+  }
+  // the same after exactly one round of looks by every thread, at 4 CTAs of 256 per SM: the lazy LR step's row groups
+  // (one token per thread) look at all of a row's first rows in one round and deposit after it
+  {
+    const uint64_t nl = 32000000;
+    const int bps = 4;
+    const uint64_t T = (uint64_t)g_sms * bps * 256;
+    cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 128);
+    const float look = run<M_READ_PAIR>("", base, nsect, nl, sink, bps, 31, false);
+    printf("look, then CAS.128 after one round of looks, 4 CTAs of 256 per SM (%llu threads), L2 fetch granularity 128 B,"
+           " look alone %.2f G rows/s\n", (unsigned long long)T, (double)nl / (look * 1e-3) / 1e9);
+    for (int lag = 0; lag <= 1; ++lag) {
+      const float best = run_lag(base, nsect, nl, bps, lag, 5353 + 100 * lag, sink);
+      const double rate = (double)nl / (best * 1e-3) / 1e9;
+      printf("  D %5.1f MB (lag %d round)  %8.1f us  %6.2f G rows/s  CAS after the look %5.1f ps per row\n",
+             (double)lag * T * 128 / 1048576.0, lag, best * 1e3, rate, 1e3 / rate - (double)look * 1e9 / nl);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) printf("CUDA error: %s\n", cudaGetErrorString(e));

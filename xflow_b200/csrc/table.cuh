@@ -215,6 +215,16 @@ __device__ __forceinline__ void xf_admit_append(const XfAdmitView& a, bool r0, u
     if (r1) a.rej_keys[base + __popc(m0) + __popc(m1 & lt)] = k1;
   }
 }
+// The same for one token per lane (rejected: r, key k): one atomic per warp and 32 tokens that have rejections.
+__device__ __forceinline__ void xf_admit_append(const XfAdmitView& a, bool r, uint64_t k) {
+  const unsigned m = __ballot_sync(0xffffffffu, r);
+  if (m == 0u) return;
+  const unsigned lane = threadIdx.x & 31u;
+  unsigned long long base = 0ull;
+  if (lane == 0u) base = atomicAdd(a.rej_n, (unsigned long long)__popc(m));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (a.rej_keys && r) a.rej_keys[base + __popc(m & ((1u << lane) - 1u))] = k;
+}
 
 __device__ __forceinline__ float xf_counter_normal(uint64_t key, uint32_t k, uint64_t seed) {
   uint64_t base = xf_splitmix64(key ^ xf_splitmix64(seed + 0x632BE59BD9B4E019ull * (uint64_t)(k + 1)));
