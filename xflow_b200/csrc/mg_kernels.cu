@@ -197,7 +197,7 @@ xf_k_pull_tokens(XfTableView t, const uint64_t* __restrict__ in_keys, const uint
       // batch ever has, and the Push takes a fresh look at it instead.
       const uint64_t q1 = xf_raw_q1(h), q2 = xf_raw_q2(h);
       uint64_t q3 = xf_raw_q3(h);
-      if ((uint32_t)(q1 >> 32) == xf_lazy_check(q2)) q3 |= XF_TAG_MASK;
+      if (xf_lazy_given(q1, q2, q3)) q3 |= XF_TAG_MASK;
       __stcs(stash + ((uint64_t)s * cap + i), make_uint4((uint32_t)q2, (uint32_t)(q2 >> 32), (uint32_t)q3, (uint32_t)(q3 >> 32)));
     }
     if (r >= 0) {
@@ -420,7 +420,10 @@ xf_k_push_tokens_lr(XfTableView t, const uint32_t* __restrict__ slots, const uin
         const XfHead h = xf_load_head(rowp);
         uint64_t r2n;
         xf_lazy_fold(t, xf_raw_q1(h), xf_raw_q2(h), xf_raw_q3(h), seq, r2n);
-        if (xf_lazy_deposit(t, rowp, xf_raw_q2(h), xf_raw_q3(h), r2n, seq, fix[u])) ++open_acc;
+        if (xf_lazy_deposit(t, rowp, xf_raw_q2(h), xf_raw_q3(h), r2n, seq, fix[u])) {
+          xf_lazy_mark_open(rowp, xf_raw_q1(h), xf_raw_q2(h), xf_raw_q3(h), seq);
+          ++open_acc;
+        }
       }
     }
   }

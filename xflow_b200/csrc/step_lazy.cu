@@ -147,6 +147,7 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
     // the row's second half as it looked (q2, q3) and as it will be published (q2n)
     uint32_t lead_s = XF_NO_SLOT, cnt = 0;
     uint64_t lq2 = 0ull, lq3 = 0ull, lq2n = 0ull;
+    bool lmark = false;  // the row carries an imported weight and has not been opened since (xf_lazy_mark_open)
 
     // ---------------- phase A: pull every token's row; nothing is written
     for (int rd = 0; rd < rounds; ++rd) {
@@ -184,9 +185,13 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
         const unsigned gm = __match_any_sync(0xffffffffu, (s != XF_NO_SLOT) ? s : (0xFFFFFF00u | (uint32_t)lane));
         const bool L = s != XF_NO_SLOT && lane == __ffs(gm) - 1;
         if (rd == 0) {
-          if (L) { lead_s = s; cnt = (uint32_t)__popc(gm); lq2 = a2; lq3 = a3; lq2n = a2n; }
+          if (L) {
+            lead_s = s; cnt = (uint32_t)__popc(gm); lq2 = a2; lq3 = a3; lq2n = a2n;
+            lmark = (a3 & XF_TAG_MASK) == 0ull && (uint32_t)(a1 >> 32) == xf_lazy_check(a2);
+          }
         } else if (L && xf_lazy_deposit(t, xf_row(t, s), a2, a3, a2n, seq, 0ll)) {
           // long rows (> G tokens): nothing is remembered for phase B; open the row now with an empty deposit
+          xf_lazy_mark_open(xf_row(t, s), a1, a2, a3, seq);
           ++open_acc;
           if (STAMP) sv.stamp[s] = sv.now;
         }
@@ -227,6 +232,7 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       bool stale = false;
       const bool issued = xf_lazy_deposit_issue(rowp, lq2, lq3, lq2n, seq, fix, o2, o3);
       if (issued && xf_lazy_deposit_resolve(rowp, true, lq2, lq3, o2, o3, seq, fix, &stale)) {
+        if (lmark) *reinterpret_cast<uint32_t*>(rowp + 12) = xf_lazy_open_check(lq2, seq);  // xf_lazy_mark_open
         ++open_acc;
         if (STAMP) sv.stamp[lead_s] = sv.now;
       }

@@ -23,9 +23,10 @@
 //                                      reference's handle evaluates after every push, ftrl.h:66-74)
 //              f32 w, byte 20 unused  (SGD)
 //     byte  8  f32 w_given, u32 check   a weight set from outside (xf_table_import) that is NOT f(z, n): it stands
-//                                      for w until the row's state changes (check = a digest of bytes 16..23;
-//                                      the reference would likewise use the stored w in its next step and then
-//                                      overwrite it with f(z', n'))
+//                                      for w until the first optimizer step after the import is folded in
+//                                      (check = a digest of bytes 16..23, re-marked by the batch that first opens
+//                                      the row: xf_lazy_given; the reference would likewise use the stored w in its
+//                                      next step and then overwrite it with f(z', n'))
 //     byte 24  u64 { tag : 16 (low) | g : 48 (high) }   tag = the batch whose residual sum is pending in g
 //                                      (0: none); g = that sum as a signed FIXED-POINT integer of the batch's
 //                                      unit 2^-s (xf_fix_shift: s = 27 below 2^20 tokens, smaller above, so
@@ -543,6 +544,25 @@ __device__ __forceinline__ uint32_t xf_lazy_check(uint64_t q2) {
   const uint32_t c = (uint32_t)q2 ^ (uint32_t)(q2 >> 32) ^ 0xA5A5A5A5u;
   return c ? c : 1u;
 }
+// The imported weight stands for w until the first optimizer step after the import folds in; that step can leave the
+// state word as it was (a residual sum of exactly 0), so the check alone cannot end it.  The batch that first opens
+// the row therefore re-marks it with its own tag (xf_lazy_mark_open): check = (top half of the digest, complemented)
+// << 16 | tag, valid only while the row's tag is still that batch's, i.e. until the next batch opens the row and folds
+// the step.  A row that was never opened since the import keeps the plain digest (tag 0).
+__device__ __forceinline__ uint32_t xf_lazy_open_check(uint64_t q2, uint32_t tag) {
+  return (((xf_lazy_check(q2) >> 16) ^ 0xFFFFu) << 16) | tag;
+}
+// does bytes 8..15 (q1) hold a weight that stands for w of the lazy row (q2, q3)?
+__device__ __forceinline__ bool xf_lazy_given(uint64_t q1, uint64_t q2, uint64_t q3) {
+  const uint32_t c = (uint32_t)(q1 >> 32), tag = (uint32_t)(q3 & XF_TAG_MASK);
+  return c == xf_lazy_check(q2) || (tag != 0u && c == xf_lazy_open_check(q2, tag));
+}
+// After the deposit that opened a row for batch `seq` from the look (q1, q2, q3): a row still carrying its imported
+// weight unopened (tag 0) is re-marked for seq (a 32-bit store of the check; readers in between accept either form).
+__device__ __forceinline__ void xf_lazy_mark_open(uint8_t* rowp, uint64_t q1, uint64_t q2, uint64_t q3, uint32_t seq) {
+  if ((q3 & XF_TAG_MASK) == 0ull && (uint32_t)(q1 >> 32) == xf_lazy_check(q2))
+    *reinterpret_cast<uint32_t*>(rowp + 12) = xf_lazy_open_check(q2, seq);
+}
 // What batch `seq` pulls from a lazy row whose second half is (q2, q3): the weight with the pending optimizer
 // step (the Push of the batch named by the tag, gradient = (float)(residual sum) / rows, lr_worker.cc:116-118)
 // applied.  q2_new = the first word the row gets when it is opened (its state after that step).  Pure.
@@ -561,7 +581,7 @@ __device__ __forceinline__ float xf_lazy_fold(const XfTableView& t, uint64_t q1,
   const float a = __uint_as_float((uint32_t)q2), b = __uint_as_float((uint32_t)(q2 >> 32));
   if (t.opt == XF_OPT_FTRL) {
     float n = a, z = b;
-    float w = ((uint32_t)(q1 >> 32) == xf_lazy_check(q2)) ? __uint_as_float((uint32_t)q1) : xf_ftrl_w(t, z, n);
+    float w = xf_lazy_given(q1, q2, q3) ? __uint_as_float((uint32_t)q1) : xf_ftrl_w(t, z, n);
     if (pending) xf_ftrl_coord(t, g, w, n, z);
     q2_new = (uint64_t)__float_as_uint(n) | ((uint64_t)__float_as_uint(z) << 32);
     return w;
