@@ -121,6 +121,7 @@ class XF_CXX_API WorkerBase {
   uint64_t loader_block_ = 0;
   xf_trainer* trainer_ = nullptr;
   uint32_t trainer_rows_ = 0, trainer_nnz_ = 0;
+  xf_pv* pv_ = nullptr;           // XFLOW_PROGRESSIVE = 1: the training steps' progressive validation
   // current block (valid inside batch_training / predict)
   const uint32_t* cur_row_ptr_ = nullptr;
   const uint64_t* cur_keys_ = nullptr;

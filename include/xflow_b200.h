@@ -21,6 +21,7 @@
  *   6. serving model          xf_model_*   = a trained table frozen for prediction only (no reference counterpart:
  *                                            the reference predicts on its training servers, lr_worker.cc:25-77)
  *   7. serving model deltas   xf_model_diff / _apply_delta, xf_delta_* = one model carried to the next
+ *   8. progressive validation xf_pv_*      = each training row scored before its step learns from it
  */
 #ifndef XFLOW_B200_H_
 #define XFLOW_B200_H_
@@ -826,6 +827,72 @@ XF_DLL int xf_delta_save(xf_delta* d, const char* path);
 XF_DLL int xf_delta_load(xf_delta** out, const char* path, int device);
 XF_DLL int xf_delta_get_info(xf_delta* d, xf_delta_info* out);
 XF_DLL int xf_delta_destroy(xf_delta* d);
+
+/* ------------------------------------------------------------------------------------------------
+ * 8. Progressive validation (csrc/validate.cu).  Each training row is scored by the model as it stood just before
+ *    the step that trains on it; the weighted mean over the stream estimates hold-out quality without setting data
+ *    aside (Blum, Kalai and Langford 1999; McMahan et al. 2013).  An xf_pv is a streaming, binned metric in constant
+ *    device memory whose report depends only on the multiset of (p, label, e) added to it: not on call boundaries,
+ *    streams, grid shape or atomic order.  Every accumulator is an integer.
+ *
+ *    Rows.  A row (p, label, e), label != 0 positive, e its weight (1 when no weights are given):
+ *      - e == 0 (either sign): adds nothing;
+ *      - e NaN, infinite, negative or >= 2^31: counted in overflow_rows, adds nothing else;
+ *      - p NaN: counted in nan_rows, adds nothing else;
+ *      - otherwise the row is scored: rows, positives or negatives count it.
+ *    Binning, with m = mantissa_bits and pc = p clamped to [2^-20, 1] (float; xf_sigmoid already returns values in
+ *    [1e-6, 1], so the clamp never changes a step's prediction):
+ *      bin(pc) = (bits(pc) >> (23 - m)) - (bits(2^-20) >> (23 - m)),  20 * 2^m + 1 bins, in the order of p.
+ *    Fixed-point sums, unit 2^-32, each row's term rounded to nearest even after exact scaling:
+ *      per bin and class   the row count (u64) and the weight mass sum e (128 bits);
+ *      globally            sum e * l (192 bits) and sum e * pc (128 bits), where l = -ln(q) for a positive row and
+ *                          -ln(1 - q) for a negative one, q = p clamped to [1e-15, 1 - 1e-15] in double (the clamp of
+ *                          xf_metric's out[4]), e * l rounded once in double; e * pc is exact in double.
+ *    No sum can wrap before 2^64 rows.  Memory: 48 bytes per bin (about 1 MB at m = 10, 63 MB at m = 16).  An add
+ *    aggregates the rows of a warp that share a bin and class before its atomics (__match_any_sync).
+ *
+ *    Report.  With W+ and W- the exact weight masses and W = W+ + W-:
+ *      weight_pos, weight_neg   W+, W- correctly rounded to double;
+ *      logloss = sum e l / W,  mean_pctr = sum e pc / W,  ctr = W+ / W   (exact ratios, correctly rounded; NaN if W = 0);
+ *      auc_lo = sum_b W-_b W+_{>b} / (W+ W-),  auc_hi = auc_lo + sum_b W-_b W+_b / (W+ W-),  auc = their midpoint,
+ *      over the bins in ascending order, in double on the device (a scan over the bins, then one reduction in a fixed
+ *      order); NaN if W+ or W- is 0.  The exact weighted AUC of the raw floats with ties counted 1/2 lies in
+ *      [auc_lo, auc_hi]: the bin width m chooses is the error bar.  Equal inputs give identical report bytes.
+ *
+ *    Training.  xf_trainer_set_validation attaches a pv to a trainer: every later TRAINING step (every entry point:
+ *    _host, _device, _host_async, _host_ids_async, _ingested, the _weighted pair, _values, _fields; LR lazy or eager,
+ *    FM, canonical FM, MVM) adds, for each of its rows, the pctr it computed from the table before its update, the
+ *    row's label and its effective weight e_r (importance weighting, section 3; 1 without weighting).  Rows that
+ *    weighting skips (e_r = 0) add nothing.  Predict never adds.  The step kernels store their predictions and one more
+ *    kernel scores them on the table's stream: xf_trainer_launches counts +1 per step while a pv is attached.
+ *    Attaching changes no bit of training: tables, state images and every other output are those of a run without.
+ *    Not in the state image: a resumed run starts its pv afresh.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct xf_pv xf_pv;
+/* the report of xf_pv_report; a struct tag only (like POSIX's struct stat), the function has the name */
+struct xf_pv_report {
+  uint64_t rows;            /* scored rows = positives + negatives */
+  uint64_t positives, negatives, nan_rows, overflow_rows;
+  double weight_pos, weight_neg;
+  double logloss, mean_pctr, ctr;
+  double auc, auc_lo, auc_hi;
+};
+/* a pv on `device` with 20 * 2^mantissa_bits + 1 bins; mantissa_bits 4 .. 16, else XF_ERR_ARG */
+XF_DLL int xf_pv_create(xf_pv** out, int device, uint32_t mantissa_bits);
+/* XF_ERR_STATE while a trainer has it attached */
+XF_DLL int xf_pv_destroy(xf_pv* pv);
+/* clears every sum, stream-ordered after every add enqueued so far; later adds come after it */
+XF_DLL int xf_pv_reset(xf_pv* pv);
+/* n predictions, labels (!= 0 positive) and weights (NULL: all 1) in device memory on pv's device; asynchronous on
+ * cuda_stream (cudaStream_t or NULL): the arrays must stay untouched until that stream has run the add */
+XF_DLL int xf_pv_add_device(xf_pv* pv, const float* d_pctr, const uint8_t* d_labels, const float* d_weights,
+                            uint64_t n, void* cuda_stream);
+/* waits for every add enqueued so far, on any stream; does not reset */
+XF_DLL int xf_pv_report(xf_pv* pv, struct xf_pv_report* out);
+/* every later training step of tr feeds pv (above); NULL detaches.  XF_ERR_ARG, naming the reason, for a trainer that
+ * runs the sharded step (a comm of more than one rank, or XFLOW_MG_FORCE=1) and for a pv on another device than the
+ * table.  A pv may feed several trainers; the caller resets it (for windows, epochs). */
+XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv);
 
 /* ------------------------------------------------------------------------------------------------
  * 1. Reference C API (src/c_api/c_api.h:26-29), unchanged signatures.

@@ -63,6 +63,13 @@ class TrainerConfig(C.Structure):
     _fields_ = [("model", C.c_int), ("max_rows", C.c_uint32), ("max_nnz", C.c_uint32), ("keep_loss", C.c_int)]
 
 
+class PvReport(C.Structure):
+    _fields_ = [("rows", C.c_uint64), ("positives", C.c_uint64), ("negatives", C.c_uint64), ("nan_rows", C.c_uint64),
+                ("overflow_rows", C.c_uint64), ("weight_pos", C.c_double), ("weight_neg", C.c_double),
+                ("logloss", C.c_double), ("mean_pctr", C.c_double), ("ctr", C.c_double), ("auc", C.c_double),
+                ("auc_lo", C.c_double), ("auc_hi", C.c_double)]
+
+
 # name -> (restype, argtypes); also the list the symbol-export test checks against the header
 _vp, _u64, _u32, _i, _f = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_float
 SIGNATURES = {
@@ -183,6 +190,12 @@ SIGNATURES = {
     "xf_delta_load": (_i, [_vp, C.c_char_p, _i]),
     "xf_delta_get_info": (_i, [_vp, _vp]),
     "xf_delta_destroy": (_i, [_vp]),
+    "xf_pv_create": (_i, [_vp, _i, _u32]),
+    "xf_pv_destroy": (_i, [_vp]),
+    "xf_pv_reset": (_i, [_vp]),
+    "xf_pv_add_device": (_i, [_vp, _vp, _vp, _vp, _u64, _vp]),
+    "xf_pv_report": (_i, [_vp, _vp]),
+    "xf_trainer_set_validation": (_i, [_vp, _vp]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
     "XFCreateEx": (_i, [_vp, C.c_char_p, C.c_char_p, _i, _i, _i, _i]),
@@ -678,6 +691,44 @@ class Comm:
             self.h = None
 
 
+class ProgressiveValidation:
+    """A streaming, binned metric on the device (xf_pv_*): 20 * 2^mantissa_bits + 1 bins of the prediction, exact
+    integer sums, a report that depends only on the rows added.  Fed by add_device or by Trainer.set_validation."""
+
+    def __init__(self, device=0, mantissa_bits=10):
+        self.device = device
+        self.h = C.c_void_p()
+        _check(lib().xf_pv_create(C.byref(self.h), int(device), int(mantissa_bits)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            _check(lib().xf_pv_destroy(self.h))
+            self.h = None
+
+    def __del__(self):
+        if getattr(self, "h", None):
+            lib().xf_pv_destroy(self.h)
+            self.h = None
+
+    def add_device(self, d_pctr, d_labels, n, d_weights=None, stream=0):
+        """n predictions (float32), labels (uint8) and weights (float32 or None: all 1) at device addresses."""
+        _check(lib().xf_pv_add_device(self.h, _p(d_pctr), _p(d_labels), _p(d_weights) if d_weights else None, int(n),
+                                      _p(stream) if stream else None))
+
+    def report_bytes(self):
+        """The raw struct xf_pv_report, for byte comparisons."""
+        r = PvReport()
+        _check(lib().xf_pv_report(self.h, C.byref(r)))
+        return bytes(r)
+
+    def report(self):
+        r = PvReport.from_buffer_copy(self.report_bytes())
+        return {name: getattr(r, name) for name, _ in PvReport._fields_}
+
+    def reset(self):
+        _check(lib().xf_pv_reset(self.h))
+
+
 class Trainer:
     def __init__(self, table, model=MODEL_LR, max_rows=65536, max_nnz=65536 * 64, keep_loss=False, comm=None):
         cfg = TrainerConfig(model, max_rows, max_nnz, 1 if keep_loss else 0)
@@ -727,6 +778,12 @@ class Trainer:
     def set_negative_sampling(self, rate, seed=0):
         """Keep each negative row of every later training step with probability `rate`, weighted 1 / rate (1: off)."""
         _check(lib().xf_trainer_set_negative_sampling(self.h, float(rate), int(seed)))
+
+    def set_validation(self, pv):
+        """Every later training step adds its rows' pre-update predictions to `pv` (a ProgressiveValidation); None
+        detaches.  The trainer keeps a reference so that the pv outlives the attachment."""
+        _check(lib().xf_trainer_set_validation(self.h, pv.h if pv is not None else None))
+        self.pv = pv
 
     def skipped_rows(self):
         """Rows trained with effective weight 0 since the trainer was created."""

@@ -878,6 +878,7 @@ XF_DLL int xf_trainer_destroy(xf_trainer* tr) {
   cudaSetDevice(tr->table->cfg.device);
   cudaStreamSynchronize(tr->table->stream);
   cudaStreamSynchronize(tr->copy_stream);
+  if (tr->pv) xf_pv_detach(tr->pv);
   if (tr->mg) xf_mg_destroy(tr);
   for (int i = 0; i < 2; ++i) {
     XfBatchBuf& b = tr->buf[i];
@@ -1027,7 +1028,8 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   XfWeightView wv{nullptr, nullptr};
   if (mode == 0) XF_TRY(xf_row_weights(tr, d_row_ptr, d_keys, d_labels, d_w, rows, &wv));
   float* loss_out = (mode == 0 && tr->cfg.keep_loss) ? tr->loss.as<float>() : nullptr;
-  float* pctr_out = mode == 1 ? tr->pctr.as<float>() : nullptr;
+  // training keeps its predictions only for an attached pv (xf_trainer_set_validation)
+  float* pctr_out = (mode == 1 || tr->pv) ? tr->pctr.as<float>() : nullptr;
   uint32_t extra = 0;  // eager: touched[] positions past the tokens (the FM hot-key cache's flushes)
   if (t->view.lazy) {
     // one kernel: the optimizer step of earlier batches is folded in as rows are touched
@@ -1062,6 +1064,11 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     ++tr->launches;
   }
   if (prof) XF_CUDA_TRY(cudaEventRecord(pe[3], st));
+  if (mode == 0 && tr->pv) {
+    // the rows' pre-update predictions, labels and effective weights (NULL: all 1) into the pv
+    XF_TRY(xf_pv_add_device(tr->pv, pctr_out, d_labels, wv.e, rows, st));
+    ++tr->launches;
+  }
   if (mode == 0) xf_admit_after_step(tr, adm, nnz);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
@@ -1291,6 +1298,21 @@ XF_DLL int xf_trainer_skipped_rows(xf_trainer* tr, uint64_t* skipped) {
   XF_CUDA_TRY(cudaMemcpyAsync(&n, tr->d_wstat + 1, sizeof(n), cudaMemcpyDeviceToHost, tr->table->stream));
   XF_CUDA_TRY(cudaStreamSynchronize(tr->table->stream));
   *skipped = n;
+  return XF_OK;
+}
+
+// ---- progressive validation (validate.cu): the pv every later training step feeds
+XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv) {
+  if (!tr) return XF_ERR_ARG;
+  if (pv && tr->mg) {
+    xf_set_error("xf_trainer_set_validation: progressive validation is single-GPU only: the sharded step does not keep "
+                 "its rows' predictions");
+    return XF_ERR_ARG;
+  }
+  if (pv == tr->pv) return XF_OK;
+  if (pv) XF_TRY(xf_pv_attach(pv, tr->table->cfg.device));
+  if (tr->pv) xf_pv_detach(tr->pv);
+  tr->pv = pv;
   return XF_OK;
 }
 

@@ -134,6 +134,8 @@ struct xf_trainer {
   uint64_t neg_seed = 0;
   XfDevBuf row_w;
   unsigned long long* d_wstat = nullptr;
+  // progressive validation (xf_trainer_set_validation, validate.cu): the pv every training step feeds, or nullptr
+  xf_pv* pv = nullptr;
   // device-side ingest (xf_trainer_ingest_begin / _end): two sets of {raw text, the block's CSR}, so that
   // block i+1 is copied and parsed on the ingest stream while block i is being trained on the table stream
   struct IngestSet {
@@ -189,6 +191,11 @@ int xf_launch_hash_ids(const uint32_t* d_ids, uint32_t n, uint64_t* d_keys, cuda
 // capi.cu: XF_ERR_ARG unless [row_start, row_end) lies in the current ingested block (sharded: is all of it)
 int xf_ingested_range(xf_trainer* tr, uint32_t row_start, uint32_t row_end);
 int xf_trainer_forward_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row_end);
+
+// validate.cu: a trainer whose table lives on `device` starts (XF_ERR_ARG, naming both devices, if pv lives on
+// another) or stops feeding pv; xf_pv_destroy refuses a pv that trainers feed
+int xf_pv_attach(xf_pv* pv, int device);
+void xf_pv_detach(xf_pv* pv);
 
 // multi-GPU pieces implemented in comm.cu
 int xf_mg_create(xf_trainer* tr);

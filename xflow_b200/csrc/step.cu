@@ -127,10 +127,8 @@ xf_k_step(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* _
       arg = __fadd_rn(wx, v_y);
     }
     const float pctr = xf_sigmoid(arg);
-    if (mode == 1) {
-      if (lane == 0 && pctr_out) pctr_out[row] = pctr;
-      continue;
-    }
+    if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
+    if (mode == 1) continue;
     float loss = __fsub_rn(pctr, (float)labels[row]);  // lr_worker.cc:141 ; fm_worker.cc:200
     if (lane == 0 && loss_out) loss_out[row] = loss;
     if (WEIGHT) loss = __fmul_rn(__ldg(wv.e + row), loss);

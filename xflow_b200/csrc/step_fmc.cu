@@ -76,10 +76,8 @@ xf_k_step_fmc(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
     Q = xf_warp_sum(Q);
     wx = xf_warp_sum(wx);
     const float pctr = xf_sigmoid(wx + 0.5f * (s2 - Q));
-    if (mode == 1) {
-      if (lane == 0 && pctr_out) pctr_out[row] = pctr;
-      continue;
-    }
+    if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
+    if (mode == 1) continue;
     const float loss = pctr - (float)labels[row];
     if (lane == 0 && loss_out) loss_out[row] = loss;
     abs_acc += fabsf(loss);

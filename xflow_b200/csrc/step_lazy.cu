@@ -207,9 +207,8 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
     if (summer) {
       const float wx = xf_warp_sum(wsum);
       const float pctr = xf_sigmoid(wx);
-      if (mode == 1) {
-        if (lane == 0 && pctr_out) pctr_out[row] = pctr;
-      } else {
+      if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
+      if (mode == 0) {
         float loss = __fsub_rn(pctr, (float)label);  // lr_worker.cc:141
         if (lane == 0 && loss_out) loss_out[row] = loss;
         if (WEIGHT) loss = __fmul_rn(__ldg(wv.e + row), loss);  // read again: not kept live through phase A

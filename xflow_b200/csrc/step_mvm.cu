@@ -88,8 +88,8 @@ xf_k_step_mvm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
       for (unsigned m = present; m; m &= m - 1) P *= S[__ffs(m) - 1][lane];
     }
     const float pctr = xf_sigmoid(xf_warp_sum(P));
+    if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
     if (mode == 1) {
-      if (lane == 0 && pctr_out) pctr_out[row] = pctr;
       __syncwarp();
       continue;
     }

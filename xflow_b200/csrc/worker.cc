@@ -130,6 +130,18 @@ static float NegSampleFromEnv(int world) {
   return (float)r;
 }
 
+// Progressive validation (xf_pv_*, xf_trainer_set_validation): XFLOW_PROGRESSIVE = 1 scores every training row with
+// the model as it stood before the step that trains on it, and prints one line per epoch, then starts afresh.  Single
+// GPU only.
+static bool ProgressiveFromEnv(int world) {
+  const char* e = getenv("XFLOW_PROGRESSIVE");
+  if (!e || !*e || strcmp(e, "0") == 0) return false;
+  if (strcmp(e, "1") != 0) throw std::runtime_error(std::string("XFLOW_PROGRESSIVE must be 0 or 1, got '") + e + "'");
+  if (world > 1)
+    throw std::runtime_error("XFLOW_PROGRESSIVE is single-GPU only: unset it or run with XFLOW_WORLD = 1");
+  return true;
+}
+
 // the table's training-batch number (host state, no device sync)
 static uint64_t TableBatches(xf_table* t) {
   uint64_t b = 0;
@@ -292,6 +304,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   uint64_t every = 0;
   EvictionFromEnv(world_, &every);  // likewise XFLOW_EVICT_*
   NegSampleFromEnv(world_);         // and XFLOW_NEG_SAMPLE
+  ProgressiveFromEnv(world_);       // and XFLOW_PROGRESSIVE
   env_path("XFLOW_CHECKPOINT", world_);
   env_path("XFLOW_RESUME", world_);
   env_path("XFLOW_EXPORT_MODEL", world_);
@@ -393,6 +406,7 @@ WorkerBase::WorkerBase(const char* train_file, const char* test_file, int model)
 
 WorkerBase::~WorkerBase() {
   if (trainer_) xf_trainer_destroy(trainer_);
+  if (pv_) xf_pv_destroy(pv_);
   if (loader_) xf_loader_close(loader_);
 }
 
@@ -419,6 +433,7 @@ void WorkerBase::ensure_trainer(uint32_t rows, uint32_t nnz) {
   if (neg_rate < 1.f)
     must(xf_trainer_set_negative_sampling(trainer_, neg_rate, (uint64_t)env_int("XFLOW_SEED", 0)),
          "xf_trainer_set_negative_sampling");
+  if (pv_) must(xf_trainer_set_validation(trainer_, pv_), "xf_trainer_set_validation");
   trainer_rows_ = cfg.max_rows;
   trainer_nnz_ = cfg.max_nnz;
 }
@@ -528,6 +543,16 @@ void WorkerBase::run_blocks(uint64_t collective_blocks, const std::function<void
   }
 }
 
+// one line per epoch: the progressive metric of that epoch's training rows (%.17g: the report's doubles exactly)
+static void PrintProgressive(xf_pv* pv, int epoch) {
+  struct xf_pv_report r;
+  must(xf_pv_report(pv, &r), "xf_pv_report");
+  printf("progressive epoch %d : logloss = %.17g  auc = %.17g [%.17g, %.17g]  mean_pctr = %.17g  ctr = %.17g  "
+         "rows = %llu\n", epoch, r.logloss, r.auc, r.auc_lo, r.auc_hi, r.mean_pctr, r.ctr, (unsigned long long)r.rows);
+  fflush(stdout);
+  must(xf_pv_reset(pv), "xf_pv_reset");
+}
+
 void WorkerBase::batch_training() {
   const bool host_parse = env_int("XFLOW_HOST_PARSE", 0) != 0 && !comm_;
   const uint64_t block_bytes = (uint64_t)block_size << 20;
@@ -543,6 +568,10 @@ void WorkerBase::batch_training() {
     CheckResumedPolicies(table_);
   } else {
     must(xf_trainer_init_push(trainer_), "xf_trainer_init_push");  // lr_worker.cc:180-182
+  }
+  if (!pv_ && ProgressiveFromEnv(1)) {  // XFLOW_WORLD > 1 was refused at Server creation
+    must(xf_pv_create(&pv_, Server::Get()->device(), 10), "xf_pv_create");
+    must(xf_trainer_set_validation(trainer_, pv_), "xf_trainer_set_validation");
   }
   uint64_t collective_blocks = 0;
   if (comm_) {
@@ -575,6 +604,7 @@ void WorkerBase::batch_training() {
       for (int i = 0; i < core_num; ++i) update(i * thread_size, (i + 1) * thread_size);  // :192-196
     }
     must(xf_trainer_sync(trainer_), "xf_trainer_sync");
+    if (pv_) PrintProgressive(pv_, epoch);
     if (!checkpoint.empty())
       must(xf_table_save_state(table_, checkpoint.c_str(), (uint64_t)epoch + 1), "xf_table_save_state");
     if (!deltas.empty()) ExportEpoch(table_, deltas, (uint64_t)epoch + 1, exported);
