@@ -238,7 +238,9 @@ XF_DLL int xf_table_last_touch(xf_table* t, const uint64_t* keys, uint64_t n, ui
  * tables' pending-step ring, the config fields that define the rows and their arithmetic, and the caller's `user`
  * value (the CLI stores the epochs done there).  A table loaded from it is byte-identical to the saved one and trains
  * on bit for bit as the saved table would have: a run that saves and continues, and a run resumed from the image,
- * both equal the run that never saved.  Not in the image: the trainers' state (xf_trainer_stats counters, the
+ * both equal the run that never saved.  For XF_MODEL_FM_CANONICAL and XF_MODEL_MVM that holds on batches with repeated
+ * keys in deterministic mode (xf_trainer_set_deterministic); their default steps sum a repeated key's terms in atomic
+ * order.  Not in the image: the trainers' state (xf_trainer_stats counters, the
  * negative-sampling policy, which is caller config) and xf_table_set_stream's choice.
  * Save runs stream-ordered after everything enqueued on the table's stream, waits for it, and changes nothing in the
  * table.  It writes <path>.tmp and renames it to <path>; on failure no .tmp is left.  Saving the same state twice
@@ -338,6 +340,43 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
 XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
                                           const uint8_t* fields, const float* vals, uint32_t rows, uint32_t nnz,
                                           float* pctr_out);
+/* Deterministic mode for XF_MODEL_FM_CANONICAL and XF_MODEL_MVM trainers (csrc/step_det.cu).  The default steps of
+ * these two models add each token's gradient terms into its key's accumulators with float atomics (and the machine's
+ * forward adds a row's same-field terms with shared-memory atomics), so a key with several tokens in a batch gets bits
+ * that depend on the order the atomics land in.  on != 0: every later step of tr, training and predict, sums in one
+ * fixed order instead; on = 0 restores the default kernels.  LR and FM trainers are refused (XF_ERR_ARG): their
+ * per-key sums are fixed point or f64 already and this mode does not change them.  Turning the mode on allocates its
+ * scratch for the trainer's max_rows / max_nnz: canonical FM 4K + 4 bytes per row and 20 bytes per token, the machine
+ * 4 bytes per row and 4K + 16 bytes per token; both about K / 4 + 5 more bytes per token for the run sums of keys with
+ * more than 32 tokens, and the sort's temporary storage.  If that fails the call returns XF_ERR_CUDA and the trainer is
+ * unchanged.  The switch waits for the table's stream.
+ *   1. Per-token terms, today's op for op.  Canonical FM, token j of row r (residual r, value x): A term
+ *      fl(fl(r x) S_k), G term (double)r (double)x, L2 term (double)r (double)x (double)x.  The machine: A term
+ *      fl(fl(r x) o_k), o_k the product of the other present fields' sums in ascending field order from 1; g term +0.0.
+ *   2. Association.  Each key's tokens in ascending position in the batch's token array, cut into consecutive runs of
+ *      32.  A run is summed by a butterfly: term i in lane i, -0.0 (the exact additive identity) in the lanes past the
+ *      run; for o = 16, 8, 4, 2, 1: a_i = a_i + a_(i^o); the run's sum is a_0.  The run sums are then added in order
+ *      onto the row's accumulator as it stood (g from -0.0, A and L2 from +0).  Every add rounds to nearest, no FMA,
+ *      no flush; A in float, G and L2 in double.  So the result depends only on the table before the step and on the
+ *      batch, not on grid, scheduling, streams or the other keys; a key with one token in the batch gets exactly the
+ *      bits of the default step.
+ *   3. The machine's forward, training and predict, is the frozen model's (section 6, "Forward, row r"): field sums as
+ *      a left fold in token order from +0, P_k over the present fields ascending, y by the xor 16 .. 1 tree.  With the
+ *      mode on, xf_trainer_predict_host_fields returns on every row, bit for bit, what xf_model_predict_host_fields
+ *      returns on a model frozen from the table at that moment.  The canonical FM's forward has a fixed order already
+ *      (lane-sequential passes, then a shuffle tree) and is unchanged.
+ *   4. mean_abs_loss and the _async abs-loss sum: thread t of 256 adds the rows' |r| for rows t, t + 256, ... in row
+ *      order from +0, then the 256 partial sums are added as s_i = s_i + s_(i+o) for o = 128, 64, .., 1; s_0 is the
+ *      sum.  The order depends only on the row count.
+ *   5. Reproducible, per key: xf_table_export of every key, the set of keys, xf_trainer_get_loss, predictions,
+ *      xf_trainer_stats and pv reports; two runs on the same batches freeze to byte-identical xf_model_save files.  Not
+ *      per slot: a key's slot depends on insertion races between keys.
+ *   6. Kernels per training step with tokens (xf_trainer_launches): the step kernel, the radix sort's (1 up to 4864
+ *      tokens, else 2 + ceil((log2(capacity) + 1) / 8)), three for the per-key sums, the optimizer pass, and one more
+ *      for the abs-loss sum on the host-batch entry points (_host_values, _host_fields, the _async ones, which report
+ *      it); a pv adds its one.  Predict
+ *      launches one kernel, as without the mode. */
+XF_DLL int xf_trainer_set_deterministic(xf_trainer* tr, int on);
 /* Importance-weighted training (McMahan et al., "Ad Click Prediction: a View from the Trenches", section 6.1):
  * per-row weights and negative subsampling for XF_MODEL_LR / XF_MODEL_FM.  Each row r of a training step has an
  * effective weight e_r = c_r * s_r (float product, rounded to nearest):
@@ -591,8 +630,9 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *      the row's first), whose order among contending lanes the hardware picks, and token order is one of those
  *      orders.  So the model returns, bit for bit, what the table's predict returns at the moment of the freeze (under
  *      ZERO: with zero rows imported for the absent keys) on every row where no field has more than two tokens (0 + a
- *      + b is commutative) or no pass holds two tokens of one field.  On other rows the table's own result is not
- *      reproducible, and the model's is the order above, the same bits on every call and every entry point.
+ *      + b is commutative) or no pass holds two tokens of one field.  On other rows the table's own default result is not
+ *      reproducible, and the model's is the order above, the same bits on every call and every entry point; in
+ *      deterministic mode (xf_trainer_set_deterministic) the table's predict is this order on every row.
  *      The XFSM and XFSD files keep version 1 and record fm = 3, latent_dim and these row bytes; a load refuses a
  *      non-zero byte 8 .. 15 or padding byte.  Diff, apply and convert serve these models as canonical ones (a
  *      canonical model and a multi-view machine's differ in fm and are never diffed or applied to one another);

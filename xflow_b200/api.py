@@ -196,6 +196,7 @@ SIGNATURES = {
     "xf_pv_add_device": (_i, [_vp, _vp, _vp, _vp, _u64, _vp]),
     "xf_pv_report": (_i, [_vp, _vp]),
     "xf_trainer_set_validation": (_i, [_vp, _vp]),
+    "xf_trainer_set_deterministic": (_i, [_vp, _i]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
     "XFCreateEx": (_i, [_vp, C.c_char_p, C.c_char_p, _i, _i, _i, _i]),
@@ -784,6 +785,11 @@ class Trainer:
         detaches.  The trainer keeps a reference so that the pv outlives the attachment."""
         _check(lib().xf_trainer_set_validation(self.h, pv.h if pv is not None else None))
         self.pv = pv
+
+    def set_deterministic(self, on=True):
+        """Canonical FM / multi-view machine trainers: sum each key's gradient in token order (xf_trainer_set_deterministic),
+        so that runs on the same batches give the same bits; False restores the default atomic kernels."""
+        _check(lib().xf_trainer_set_deterministic(self.h, 1 if on else 0))
 
     def skipped_rows(self):
         """Rows trained with effective weight 0 since the trainer was created."""

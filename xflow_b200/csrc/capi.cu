@@ -888,6 +888,7 @@ XF_DLL int xf_trainer_destroy(xf_trainer* tr) {
     cudaEventDestroy(b.copied); cudaEventDestroy(b.consumed); cudaEventDestroy(b.staged);
   }
   tr->touched.release(); tr->loss.release(); tr->pctr.release(); tr->rejected.release(); tr->row_w.release();
+  if (tr->det) { tr->det->release(); delete tr->det; }
   cudaStreamSynchronize(tr->ing_copy_stream);
   cudaStreamSynchronize(tr->ing_stream);
   for (int i = 0; i < 2; ++i) {
@@ -1042,7 +1043,13 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
     if (mvm && !d_fields && nnz) { xf_set_error("XF_MODEL_MVM steps need the tokens' field ids (xf_trainer_step_host_fields)"); return XF_ERR_ARG; }
     extra = canon ? 0u : xf_step_touched_extra(t->view.K, (int)rows);
     XF_TRY(tr->touched.ensure(((size_t)nnz + extra) * 4));
-    if (mvm)
+    // deterministic mode: every training step, and the machine's predict (the canonical FM's forward has a fixed
+    // order already, so its predict stays xf_k_step_fmc's)
+    if (tr->det && (mode == 0 || mvm)) {
+      XF_TRY(xf_det_step(t->view, *tr->det, mvm, d_row_ptr, d_keys, d_vals, d_fields, d_labels, rows, nnz, mode,
+                         tr->touched.as<uint32_t>(), loss_out, pctr_out, d_abs, st));
+      if (mode == 0) tr->launches += xf_det_extra_launches(nnz, t->view.log2cap, d_abs != nullptr);
+    } else if (mvm)
       xf_launch_step_mvm(t->view, d_row_ptr, d_keys, d_fields, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
                          loss_out, pctr_out, d_abs, st);
     else if (canon)
@@ -1313,6 +1320,38 @@ XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv) {
   if (pv) XF_TRY(xf_pv_attach(pv, tr->table->cfg.device));
   if (tr->pv) xf_pv_detach(tr->pv);
   tr->pv = pv;
+  return XF_OK;
+}
+
+// ---- deterministic mode (step_det.cu): per-key sums in token order for the canonical FM and the multi-view machine
+XF_DLL int xf_trainer_set_deterministic(xf_trainer* tr, int on) {
+  if (!tr) return XF_ERR_ARG;
+  if (tr->cfg.model != XF_MODEL_FM_CANONICAL && tr->cfg.model != XF_MODEL_MVM) {
+    xf_set_error("xf_trainer_set_deterministic: XF_MODEL_FM_CANONICAL and XF_MODEL_MVM only: the LR and FM steps sum "
+                 "each key's gradient in fixed point or f64 already, in an order that does not change the result, and "
+                 "this mode would not change them");
+    return XF_ERR_ARG;
+  }
+  if ((on != 0) == (tr->det != nullptr)) return XF_OK;
+  XF_CUDA_TRY(cudaSetDevice(tr->table->cfg.device));
+  // the steps enqueued so far may still use the scratch (off) or the old kernels' state; both modes leave the
+  // accumulators clear after every step, so the switch needs nothing else
+  XF_CUDA_TRY(cudaStreamSynchronize(tr->table->stream));
+  if (!on) {
+    tr->det->release();
+    delete tr->det;
+    tr->det = nullptr;
+    return XF_OK;
+  }
+  XfDetBufs* d = new XfDetBufs;
+  const int r = d->alloc(tr->cfg.model == XF_MODEL_MVM, tr->table->view.K, tr->cfg.max_rows, tr->cfg.max_nnz);
+  if (r != XF_OK) {
+    d->release();
+    delete d;
+    cudaGetLastError();  // a failed cudaMalloc is not sticky: later calls must not report it
+    return r;
+  }
+  tr->det = d;
   return XF_OK;
 }
 

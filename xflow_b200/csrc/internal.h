@@ -104,6 +104,26 @@ struct xf_table {
   int check_error();
 };
 
+// deterministic training steps (xf_trainer_set_deterministic, step_det.cu): the scratch of one step, allocated for the
+// trainer's max_rows / max_nnz when the mode is turned on
+struct XfDetBufs {
+  XfDevBuf keys_in, keys_out, toks_in, toks_out;  // the (slot, token position) pairs before and after the sort
+  XfDevBuf tok_row, row_s;                        // canonical FM: each token's row, each row's S[K]
+  XfDevBuf terms;                                 // multi-view machine: each token's K terms
+  XfDevBuf res;                                   // each row's residual
+  XfDevBuf run_a, run_d, rdesc, longs, cnt;       // segments of more than 32 tokens: their runs' sums
+  XfDevBuf tmp;                                   // the sort's temporary storage
+  int alloc(bool mvm, int K, uint32_t max_rows, uint32_t max_nnz);  // on failure some buffers may be held: release()
+  void release();
+};
+// one deterministic step (mode 0 train, 1 predict: the multi-view machine only); touched[] gets nnz entries
+int xf_det_step(const XfTableView& t, XfDetBufs& b, bool mvm, const uint32_t* row_ptr, const uint64_t* keys,
+                const float* vals, const uint8_t* fields, const uint8_t* labels, uint32_t rows, uint32_t nnz, int mode,
+                uint32_t* touched, float* loss_out, float* pctr_out, float* abs_loss_sum, cudaStream_t st);
+// kernels a deterministic training step launches besides its step kernel and the optimizer pass: the sort's, the
+// three of the per-key sums (none without tokens) and the abs-loss sum's (abs_sum)
+uint64_t xf_det_extra_launches(uint32_t nnz, uint32_t log2cap, bool abs_sum);
+
 struct XfBatchBuf {
   XfDevBuf row_ptr, keys, labels, ids, vals, fields, weights;
   XfPinBuf h_row_ptr, h_keys, h_labels;
@@ -136,6 +156,8 @@ struct xf_trainer {
   unsigned long long* d_wstat = nullptr;
   // progressive validation (xf_trainer_set_validation, validate.cu): the pv every training step feeds, or nullptr
   xf_pv* pv = nullptr;
+  // deterministic mode (xf_trainer_set_deterministic, step_det.cu): its scratch, or nullptr when the mode is off
+  XfDetBufs* det = nullptr;
   // device-side ingest (xf_trainer_ingest_begin / _end): two sets of {raw text, the block's CSR}, so that
   // block i+1 is copied and parsed on the ingest stream while block i is being trained on the table stream
   struct IngestSet {
