@@ -779,6 +779,48 @@ XF_DLL int xf_model_predict_host_fields(xf_model* m, const uint32_t* row_ptr, co
 XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                           const uint8_t* d_fields, const float* d_vals, uint32_t rows, uint32_t nnz,
                                           float* d_pctr_out, void* cuda_stream);
+/* Candidate scoring.  A ranking request scores one context (the user, page and device features) against N candidates,
+ * each with features of its own.  A batch of R requests gives each its context once:
+ *   request q's context is tokens ctx_ptr[q] .. ctx_ptr[q+1] - 1 of ctx_keys (ctx_vals, ctx_fields);
+ *   its candidates are rows cand_ptr[q] .. cand_ptr[q+1] - 1, candidate c being tokens row_ptr[c] .. row_ptr[c+1] - 1
+ *   of keys (vals, fields), with cand_ptr[0] = 0 and cand_ptr[R] = candidates.
+ * Candidate c of request q is scored as the concatenated row "request q's context tokens in order, then row c's
+ * tokens", values and field ids concatenated alike (a NULL vals side reads as every value 1): pctr_out[c] is, bit for
+ * bit, what the model's flat predict returns for that row (xf_model_predict_host / _host_values for LR, FM and
+ * canonical models, _host_fields for multi-view machines; F32 and F16 models, either absent policy, pruned or not).
+ * A request without candidates produces nothing; an empty context gives the flat predict of the candidate rows, an
+ * empty candidate row that of the context.  Values are read by canonical and multi-view machine models only (non-NULL
+ * vals on an LR or FM model: XF_ERR_ARG); field ids are required by multi-view machine models (NULL with tokens: XF_ERR_ARG)
+ * and refused by every other model.
+ * The device folds each context once per run of up to 16 candidates of its request and starts every candidate's forward
+ * from that state, so a context's rows are looked up about N / 16 times rather than N times. */
+typedef struct xf_candidate_batch {
+  uint32_t requests;            /* R */
+  const uint32_t* ctx_ptr;      /* [R + 1] */
+  const uint64_t* ctx_keys;     /* [ctx_nnz] */
+  const float* ctx_vals;        /* [ctx_nnz] or NULL (every value 1); canonical and multi-view machine models only */
+  const uint8_t* ctx_fields;    /* [ctx_nnz]; multi-view machine models only, and required by them */
+  uint32_t ctx_nnz;
+  const uint32_t* cand_ptr;     /* [R + 1]: cand_ptr[0] = 0, cand_ptr[R] = candidates */
+  uint32_t candidates;
+  const uint32_t* row_ptr;      /* [candidates + 1] into keys / vals / fields, as a flat predict's row_ptr */
+  const uint64_t* keys;         /* [nnz] */
+  const float* vals;            /* as ctx_vals */
+  const uint8_t* fields;        /* as ctx_fields */
+  uint32_t nnz;
+} xf_candidate_batch;
+/* _host: host arrays.  Refused with XF_ERR_ARG, naming the cause: null arguments, a decreasing ctx_ptr, cand_ptr or
+ * row_ptr, cand_ptr[0] != 0 or cand_ptr[R] != candidates, ctx_ptr[R] > ctx_nnz or row_ptr[candidates] > nnz, the key
+ * 2^64 - 1 on either side, a field id of 32 or more on either side; a part with XF_ERR_STATE.  Stages the batch through
+ * the model's buffers in one upload (each context once), runs on the model's stream and returns when pctr_out
+ * [candidates] is filled; calls on one model are serialised. */
+XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batch* b, float* pctr_out);
+/* _device: the struct on the host, its arrays in device memory on the model's device.  The contract of
+ * xf_model_predict_device: asynchronous on `cuda_stream`, reads nothing on the host, uses no state of the model but its
+ * rows, any number in flight.  The arrays are the caller's contract (the _host checks are not made; field ids are read
+ * & 31). */
+XF_DLL int xf_model_predict_candidates_device(xf_model* m, const xf_candidate_batch* b, float* d_pctr_out,
+                                              void* cuda_stream);
 /* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL.  On a
  * canonical or multi-view machine's model st and qt must be NULL (XF_ERR_ARG): its rows are read with
  * xf_model_lookup_latent. */

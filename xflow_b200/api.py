@@ -52,6 +52,14 @@ class ModelInfo(C.Structure):
                 ("absent", C.c_int), ("fm", C.c_int), ("precision", C.c_int)]
 
 
+class CandidateBatch(C.Structure):
+    """xf_candidate_batch: R requests, each a context and a run of candidate rows (include/xflow_b200.h)."""
+    _fields_ = [("requests", C.c_uint32), ("ctx_ptr", C.c_void_p), ("ctx_keys", C.c_void_p), ("ctx_vals", C.c_void_p),
+                ("ctx_fields", C.c_void_p), ("ctx_nnz", C.c_uint32), ("cand_ptr", C.c_void_p), ("candidates", C.c_uint32),
+                ("row_ptr", C.c_void_p), ("keys", C.c_void_p), ("vals", C.c_void_p), ("fields", C.c_void_p),
+                ("nnz", C.c_uint32)]
+
+
 class DeltaInfo(C.Structure):
     _fields_ = [("upserts", C.c_uint64), ("deletes", C.c_uint64), ("base_keys", C.c_uint64),
                 ("base_fingerprint", C.c_uint64), ("result_keys", C.c_uint64), ("result_fingerprint", C.c_uint64),
@@ -180,6 +188,8 @@ SIGNATURES = {
     "xf_model_predict_device_values": (_i, [_vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_predict_host_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "xf_model_predict_device_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "xf_model_predict_candidates_host": (_i, [_vp, _vp, _vp]),
+    "xf_model_predict_candidates_device": (_i, [_vp, _vp, _vp, _vp]),
     "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
     "xf_model_lookup_latent": (_i, [_vp, _vp, _u64, _vp, _vp, _vp]),
     "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
@@ -595,6 +605,52 @@ class Model:
         st = C.c_void_p(int(stream)) if stream else None
         _check(lib().xf_model_predict_device_fields(self.h, _p(d_row_ptr), _p(d_keys), _p(d_fields),
                                                     _p(d_vals) if d_vals else None, rows, nnz, _p(d_out), st))
+
+    def predict_candidates(self, ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals=None, vals=None, ctx_fields=None,
+                           fields=None):
+        """Score each request's candidates against its context (xf_model_predict_candidates_host): request q's context
+        is ctx_keys[ctx_ptr[q] .. ctx_ptr[q+1]), its candidates rows cand_ptr[q] .. cand_ptr[q+1] - 1 of the CSR
+        (row_ptr, keys).  Returns float32 [candidates]: for each candidate, the flat predict of its request's context
+        followed by its own tokens, bit for bit.  Values (None: all 1) for canonical and multi-view machine models,
+        field ids for multi-view machine models, on either side."""
+        ctx_ptr = np.ascontiguousarray(ctx_ptr, np.uint32)
+        cand_ptr = np.ascontiguousarray(cand_ptr, np.uint32)
+        row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
+        ctx_keys = np.ascontiguousarray(ctx_keys, np.uint64)
+        keys = np.ascontiguousarray(keys, np.uint64)
+        if ctx_ptr.size != cand_ptr.size or cand_ptr.size < 1:
+            raise ValueError("one context per request: ctx_ptr has %d entries, cand_ptr %d" % (ctx_ptr.size, cand_ptr.size))
+
+        def side(a, dtype, n, what):
+            if a is None:
+                return None
+            a = np.ascontiguousarray(a, dtype)
+            if a.size != n:
+                raise ValueError("one %s per token: %d for %d keys" % (what, a.size, n))
+            return a
+
+        ctx_vals, vals = side(ctx_vals, np.float32, ctx_keys.size, "value"), side(vals, np.float32, keys.size, "value")
+        ctx_fields = side(ctx_fields, np.uint8, ctx_keys.size, "field id")
+        fields = side(fields, np.uint8, keys.size, "field id")
+        n = row_ptr.size - 1
+        out = np.empty(max(n, 0), np.float32)
+        b = CandidateBatch(cand_ptr.size - 1, ctx_ptr.ctypes.data, ctx_keys.ctypes.data,
+                           None if ctx_vals is None else ctx_vals.ctypes.data,
+                           None if ctx_fields is None else ctx_fields.ctypes.data, ctx_keys.size, cand_ptr.ctypes.data, n,
+                           row_ptr.ctypes.data, keys.ctypes.data, None if vals is None else vals.ctypes.data,
+                           None if fields is None else fields.ctypes.data, keys.size)
+        _check(lib().xf_model_predict_candidates_host(self.h, C.byref(b), _p(out)))
+        return out
+
+    def predict_candidates_device(self, requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr,
+                                  d_keys, nnz, d_out, stream=0, d_ctx_vals=0, d_vals=0, d_ctx_fields=0, d_fields=0):
+        """Asynchronous predict_candidates on device pointers (raw addresses) on the CUDA stream `stream`; d_out
+        [candidates].  A 0 address for values reads every value as 1."""
+        st = C.c_void_p(int(stream)) if stream else None
+        a = lambda x: int(x) or None
+        b = CandidateBatch(requests, a(d_ctx_ptr), a(d_ctx_keys), a(d_ctx_vals), a(d_ctx_fields), ctx_nnz, a(d_cand_ptr),
+                           candidates, a(d_row_ptr), a(d_keys), a(d_vals), a(d_fields), nnz)
+        _check(lib().xf_model_predict_candidates_device(self.h, C.byref(b), _p(d_out), st))
 
     def lookup(self, keys):
         """What the model holds for `keys`: dict of w, st, qt (0 for LR) and present."""

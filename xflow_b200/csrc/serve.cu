@@ -352,6 +352,306 @@ static void xf_launch_serve(const xf_model* m, const uint32_t* row_ptr, const ui
   else xf_k_serve<false, false><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, (int)rows, pctr_out);
 }
 
+// ---- candidate scoring: a request's context scored against each of its candidates (xf_model_predict_candidates_*)
+// Candidate c of request q is the row "context q, then row c".  Every forward above is a per-lane (LR, FM, canonical)
+// or per-entry (multi-view machine) left fold over the row's positions in increasing order, so the fold over the context
+// is a prefix of the fold over every such row.  A warp folds the context once and starts each candidate's fold from
+// that state: candidate token i sits at position n_c + i, on the lane (LR, FM) or lane group (canonical) that the flat
+// kernel gives that position, so the result is the flat kernel's on the concatenated row, bit for bit.
+//
+// Work: the candidates in runs of XF_CAND_RUN, a warp per run.  A run that crosses a request boundary is scored a
+// request at a time, each request's context folded once; a warp finds its first request by a binary search over
+// cand_ptr.  Nothing is written but pctr_out.
+#define XF_CAND_RUN 16u
+
+struct XfCandView {
+  const uint32_t* ctx_ptr;
+  const uint64_t* ctx_keys;
+  const float* ctx_vals;
+  const uint8_t* ctx_fields;
+  const uint32_t* cand_ptr;
+  const uint32_t* row_ptr;
+  const uint64_t* keys;
+  const float* vals;
+  const uint8_t* fields;
+  uint32_t requests, candidates;
+};
+
+// the request that holds candidate c: the q < R with cand_ptr[q] <= c < cand_ptr[q + 1] (cand_ptr[0] = 0 <= c <
+// cand_ptr[R])
+__device__ __forceinline__ uint32_t xf_cand_request(const uint32_t* __restrict__ cand_ptr, uint32_t R, uint32_t c) {
+  uint32_t lo = 0, hi = R;
+  while (hi - lo > 1u) {
+    const uint32_t mid = lo + (hi - lo) / 2u;
+    if (__ldg(cand_ptr + mid) <= c) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// The walk every candidate kernel makes: each run of XF_CAND_RUN candidates, split at request boundaries; for each
+// request q met, state = context(q) once, candidate(state, c) for its candidates in the run, then done(state).  The
+// state goes by value, so that it stays in registers.
+template <typename Ctx, typename Cand, typename Done>
+__device__ __forceinline__ void xf_cand_walk(const XfCandView& b, int gwarp, int nwarps, Ctx context, Cand candidate,
+                                             Done done) {
+  const uint32_t runs = (uint32_t)(((uint64_t)b.candidates + XF_CAND_RUN - 1u) / XF_CAND_RUN);
+  for (uint32_t run = (uint32_t)gwarp; run < runs; run += (uint32_t)nwarps) {
+    uint32_t c = run * XF_CAND_RUN;
+    const uint32_t c_end = b.candidates - c > XF_CAND_RUN ? c + XF_CAND_RUN : b.candidates;
+    for (uint32_t q = xf_cand_request(b.cand_ptr, b.requests, c); c < c_end; ++q) {
+      const uint32_t last = min(c_end, __ldg(b.cand_ptr + q + 1));
+      if (c >= last) continue;  // a request without candidates
+      const auto state = context(q);
+      for (; c < last; ++c) candidate(state, c);
+      done(state);
+    }
+  }
+}
+
+// xf_k_serve's loop over the positions [lo, hi) of a row whose token at position p is keys[beg + p - lo]: lane l takes
+// the positions = l (mod 32) in increasing order, two in flight, into its sums
+template <bool FM, bool H>
+__device__ __forceinline__ void xf_serve_fold(const XfTableView& m, int absent, const uint64_t* __restrict__ keys,
+                                              uint32_t beg, uint32_t lo, uint32_t hi, float& wsum, float& ssum,
+                                              float& qsum) {
+  const uint32_t lane = threadIdx.x & 31u;
+  for (uint32_t p0 = lo & ~63u; p0 < hi; p0 += 64u) {
+    const uint32_t pa = p0 + lane, pb = pa + 32u;
+    const bool v0 = pa >= lo && pa < hi, v1 = pb >= lo && pb < hi;
+    const uint64_t k0 = v0 ? __ldcs(keys + beg + (pa - lo)) : 0ull;
+    const uint64_t k1 = v1 ? __ldcs(keys + beg + (pb - lo)) : 0ull;
+    uint64_t a = XF_EMPTY_KEY, b = XF_EMPTY_KEY;
+    float wa = 0.f, sa = 0.f, qa = 0.f, wb = 0.f, sb = 0.f, qb = 0.f;
+    if (v0) xf_serve_load<FM, H>(xf_row(m, xf_home_slot(m, k0)), a, wa, sa, qa);
+    if (v1) xf_serve_load<FM, H>(xf_row(m, xf_home_slot(m, k1)), b, wb, sb, qb);
+    if (v0) xf_serve_token<FM, H>(m, absent, k0, a, wa, sa, qa, wsum, ssum, qsum);
+    if (v1) xf_serve_token<FM, H>(m, absent, k1, b, wb, sb, qb, wsum, ssum, qsum);
+  }
+}
+
+// LR and FM: the context's three sums per lane stay in registers; a candidate's tokens start at position n_c mod 64,
+// which puts each on the lane xf_k_serve gives it
+template <bool FM, bool H>
+__global__ void __launch_bounds__(256)
+xf_k_serve_cand(XfTableView m, int absent, XfCandView b, float* __restrict__ pctr_out) {
+  const int lane = threadIdx.x & 31;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
+  struct Ctx { float wsum, ssum, qsum; uint32_t lo; };
+  xf_cand_walk(b, gwarp, gridDim.x * warps_per_block,
+               [=](uint32_t q) {
+                 const uint32_t beg = __ldg(b.ctx_ptr + q), n = __ldg(b.ctx_ptr + q + 1) - beg;
+                 Ctx x{0.f, 0.f, 0.f, n & 63u};
+                 xf_serve_fold<FM, H>(m, absent, b.ctx_keys, beg, 0u, n, x.wsum, x.ssum, x.qsum);
+                 return x;
+               },
+               [=](const Ctx& x, uint32_t c) {
+                 const uint32_t beg = __ldg(b.row_ptr + c), n = __ldg(b.row_ptr + c + 1) - beg;
+                 float wsum = x.wsum, ssum = x.ssum, qsum = x.qsum;
+                 xf_serve_fold<FM, H>(m, absent, b.keys, beg, x.lo, x.lo + n, wsum, ssum, qsum);
+                 // xf_k_serve's reductions
+                 const float wx = xf_warp_sum(wsum);
+                 float arg = wx;
+                 if (FM) {
+                   const float S = xf_warp_sum(ssum);
+                   const float Q = xf_warp_sum(qsum);
+                   arg = __fadd_rn(wx, __fsub_rn(__fmul_rn(S, S), Q));
+                 }
+                 if (lane == 0) pctr_out[c] = xf_sigmoid(arg);
+               },
+               [](const Ctx&) {});
+}
+
+// xf_k_serve_fmc's loop over the positions [lo, hi) of a row whose token at position p is keys[beg + p - lo] (vals
+// NULL: every value 1): lane group g takes the positions = g (mod T) in increasing order, two passes in flight
+template <int C, bool H>
+__device__ __forceinline__ void xf_fmc_fold(const XfTableView& m, int absent, const uint64_t* __restrict__ keys,
+                                            const float* __restrict__ vals, uint32_t beg, uint32_t lo, uint32_t hi,
+                                            float (&S)[4], float& Q, float& wx) {
+  constexpr uint32_t T = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const uint32_t tg = (uint32_t)(lane / C);
+  for (uint32_t p0 = lo & ~(2u * T - 1u); p0 < hi; p0 += 2u * T) {
+    const uint32_t pa = p0 + tg, pb = pa + T;
+    const bool va = pa >= lo && pa < hi, vb = pb >= lo && pb < hi;
+    const uint32_t ja = beg + (pa - lo), jb = beg + (pb - lo);
+    const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+    const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+    const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+    const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+    uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+    float wa = 0.f, wb = 0.f;
+    float4 qa = make_float4(0.f, 0.f, 0.f, 0.f), qb = qa;
+    if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, qa);
+    if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, qb);
+    if (va) xf_fmc_serve_token<H>(m, absent, ka, ra, wa, qa, xa, c, S, Q, wx);
+    if (vb) xf_fmc_serve_token<H>(m, absent, kb, rb, wb, qb, xb, c, S, Q, wx);
+  }
+}
+
+// canonical: the context's S[4], Q and wx per lane stay in registers; a candidate's tokens start at position
+// n_c mod 2T, which puts each on the lane group xf_k_serve_fmc gives it
+template <int C, bool H>
+__global__ void __launch_bounds__(256)
+xf_k_serve_cand_fmc(XfTableView m, int absent, XfCandView b, float* __restrict__ pctr_out) {
+  constexpr uint32_t T = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + (threadIdx.x >> 5);
+  struct Ctx { float S[4], Q, wx; uint32_t lo; };
+  xf_cand_walk(b, gwarp, gridDim.x * warps_per_block,
+               [=](uint32_t q) {
+                 const uint32_t beg = __ldg(b.ctx_ptr + q), n = __ldg(b.ctx_ptr + q + 1) - beg;
+                 Ctx x{{0.f, 0.f, 0.f, 0.f}, 0.f, 0.f, n & (2u * T - 1u)};
+                 xf_fmc_fold<C, H>(m, absent, b.ctx_keys, b.ctx_vals, beg, 0u, n, x.S, x.Q, x.wx);
+                 return x;
+               },
+               [=](const Ctx& x, uint32_t c) {
+                 const uint32_t beg = __ldg(b.row_ptr + c), n = __ldg(b.row_ptr + c + 1) - beg;
+                 float S[4] = {x.S[0], x.S[1], x.S[2], x.S[3]};
+                 float Q = x.Q, wx = x.wx;
+                 xf_fmc_fold<C, H>(m, absent, b.keys, b.vals, beg, x.lo, x.lo + n, S, Q, wx);
+                 const float arg = xf_fmc_arg<C>(S, Q, wx);
+                 if (lane == 0) pctr_out[c] = xf_sigmoid(arg);
+               },
+               [](const Ctx&) {});
+}
+
+template <bool H>
+static void xf_launch_cand_fmc(const xf_model* m, const XfCandView& b, float* pctr_out, int grid, cudaStream_t st) {
+  switch (m->view.K) {
+    case 4: xf_k_serve_cand_fmc<1, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 8: xf_k_serve_cand_fmc<2, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 16: xf_k_serve_cand_fmc<4, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 32: xf_k_serve_cand_fmc<8, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 64: xf_k_serve_cand_fmc<16, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    default: xf_k_serve_cand_fmc<32, H><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+  }
+}
+
+// xf_k_serve_mvm's loop over the n tokens of a row from keys[beg] (vals NULL: every value 1) into the warp's sums S, in
+// token order; returns the lane's fields present (the caller reduces them over the warp)
+template <int C, bool H>
+__device__ __forceinline__ unsigned xf_mvm_fold(const XfTableView& m, int absent, const uint64_t* __restrict__ keys,
+                                                const uint8_t* __restrict__ fields, const float* __restrict__ vals,
+                                                uint32_t beg, uint32_t n, float (*S)[4 * C]) {
+  constexpr uint32_t T = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const uint32_t tg = (uint32_t)(lane / C);
+  unsigned present = 0u;
+  for (uint32_t i0 = 0; i0 < n; i0 += 2u * T) {
+    const uint32_t ia = i0 + tg, ib = ia + T;
+    const bool va = ia < n, vb = ib < n;
+    const uint32_t ja = beg + ia, jb = beg + ib;
+    const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+    const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+    const uint32_t fa = va ? (uint32_t)__ldcs(fields + ja) & (XF_MVM_FIELDS - 1) : 0u;
+    const uint32_t fb = vb ? (uint32_t)__ldcs(fields + jb) & (XF_MVM_FIELDS - 1) : 0u;
+    const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+    const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+    uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+    float wa, wb;  // a multi-view machine's row holds no w
+    float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
+    if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+    if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+    if (va) pa = xf_mvm_serve_token<H>(m, absent, ka, ra, pa, c);
+    if (vb) pb = xf_mvm_serve_token<H>(m, absent, kb, rb, pb, c);
+    present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
+    xf_mvm_add<4 * C>(S, va, fa, c, pa, xa);  // pass a, then pass b
+    xf_mvm_add<4 * C>(S, vb, fb, c, pb, xb);
+  }
+  return present;
+}
+
+// Multi-view machine: a warp's working sums S[f][k] and a copy S0 of the context's, both in shared memory (2 x 32 x K
+// floats per warp, 4 warps per block: 32 KB at K = 32).  Each candidate adds its tokens to S in token order; then lane
+// k < K forms P_k over the fields present in the context or the candidate, as xf_k_serve_mvm, and puts the candidate's
+// fields back to the context's sums.  After a request's last candidate in the run, its context's fields are cleared in
+// both.  The candidate tokens' lanes do not matter: S is the warp's, each entry a fold in token order.
+#define XF_CAND_MVM_WARPS 4
+template <int C, bool H>
+__global__ void __launch_bounds__(32 * XF_CAND_MVM_WARPS)
+xf_k_serve_cand_mvm(XfTableView m, int absent, XfCandView b, float* __restrict__ pctr_out) {
+  constexpr int K = 4 * C;
+  __shared__ __align__(16) float s_sum[XF_CAND_MVM_WARPS][2][XF_MVM_FIELDS][K];
+  const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
+  const int gwarp = blockIdx.x * XF_CAND_MVM_WARPS + wib;
+  float (*S)[K] = s_sum[wib][0];
+  float (*S0)[K] = s_sum[wib][1];
+  if (lane < K)
+    for (int f = 0; f < XF_MVM_FIELDS; ++f) S[f][lane] = S0[f][lane] = 0.f;
+  __syncwarp();
+  xf_cand_walk(b, gwarp, gridDim.x * XF_CAND_MVM_WARPS,
+               [=](uint32_t q) {
+                 const uint32_t beg = __ldg(b.ctx_ptr + q), n = __ldg(b.ctx_ptr + q + 1) - beg;
+                 const unsigned ctx_present = __reduce_or_sync(
+                     0xffffffffu, xf_mvm_fold<C, H>(m, absent, b.ctx_keys, b.ctx_fields, b.ctx_vals, beg, n, S));
+                 __syncwarp();
+                 if (lane < K)
+                   for (unsigned f = ctx_present; f; f &= f - 1) S0[__ffs(f) - 1][lane] = S[__ffs(f) - 1][lane];
+                 return ctx_present;
+               },
+               [=](unsigned ctx_present, uint32_t c) {
+                 const uint32_t beg = __ldg(b.row_ptr + c), n = __ldg(b.row_ptr + c + 1) - beg;
+                 __syncwarp();
+                 const unsigned own = __reduce_or_sync(0xffffffffu, xf_mvm_fold<C, H>(m, absent, b.keys, b.fields,
+                                                                                      b.vals, beg, n, S));
+                 __syncwarp();
+                 const unsigned present = ctx_present | own;
+                 float P = 0.f;
+                 if (lane < K && present) {
+                   P = 1.f;
+                   for (unsigned q = present; q; q &= q - 1) P = __fmul_rn(P, S[__ffs(q) - 1][lane]);
+                   for (unsigned q = own; q; q &= q - 1) S[__ffs(q) - 1][lane] = S0[__ffs(q) - 1][lane];
+                 }
+                 const float y = xf_warp_sum(P);
+                 if (lane == 0) pctr_out[c] = xf_sigmoid(y);
+               },
+               [=](unsigned ctx_present) {
+                 // the context leaves both copies before the warp's next request
+                 if (lane < K)
+                   for (unsigned f = ctx_present; f; f &= f - 1) S[__ffs(f) - 1][lane] = S0[__ffs(f) - 1][lane] = 0.f;
+                 __syncwarp();
+               });
+}
+
+template <bool H>
+static void xf_launch_cand_mvm(const xf_model* m, const XfCandView& b, float* pctr_out, int grid, cudaStream_t st) {
+  constexpr int T = 32 * XF_CAND_MVM_WARPS;
+  switch (m->view.K) {
+    case 4: xf_k_serve_cand_mvm<1, H><<<grid, T, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 8: xf_k_serve_cand_mvm<2, H><<<grid, T, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    case 16: xf_k_serve_cand_mvm<4, H><<<grid, T, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+    default: xf_k_serve_cand_mvm<8, H><<<grid, T, 0, st>>>(m->view, m->absent, b, pctr_out); break;
+  }
+}
+
+// the candidate forward of any model on device arrays
+static void xf_launch_candidates(const xf_model* m, const XfCandView& b, float* pctr_out, cudaStream_t st) {
+  if (b.candidates == 0) return;
+  const uint64_t warps = ((uint64_t)b.candidates + XF_CAND_RUN - 1u) / XF_CAND_RUN;
+  const bool half = m->precision == XF_PRECISION_F16;
+  if (m->fm == XF_SERVE_MVM) {
+    const int grid = xf_grid_for(warps * 32, 32 * XF_CAND_MVM_WARPS, 16);
+    if (half) xf_launch_cand_mvm<true>(m, b, pctr_out, grid, st);
+    else xf_launch_cand_mvm<false>(m, b, pctr_out, grid, st);
+    return;
+  }
+  const int grid = xf_grid_for(warps * 32, 256, 8);
+  if (m->fm == XF_SERVE_FMC) {
+    if (half) xf_launch_cand_fmc<true>(m, b, pctr_out, grid, st);
+    else xf_launch_cand_fmc<false>(m, b, pctr_out, grid, st);
+    return;
+  }
+  if (m->fm && half) xf_k_serve_cand<true, true><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out);
+  else if (m->fm) xf_k_serve_cand<true, false><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out);
+  else xf_k_serve_cand<false, false><<<grid, 256, 0, st>>>(m->view, m->absent, b, pctr_out);
+}
+
 // ---- building a model's table
 __global__ void xf_k_model_fill(uint4* base, uint64_t chunks16, uint32_t per_row) {
   for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < chunks16; c += (uint64_t)gridDim.x * blockDim.x)
@@ -1014,6 +1314,122 @@ XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr
                                           float* d_pctr_out, void* cuda_stream) {
   return xf_predict_device(m, d_row_ptr, d_keys, d_fields, d_vals, rows, nnz, d_pctr_out, cuda_stream, true,
                            "xf_model_predict_device_fields");
+}
+
+// what both candidate entry points check without reading the arrays: null pointers, a part, the model's kind
+static int xf_check_candidates(xf_model* m, const xf_candidate_batch* b, const void* pctr_out, const char* fn) {
+  const bool mvm = m && m->fm == XF_SERVE_MVM;
+  if (!m || !b || !b->ctx_ptr || !b->cand_ptr || !b->row_ptr || (!b->ctx_keys && b->ctx_nnz) || (!b->keys && b->nnz) ||
+      (!pctr_out && b->candidates) || (mvm && ((!b->ctx_fields && b->ctx_nnz) || (!b->fields && b->nnz)))) {
+    xf_set_error("null argument");
+    return XF_ERR_ARG;
+  }
+  XF_TRY(xf_refuse_part(m, fn));
+  XF_TRY(xf_check_fields_kind(m, mvm || b->ctx_fields || b->fields, fn));
+  XF_TRY(xf_check_vals(m, b->ctx_vals, fn));
+  XF_TRY(xf_check_vals(m, b->vals, fn));
+  return XF_OK;
+}
+
+static XfCandView xf_cand_view(const xf_candidate_batch& b) {
+  return XfCandView{b.ctx_ptr, b.ctx_keys, b.ctx_vals, b.ctx_fields, b.cand_ptr, b.row_ptr, b.keys, b.vals, b.fields,
+                    b.requests, b.candidates};
+}
+
+// XF_ERR_ARG, naming the array and the index, where ptr[0 .. n] decreases
+static int xf_check_nondecreasing(const uint32_t* ptr, uint32_t n, const char* what, const char* fn) {
+  for (uint32_t i = 0; i < n; ++i)
+    if (ptr[i] > ptr[i + 1]) {
+      xf_set_error("%s: %s decreases at %u (%u > %u)", fn, what, i, ptr[i], ptr[i + 1]);
+      return XF_ERR_ARG;
+    }
+  return XF_OK;
+}
+
+static int xf_check_host_fields(const uint8_t* fields, uint32_t n, const char* what, const char* fn) {
+  for (uint32_t j = 0; j < n; ++j)
+    if (fields[j] >= XF_MVM_FIELDS) {
+      xf_set_error("%s: %s: field id %u of token %u: a multi-view machine takes field ids below %d", fn, what,
+                   (unsigned)fields[j], j, XF_MVM_FIELDS);
+      return XF_ERR_ARG;
+    }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batch* b, float* pctr_out) {
+  static const char* const fn = "xf_model_predict_candidates_host";
+  XF_TRY(xf_check_candidates(m, b, pctr_out, fn));
+  const uint32_t R = b->requests, N = b->candidates;
+  XF_TRY(xf_check_nondecreasing(b->ctx_ptr, R, "ctx_ptr", fn));
+  XF_TRY(xf_check_nondecreasing(b->cand_ptr, R, "cand_ptr", fn));
+  XF_TRY(xf_check_nondecreasing(b->row_ptr, N, "row_ptr", fn));
+  if (b->cand_ptr[0] != 0 || b->cand_ptr[R] != N) {
+    xf_set_error("%s: cand_ptr runs from %u to %u: it must run from 0 to candidates = %u", fn, b->cand_ptr[0],
+                 b->cand_ptr[R], N);
+    return XF_ERR_ARG;
+  }
+  if (b->ctx_ptr[R] > b->ctx_nnz) {
+    xf_set_error("%s: ctx_ptr ends at %u, past ctx_nnz = %u", fn, b->ctx_ptr[R], b->ctx_nnz);
+    return XF_ERR_ARG;
+  }
+  if (b->row_ptr[N] > b->nnz) {
+    xf_set_error("%s: row_ptr ends at %u, past nnz = %u", fn, b->row_ptr[N], b->nnz);
+    return XF_ERR_ARG;
+  }
+  XF_TRY(xf_check_host_keys(b->ctx_keys, b->ctx_nnz, "xf_model_predict_candidates_host: ctx_keys"));
+  XF_TRY(xf_check_host_keys(b->keys, b->nnz, "xf_model_predict_candidates_host: keys"));
+  const bool mvm = m->fm == XF_SERVE_MVM;
+  if (mvm) {
+    XF_TRY(xf_check_host_fields(b->ctx_fields, b->ctx_nnz, "ctx_fields", fn));
+    XF_TRY(xf_check_host_fields(b->fields, b->nnz, "fields", fn));
+  }
+  if (N == 0) return XF_OK;
+  // every array into one pinned image, 16-byte aligned sections, and one upload: each context crosses once
+  const struct { const void* src; size_t bytes; } part[] = {
+      {b->ctx_ptr, ((size_t)R + 1) * 4},
+      {b->cand_ptr, ((size_t)R + 1) * 4},
+      {b->row_ptr, ((size_t)N + 1) * 4},
+      {b->ctx_keys, (size_t)b->ctx_nnz * 8},
+      {b->keys, (size_t)b->nnz * 8},
+      {b->ctx_vals, b->ctx_vals ? (size_t)b->ctx_nnz * 4 : 0},
+      {b->vals, b->vals ? (size_t)b->nnz * 4 : 0},
+      {b->ctx_fields, mvm ? (size_t)b->ctx_nnz : 0},
+      {b->fields, mvm ? (size_t)b->nnz : 0},
+  };
+  constexpr int NP = sizeof(part) / sizeof(part[0]);
+  size_t off[NP + 1];
+  off[0] = 0;
+  for (int i = 0; i < NP; ++i) off[i + 1] = off[i] + ((part[i].bytes + 15) & ~(size_t)15);
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  XF_TRY(m->h_in.ensure(off[NP]));
+  XF_TRY(m->s_aux.ensure(off[NP]));
+  XF_TRY(m->h_out.ensure((size_t)N * 4));
+  XF_TRY(m->s_out.ensure((size_t)N * 4));
+  for (int i = 0; i < NP; ++i)
+    if (part[i].bytes) memcpy(m->h_in.as<uint8_t>() + off[i], part[i].src, part[i].bytes);
+  XF_CUDA_TRY(cudaMemcpyAsync(m->s_aux.p, m->h_in.p, off[NP], cudaMemcpyHostToDevice, m->stream));
+  const uint8_t* d = m->s_aux.as<uint8_t>();
+  auto at = [&](int i) -> const void* { return part[i].bytes ? d + off[i] : nullptr; };
+  XfCandView v{static_cast<const uint32_t*>(at(0)), static_cast<const uint64_t*>(at(3)), static_cast<const float*>(at(5)),
+               static_cast<const uint8_t*>(at(7)), static_cast<const uint32_t*>(at(1)), static_cast<const uint32_t*>(at(2)),
+               static_cast<const uint64_t*>(at(4)), static_cast<const float*>(at(6)), static_cast<const uint8_t*>(at(8)),
+               R, N};
+  xf_launch_candidates(m, v, m->s_out.as<float>(), m->stream);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_out.p, (size_t)N * 4, cudaMemcpyDeviceToHost, m->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
+  memcpy(pctr_out, m->h_out.p, (size_t)N * 4);
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_candidates_device(xf_model* m, const xf_candidate_batch* b, float* d_pctr_out,
+                                              void* cuda_stream) {
+  XF_TRY(xf_check_candidates(m, b, d_pctr_out, "xf_model_predict_candidates_device"));
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  xf_launch_candidates(m, xf_cand_view(*b), d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
 }
 
 XF_DLL int xf_model_predict_ingested(xf_model* m, xf_trainer* tr, uint32_t row_start, uint32_t row_end, float* pctr_out,
