@@ -1,9 +1,11 @@
 // The forward passes' arithmetic shared by the serving kernels (serve.cu) and the deterministic training step
-// (step_det.cu): the canonical FM's per-lane sums in xf_k_step_fmc's order, and the multi-view machine's same-field
-// adds in token order.
+// (step_det.cu): the canonical FM's per-lane sums in xf_k_step_fmc's order, the multi-view machine's same-field adds in
+// token order and its product over the present fields, and the launchers' map from K to the lane count C.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "kernels.h"
 
@@ -55,5 +57,28 @@ __device__ __forceinline__ void xf_mvm_add(float (*S)[K], bool live, uint32_t f,
     }
     __syncwarp();
   }
+}
+
+// Lane k < K's P_k = the product of S[f][k] over the present fields in ascending order; 0 on the other lanes and when
+// no field is present.  The warp sum of the P_k is the machine's y.
+template <int K>
+__device__ __forceinline__ float xf_mvm_product(float (*S)[K], unsigned present) {
+  const int lane = threadIdx.x & 31;
+  float P = 0.f;
+  if (lane < K && present) {
+    P = 1.f;
+    for (unsigned q = present; q; q &= q - 1) P = __fmul_rn(P, S[__ffs(q) - 1][lane]);
+  }
+  return P;
+}
+
+// f(std::integral_constant<int, C>()) for the lane count C = K/4 of latent dimension K, C <= MAX_C; a K that is not
+// 4C for such a C takes C = MAX_C (the multi-view machine's kernels stop at 8: their shared memory grows with K)
+template <int MAX_C, int C = 1, typename F>
+inline void xf_with_lanes(int K, F&& f) {
+  if constexpr (C < MAX_C) {
+    if (K != 4 * C) return xf_with_lanes<MAX_C, 2 * C>(K, static_cast<F&&>(f));
+  }
+  f(std::integral_constant<int, C>());
 }
 

@@ -27,7 +27,7 @@ struct xf_model {
   cudaStream_t stream = nullptr;
   // staging of the host entry points, grown on demand; those calls are serialised by the mutex
   std::mutex mu;
-  XfDevBuf s_row_ptr, s_keys, s_out, s_aux, s_vals, s_fields;
+  XfDevBuf s_keys, s_out, s_aux;  // s_aux: a host batch's upload image (xf_model_upload), or a lookup's outputs
   XfPinBuf h_in, h_out;
 };
 

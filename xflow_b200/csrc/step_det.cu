@@ -161,12 +161,7 @@ xf_k_det_mvm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t
       xf_mvm_add<K>(S, on, f, c, v, x);
     }
     present = __reduce_or_sync(0xffffffffu, present);
-    float P = 0.f;
-    if (lane < K && present) {
-      P = 1.f;
-      for (unsigned q = present; q; q &= q - 1) P = __fmul_rn(P, S[__ffs(q) - 1][lane]);
-    }
-    const float pctr = xf_sigmoid(xf_warp_sum(P));
+    const float pctr = xf_sigmoid(xf_warp_sum(xf_mvm_product<K>(S, present)));
     if (lane == 0 && pctr_out) pctr_out[row] = pctr;
     if (mode == 0) {
       const float loss = __fsub_rn(pctr, (float)labels[row]);
@@ -504,23 +499,14 @@ int xf_det_step(const XfTableView& t, XfDetBufs& b, bool mvm, const uint32_t* ro
   const int grid = xf_grid_for((uint64_t)B * 32, 256, 8);
   // positions outside the rows (a slice of an ingested block) keep no slot
   if (mode == 0 && nnz) XF_CUDA_TRY(cudaMemsetAsync(d.keys_in, 0xFF, (size_t)nnz * 4, st));
-  if (mvm) {
-    switch (t.K) {
-      case 4: xf_k_det_mvm<1><<<grid, 256, 0, st>>>(t, row_ptr, keys, fields, vals, labels, B, mode, d, loss_out, pctr_out); break;
-      case 8: xf_k_det_mvm<2><<<grid, 256, 0, st>>>(t, row_ptr, keys, fields, vals, labels, B, mode, d, loss_out, pctr_out); break;
-      case 16: xf_k_det_mvm<4><<<grid, 256, 0, st>>>(t, row_ptr, keys, fields, vals, labels, B, mode, d, loss_out, pctr_out); break;
-      default: xf_k_det_mvm<8><<<grid, 256, 0, st>>>(t, row_ptr, keys, fields, vals, labels, B, mode, d, loss_out, pctr_out); break;
-    }
-  } else {
-    switch (t.K) {
-      case 4: xf_k_det_fmc<1><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-      case 8: xf_k_det_fmc<2><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-      case 16: xf_k_det_fmc<4><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-      case 32: xf_k_det_fmc<8><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-      case 64: xf_k_det_fmc<16><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-      default: xf_k_det_fmc<32><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out); break;
-    }
-  }
+  if (mvm)
+    xf_with_lanes<8>(t.K, [&](auto C) {
+      xf_k_det_mvm<C><<<grid, 256, 0, st>>>(t, row_ptr, keys, fields, vals, labels, B, mode, d, loss_out, pctr_out);
+    });
+  else
+    xf_with_lanes<32>(t.K, [&](auto C) {
+      xf_k_det_fmc<C><<<grid, 256, 0, st>>>(t, row_ptr, keys, vals, labels, B, d, loss_out, pctr_out);
+    });
   if (mode != 0) return XF_OK;
   if (nnz) {
     const int bits = (int)t.log2cap + 1;
@@ -532,23 +518,8 @@ int xf_det_step(const XfTableView& t, XfDetBufs& b, bool mvm, const uint32_t* ro
     XF_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp.p, tb, b.keys_in.as<uint32_t>(), b.keys_out.as<uint32_t>(),
                                                 b.toks_in.as<uint32_t>(), b.toks_out.as<uint32_t>(), (int)nnz, 0, bits, st));
     XF_CUDA_TRY(cudaMemsetAsync(d.cnt, 0, 2 * sizeof(unsigned), st));
-    if (mvm) {
-      switch (t.K) {
-        case 4: xf_det_launch_reduce<true, 4>(t, d, nnz, touched, st); break;
-        case 8: xf_det_launch_reduce<true, 8>(t, d, nnz, touched, st); break;
-        case 16: xf_det_launch_reduce<true, 16>(t, d, nnz, touched, st); break;
-        default: xf_det_launch_reduce<true, 32>(t, d, nnz, touched, st); break;
-      }
-    } else {
-      switch (t.K) {
-        case 4: xf_det_launch_reduce<false, 4>(t, d, nnz, touched, st); break;
-        case 8: xf_det_launch_reduce<false, 8>(t, d, nnz, touched, st); break;
-        case 16: xf_det_launch_reduce<false, 16>(t, d, nnz, touched, st); break;
-        case 32: xf_det_launch_reduce<false, 32>(t, d, nnz, touched, st); break;
-        case 64: xf_det_launch_reduce<false, 64>(t, d, nnz, touched, st); break;
-        default: xf_det_launch_reduce<false, 128>(t, d, nnz, touched, st); break;
-      }
-    }
+    if (mvm) xf_with_lanes<8>(t.K, [&](auto C) { xf_det_launch_reduce<true, 4 * C>(t, d, nnz, touched, st); });
+    else xf_with_lanes<32>(t.K, [&](auto C) { xf_det_launch_reduce<false, 4 * C>(t, d, nnz, touched, st); });
   }
   if (abs_loss_sum) xf_k_det_abs<<<1, 256, 0, st>>>(d.res, B, abs_loss_sum);
   return XF_OK;
