@@ -821,6 +821,29 @@ XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batc
  * & 31). */
 XF_DLL int xf_model_predict_candidates_device(xf_model* m, const xf_candidate_batch* b, float* d_pctr_out,
                                               void* cuda_stream);
+/* Candidate ranking: each request's top k candidates by pctr, selected on the device.  Candidate i of request q
+ * (0 <= i < n_q = cand_ptr[q+1] - cand_ptr[q], its local index) has the score p_i that xf_model_predict_candidates_*
+ * returns for candidate cand_ptr[q] + i, bit for bit, and the key
+ *   r_i = ord(p_i) << 32 | (2^32 - 1 - i),  ord(NaN) = 0,  ord(p) = bits(p) ^ 0x80000000 (sign clear), ~bits(p) (set);
+ * a candidate ranks before another iff its key is larger.  So a higher pctr ranks first, equal pctr bits rank by
+ * smaller index, and NaN ranks after every number.  Ties are common at the ends: xf_sigmoid returns exactly 1.0f for
+ * y > 30 and rounds to 1.0f above about y = 17, and returns 1e-6 for y < -30; such candidates rank by index.
+ * For j < m_q = min(k, n_q), top_index[q k + j] is the local index of request q's j-th ranked candidate and
+ * top_pctr[q k + j] its score, bit for bit; every slot j >= m_q holds index 0xFFFFFFFF and pctr bits 0x7FC00000.  All
+ * R k slots are written, also when candidates == 0.
+ * _host: every check of xf_model_predict_candidates_host, with its codes; XF_ERR_ARG for k = 0, k > XF_RANK_MAX_K and
+ * a NULL top_index with R > 0.  Uploads the batch as xf_model_predict_candidates_host does and scores into the model's
+ * buffers; downloads the R k indices (and the R k scores when top_pctr is not NULL), never the candidates' scores.
+ * Runs on the model's stream; calls on one model are serialised.
+ * _device: the contract of xf_model_predict_candidates_device.  d_pctr [candidates] receives every candidate's score,
+ * the bytes xf_model_predict_candidates_device writes, and the selection reads them; d_top_pctr may be NULL.  Uses no
+ * device memory but its arguments. */
+enum { XF_RANK_MAX_K = 1024 };
+XF_DLL int xf_model_rank_candidates_host(xf_model* m, const xf_candidate_batch* b, uint32_t k,
+                                         uint32_t* top_index /* [R * k] */, float* top_pctr /* [R * k] or NULL */);
+XF_DLL int xf_model_rank_candidates_device(xf_model* m, const xf_candidate_batch* b, uint32_t k,
+                                           float* d_pctr /* [candidates] */, uint32_t* d_top_index /* [R * k] */,
+                                           float* d_top_pctr /* [R * k] or NULL */, void* cuda_stream);
 /* what the model holds for n host keys: w[n], st[n], qt[n] (0 for LR), present[n]; any output may be NULL.  On a
  * canonical or multi-view machine's model st and qt must be NULL (XF_ERR_ARG): its rows are read with
  * xf_model_lookup_latent. */

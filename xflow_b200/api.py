@@ -190,6 +190,8 @@ SIGNATURES = {
     "xf_model_predict_device_fields": (_i, [_vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "xf_model_predict_candidates_host": (_i, [_vp, _vp, _vp]),
     "xf_model_predict_candidates_device": (_i, [_vp, _vp, _vp, _vp]),
+    "xf_model_rank_candidates_host": (_i, [_vp, _vp, _u32, _vp, _vp]),
+    "xf_model_rank_candidates_device": (_i, [_vp, _vp, _u32, _vp, _vp, _vp, _vp]),
     "xf_model_lookup": (_i, [_vp, _vp, _u64, _vp, _vp, _vp, _vp]),
     "xf_model_lookup_latent": (_i, [_vp, _vp, _u64, _vp, _vp, _vp]),
     "xf_model_predict_ingested": (_i, [_vp, _vp, _u32, _u32, _vp, _vp]),
@@ -606,13 +608,9 @@ class Model:
         _check(lib().xf_model_predict_device_fields(self.h, _p(d_row_ptr), _p(d_keys), _p(d_fields),
                                                     _p(d_vals) if d_vals else None, rows, nnz, _p(d_out), st))
 
-    def predict_candidates(self, ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals=None, vals=None, ctx_fields=None,
-                           fields=None):
-        """Score each request's candidates against its context (xf_model_predict_candidates_host): request q's context
-        is ctx_keys[ctx_ptr[q] .. ctx_ptr[q+1]), its candidates rows cand_ptr[q] .. cand_ptr[q+1] - 1 of the CSR
-        (row_ptr, keys).  Returns float32 [candidates]: for each candidate, the flat predict of its request's context
-        followed by its own tokens, bit for bit.  Values (None: all 1) for canonical and multi-view machine models,
-        field ids for multi-view machine models, on either side."""
+    @staticmethod
+    def _candidate_batch(ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals, vals, ctx_fields, fields):
+        """(CandidateBatch, the arrays it points into) for host arrays, their sizes checked."""
         ctx_ptr = np.ascontiguousarray(ctx_ptr, np.uint32)
         cand_ptr = np.ascontiguousarray(cand_ptr, np.uint32)
         row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
@@ -633,12 +631,29 @@ class Model:
         ctx_fields = side(ctx_fields, np.uint8, ctx_keys.size, "field id")
         fields = side(fields, np.uint8, keys.size, "field id")
         n = row_ptr.size - 1
-        out = np.empty(max(n, 0), np.float32)
         b = CandidateBatch(cand_ptr.size - 1, ctx_ptr.ctypes.data, ctx_keys.ctypes.data,
                            None if ctx_vals is None else ctx_vals.ctypes.data,
                            None if ctx_fields is None else ctx_fields.ctypes.data, ctx_keys.size, cand_ptr.ctypes.data, n,
                            row_ptr.ctypes.data, keys.ctypes.data, None if vals is None else vals.ctypes.data,
                            None if fields is None else fields.ctypes.data, keys.size)
+        return b, (ctx_ptr, cand_ptr, row_ptr, ctx_keys, keys, ctx_vals, vals, ctx_fields, fields)
+
+    @staticmethod
+    def _device_batch(requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr, d_keys, nnz,
+                      d_ctx_vals, d_vals, d_ctx_fields, d_fields):
+        a = lambda x: int(x) or None
+        return CandidateBatch(requests, a(d_ctx_ptr), a(d_ctx_keys), a(d_ctx_vals), a(d_ctx_fields), ctx_nnz,
+                              a(d_cand_ptr), candidates, a(d_row_ptr), a(d_keys), a(d_vals), a(d_fields), nnz)
+
+    def predict_candidates(self, ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals=None, vals=None, ctx_fields=None,
+                           fields=None):
+        """Score each request's candidates against its context (xf_model_predict_candidates_host): request q's context
+        is ctx_keys[ctx_ptr[q] .. ctx_ptr[q+1]), its candidates rows cand_ptr[q] .. cand_ptr[q+1] - 1 of the CSR
+        (row_ptr, keys).  Returns float32 [candidates]: for each candidate, the flat predict of its request's context
+        followed by its own tokens, bit for bit.  Values (None: all 1) for canonical and multi-view machine models,
+        field ids for multi-view machine models, on either side."""
+        b, arrays = self._candidate_batch(ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals, vals, ctx_fields, fields)
+        out = np.empty(max(arrays[2].size - 1, 0), np.float32)
         _check(lib().xf_model_predict_candidates_host(self.h, C.byref(b), _p(out)))
         return out
 
@@ -647,10 +662,33 @@ class Model:
         """Asynchronous predict_candidates on device pointers (raw addresses) on the CUDA stream `stream`; d_out
         [candidates].  A 0 address for values reads every value as 1."""
         st = C.c_void_p(int(stream)) if stream else None
-        a = lambda x: int(x) or None
-        b = CandidateBatch(requests, a(d_ctx_ptr), a(d_ctx_keys), a(d_ctx_vals), a(d_ctx_fields), ctx_nnz, a(d_cand_ptr),
-                           candidates, a(d_row_ptr), a(d_keys), a(d_vals), a(d_fields), nnz)
+        b = self._device_batch(requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr, d_keys, nnz,
+                               d_ctx_vals, d_vals, d_ctx_fields, d_fields)
         _check(lib().xf_model_predict_candidates_device(self.h, C.byref(b), _p(d_out), st))
+
+    def rank_candidates(self, ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, k, ctx_vals=None, vals=None, ctx_fields=None,
+                        fields=None):
+        """Each request's top k candidates by pctr (xf_model_rank_candidates_host), selected on the device from the
+        scores predict_candidates returns.  Returns (index uint32 [R, k], pctr float32 [R, k]): row q holds request
+        q's local candidate indices (0 .. n_q - 1), highest pctr first, equal pctr by smaller index, NaN last, and
+        their scores; slots past n_q hold index 0xFFFFFFFF and a NaN."""
+        b, arrays = self._candidate_batch(ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals, vals, ctx_fields, fields)
+        index = np.empty((b.requests, k), np.uint32)
+        pctr = np.empty((b.requests, k), np.float32)
+        _check(lib().xf_model_rank_candidates_host(self.h, C.byref(b), k, _p(index), _p(pctr)))
+        return index, pctr
+
+    def rank_candidates_device(self, requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr,
+                               d_keys, nnz, k, d_pctr, d_top_index, d_top_pctr=0, stream=0, d_ctx_vals=0, d_vals=0,
+                               d_ctx_fields=0, d_fields=0):
+        """Asynchronous rank_candidates on device pointers (raw addresses) on the CUDA stream `stream`: d_pctr
+        [candidates] receives every score, d_top_index [R * k] and d_top_pctr [R * k] (0: not written) the ranking."""
+        st = C.c_void_p(int(stream)) if stream else None
+        b = self._device_batch(requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr, d_keys, nnz,
+                               d_ctx_vals, d_vals, d_ctx_fields, d_fields)
+        _check(lib().xf_model_rank_candidates_device(self.h, C.byref(b), k, _p(d_pctr) if d_pctr else None,
+                                                     _p(d_top_index) if d_top_index else None,
+                                                     _p(d_top_pctr) if d_top_pctr else None, st))
 
     def lookup(self, keys):
         """What the model holds for `keys`: dict of w, st, qt (0 for LR) and present."""

@@ -1326,9 +1326,8 @@ static XfCandView xf_cand_view(const xf_candidate_batch& b) {
                     b.requests, b.candidates};
 }
 
-XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batch* b, float* pctr_out) {
-  static const char* const fn = "xf_model_predict_candidates_host";
-  XF_TRY(xf_check_candidates(m, b, pctr_out, fn));
+// the checks xf_model_predict_candidates_host makes on a batch's host arrays, after xf_check_candidates
+static int xf_check_candidates_host(const xf_model* m, const xf_candidate_batch* b, const char* fn) {
   const uint32_t R = b->requests, N = b->candidates;
   XF_TRY(xf_check_nondecreasing(b->ctx_ptr, R, "ctx_ptr", fn));
   XF_TRY(xf_check_nondecreasing(b->cand_ptr, R, "cand_ptr", fn));
@@ -1346,19 +1345,23 @@ XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batc
     xf_set_error("%s: row_ptr ends at %u, past nnz = %u", fn, b->row_ptr[N], b->nnz);
     return XF_ERR_ARG;
   }
-  XF_TRY(xf_check_host_keys(b->ctx_keys, b->ctx_nnz, "xf_model_predict_candidates_host: ctx_keys"));
-  XF_TRY(xf_check_host_keys(b->keys, b->nnz, "xf_model_predict_candidates_host: keys"));
-  const bool mvm = m->fm == XF_SERVE_MVM;
-  if (mvm) {
+  char what[96];
+  snprintf(what, sizeof what, "%s: ctx_keys", fn);
+  XF_TRY(xf_check_host_keys(b->ctx_keys, b->ctx_nnz, what));
+  snprintf(what, sizeof what, "%s: keys", fn);
+  XF_TRY(xf_check_host_keys(b->keys, b->nnz, what));
+  if (m->fm == XF_SERVE_MVM) {
     XF_TRY(xf_check_host_fields(b->ctx_fields, b->ctx_nnz, "ctx_fields", fn));
     XF_TRY(xf_check_host_fields(b->fields, b->nnz, "fields", fn));
   }
-  if (N == 0) return XF_OK;
-  std::lock_guard<std::mutex> lock(m->mu);
-  XF_CUDA_TRY(cudaSetDevice(m->device));
-  XF_TRY(m->h_out.ensure((size_t)N * 4));
-  XF_TRY(m->s_out.ensure((size_t)N * 4));
-  // each context crosses once
+  return XF_OK;
+}
+
+// A checked host batch onto the device as one image (xf_model_upload), each context once; *v: its arrays there.  The
+// caller holds the model's mutex with its device current.
+static int xf_upload_candidates(xf_model* m, const xf_candidate_batch* b, XfCandView* v) {
+  const uint32_t R = b->requests, N = b->candidates;
+  const bool mvm = m->fm == XF_SERVE_MVM;
   const XfUpload part[] = {
       {b->ctx_ptr, ((size_t)R + 1) * 4},
       {b->cand_ptr, ((size_t)R + 1) * 4},
@@ -1372,10 +1375,25 @@ XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batc
   };
   const void* d[9];
   XF_TRY(xf_model_upload(m, part, d));
-  XfCandView v{static_cast<const uint32_t*>(d[0]), static_cast<const uint64_t*>(d[3]), static_cast<const float*>(d[5]),
-               static_cast<const uint8_t*>(d[7]), static_cast<const uint32_t*>(d[1]), static_cast<const uint32_t*>(d[2]),
-               static_cast<const uint64_t*>(d[4]), static_cast<const float*>(d[6]), static_cast<const uint8_t*>(d[8]),
-               R, N};
+  *v = XfCandView{static_cast<const uint32_t*>(d[0]), static_cast<const uint64_t*>(d[3]), static_cast<const float*>(d[5]),
+                  static_cast<const uint8_t*>(d[7]), static_cast<const uint32_t*>(d[1]), static_cast<const uint32_t*>(d[2]),
+                  static_cast<const uint64_t*>(d[4]), static_cast<const float*>(d[6]), static_cast<const uint8_t*>(d[8]),
+                  R, N};
+  return XF_OK;
+}
+
+XF_DLL int xf_model_predict_candidates_host(xf_model* m, const xf_candidate_batch* b, float* pctr_out) {
+  static const char* const fn = "xf_model_predict_candidates_host";
+  XF_TRY(xf_check_candidates(m, b, pctr_out, fn));
+  XF_TRY(xf_check_candidates_host(m, b, fn));
+  const uint32_t N = b->candidates;
+  if (N == 0) return XF_OK;
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  XF_TRY(m->h_out.ensure((size_t)N * 4));
+  XF_TRY(m->s_out.ensure((size_t)N * 4));
+  XfCandView v;
+  XF_TRY(xf_upload_candidates(m, b, &v));
   xf_launch_candidates(m, v, m->s_out.as<float>(), m->stream);
   XF_CUDA_TRY(cudaGetLastError());
   XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_out.p, (size_t)N * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -1389,6 +1407,61 @@ XF_DLL int xf_model_predict_candidates_device(xf_model* m, const xf_candidate_ba
   XF_TRY(xf_check_candidates(m, b, d_pctr_out, "xf_model_predict_candidates_device"));
   XF_CUDA_TRY(cudaSetDevice(m->device));
   xf_launch_candidates(m, xf_cand_view(*b), d_pctr_out, reinterpret_cast<cudaStream_t>(cuda_stream));
+  XF_CUDA_TRY(cudaGetLastError());
+  return XF_OK;
+}
+
+// what both rank entry points check besides xf_check_candidates: k, and the index output
+static int xf_check_rank(const xf_candidate_batch* b, uint32_t k, const void* top_index, const char* fn) {
+  if (k == 0 || k > XF_RANK_MAX_K) {
+    xf_set_error("%s: k = %u: it must run from 1 to XF_RANK_MAX_K = %d", fn, k, XF_RANK_MAX_K);
+    return XF_ERR_ARG;
+  }
+  if (b && b->requests && !top_index) {
+    xf_set_error("%s: top_index is NULL with %u requests", fn, b->requests);
+    return XF_ERR_ARG;
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_model_rank_candidates_host(xf_model* m, const xf_candidate_batch* b, uint32_t k, uint32_t* top_index,
+                                         float* top_pctr) {
+  static const char* const fn = "xf_model_rank_candidates_host";
+  XF_TRY(xf_check_rank(b, k, top_index, fn));
+  XF_TRY(xf_check_candidates(m, b, top_index, fn));
+  XF_TRY(xf_check_candidates_host(m, b, fn));
+  const uint32_t R = b->requests, N = b->candidates;
+  if (R == 0) return XF_OK;
+  const size_t slots = (size_t)R * k, back = slots * (top_pctr ? 8 : 4);
+  std::lock_guard<std::mutex> lock(m->mu);
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  // the scores stay on the device in s_out; the outputs, indices then scores, in s_keys
+  XF_TRY(m->s_out.ensure((size_t)N * 4));
+  XF_TRY(m->s_keys.ensure(slots * 8));
+  XF_TRY(m->h_out.ensure(back));
+  XfCandView v;
+  XF_TRY(xf_upload_candidates(m, b, &v));
+  uint32_t* d_index = m->s_keys.as<uint32_t>();
+  xf_launch_candidates(m, v, m->s_out.as<float>(), m->stream);
+  xf_launch_rank(m->s_out.as<float>(), v.cand_ptr, R, k, d_index,
+                 top_pctr ? reinterpret_cast<float*>(d_index + slots) : nullptr, m->stream);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(m->h_out.p, m->s_keys.p, back, cudaMemcpyDeviceToHost, m->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(m->stream));
+  memcpy(top_index, m->h_out.p, slots * 4);
+  if (top_pctr) memcpy(top_pctr, m->h_out.as<uint8_t>() + slots * 4, slots * 4);
+  return XF_OK;
+}
+
+XF_DLL int xf_model_rank_candidates_device(xf_model* m, const xf_candidate_batch* b, uint32_t k, float* d_pctr,
+                                           uint32_t* d_top_index, float* d_top_pctr, void* cuda_stream) {
+  static const char* const fn = "xf_model_rank_candidates_device";
+  XF_TRY(xf_check_rank(b, k, d_top_index, fn));
+  XF_TRY(xf_check_candidates(m, b, d_pctr, fn));
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
+  xf_launch_candidates(m, xf_cand_view(*b), d_pctr, st);
+  xf_launch_rank(d_pctr, b->cand_ptr, b->requests, k, d_top_index, d_top_pctr, st);
   XF_CUDA_TRY(cudaGetLastError());
   return XF_OK;
 }

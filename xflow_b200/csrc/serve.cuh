@@ -226,6 +226,12 @@ int xf_model_gather(const XfTableView& v, const uint32_t* slots, uint64_t n, voi
 // *error
 int xf_model_insert_rows(const XfTableView& v, const uint8_t* rows, uint64_t n, int* error, cudaStream_t st);
 
+// Each request's top k candidates (rank.cu): request q's scores are pctr[cand_ptr[q] .. cand_ptr[q+1]); slots
+// [q k, q k + k) of top_index (and of top_pctr, unless NULL) receive its ranked local indices and their scores, padded
+// with 0xFFFFFFFF (and the NaN 0x7FC00000).  1 <= k <= XF_RANK_MAX_K.  Reads cand_ptr on the device only; no scratch.
+void xf_launch_rank(const float* pctr, const uint32_t* cand_ptr, uint32_t requests, uint32_t k, uint32_t* top_index,
+                    float* top_pctr, cudaStream_t st);
+
 // ---- the files' chunked sections (XFSM and XFSP rows, XFSD upserts and delete keys)
 // A section of n entries of `bytes` bytes is a sequence of chunks of per_chunk entries (the last may be shorter), each a
 // head {u64 first entry, u64 entries, u64 checksum, u64 0} and its entries.  The checksum is xf_st_host_sum over the
