@@ -122,6 +122,7 @@ class XF_CXX_API WorkerBase {
   xf_trainer* trainer_ = nullptr;
   uint32_t trainer_rows_ = 0, trainer_nnz_ = 0;
   xf_pv* pv_ = nullptr;           // XFLOW_PROGRESSIVE = 1: the training steps' progressive validation
+  uint32_t pv_slices_ = 0;        // XFLOW_PV_SLICES: the slices pv_ reports
   // current block (valid inside batch_training / predict)
   const uint32_t* cur_row_ptr_ = nullptr;
   const uint64_t* cur_keys_ = nullptr;

@@ -972,6 +972,23 @@ XF_DLL int xf_delta_destroy(xf_delta* d);
  *    kernel scores them on the table's stream: xf_trainer_launches counts +1 per step while a pv is attached.
  *    Attaching changes no bit of training: tables, state images and every other output are those of a run without.
  *    Not in the state image: a resumed run starts its pv afresh.
+ *
+ *    Slices.  xf_pv_set_slices gives a pv a slice map: a set of (key, slice) pairs, slice < n_slices.  Many keys may
+ *    name one slice; a key names at most one.  A row belongs to slice s when at least one of its tokens has a key that
+ *    the map sends to s: a row belongs to every slice its keys name, and counts once per slice however many of its
+ *    tokens name it and wherever they sit in the row.  A row whose keys name no slice is in no slice (the global sums
+ *    still count it).  Membership depends only on the batch's keys, not on the table, admission or eviction.  Each
+ *    slice has the pv's accumulators with the same row classification (e == 0 adds nothing; overflow and NaN rows are
+ *    counted per slice), fixed-point units and sums, binned with the slice mantissa bits ms chosen at set time:
+ *      slice s's report is, byte for byte, the xf_pv_report of an unsliced pv with mantissa_bits = ms fed exactly the
+ *      rows of slice s, and the sliced pv's own xf_pv_report is that of an unsliced pv with its m fed every row;
+ *    so the slice reports too depend only on the rows added, not on batch cuts, streams, grid or atomic order.  A
+ *    sliced pv needs each row's tokens: xf_pv_add_device_rows (xf_pv_add_device refuses it).  A trainer feeding a
+ *    sliced pv passes its batch's row_ptr and keys, and xf_trainer_launches counts +2 per step instead of +1; the
+ *    training itself changes no bit.  Memory: n_slices * (20 * 2^ms + 1) * 48 bytes for the bins, and a map of 12
+ *    bytes per slot with at least 2 slots per key.  One table lookup per token (one 32-byte sector for a key that
+ *    names no slice, almost always); a row's (row, slice) pairs add with the same multi-word atomics as the bins.
+ *    Made for up to about 10^4 segments (ms = 8: 246 KB of bins per slice), not one slice per user.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct xf_pv xf_pv;
 /* the report of xf_pv_report; a struct tag only (like POSIX's struct stat), the function has the name */
@@ -989,12 +1006,29 @@ XF_DLL int xf_pv_destroy(xf_pv* pv);
 /* clears every sum, stream-ordered after every add enqueued so far; later adds come after it */
 XF_DLL int xf_pv_reset(xf_pv* pv);
 /* n predictions, labels (!= 0 positive) and weights (NULL: all 1) in device memory on pv's device; asynchronous on
- * cuda_stream (cudaStream_t or NULL): the arrays must stay untouched until that stream has run the add */
+ * cuda_stream (cudaStream_t or NULL): the arrays must stay untouched until that stream has run the add.  XF_ERR_STATE
+ * on a pv with slices (xf_pv_add_device_rows) */
 XF_DLL int xf_pv_add_device(xf_pv* pv, const float* d_pctr, const uint8_t* d_labels, const float* d_weights,
                             uint64_t n, void* cuda_stream);
 /* waits for every add enqueued so far, on any stream; does not reset */
 XF_DLL int xf_pv_report(xf_pv* pv, struct xf_pv_report* out);
-/* every later training step of tr feeds pv (above); NULL detaches.  XF_ERR_ARG, naming the reason, for a trainer that
+/* Replace pv's slice map and clear every sum (global and per slice), like xf_pv_reset.  n_slices = 0 (with
+ * n_keys = 0) removes slicing; slice_mantissa_bits is then ignored.  XF_ERR_STATE while a trainer feeds pv.
+ * XF_ERR_ARG, naming the reason, leaving pv as it was, for: slice_of[i] >= n_slices, a key listed twice, the reserved
+ * key 2^64-1, n_slices > 65536, n_keys > 2^24, slice_mantissa_bits outside 4..16, and slice accumulators over 1 GiB
+ * (n_slices * ((20 << ms) + 1) * 48 bytes + 56 bytes of sums per slice).  Waits for every add enqueued so far. */
+XF_DLL int xf_pv_set_slices(xf_pv* pv, const uint64_t* keys, const uint32_t* slice_of, uint64_t n_keys,
+                            uint32_t n_slices, uint32_t slice_mantissa_bits);
+/* rows predictions/labels/weights as xf_pv_add_device, plus each row's tokens: d_keys[d_row_ptr[r] .. d_row_ptr[r+1]).
+ * d_row_ptr[0] need not be 0 (the ingested path passes absolute offsets).  On a pv without slices it equals
+ * xf_pv_add_device (d_row_ptr and d_keys are then not read).  Asynchronous on cuda_stream, like xf_pv_add_device. */
+XF_DLL int xf_pv_add_device_rows(xf_pv* pv, const float* d_pctr, const uint8_t* d_labels, const float* d_weights,
+                                 const uint32_t* d_row_ptr, const uint64_t* d_keys, uint64_t rows, void* cuda_stream);
+/* out[n_slices], slice s at out[s]; XF_ERR_ARG unless n equals the pv's n_slices (> 0); waits like xf_pv_report;
+ * does not reset */
+XF_DLL int xf_pv_report_slices(xf_pv* pv, struct xf_pv_report* out, uint32_t n);
+/* every later training step of tr feeds pv (above); NULL detaches.  With a sliced pv the steps add their rows' keys
+ * too (xf_pv_add_device_rows).  XF_ERR_ARG, naming the reason, for a trainer that
  * runs the sharded step (a comm of more than one rank, or XFLOW_MG_FORCE=1) and for a pv on another device than the
  * table.  A pv may feed several trainers; the caller resets it (for windows, epochs). */
 XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv);

@@ -207,6 +207,9 @@ SIGNATURES = {
     "xf_pv_reset": (_i, [_vp]),
     "xf_pv_add_device": (_i, [_vp, _vp, _vp, _vp, _u64, _vp]),
     "xf_pv_report": (_i, [_vp, _vp]),
+    "xf_pv_set_slices": (_i, [_vp, _vp, _vp, _u64, _u32, _u32]),
+    "xf_pv_add_device_rows": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp]),
+    "xf_pv_report_slices": (_i, [_vp, _vp, _u32]),
     "xf_trainer_set_validation": (_i, [_vp, _vp]),
     "xf_trainer_set_deterministic": (_i, [_vp, _i]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
@@ -792,6 +795,7 @@ class ProgressiveValidation:
 
     def __init__(self, device=0, mantissa_bits=10):
         self.device = device
+        self.num_slices = 0
         self.h = C.c_void_p()
         _check(lib().xf_pv_create(C.byref(self.h), int(device), int(mantissa_bits)))
 
@@ -822,6 +826,36 @@ class ProgressiveValidation:
 
     def reset(self):
         _check(lib().xf_pv_reset(self.h))
+
+    def set_slices(self, keys, slice_of, num_slices, mantissa_bits=8):
+        """The slice map: keys[i] (uint64) names slice slice_of[i] (< num_slices).  Clears every sum; num_slices = 0
+        with no keys removes slicing."""
+        keys = np.ascontiguousarray(keys, np.uint64)
+        slice_of = np.ascontiguousarray(slice_of, np.uint32)
+        if keys.size != slice_of.size:
+            raise ValueError("keys and slice_of differ in length")
+        _check(lib().xf_pv_set_slices(self.h, _p(keys), _p(slice_of), keys.size, int(num_slices), int(mantissa_bits)))
+        self.num_slices = int(num_slices)
+
+    def add_device_rows(self, d_pctr, d_labels, d_row_ptr, d_keys, rows, d_weights=None, stream=0):
+        """add_device plus each row's tokens: keys d_keys[row_ptr[r] .. row_ptr[r + 1]) (uint32 row_ptr, uint64 keys at
+        device addresses), which name its slices."""
+        _check(lib().xf_pv_add_device_rows(self.h, _p(d_pctr), _p(d_labels), _p(d_weights) if d_weights else None,
+                                           _p(d_row_ptr), _p(d_keys), int(rows), _p(stream) if stream else None))
+
+    def report_slices_bytes(self, n=None):
+        """The raw struct xf_pv_report of each slice, in slice order, for byte comparisons."""
+        n = self.num_slices if n is None else int(n)
+        arr = (PvReport * max(n, 1))()
+        _check(lib().xf_pv_report_slices(self.h, arr, n))
+        return [bytes(arr[s]) for s in range(n)]
+
+    def report_slices(self):
+        out = []
+        for raw in self.report_slices_bytes():
+            r = PvReport.from_buffer_copy(raw)
+            out.append({name: getattr(r, name) for name, _ in PvReport._fields_})
+        return out
 
 
 class Trainer:

@@ -1072,9 +1072,10 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
   }
   if (prof) XF_CUDA_TRY(cudaEventRecord(pe[3], st));
   if (mode == 0 && tr->pv) {
-    // the rows' pre-update predictions, labels and effective weights (NULL: all 1) into the pv
-    XF_TRY(xf_pv_add_device(tr->pv, pctr_out, d_labels, wv.e, rows, st));
-    ++tr->launches;
+    // the rows' pre-update predictions, labels and effective weights (NULL: all 1) into the pv; a sliced pv also
+    // reads each row's keys (xf_pv_set_slices is refused while a trainer feeds the pv)
+    XF_TRY(xf_pv_add_device_rows(tr->pv, pctr_out, d_labels, wv.e, d_row_ptr, d_keys, rows, st));
+    tr->launches += xf_pv_sliced(tr->pv) ? 2 : 1;
   }
   if (mode == 0) xf_admit_after_step(tr, adm, nnz);
   XF_CUDA_TRY(cudaGetLastError());

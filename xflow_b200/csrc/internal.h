@@ -218,6 +218,8 @@ int xf_trainer_forward_ingested(xf_trainer* tr, uint32_t row_start, uint32_t row
 // another) or stops feeding pv; xf_pv_destroy refuses a pv that trainers feed
 int xf_pv_attach(xf_pv* pv, int device);
 void xf_pv_detach(xf_pv* pv);
+// does pv have slices (xf_pv_set_slices)?  Its adds then launch two kernels, not one
+bool xf_pv_sliced(xf_pv* pv);
 
 // multi-GPU pieces implemented in comm.cu
 int xf_mg_create(xf_trainer* tr);

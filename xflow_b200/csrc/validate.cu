@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <mutex>
+#include <vector>
 
 #include "internal.h"
 
@@ -40,6 +41,17 @@ struct XfPvOut {
 constexpr int XF_PV_THREADS = 256;
 constexpr int XF_PV_REPORT_THREADS = 1024;
 
+constexpr u64 XF_PV_EMPTY_KEY = ~0ull;  // the reserved key
+constexpr uint32_t XF_PV_NO_SLICE = 0xFFFFFFFFu;
+constexpr uint32_t XF_PV_MAP_PROBES = 8;  // buckets past the home one
+struct XfPvSliceMap {
+  const u64* keys = nullptr;          // 4 per bucket, XF_PV_EMPTY_KEY where free
+  const uint32_t* slice = nullptr;    // per slot
+  u64 seed = 0;
+  uint32_t shift = 63, mask = 1;      // bucket = mix(key ^ seed) >> shift, 2^(64 - shift) buckets
+  uint32_t probes = 0;                // the longest probe of a present key: buckets past its home
+};
+
 }  // namespace
 
 struct xf_pv {
@@ -54,6 +66,15 @@ struct xf_pv {
   cudaEvent_t added = nullptr;      // recorded on an add's stream after the add
   cudaEvent_t cleared = nullptr;    // recorded on `stream` after the last reset: adds wait for it
   int attached = 0;                 // trainers feeding this pv
+  // slices (xf_pv_set_slices): n_slices sets of nbins_s bins and sums, and the map on the device
+  uint32_t n_slices = 0, ms = 0, nbins_s = 0;
+  XfPvBin* d_sbins = nullptr;
+  XfPvSums* d_ssums = nullptr;
+  XfPvOut* d_sout = nullptr;
+  XfPvOut* h_sout = nullptr;        // page-locked
+  u64* d_map_keys = nullptr;
+  uint32_t* d_map_slice = nullptr;
+  XfPvSliceMap map;
   std::mutex mu;
 };
 
@@ -84,6 +105,47 @@ __device__ __forceinline__ void xf_atomic_add192(u64* w, u64 a0, u64 a1, u64 a2)
 }
 
 __device__ __forceinline__ double xf_u128_to_double(u64 lo, u64 hi) { return (double)hi * 0x1p64 + (double)lo; }
+
+// a row's class and fixed-point terms (section 8): cls 0 / 1 for a scored negative / positive row, else one of the codes
+// below; bin, u (e), t (e * pc) and xl + 2^64 xh (e * l) are set for a scored row only.  The slice kernel's; xf_k_pv_add
+// keeps its own inline copy of the same arithmetic (through this function it compiles to 36 registers instead of 32),
+// and the tests hold the two to equal report bytes.
+enum { XF_PV_SKIP = -1, XF_PV_OVERFLOW = -2, XF_PV_NAN = -3 };
+struct XfPvRow {
+  int cls;
+  uint32_t bin;
+  u64 u, t, xl, xh;
+};
+__device__ __forceinline__ XfPvRow xf_pv_row(float e, const float* __restrict__ pctr, const uint8_t* __restrict__ labels,
+                                             uint64_t i, uint32_t m) {
+  XfPvRow v{XF_PV_SKIP, 0u, 0ull, 0ull, 0ull, 0ull};
+  if (e == 0.f) return v;
+  if (!(e >= 0.f && e < 2147483648.f)) {
+    v.cls = XF_PV_OVERFLOW;
+    return v;
+  }
+  const float p = pctr[i];
+  if (p != p) {
+    v.cls = XF_PV_NAN;
+    return v;
+  }
+  v.cls = labels[i] != 0 ? 1 : 0;
+  const uint32_t first_bin = 107u << m;  // bits(2^-20) >> (23 - m)
+  const float pc = fminf(fmaxf(p, 0x1p-20f), 1.f);
+  v.bin = (__float_as_uint(pc) >> (23 - m)) - first_bin;
+  v.u = __double2ull_rn((double)e * 4294967296.0);
+  v.t = __double2ull_rn((double)e * (double)pc * 4294967296.0);  // e * pc exact, < 2^63 units
+  const double q = fmin(fmax((double)p, 1e-15), 1.0 - 1e-15);
+  const double l = v.cls ? -log(q) : -log(1.0 - q);
+  const double x = (double)e * l * 4294967296.0;  // < 2^69 units
+  if (x < 0x1p64) {
+    v.xl = __double2ull_rn(x);
+  } else {  // an integer: the split is exact
+    v.xh = (u64)(x * 0x1p-64);
+    v.xl = (u64)(x - (double)v.xh * 0x1p64);
+  }
+  return v;
+}
 
 __global__ void __launch_bounds__(XF_PV_THREADS)
 xf_k_pv_add(const float* __restrict__ pctr, const uint8_t* __restrict__ labels, const float* __restrict__ weights,
@@ -187,10 +249,105 @@ xf_k_pv_add(const float* __restrict__ pctr, const uint8_t* __restrict__ labels, 
   }
 }
 
-// one block; out zeroed before
+// ---- slices (xf_pv_set_slices): an open-addressing map key -> slice in buckets of 4 keys, one 32-byte sector each.
+// A key's home bucket comes from a mix of all its bits; it sits in the first bucket from there with a free slot, and
+// slots fill in order, so a bucket whose last slot is free ends every probe through it.  The host builds the map and
+// bounds the longest probe (XF_PV_MAP_PROBES) by reseeding or doubling it.
+__host__ __device__ __forceinline__ u64 xf_pv_mix(u64 z) {  // splitmix64's finalizer: a bijection on 64 bits
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ uint32_t xf_pv_slice_of(const XfPvSliceMap& mp, u64 key) {
+  if (key == XF_PV_EMPTY_KEY) return XF_PV_NO_SLICE;
+  uint32_t b = (uint32_t)(xf_pv_mix(key ^ mp.seed) >> mp.shift);
+  for (uint32_t p = 0; p <= mp.probes; ++p, b = (b + 1) & mp.mask) {
+    const ulonglong2* q = reinterpret_cast<const ulonglong2*>(mp.keys + 4 * (size_t)b);
+    const ulonglong2 k01 = __ldg(q), k23 = __ldg(q + 1);
+    if (k01.x == key) return __ldg(mp.slice + 4 * (size_t)b);
+    if (k01.y == key) return __ldg(mp.slice + 4 * (size_t)b + 1);
+    if (k23.x == key) return __ldg(mp.slice + 4 * (size_t)b + 2);
+    if (k23.y == key) return __ldg(mp.slice + 4 * (size_t)b + 3);
+    if (k23.y == XF_PV_EMPTY_KEY) break;
+  }
+  return XF_PV_NO_SLICE;
+}
+
+// does a token in keys[beg, end) name slice s?  (warp-uniform arguments; the whole warp runs it)
+__device__ __forceinline__ bool xf_pv_named_in(XfPvSliceMap mp, const uint64_t* __restrict__ keys, uint32_t beg,
+                                            uint32_t end, uint32_t s, int lane) {
+  for (uint32_t base = beg; base < end; base += 32) {
+    const uint32_t j = base + lane;
+    if (__any_sync(0xffffffffu, j < end && xf_pv_slice_of(mp, keys[j]) == s)) return true;
+  }
+  return false;
+}
+
+// one warp per row, its lanes over 32-token chunks.  Each (row, slice) pair is added once, by the lowest lane of the
+// first chunk whose tokens name the slice: __match_any_sync finds a chunk's distinct slices, and the slices the row
+// has added so far sit one per lane in `seen` (the first 32; past those, earlier chunks are looked up again).
+__global__ void __launch_bounds__(XF_PV_THREADS)
+xf_k_pv_slice_add(const float* __restrict__ pctr, const uint8_t* __restrict__ labels,
+                  const float* __restrict__ weights, const uint32_t* __restrict__ row_ptr,
+                  const uint64_t* __restrict__ keys, uint64_t rows, XfPvSliceMap mp, uint32_t ms, uint32_t nbins_s,
+                  XfPvBin* __restrict__ bins, XfPvSums* __restrict__ sums) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+  for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < rows; r += warps) {
+    const float e = weights ? weights[r] : 1.f;
+    if (e == 0.f) continue;  // adds nothing anywhere
+    const uint32_t beg = row_ptr[r], end = row_ptr[r + 1];
+    uint32_t seen = XF_PV_NO_SLICE, n_seen = 0;
+    for (uint32_t base = beg; base < end; base += 32) {
+      const uint32_t j = base + lane;
+      const uint32_t s = j < end ? xf_pv_slice_of(mp, keys[j]) : XF_PV_NO_SLICE;
+      if (!__any_sync(0xffffffffu, s != XF_PV_NO_SLICE)) continue;
+      const unsigned peers = __match_any_sync(0xffffffffu, s);
+      unsigned leaders = __ballot_sync(0xffffffffu, s != XF_PV_NO_SLICE && lane == __ffs(peers) - 1);
+      unsigned fresh = 0;
+      while (leaders) {
+        const int l = __ffs(leaders) - 1;
+        leaders &= leaders - 1;
+        const uint32_t sl = __shfl_sync(0xffffffffu, s, l);
+        bool added = __any_sync(0xffffffffu, seen == sl);
+        if (!added && n_seen > 32) added = xf_pv_named_in(mp, keys, beg, base, sl, lane);
+        if (!added) {
+          if (lane == (int)n_seen) seen = sl;
+          ++n_seen;
+          fresh |= 1u << l;
+        }
+      }
+      if ((fresh >> lane) & 1u) {
+        const XfPvRow v = xf_pv_row(e, pctr, labels, r, ms);
+        XfPvSums* sp = sums + s;
+        if (v.cls == XF_PV_OVERFLOW) {
+          atomicAdd(&sp->overflow_rows, 1ull);
+        } else if (v.cls == XF_PV_NAN) {
+          atomicAdd(&sp->nan_rows, 1ull);
+        } else {
+          // the low words first, all three in flight at once; each carry then goes on as in xf_atomic_add128
+          XfPvBin* bp = bins + (size_t)s * nbins_s + v.bin;
+          atomicAdd(&bp->n[v.cls], 1ull);
+          const u64 ow = atomicAdd(&bp->w[v.cls][0], v.u);
+          const u64 oe = atomicAdd(&sp->el[0], v.xl);
+          const u64 op = atomicAdd(&sp->ep[0], v.t);
+          if (ow + v.u < ow) atomicAdd(&bp->w[v.cls][1], 1ull);
+          xf_atomic_add128(sp->el + 1, v.xh + (oe + v.xl < oe ? 1ull : 0ull), 0ull);
+          if (op + v.t < op) atomicAdd(&sp->ep[1], 1ull);
+        }
+      }
+    }
+  }
+}
+
+// one block per accumulator set (the global one, or one per slice); out zeroed before
 __global__ void __launch_bounds__(XF_PV_REPORT_THREADS)
 xf_k_pv_report(const XfPvBin* __restrict__ bins, uint32_t nbins, const XfPvSums* __restrict__ sums,
                XfPvOut* __restrict__ out) {
+  bins += (size_t)blockIdx.x * nbins;
+  sums += blockIdx.x;
+  out += blockIdx.x;
   __shared__ u64 s_lo[XF_PV_REPORT_THREADS], s_hi[XF_PV_REPORT_THREADS];
   __shared__ double s_a[XF_PV_REPORT_THREADS], s_t[XF_PV_REPORT_THREADS];
   const int t = threadIdx.x;
@@ -348,6 +505,23 @@ XF_DLL int xf_pv_create(xf_pv** out, int device, uint32_t mantissa_bits) {
   return XF_OK;
 }
 
+static void xf_pv_free_slices(xf_pv* pv) {
+  cudaFree(pv->d_sbins);
+  cudaFree(pv->d_ssums);
+  cudaFree(pv->d_sout);
+  if (pv->h_sout) cudaFreeHost(pv->h_sout);
+  cudaFree(pv->d_map_keys);
+  cudaFree(pv->d_map_slice);
+  pv->d_sbins = nullptr;
+  pv->d_ssums = nullptr;
+  pv->d_sout = nullptr;
+  pv->h_sout = nullptr;
+  pv->d_map_keys = nullptr;
+  pv->d_map_slice = nullptr;
+  pv->map = XfPvSliceMap();
+  pv->n_slices = pv->ms = pv->nbins_s = 0;
+}
+
 XF_DLL int xf_pv_destroy(xf_pv* pv) {
   if (!pv) return XF_OK;
   if (pv->attached) {
@@ -361,6 +535,7 @@ XF_DLL int xf_pv_destroy(xf_pv* pv) {
   cudaFree(pv->d_sums);
   cudaFree(pv->d_out);
   if (pv->h_out) cudaFreeHost(pv->h_out);
+  xf_pv_free_slices(pv);
   if (pv->added) cudaEventDestroy(pv->added);
   if (pv->cleared) cudaEventDestroy(pv->cleared);
   if (pv->stream) cudaStreamDestroy(pv->stream);
@@ -368,21 +543,157 @@ XF_DLL int xf_pv_destroy(xf_pv* pv) {
   return XF_OK;
 }
 
-XF_DLL int xf_pv_reset(xf_pv* pv) {
-  if (!pv) return XF_ERR_ARG;
-  std::lock_guard<std::mutex> lk(pv->mu);
+// under pv->mu
+static int xf_pv_clear(xf_pv* pv) {
   XF_CUDA_TRY(cudaSetDevice(pv->device));
   XF_CUDA_TRY(cudaMemsetAsync(pv->d_bins, 0, (size_t)pv->nbins * sizeof(XfPvBin), pv->stream));
   XF_CUDA_TRY(cudaMemsetAsync(pv->d_sums, 0, sizeof(XfPvSums), pv->stream));
+  if (pv->n_slices) {
+    XF_CUDA_TRY(cudaMemsetAsync(pv->d_sbins, 0, (size_t)pv->n_slices * pv->nbins_s * sizeof(XfPvBin), pv->stream));
+    XF_CUDA_TRY(cudaMemsetAsync(pv->d_ssums, 0, (size_t)pv->n_slices * sizeof(XfPvSums), pv->stream));
+  }
   XF_CUDA_TRY(cudaEventRecord(pv->cleared, pv->stream));
   return XF_OK;
+}
+
+XF_DLL int xf_pv_reset(xf_pv* pv) {
+  if (!pv) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(pv->mu);
+  return xf_pv_clear(pv);
+}
+
+// The slice map on the host: 2^log2b buckets of 4 slots, the key in the first bucket from its home with a free slot.
+// XF_ERR_ARG, naming the key, for a key listed twice.  probes: the longest walk past a key's home bucket.
+static int xf_pv_build_map(const uint64_t* keys, const uint32_t* slice_of, uint64_t n, uint32_t log2b, u64 seed,
+                           std::vector<u64>& mk, std::vector<uint32_t>& ms, uint32_t* probes) {
+  const uint64_t nb = 1ull << log2b, mask = nb - 1;
+  mk.assign(4 * nb, XF_PV_EMPTY_KEY);
+  ms.assign(4 * nb, XF_PV_NO_SLICE);
+  *probes = 0;
+  for (uint64_t i = 0; i < n; ++i) {
+    uint64_t b = xf_pv_mix(keys[i] ^ seed) >> (64 - log2b);
+    for (uint32_t p = 0;; ++p, b = (b + 1) & mask) {
+      int k = 0;
+      while (k < 4 && mk[4 * b + k] != XF_PV_EMPTY_KEY && mk[4 * b + k] != keys[i]) ++k;
+      if (k == 4) continue;
+      if (mk[4 * b + k] == keys[i]) {
+        xf_set_error("xf_pv_set_slices: key %llu is listed twice (a key names at most one slice)",
+                     (unsigned long long)keys[i]);
+        return XF_ERR_ARG;
+      }
+      mk[4 * b + k] = keys[i];
+      ms[4 * b + k] = slice_of[i];
+      if (p > *probes) *probes = p;
+      break;
+    }
+  }
+  return XF_OK;
+}
+
+XF_DLL int xf_pv_set_slices(xf_pv* pv, const uint64_t* keys, const uint32_t* slice_of, uint64_t n_keys,
+                            uint32_t n_slices, uint32_t slice_mantissa_bits) {
+  if (!pv || ((!keys || !slice_of) && n_keys)) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(pv->mu);
+  if (pv->attached) {
+    xf_set_error("xf_pv_set_slices: %d trainer(s) feed this pv; detach it (xf_trainer_set_validation(tr, NULL)), set "
+                 "the slices, then attach it again", pv->attached);
+    return XF_ERR_STATE;
+  }
+  if (n_slices > 65536) {
+    xf_set_error("xf_pv_set_slices: n_slices must be at most 65536, got %u", n_slices);
+    return XF_ERR_ARG;
+  }
+  if (n_keys > (1ull << 24)) {
+    xf_set_error("xf_pv_set_slices: n_keys must be at most 2^24, got %llu", (unsigned long long)n_keys);
+    return XF_ERR_ARG;
+  }
+  const uint32_t ms = slice_mantissa_bits;
+  if (n_slices && (ms < 4 || ms > 16)) {
+    xf_set_error("xf_pv_set_slices: slice_mantissa_bits must be 4 .. 16, got %u", ms);
+    return XF_ERR_ARG;
+  }
+  const uint64_t nbins_s = n_slices ? (20ull << ms) + 1 : 0;
+  const uint64_t bytes = (uint64_t)n_slices * (nbins_s * sizeof(XfPvBin) + sizeof(XfPvSums));
+  if (bytes > (1ull << 30)) {
+    xf_set_error("xf_pv_set_slices: %u slices at slice_mantissa_bits %u need %llu bytes of accumulators, over 1 GiB "
+                 "(fewer slices or fewer mantissa bits)", n_slices, ms, (unsigned long long)bytes);
+    return XF_ERR_ARG;
+  }
+  for (uint64_t i = 0; i < n_keys; ++i) {
+    if (slice_of[i] >= n_slices) {
+      xf_set_error("xf_pv_set_slices: slice_of[%llu] = %u is not below n_slices = %u", (unsigned long long)i,
+                   slice_of[i], n_slices);
+      return XF_ERR_ARG;
+    }
+    if (keys[i] == XF_PV_EMPTY_KEY) {
+      xf_set_error("xf_pv_set_slices: keys[%llu] is the reserved key 2^64 - 1", (unsigned long long)i);
+      return XF_ERR_ARG;
+    }
+  }
+  // at least twice the slots as keys; reseeded, then doubled, while a key sits more than XF_PV_MAP_PROBES buckets
+  // past its home (a bound that only an adversarial key set should reach; past it lookups stay exact, only longer)
+  std::vector<u64> mk;
+  std::vector<uint32_t> msl;
+  uint32_t log2b = 1, probes = 0;
+  u64 seed = 0;
+  if (n_slices) {
+    uint32_t base = 1;
+    while ((4ull << base) < 2 * n_keys) ++base;
+    for (int attempt = 0; attempt < 8; ++attempt) {
+      seed = xf_pv_mix(0x9e3779b97f4a7c15ull * (u64)(attempt + 1));
+      log2b = base + (uint32_t)attempt / 4;
+      XF_TRY(xf_pv_build_map(keys, slice_of, n_keys, log2b, seed, mk, msl, &probes));
+      if (probes <= XF_PV_MAP_PROBES) break;
+    }
+  }
+  // the adds enqueued so far (pv->stream waits for each) may still read the old map and accumulators
+  XF_CUDA_TRY(cudaSetDevice(pv->device));
+  XF_CUDA_TRY(cudaStreamSynchronize(pv->stream));
+  xf_pv_free_slices(pv);
+  if (n_slices) {
+    int rc = XF_OK;
+    auto fail = [&](cudaError_t e) {
+      if (e != cudaSuccess && rc == XF_OK) {
+        xf_set_error("xf_pv_set_slices: %s", cudaGetErrorString(e));
+        rc = XF_ERR_CUDA;
+      }
+    };
+    fail(cudaMalloc(&pv->d_sbins, (size_t)n_slices * nbins_s * sizeof(XfPvBin)));
+    if (rc == XF_OK) fail(cudaMalloc(&pv->d_ssums, (size_t)n_slices * sizeof(XfPvSums)));
+    if (rc == XF_OK) fail(cudaMalloc(&pv->d_sout, (size_t)n_slices * sizeof(XfPvOut)));
+    if (rc == XF_OK) fail(cudaHostAlloc(&pv->h_sout, (size_t)n_slices * sizeof(XfPvOut), cudaHostAllocDefault));
+    if (rc == XF_OK) fail(cudaMalloc(&pv->d_map_keys, mk.size() * sizeof(u64)));
+    if (rc == XF_OK) fail(cudaMalloc(&pv->d_map_slice, msl.size() * sizeof(uint32_t)));
+    if (rc == XF_OK) fail(cudaMemcpy(pv->d_map_keys, mk.data(), mk.size() * sizeof(u64), cudaMemcpyHostToDevice));
+    if (rc == XF_OK)
+      fail(cudaMemcpy(pv->d_map_slice, msl.data(), msl.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (rc != XF_OK) {  // the pv is left without slices, its sums cleared
+      xf_pv_free_slices(pv);
+      xf_pv_clear(pv);
+      return rc;
+    }
+    pv->n_slices = n_slices;
+    pv->ms = ms;
+    pv->nbins_s = (uint32_t)nbins_s;
+    pv->map.keys = pv->d_map_keys;
+    pv->map.slice = pv->d_map_slice;
+    pv->map.seed = seed;
+    pv->map.shift = 64 - log2b;
+    pv->map.mask = (1u << log2b) - 1;
+    pv->map.probes = probes;
+  }
+  return xf_pv_clear(pv);
 }
 
 XF_DLL int xf_pv_add_device(xf_pv* pv, const float* d_pctr, const uint8_t* d_labels, const float* d_weights,
                             uint64_t n, void* cuda_stream) {
   if (!pv || ((!d_pctr || !d_labels) && n)) return XF_ERR_ARG;
-  if (n == 0) return XF_OK;
   std::lock_guard<std::mutex> lk(pv->mu);
+  if (pv->n_slices) {
+    xf_set_error("xf_pv_add_device: a sliced pv needs each row's keys: xf_pv_add_device_rows");
+    return XF_ERR_STATE;
+  }
+  if (n == 0) return XF_OK;
   XF_CUDA_TRY(cudaSetDevice(pv->device));
   cudaStream_t st = (cudaStream_t)cuda_stream;
   // after the last reset; the pv's stream (resets, reports) after this add
@@ -395,16 +706,34 @@ XF_DLL int xf_pv_add_device(xf_pv* pv, const float* d_pctr, const uint8_t* d_lab
   return XF_OK;
 }
 
-XF_DLL int xf_pv_report(xf_pv* pv, struct xf_pv_report* out) {
-  if (!pv || !out) return XF_ERR_ARG;
-  std::lock_guard<std::mutex> lk(pv->mu);
-  XF_CUDA_TRY(cudaSetDevice(pv->device));
-  XF_CUDA_TRY(cudaMemsetAsync(pv->d_out, 0, sizeof(XfPvOut), pv->stream));
-  xf_k_pv_report<<<1, XF_PV_REPORT_THREADS, 0, pv->stream>>>(pv->d_bins, pv->nbins, pv->d_sums, pv->d_out);
-  XF_CUDA_TRY(cudaGetLastError());
-  XF_CUDA_TRY(cudaMemcpyAsync(pv->h_out, pv->d_out, sizeof(XfPvOut), cudaMemcpyDeviceToHost, pv->stream));
-  XF_CUDA_TRY(cudaStreamSynchronize(pv->stream));
-  const XfPvOut& h = *pv->h_out;
+XF_DLL int xf_pv_add_device_rows(xf_pv* pv, const float* d_pctr, const uint8_t* d_labels, const float* d_weights,
+                                 const uint32_t* d_row_ptr, const uint64_t* d_keys, uint64_t rows, void* cuda_stream) {
+  if (!pv || ((!d_pctr || !d_labels) && rows)) return XF_ERR_ARG;
+  if (rows == 0) return XF_OK;
+  {
+    std::lock_guard<std::mutex> lk(pv->mu);
+    if (pv->n_slices) {
+      if (!d_row_ptr || !d_keys) return XF_ERR_ARG;
+      XF_CUDA_TRY(cudaSetDevice(pv->device));
+      cudaStream_t st = (cudaStream_t)cuda_stream;
+      XF_CUDA_TRY(cudaStreamWaitEvent(st, pv->cleared, 0));
+      xf_k_pv_add<<<xf_grid_for(rows, XF_PV_THREADS, 4), XF_PV_THREADS, 0, st>>>(d_pctr, d_labels, d_weights, rows,
+                                                                                 pv->m, pv->d_bins, pv->d_sums);
+      XF_CUDA_TRY(cudaGetLastError());
+      xf_k_pv_slice_add<<<xf_grid_for(rows * 32, XF_PV_THREADS, 8), XF_PV_THREADS, 0, st>>>(
+          d_pctr, d_labels, d_weights, d_row_ptr, d_keys, rows, pv->map, pv->ms, pv->nbins_s, pv->d_sbins,
+          pv->d_ssums);
+      XF_CUDA_TRY(cudaGetLastError());
+      XF_CUDA_TRY(cudaEventRecord(pv->added, st));
+      XF_CUDA_TRY(cudaStreamWaitEvent(pv->stream, pv->added, 0));
+      return XF_OK;
+    }
+  }
+  return xf_pv_add_device(pv, d_pctr, d_labels, d_weights, rows, cuda_stream);
+}
+
+// one report record from the device's exact sums
+static void xf_pv_fill_report(const XfPvOut& h, struct xf_pv_report* out) {
   memset(out, 0, sizeof(*out));
   out->negatives = h.n[0];
   out->positives = h.n[1];
@@ -431,10 +760,46 @@ XF_DLL int xf_pv_report(xf_pv* pv, struct xf_pv_report* out) {
   } else {
     out->auc_lo = out->auc_hi = out->auc = NAN;
   }
+}
+
+XF_DLL int xf_pv_report(xf_pv* pv, struct xf_pv_report* out) {
+  if (!pv || !out) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(pv->mu);
+  XF_CUDA_TRY(cudaSetDevice(pv->device));
+  XF_CUDA_TRY(cudaMemsetAsync(pv->d_out, 0, sizeof(XfPvOut), pv->stream));
+  xf_k_pv_report<<<1, XF_PV_REPORT_THREADS, 0, pv->stream>>>(pv->d_bins, pv->nbins, pv->d_sums, pv->d_out);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(pv->h_out, pv->d_out, sizeof(XfPvOut), cudaMemcpyDeviceToHost, pv->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(pv->stream));
+  xf_pv_fill_report(*pv->h_out, out);
+  return XF_OK;
+}
+
+XF_DLL int xf_pv_report_slices(xf_pv* pv, struct xf_pv_report* out, uint32_t n) {
+  if (!pv || (!out && n)) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(pv->mu);
+  if (n != pv->n_slices || n == 0) {
+    xf_set_error("xf_pv_report_slices: n = %u, but the pv has %u slices%s", n, pv->n_slices,
+                 pv->n_slices ? "" : " (xf_pv_set_slices sets them)");
+    return XF_ERR_ARG;
+  }
+  XF_CUDA_TRY(cudaSetDevice(pv->device));
+  const size_t bytes = (size_t)n * sizeof(XfPvOut);
+  XF_CUDA_TRY(cudaMemsetAsync(pv->d_sout, 0, bytes, pv->stream));
+  xf_k_pv_report<<<n, XF_PV_REPORT_THREADS, 0, pv->stream>>>(pv->d_sbins, pv->nbins_s, pv->d_ssums, pv->d_sout);
+  XF_CUDA_TRY(cudaGetLastError());
+  XF_CUDA_TRY(cudaMemcpyAsync(pv->h_sout, pv->d_sout, bytes, cudaMemcpyDeviceToHost, pv->stream));
+  XF_CUDA_TRY(cudaStreamSynchronize(pv->stream));
+  for (uint32_t s = 0; s < n; ++s) xf_pv_fill_report(pv->h_sout[s], out + s);
   return XF_OK;
 }
 
 // ---- the trainers' side (capi.cu)
+bool xf_pv_sliced(xf_pv* pv) {
+  std::lock_guard<std::mutex> lk(pv->mu);
+  return pv->n_slices != 0;
+}
+
 int xf_pv_attach(xf_pv* pv, int device) {
   if (pv->device != device) {
     xf_set_error("xf_trainer_set_validation: the pv lives on device %d, the trainer's table on device %d", pv->device,

@@ -7,12 +7,15 @@
 #include <string.h>
 
 #include <algorithm>
+#include <fstream>
 #include <functional>
 #include <iostream>
 #include <memory>
 #include <mutex>
+#include <sstream>
 #include <stdexcept>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/xflow/xflow.h"
@@ -140,6 +143,47 @@ static bool ProgressiveFromEnv(int world) {
   if (world > 1)
     throw std::runtime_error("XFLOW_PROGRESSIVE is single-GPU only: unset it or run with XFLOW_WORLD = 1");
   return true;
+}
+
+// Sliced progressive validation (xf_pv_set_slices): XFLOW_PV_SLICES = <path> reports the progressive metric per
+// segment too.  The file holds one "<feature id> <slice>" pair per line; the id is hashed as the loader hashes the
+// text's ids, so a row belongs to every slice its ids name.  n_slices is the largest slice + 1, binned with 8 mantissa
+// bits.  Needs XFLOW_PROGRESSIVE = 1; single GPU only.  A malformed file or an id listed twice fails here.
+struct PvSlices {
+  std::vector<uint64_t> keys;
+  std::vector<uint32_t> slice_of;
+  uint32_t n = 0;  // 0: no slices
+};
+static PvSlices PvSlicesFromEnv(int world) {
+  PvSlices ps;
+  const char* path = getenv("XFLOW_PV_SLICES");
+  if (!path || !*path) return ps;
+  if (world > 1) throw std::runtime_error("XFLOW_PV_SLICES is single-GPU only: unset it or run with XFLOW_WORLD = 1");
+  if (!ProgressiveFromEnv(1)) throw std::runtime_error("XFLOW_PV_SLICES needs XFLOW_PROGRESSIVE = 1");
+  std::ifstream in(path);
+  if (!in) throw std::runtime_error(std::string("XFLOW_PV_SLICES: cannot open '") + path + "'");
+  std::unordered_map<uint64_t, uint64_t> line_of;  // key -> the line that named it
+  std::string text, id, slice, extra;
+  for (uint64_t line = 1; std::getline(in, text); ++line) {
+    const std::string where = std::string("XFLOW_PV_SLICES: ") + path + " line " + std::to_string(line);
+    std::istringstream ss(text);
+    id.clear();
+    slice.clear();
+    if (!(ss >> id >> slice) || (ss >> extra) || slice.size() > 5 ||
+        slice.find_first_not_of("0123456789") != std::string::npos)
+      throw std::runtime_error(where + " is not '<feature id> <slice>'");
+    const unsigned long s = strtoul(slice.c_str(), nullptr, 10);
+    if (s >= 65536) throw std::runtime_error(where + ": slice " + slice + " is over 65535");
+    const uint64_t key = xf_hash_bytes(id.data(), id.size());
+    const auto ins = line_of.emplace(key, line);
+    if (!ins.second)
+      throw std::runtime_error(where + ": id '" + id + "' was named on line " + std::to_string(ins.first->second));
+    ps.keys.push_back(key);
+    ps.slice_of.push_back((uint32_t)s);
+    ps.n = std::max(ps.n, (uint32_t)s + 1);
+  }
+  if (ps.n == 0) throw std::runtime_error(std::string("XFLOW_PV_SLICES: ") + path + " names no slice");
+  return ps;
 }
 
 // the table's training-batch number (host state, no device sync)
@@ -304,6 +348,7 @@ Server::Server(Optimizer opt, int latent_dim, int device)
   uint64_t every = 0;
   EvictionFromEnv(world_, &every);  // likewise XFLOW_EVICT_*
   NegSampleFromEnv(world_);         // and XFLOW_NEG_SAMPLE
+  PvSlicesFromEnv(world_);          // and XFLOW_PV_SLICES (its file too)
   ProgressiveFromEnv(world_);       // and XFLOW_PROGRESSIVE
   env_path("XFLOW_CHECKPOINT", world_);
   env_path("XFLOW_RESUME", world_);
@@ -543,12 +588,21 @@ void WorkerBase::run_blocks(uint64_t collective_blocks, const std::function<void
   }
 }
 
-// one line per epoch: the progressive metric of that epoch's training rows (%.17g: the report's doubles exactly)
-static void PrintProgressive(xf_pv* pv, int epoch) {
+// one line per epoch: the progressive metric of that epoch's training rows (%.17g: the report's doubles exactly),
+// then one per slice (XFLOW_PV_SLICES)
+static void PrintProgressive(xf_pv* pv, int epoch, uint32_t n_slices) {
   struct xf_pv_report r;
   must(xf_pv_report(pv, &r), "xf_pv_report");
   printf("progressive epoch %d : logloss = %.17g  auc = %.17g [%.17g, %.17g]  mean_pctr = %.17g  ctr = %.17g  "
          "rows = %llu\n", epoch, r.logloss, r.auc, r.auc_lo, r.auc_hi, r.mean_pctr, r.ctr, (unsigned long long)r.rows);
+  if (n_slices) {
+    std::vector<struct xf_pv_report> rs(n_slices);
+    must(xf_pv_report_slices(pv, rs.data(), n_slices), "xf_pv_report_slices");
+    for (uint32_t s = 0; s < n_slices; ++s)
+      printf("progressive epoch %d slice %u : logloss = %.17g  auc = %.17g [%.17g, %.17g]  mean_pctr = %.17g  "
+             "ctr = %.17g  rows = %llu\n", epoch, s, rs[s].logloss, rs[s].auc, rs[s].auc_lo, rs[s].auc_hi,
+             rs[s].mean_pctr, rs[s].ctr, (unsigned long long)rs[s].rows);
+  }
   fflush(stdout);
   must(xf_pv_reset(pv), "xf_pv_reset");
 }
@@ -571,6 +625,10 @@ void WorkerBase::batch_training() {
   }
   if (!pv_ && ProgressiveFromEnv(1)) {  // XFLOW_WORLD > 1 was refused at Server creation
     must(xf_pv_create(&pv_, Server::Get()->device(), 10), "xf_pv_create");
+    const PvSlices ps = PvSlicesFromEnv(1);
+    if (ps.n)
+      must(xf_pv_set_slices(pv_, ps.keys.data(), ps.slice_of.data(), ps.keys.size(), ps.n, 8), "xf_pv_set_slices");
+    pv_slices_ = ps.n;
     must(xf_trainer_set_validation(trainer_, pv_), "xf_trainer_set_validation");
   }
   uint64_t collective_blocks = 0;
@@ -604,7 +662,7 @@ void WorkerBase::batch_training() {
       for (int i = 0; i < core_num; ++i) update(i * thread_size, (i + 1) * thread_size);  // :192-196
     }
     must(xf_trainer_sync(trainer_), "xf_trainer_sync");
-    if (pv_) PrintProgressive(pv_, epoch);
+    if (pv_) PrintProgressive(pv_, epoch, pv_slices_);
     if (!checkpoint.empty())
       must(xf_table_save_state(table_, checkpoint.c_str(), (uint64_t)epoch + 1), "xf_table_save_state");
     if (!deltas.empty()) ExportEpoch(table_, deltas, (uint64_t)epoch + 1, exported);
