@@ -48,7 +48,8 @@ enum {
 
 enum { XF_MODEL_LR = 0, XF_MODEL_FM = 1,              /* main.cc:26-39: '0' = LR, '1' = FM */
        XF_MODEL_FM_CANONICAL = 2,                     /* NOT the reference's model: the textbook FM, see below */
-       XF_MODEL_MVM = 3 };                            /* a DEFINED multi-view machine (mvm_worker.cc is not), see below */
+       XF_MODEL_MVM = 3,                              /* a DEFINED multi-view machine (mvm_worker.cc is not), see below */
+       XF_MODEL_FFM = 4 };                            /* the field-aware FM (libffm's model), see below */
 enum { XF_OPTIMIZER_FTRL = 0, XF_OPTIMIZER_SGD = 1 }; /* server.h:24-29 (comment toggle in the reference) */
 enum {
   XF_VINIT_DEFAULT = 0,  /* FTRL: N(0,1)*1e-2 (ftrl.h:114-120, counter-based here); SGD: 0.001 (sgd.h:68-70) */
@@ -80,7 +81,8 @@ typedef struct xf_table_config {
   uint64_t capacity;     /* initial slot count (rounded up to a power of two); 0 = 1<<20.  Grows on demand. */
   int shard_index;       /* this table owns keys of shard_index out of num_shards (postoffice.cc:134-143) */
   int num_shards;        /* 1 = whole key space */
-  int canonical_fm;      /* 1: rows carry the accumulators of XF_MODEL_FM_CANONICAL / XF_MODEL_MVM (latent_dim in {4,8,16,32,64,128}) */
+  int canonical_fm;      /* 1: rows carry the accumulators of XF_MODEL_FM_CANONICAL / XF_MODEL_MVM / XF_MODEL_FFM
+                            (latent_dim in {4,8,16,32,64,128}) */
 } xf_table_config;
 
 /* fills *cfg with the reference's compile-time defaults (ftrl.h:15-20, sgd.h:16) */
@@ -240,7 +242,7 @@ XF_DLL int xf_table_last_touch(xf_table* t, const uint64_t* keys, uint64_t n, ui
  * on bit for bit as the saved table would have: a run that saves and continues, and a run resumed from the image,
  * both equal the run that never saved.  For XF_MODEL_FM_CANONICAL and XF_MODEL_MVM that holds on batches with repeated
  * keys in deterministic mode (xf_trainer_set_deterministic); their default steps sum a repeated key's terms in atomic
- * order.  Not in the image: the trainers' state (xf_trainer_stats counters, the
+ * order.  XF_MODEL_FFM has no deterministic mode: it holds on batches in which no key repeats.  Not in the image: the trainers' state (xf_trainer_stats counters, the
  * negative-sampling policy, which is caller config) and xf_table_set_stream's choice.
  * Save runs stream-ordered after everything enqueued on the table's stream, waits for it, and changes nothing in the
  * table.  It writes <path>.tmp and renames it to <path>; on failure no .tmp is left.  Saving the same state twice
@@ -340,6 +342,32 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
 XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_ptr, const uint64_t* keys,
                                           const uint8_t* fields, const float* vals, uint32_t rows, uint32_t nnz,
                                           float* pctr_out);
+/* The field-aware factorisation machine, XF_MODEL_FFM (Juan, Zhuang, Chin, Lin, RecSys 2016; libffm's model;
+ * csrc/step_ffm.cu), through the same two entry points.  Needs a table created with canonical_fm = 1 (any latent_dim
+ * L in {4,8,16,32,64,128}) and no comm.
+ *   Layout: the per-field latent dimension is 4 (libffm's default -k 4), so the table holds F = L / 4 fields.  A key's
+ *   latent row v[L] is F pieces of 4 floats: piece b (coordinates 4b .. 4b+3) is v_{i,b}, the key's vector for
+ *   interacting with field b.  Rows, optimizer state, xf_table_export / _import and the state image are the canonical
+ *   tables' own.  Field ids must be < F (18 fields need L = 128, of whose 32 pieces 14 are then never used: the rows
+ *   cost what 32 fields would).
+ *   Definition, row r with tokens i (key k_i, field f_i, value x_i; vals NULL = all 1):
+ *     y = sum_i w_i x_i + sum_{i<j} <v_{i,f_j}, v_{j,f_i}> x_i x_j      (pairs of token positions, same field included)
+ *     p = sigmoid(y) ,  r = p - label                                    (a row without tokens: y = 0; no global bias)
+ *     dL/dw_i = r x_i ,  dL/dv_{i,b} = r x_i ( T[b][f_i] - [b = f_i] x_i v_{i,f_i} ) ,  T[a][b] = sum_{f_i = a} x_i v_{i,b}
+ *   gradients / rows and one FTRL or SGD step per touched key on w and all L coordinates, as XF_MODEL_FM_CANONICAL.
+ *   Absent keys are inserted on pull, in training and in predict.
+ *   Fixed-order forward: T[a][b], sum w x and Q = sum x^2 |v_{i,f_i}|^2 are added in ascending token position from +0,
+ *   the pair sum over the present fields a ascending, the warp reduction by the xor 16 .. 1 tree.  So a row's
+ *   prediction depends only on its tokens and on the table, not on its batch, its place in it or the grid, and
+ *   xf_trainer_predict_host_fields returns, bit for bit, what a training step on that table state computes (and
+ *   feeds an attached pv).  Per-key gradient sums are float atomics: a key repeated within a batch gets bits that
+ *   depend on the order they land in (see xf_table_save_state).
+ *   Refused with XF_ERR_ARG: every entry point without field ids when nnz > 0 (xf_trainer_step_host, _device,
+ *   _values, _async, the ingested steps and their predicts), field ids >= F (naming the token and the bound),
+ *   xf_trainer_set_deterministic, importance weighting and negative sampling.
+ *   Kernels per step (xf_trainer_launches): training, the step kernel and the optimizer pass (+1 with a pv); predict,
+ *   one.  No serving model yet: xf_table_freeze_canonical / _mvm of an FFM-trained table give those models'
+ *   forwards, not this one's. */
 /* Deterministic mode for XF_MODEL_FM_CANONICAL and XF_MODEL_MVM trainers (csrc/step_det.cu).  The default steps of
  * these two models add each token's gradient terms into its key's accumulators with float atomics (and the machine's
  * forward adds a row's same-field terms with shared-memory atomics), so a key with several tokens in a batch gets bits

@@ -11,7 +11,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libxflow_b200.so")
 
-MODEL_LR, MODEL_FM, MODEL_FM_CANONICAL, MODEL_MVM = 0, 1, 2, 3
+MODEL_LR, MODEL_FM, MODEL_FM_CANONICAL, MODEL_MVM, MODEL_FFM = 0, 1, 2, 3, 4
 OPT_FTRL, OPT_SGD = 0, 1
 VINIT_DEFAULT, VINIT_COUNTER, VINIT_ZERO = 0, 1, 3
 ADMIT_ALL, ADMIT_POISSON, ADMIT_BLOOM = 0, 1, 2
@@ -946,7 +946,8 @@ class Trainer:
         return out
 
     def step_host_fields(self, row_ptr, keys, fields, vals, labels):
-        """One step of the defined multi-view machine (XF_MODEL_MVM): host CSR arrays + the tokens' field ids."""
+        """One step of the defined multi-view machine (XF_MODEL_MVM, field ids < 32) or the field-aware FM
+        (XF_MODEL_FFM, field ids < latent_dim / 4): host CSR arrays + the tokens' field ids; vals may be None (all 1)."""
         row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
         keys = np.ascontiguousarray(keys, np.uint64)
         fields = np.ascontiguousarray(fields, np.uint8)
@@ -958,6 +959,7 @@ class Trainer:
         return loss.value
 
     def predict_host_fields(self, row_ptr, keys, fields, vals):
+        """Forward only of an XF_MODEL_MVM or XF_MODEL_FFM trainer on host CSR arrays + field ids; returns pctr[rows]."""
         row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
         keys = np.ascontiguousarray(keys, np.uint64)
         fields = np.ascontiguousarray(fields, np.uint8)

@@ -810,8 +810,13 @@ XF_DLL int xf_trainer_create(xf_trainer** out, xf_table* table, xf_comm* comm, c
     xf_set_error("XF_MODEL_MVM needs a table created with canonical_fm = 1, latent_dim <= 32 and no comm");
     return XF_ERR_ARG;
   }
-  if (cfg->model != XF_MODEL_FM_CANONICAL && cfg->model != XF_MODEL_MVM && table->view.canon) {
-    xf_set_error("canonical tables serve XF_MODEL_FM_CANONICAL and XF_MODEL_MVM only");
+  if (cfg->model == XF_MODEL_FFM && (!table->view.canon || comm)) {
+    xf_set_error("XF_MODEL_FFM needs a table created with canonical_fm = 1 and no comm");
+    return XF_ERR_ARG;
+  }
+  if (cfg->model != XF_MODEL_FM_CANONICAL && cfg->model != XF_MODEL_MVM && cfg->model != XF_MODEL_FFM &&
+      table->view.canon) {
+    xf_set_error("canonical tables serve XF_MODEL_FM_CANONICAL, XF_MODEL_MVM and XF_MODEL_FFM only");
     return XF_ERR_ARG;
   }
   if (cfg->model == XF_MODEL_LR && table->view.K != 0) { xf_set_error("LR needs latent_dim == 0"); return XF_ERR_ARG; }
@@ -1039,8 +1044,10 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
                            loss_out, pctr_out, d_abs, tr->d_unique_total, adm, sv, wv, st);
   } else {
     const bool mvm = tr->cfg.model == XF_MODEL_MVM;
-    const bool canon = tr->cfg.model == XF_MODEL_FM_CANONICAL || mvm;
+    const bool ffm = tr->cfg.model == XF_MODEL_FFM;
+    const bool canon = tr->cfg.model == XF_MODEL_FM_CANONICAL || mvm || ffm;
     if (mvm && !d_fields && nnz) { xf_set_error("XF_MODEL_MVM steps need the tokens' field ids (xf_trainer_step_host_fields)"); return XF_ERR_ARG; }
+    if (ffm && !d_fields && nnz) { xf_set_error("XF_MODEL_FFM steps need the tokens' field ids (xf_trainer_step_host_fields)"); return XF_ERR_ARG; }
     extra = canon ? 0u : xf_step_touched_extra(t->view.K, (int)rows);
     XF_TRY(tr->touched.ensure(((size_t)nnz + extra) * 4));
     // deterministic mode: every training step, and the machine's predict (the canonical FM's forward has a fixed
@@ -1049,7 +1056,10 @@ static int xf_step_device_impl(xf_trainer* tr, const uint32_t* d_row_ptr, const 
       XF_TRY(xf_det_step(t->view, *tr->det, mvm, d_row_ptr, d_keys, d_vals, d_fields, d_labels, rows, nnz, mode,
                          tr->touched.as<uint32_t>(), loss_out, pctr_out, d_abs, st));
       if (mode == 0) tr->launches += xf_det_extra_launches(nnz, t->view.log2cap, d_abs != nullptr);
-    } else if (mvm)
+    } else if (ffm)
+      xf_launch_step_ffm(t->view, d_row_ptr, d_keys, d_fields, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
+                         loss_out, pctr_out, d_abs, st);
+    else if (mvm)
       xf_launch_step_mvm(t->view, d_row_ptr, d_keys, d_fields, d_vals, d_labels, (int)rows, mode, tr->touched.as<uint32_t>(),
                          loss_out, pctr_out, d_abs, st);
     else if (canon)
@@ -1239,7 +1249,7 @@ XF_DLL int xf_trainer_predict_host(xf_trainer* tr, const uint32_t* row_ptr, cons
 // the trainers that can weight their rows: LR / FM on a single GPU
 static int xf_check_weighting(xf_trainer* tr, const char* fn) {
   if (tr->cfg.model != XF_MODEL_LR && tr->cfg.model != XF_MODEL_FM) {
-    xf_set_error("%s: importance weighting needs XF_MODEL_LR or XF_MODEL_FM (canonical FM and MVM are not weighted)", fn);
+    xf_set_error("%s: importance weighting needs XF_MODEL_LR or XF_MODEL_FM (canonical FM, MVM and FFM are not weighted)", fn);
     return XF_ERR_ARG;
   }
   if (tr->mg) {
@@ -1327,6 +1337,11 @@ XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv) {
 // ---- deterministic mode (step_det.cu): per-key sums in token order for the canonical FM and the multi-view machine
 XF_DLL int xf_trainer_set_deterministic(xf_trainer* tr, int on) {
   if (!tr) return XF_ERR_ARG;
+  if (tr->cfg.model == XF_MODEL_FFM) {
+    xf_set_error("xf_trainer_set_deterministic: XF_MODEL_FFM has no deterministic mode: its forward has a fixed order, "
+                 "but its per-key gradient sums are float atomics");
+    return XF_ERR_ARG;
+  }
   if (tr->cfg.model != XF_MODEL_FM_CANONICAL && tr->cfg.model != XF_MODEL_MVM) {
     xf_set_error("xf_trainer_set_deterministic: XF_MODEL_FM_CANONICAL and XF_MODEL_MVM only: the LR and FM steps sum "
                  "each key's gradient in fixed point or f64 already, in an order that does not change the result, and "
@@ -1391,10 +1406,23 @@ XF_DLL int xf_trainer_predict_host_values(xf_trainer* tr, const uint32_t* row_pt
   return xf_read_pctr(tr, pctr_out, rows);
 }
 
-// ---- the defined multi-view machine (XF_MODEL_MVM, step_mvm.cu): the batch with the tokens' field ids
-static int xf_check_fields(const uint8_t* fields, uint32_t nnz) {
+// ---- the defined multi-view machine (XF_MODEL_MVM, step_mvm.cu) and the field-aware FM (XF_MODEL_FFM,
+// step_ffm.cu): the batch with the tokens' field ids
+static bool xf_takes_fields(const xf_trainer* tr) { return tr->cfg.model == XF_MODEL_MVM || tr->cfg.model == XF_MODEL_FFM; }
+
+// MVM: field ids < 32; FFM: < F = latent_dim / 4, the pieces of a latent row
+static int xf_check_fields(const xf_trainer* tr, const uint8_t* fields, uint32_t nnz) {
+  const bool ffm = tr->cfg.model == XF_MODEL_FFM;
+  const unsigned bound = ffm ? (unsigned)(tr->table->view.K / 4) : (unsigned)XF_MVM_FIELDS;
   for (uint32_t j = 0; j < nnz; ++j)
-    if (fields[j] >= XF_MVM_FIELDS) { xf_set_error("field id %u of token %u: XF_MODEL_MVM takes field ids below %d", (unsigned)fields[j], j, XF_MVM_FIELDS); return XF_ERR_ARG; }
+    if (fields[j] >= bound) {
+      if (ffm)
+        xf_set_error("field id %u of token %u: XF_MODEL_FFM at latent_dim %d takes field ids below %u", (unsigned)fields[j],
+                     j, tr->table->view.K, bound);
+      else
+        xf_set_error("field id %u of token %u: XF_MODEL_MVM takes field ids below %u", (unsigned)fields[j], j, bound);
+      return XF_ERR_ARG;
+    }
   return XF_OK;
 }
 
@@ -1402,11 +1430,11 @@ XF_DLL int xf_trainer_step_host_fields(xf_trainer* tr, const uint32_t* row_ptr, 
                                        const float* vals, const uint8_t* labels, uint32_t rows, uint32_t nnz,
                                        float* mean_abs_loss) {
   if (!tr || !row_ptr || (!keys && nnz) || (!fields && nnz) || !labels) return XF_ERR_ARG;
-  if (tr->cfg.model != XF_MODEL_MVM) { xf_set_error("field ids need XF_MODEL_MVM"); return XF_ERR_ARG; }
+  if (!xf_takes_fields(tr)) { xf_set_error("field ids need XF_MODEL_MVM or XF_MODEL_FFM"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_step_host_fields"));
   if (rows == 0) { if (mean_abs_loss) *mean_abs_loss = 0.f; return XF_OK; }
-  XF_TRY(xf_check_fields(fields, nnz));
+  XF_TRY(xf_check_fields(tr, fields, nnz));
   int slot;
   XF_TRY(xf_step_host_impl(tr, 0, row_ptr, keys, nullptr, labels, rows, nnz, &slot, vals, fields));
   XF_TRY(xf_read_abs_loss(tr, slot, rows, mean_abs_loss));  // also: `fields` / `vals` may be reused by the caller
@@ -1417,11 +1445,11 @@ XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_pt
                                           const uint8_t* fields, const float* vals, uint32_t rows, uint32_t nnz,
                                           float* pctr_out) {
   if (!tr || !row_ptr || (!keys && nnz) || (!fields && nnz) || !pctr_out) return XF_ERR_ARG;
-  if (tr->cfg.model != XF_MODEL_MVM) { xf_set_error("field ids need XF_MODEL_MVM"); return XF_ERR_ARG; }
+  if (!xf_takes_fields(tr)) { xf_set_error("field ids need XF_MODEL_MVM or XF_MODEL_FFM"); return XF_ERR_ARG; }
   XF_TRY(xf_check_batch(tr, rows, nnz));
   XF_TRY(xf_check_host_keys(keys, nnz, "xf_trainer_predict_host_fields"));
   if (rows == 0) return XF_OK;
-  XF_TRY(xf_check_fields(fields, nnz));
+  XF_TRY(xf_check_fields(tr, fields, nnz));
   XF_TRY(xf_step_host_impl(tr, 1, row_ptr, keys, nullptr, nullptr, rows, nnz, nullptr, vals, fields));
   return xf_read_pctr(tr, pctr_out, rows);
 }

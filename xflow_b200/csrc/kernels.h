@@ -105,6 +105,11 @@ void xf_launch_step_mvm(const XfTableView& t, const uint32_t* row_ptr, const uin
                         const float* vals, const uint8_t* labels, int B, int mode, uint32_t* touched, float* loss_out,
                         float* pctr_out, float* abs_loss_sum, cudaStream_t st);
 
+// the field-aware FM on canonical tables (step_ffm.cu); field ids < K / 4
+void xf_launch_step_ffm(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
+                        const float* vals, const uint8_t* labels, int B, int mode, uint32_t* touched, float* loss_out,
+                        float* pctr_out, float* abs_loss_sum, cudaStream_t st);
+
 // canonical per-k FM with feature values (step_fmc.cu)
 void xf_launch_step_fmc(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
                         const uint8_t* labels, int B, int mode, uint32_t* touched, float* loss_out, float* pctr_out,
