@@ -366,7 +366,8 @@ XF_DLL int xf_trainer_predict_host_fields(xf_trainer* tr, const uint32_t* row_pt
  *   _values, _async, the ingested steps and their predicts), field ids >= F (naming the token and the bound),
  *   xf_trainer_set_deterministic, importance weighting and negative sampling.
  *   Kernels per step (xf_trainer_launches): training, the step kernel and the optimizer pass (+1 with a pv); predict,
- *   one.  No serving model yet: xf_table_freeze_canonical / _mvm of an FFM-trained table give those models'
+ *   one.  Serving: xf_table_freeze_ffm (section 6, "Field-aware FM models").  The table does not record which model
+ *   trained it, so xf_table_freeze_canonical / _mvm of an FFM-trained table are not refused: they give those models'
  *   forwards, not this one's. */
 /* Deterministic mode for XF_MODEL_FM_CANONICAL and XF_MODEL_MVM trainers (csrc/step_det.cu).  The default steps of
  * these two models add each token's gradient terms into its key's accumulators with float atomics (and the machine's
@@ -666,6 +667,39 @@ XF_DLL int xf_comm_barrier(xf_comm* c);
  *      canonical model and a multi-view machine's differ in fm and are never diffed or applied to one another);
  *      merge does not apply (canonical tables are never sharded).
  *
+ *    Field-aware FM models.  xf_table_freeze_ffm freezes a table created with canonical_fm = 1 for the field-aware FM
+ *    (XF_MODEL_FFM, which trains such tables): its predict is the FFM's forward on the tokens' field ids and feature
+ *    values, served by xf_model_predict_host_fields / _device_fields and the candidate and rank entry points only.
+ *      Row: the canonical row {u64 key, f32 w, u32 0, f32 v[L], zero padding}, the same bytes at F32 and F16; piece b
+ *      of v (coordinates 4b .. 4b+3) is the key's vector for field b, so the model serves F = L / 4 fields, L in
+ *      {4, 8, 16, 32, 64, 128}.  xf_model_info reports fm = 4 and these row bytes.
+ *      Freeze resolves w and v as xf_table_freeze_canonical does (both equal xf_table_export's bit for bit); absent =
+ *      -1 is DEFAULT.  Refused with XF_ERR_ARG: tables with canonical_fm = 0, a latent_dim outside {4, ..., 128},
+ *      num_shards > 1.  The table does not change.
+ *      Absent keys: XF_ABSENT_DEFAULT reads an absent key as the row the table would insert (w = 0, v its initial
+ *      values, evaluated on the fly).  XF_ABSENT_ZERO reads it as a row of zeros whose field is present: the token
+ *      adds 0 x to its field sums and w x = 0 x, as the table does with zero rows imported for the query's absent keys.
+ *      prune = 1 leaves out rows with w == +-0 and, under DEFAULT, a latent block that is not materialised; under ZERO,
+ *      every resolved v_k == +-0.  That never changes a prediction, NaN and Inf values included: every sum (Σwx, each
+ *      T[a][b], Q) starts at +0 and a round-to-nearest sum is never -0, so adding +-0 leaves it unchanged whatever the
+ *      sign, and 0 x is the same NaN for either sign of zero when x is NaN or Inf.
+ *      Forward, row r with tokens j = row_ptr[r] .. row_ptr[r+1] - 1 in that order, f_j = fields[j] & (F - 1) (the
+ *      host entry points refuse ids >= F), x_j = vals[j] (1 when vals is NULL), (w_j, v_j) the token's row as the
+ *      absent policy reads it, a_j = v_j x_j (L products), every sum a left fold from +0 in j's order:
+ *          T[f_j][b] += a_j[4b .. 4b+3]  (b < F);  Q += fma(a3, a3, fma(a2, a2, fma(a1, a1, a0 a0))) over piece f_j;
+ *          Σwx += w_j x_j;  lane b < F: P_b = sum over the present fields a ascending of
+ *          fma(u3, s3, fma(u2, s2, fma(u0, s0, u1 s1))), u = T[a][b], s = T[b][a];  y = fma(0.5, (the xor 16 .. 1 sum
+ *          of P over 32 lanes) - Q, Σwx);  pctr = sigmoid(y)   (round to nearest, no other contraction, no flush)
+ *      This is xf_k_step_ffm's pass 1, pair sum and sigmoid, whose order is fixed, with its fused multiply-adds.  So on
+ *      every row xf_model_predict_*_fields of a DEFAULT model returns, bit for bit, what xf_trainer_predict_host_fields
+ *      returns on the table at the moment of the freeze, and a ZERO model what it returns on that table with zero rows
+ *      imported for the query's absent keys.  A candidate's score is the flat predict of its request's context
+ *      followed by its tokens, bit for bit.
+ *      The XFSM and XFSD files keep version 1 and record fm = 4, latent_dim and these row bytes; a load refuses
+ *      non-zero padding as for canonical rows.  Diff, apply and convert serve these models as canonical ones (a
+ *      canonical model and a field-aware FM's differ in fm and are never diffed or applied to one another); merge
+ *      does not apply.
+ *
  *    Sharded tables: parts and merge.  A run sharded over S GPUs holds shard s of the key space in table s
  *    (num_shards = S; shard s owns [s width, (s + 1) width) with width = floor((2^64 - 1) / S), the last shard up to
  *    2^64 - 2, as xf_shard_of).  xf_table_freeze_part freezes one LR or FM table of any num_shards (1 included) into
@@ -721,6 +755,10 @@ XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, x
 /* A multi-view machine's model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG,
  * naming the reason, for tables with canonical_fm = 0, a latent_dim outside {4, 8, 16, 32} and num_shards > 1. */
 XF_DLL int xf_table_freeze_mvm(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
+/* A field-aware FM's model of a table with canonical_fm = 1 (above); the same config and defaults.  XF_ERR_ARG,
+ * naming the reason, for tables with canonical_fm = 0, a latent_dim outside {4, 8, 16, 32, 64, 128} and
+ * num_shards > 1.  The table does not change. */
+XF_DLL int xf_table_freeze_ffm(xf_table* t, const xf_freeze_config* cfg, xf_model** out);
 /* A part of a table of any num_shards (above); the same config and defaults.  XF_ERR_ARG for canonical tables (they
  * are never sharded); XF_ERR_STATE, naming their count, if the table holds keys outside its shard's range (a Pull,
  * Push or import can put them there). */
@@ -747,15 +785,15 @@ typedef struct xf_model_info {
   uint64_t bytes;        /* capacity x row_bytes: the model's device memory */
   uint64_t source_keys;  /* keys of the table when it was frozen */
   uint64_t pruned_keys;  /* source_keys - keys */
-  uint32_t row_bytes;    /* F32: 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical, multi-view machine); F16: 16
-                            (FM), 16 + 2K rounded up to 32 (canonical, multi-view machine) */
-  int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM, 3 multi-view machine */
+  uint32_t row_bytes;    /* F32: 16 (LR), 32 (FM), 16 + 4K rounded up to 32 (canonical, multi-view machine,
+                            field-aware FM); F16: 16 (FM), 16 + 2K rounded up to 32 (the others but LR) */
+  int latent_dim, optimizer, absent, fm;  /* fm: 0 LR, 1 FM, 2 canonical FM, 3 multi-view machine, 4 field-aware FM */
   int precision;         /* XF_PRECISION_* of the latent fields */
 } xf_model_info;
 XF_DLL int xf_model_get_info(xf_model* m, xf_model_info* out);
 /* Model file "XFSM" (little-endian): a 104-byte header
  *     0 "XFSM"   4 u32 version (1)   8 u64 header bytes (104)   16 u64 keys   24 u64 capacity   32 u32 row bytes
- *    36 i32 fm (0 LR, 1 FM, 2 canonical, 3 multi-view machine)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
+ *    36 i32 fm (0 LR, 1 FM, 2 canonical, 3 multi-view machine, 4 field-aware FM)   40 i32 latent_dim   44 i32 optimizer   48 i32 absent
  *    52 i32 resolved v_init (0 constant, 1 counter-based normal, 3 zero)   56 f32 the constant
  *    60 u32 precision (0 F32, 1 F16; the word was reserved as 0, so every F32 file is unchanged)   64 u64 seed
  *    72 u64 source keys   80 u64 pruned keys
@@ -790,18 +828,19 @@ XF_DLL int xf_model_predict_device(xf_model* m, const uint32_t* d_row_ptr, const
                                    uint32_t nnz, float* d_pctr_out, void* cuda_stream);
 /* The same with the tokens' feature values vals[nnz] (NULL: all 1; device memory for _device_values), for canonical
  * models; the contracts are those of _host / _device.  Non-NULL vals on an LR or FM model are XF_ERR_ARG: that model
- * ignores values.  These four and xf_model_predict_ingested refuse a multi-view machine's model (XF_ERR_ARG): it
- * reads field ids. */
+ * ignores values.  These four and xf_model_predict_ingested refuse a multi-view machine's or a field-aware FM's model
+ * (XF_ERR_ARG): they read field ids. */
 XF_DLL int xf_model_predict_host_values(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const float* vals,
                                         uint32_t rows, uint32_t nnz, float* pctr_out);
 XF_DLL int xf_model_predict_device_values(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
                                           const float* d_vals, uint32_t rows, uint32_t nnz, float* d_pctr_out,
                                           void* cuda_stream);
-/* The forward of a multi-view machine's model (above) with the tokens' field ids fields[nnz] and feature values
- * vals[nnz] (NULL: all 1); the contracts are those of _host_values / _device_values.  _host refuses a field id of 32 or
- * more with XF_ERR_ARG, naming the token and the id; on the device the ids are the caller's contract, and the kernel
- * reads fields[j] & 31 as the step kernel does.  NULL fields with nnz > 0 are XF_ERR_ARG.  XF_ERR_ARG on an LR, FM or
- * canonical model: they read no field ids. */
+/* The forward of a multi-view machine's or a field-aware FM's model (above) with the tokens' field ids fields[nnz] and
+ * feature values vals[nnz] (NULL: all 1); the contracts are those of _host_values / _device_values.  _host refuses a
+ * field id of 32 or more (multi-view machine) or of F = L / 4 or more (field-aware FM) with XF_ERR_ARG, naming the
+ * token, the id and, for the field-aware FM, the bound; on the device the ids are the caller's contract, and the kernel
+ * reads fields[j] & 31 or & (F - 1) as the step kernels do.  NULL fields with nnz > 0 are XF_ERR_ARG.  XF_ERR_ARG on an
+ * LR, FM or canonical model: they read no field ids. */
 XF_DLL int xf_model_predict_host_fields(xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
                                         const float* vals, uint32_t rows, uint32_t nnz, float* pctr_out);
 XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr, const uint64_t* d_keys,
@@ -827,7 +866,7 @@ typedef struct xf_candidate_batch {
   const uint32_t* ctx_ptr;      /* [R + 1] */
   const uint64_t* ctx_keys;     /* [ctx_nnz] */
   const float* ctx_vals;        /* [ctx_nnz] or NULL (every value 1); canonical and multi-view machine models only */
-  const uint8_t* ctx_fields;    /* [ctx_nnz]; multi-view machine models only, and required by them */
+  const uint8_t* ctx_fields;    /* [ctx_nnz]; multi-view machine and field-aware FM models only, and required by them */
   uint32_t ctx_nnz;
   const uint32_t* cand_ptr;     /* [R + 1]: cand_ptr[0] = 0, cand_ptr[R] = candidates */
   uint32_t candidates;
@@ -940,7 +979,7 @@ XF_DLL int xf_model_diff(xf_model* base, xf_model* next, xf_delta** out);
 XF_DLL int xf_model_apply_delta(xf_model* base, const xf_delta* d, xf_model** out);
 XF_DLL int xf_model_fingerprint(xf_model* m, uint64_t* out);
 /* Delta file "XFSD" (little-endian): a 144-byte header
- *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's: 0, 1, 2 or 3)   20 i32 latent_dim
+ *     0 "XFSD"   4 u32 version (1)   8 u64 header bytes (144)   16 i32 fm (as XFSM's: 0 .. 4)   20 i32 latent_dim
  *    24 i32 optimizer   28 i32 absent   32 i32 resolved v_init   36 f32 the constant   40 u64 seed   48 u32 row bytes
  *    52 u32 precision (as XFSM's; reserved as 0 before, so every F32 file is unchanged)
  *    56 u64 base keys   64 u64 base fingerprint   72 u64 result keys   80 u64 result source keys

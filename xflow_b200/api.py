@@ -174,6 +174,7 @@ SIGNATURES = {
     "xf_table_freeze": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_canonical": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_mvm": (_i, [_vp, _vp, _vp]),
+    "xf_table_freeze_ffm": (_i, [_vp, _vp, _vp]),
     "xf_table_freeze_part": (_i, [_vp, _vp, _vp]),
     "xf_model_part_info": (_i, [_vp, _vp, _vp]),
     "xf_model_merge": (_i, [_vp, _i, _i, _vp]),
@@ -502,6 +503,16 @@ class Table:
         _check(lib().xf_table_freeze_mvm(self.h, C.byref(cfg), C.byref(h)))
         return Model(h)
 
+    def freeze_ffm(self, absent=None, prune=True, device=None):
+        """A field-aware FM's serving Model of a canonical_fm table (xf_table_freeze_ffm): rows {key, w, v[L]} served
+        with XF_MODEL_FFM's forward on field ids (< L / 4) and feature values (Model.predict_*_fields, the candidate
+        and rank methods); arguments as for freeze.  The table does not record which model trained it: freeze a table
+        trained with MODEL_FFM with this method, not freeze_canonical or freeze_mvm."""
+        cfg = FreezeConfig(-1 if absent is None else absent, 1 if prune else 0, -1 if device is None else device)
+        h = C.c_void_p()
+        _check(lib().xf_table_freeze_ffm(self.h, C.byref(cfg), C.byref(h)))
+        return Model(h)
+
     def freeze_part(self, absent=None, prune=True, device=None):
         """The part of a shard table (xf_table_freeze_part): the rows freeze would make of it, tagged with its shard;
         Model.merge of every shard's part is the whole model.  Arguments as for freeze."""
@@ -587,8 +598,8 @@ class Model:
             _check(lib().xf_model_predict_device(self.h, _p(d_row_ptr), _p(d_keys), rows, nnz, _p(d_out), st))
 
     def predict_host_fields(self, row_ptr, keys, fields, vals=None):
-        """Forward pass of a multi-view machine's model on host CSR arrays with the tokens' field ids (< 32) and
-        feature values (None: all 1)."""
+        """Forward pass of a multi-view machine's model (field ids < 32) or a field-aware FM's model (field ids
+        < latent_dim / 4) on host CSR arrays with the tokens' field ids and feature values (None: all 1)."""
         row_ptr = np.ascontiguousarray(row_ptr, np.uint32)
         keys = np.ascontiguousarray(keys, np.uint64)
         fields = np.ascontiguousarray(fields, np.uint8)
@@ -605,8 +616,9 @@ class Model:
         return out
 
     def predict_device_fields(self, d_row_ptr, d_keys, d_fields, rows, nnz, d_out, stream=0, d_vals=0):
-        """Asynchronous forward pass of a multi-view machine's model on device pointers (raw addresses) on the CUDA
-        stream `stream`: d_fields the tokens' u8 field ids, d_vals their feature values (0: all 1)."""
+        """Asynchronous forward pass of a multi-view machine's or a field-aware FM's model on device pointers (raw
+        addresses) on the CUDA stream `stream`: d_fields the tokens' u8 field ids, d_vals their feature values (0: all
+        1)."""
         st = C.c_void_p(int(stream)) if stream else None
         _check(lib().xf_model_predict_device_fields(self.h, _p(d_row_ptr), _p(d_keys), _p(d_fields),
                                                     _p(d_vals) if d_vals else None, rows, nnz, _p(d_out), st))
@@ -653,8 +665,8 @@ class Model:
         """Score each request's candidates against its context (xf_model_predict_candidates_host): request q's context
         is ctx_keys[ctx_ptr[q] .. ctx_ptr[q+1]), its candidates rows cand_ptr[q] .. cand_ptr[q+1] - 1 of the CSR
         (row_ptr, keys).  Returns float32 [candidates]: for each candidate, the flat predict of its request's context
-        followed by its own tokens, bit for bit.  Values (None: all 1) for canonical and multi-view machine models,
-        field ids for multi-view machine models, on either side."""
+        followed by its own tokens, bit for bit.  Values (None: all 1) for canonical, multi-view machine and
+        field-aware FM models, field ids for multi-view machine and field-aware FM models, on either side."""
         b, arrays = self._candidate_batch(ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals, vals, ctx_fields, fields)
         out = np.empty(max(arrays[2].size - 1, 0), np.float32)
         _check(lib().xf_model_predict_candidates_host(self.h, C.byref(b), _p(out)))
@@ -663,7 +675,7 @@ class Model:
     def predict_candidates_device(self, requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr,
                                   d_keys, nnz, d_out, stream=0, d_ctx_vals=0, d_vals=0, d_ctx_fields=0, d_fields=0):
         """Asynchronous predict_candidates on device pointers (raw addresses) on the CUDA stream `stream`; d_out
-        [candidates].  A 0 address for values reads every value as 1."""
+        [candidates].  A 0 address for values reads every value as 1; field ids as for predict_candidates."""
         st = C.c_void_p(int(stream)) if stream else None
         b = self._device_batch(requests, d_ctx_ptr, d_ctx_keys, ctx_nnz, d_cand_ptr, candidates, d_row_ptr, d_keys, nnz,
                                d_ctx_vals, d_vals, d_ctx_fields, d_fields)
@@ -674,7 +686,8 @@ class Model:
         """Each request's top k candidates by pctr (xf_model_rank_candidates_host), selected on the device from the
         scores predict_candidates returns.  Returns (index uint32 [R, k], pctr float32 [R, k]): row q holds request
         q's local candidate indices (0 .. n_q - 1), highest pctr first, equal pctr by smaller index, NaN last, and
-        their scores; slots past n_q hold index 0xFFFFFFFF and a NaN."""
+        their scores; slots past n_q hold index 0xFFFFFFFF and a NaN.  Values and field ids as for predict_candidates
+        (field ids: multi-view machine and field-aware FM models)."""
         b, arrays = self._candidate_batch(ctx_ptr, ctx_keys, cand_ptr, row_ptr, keys, ctx_vals, vals, ctx_fields, fields)
         index = np.empty((b.requests, k), np.uint32)
         pctr = np.empty((b.requests, k), np.float32)
@@ -703,8 +716,8 @@ class Model:
         return out
 
     def lookup_latent(self, keys):
-        """What a canonical or multi-view machine's model holds for `keys`: dict of w (0 for the latter), v [n, K]
-        and present."""
+        """What a canonical, multi-view machine's or field-aware FM's model holds for `keys`: dict of w (0 for a
+        multi-view machine), v [n, K] and present."""
         keys = np.ascontiguousarray(keys, np.uint64)
         n, K = keys.size, self.info()["latent_dim"]
         out = dict(keys=keys, w=np.zeros(n, np.float32), v=np.zeros((n, K), np.float32), present=np.zeros(n, np.uint8))

@@ -39,6 +39,12 @@
 //                                          memory, added in token order without atomics: a pass's tokens of one field
 //                                          are ranked with __match_any_sync and added a rank per round
 //
+// A field-aware FM's model (xf_table_freeze_ffm, fm = XF_SERVE_FFM) serves step_ffm.cu's forward on field ids and
+// feature values: its row is the canonical one, piece c of v the key's vector for field c.
+//   freeze   xf_k_freeze_fmc<COUNT, false>  the canonical freeze
+//   predict  xf_k_serve_ffm<C>              xf_k_serve_fmc's mapping, loads and probe; the field sums T[F][F] in dynamic
+//                                           shared memory, added in token order as xf_k_step_ffm adds them (xf_ffm_add)
+//
 // An F16 model (xf_model_convert) holds its latent fields in binary16: FM {key, w, st, qt} in 16 bytes, canonical
 // {key, w, 0, v[K]} with 2-byte v.  Its predict and lookup kernels are the F32 ones' H = true instantiations, which widen
 // each field right after the load and then run the F32 arithmetic unchanged.
@@ -46,10 +52,10 @@
 //                                              converted and put into the result with xf_model_claim
 //
 // Each row kind's forward is a token loop and a finishing step: xf_serve_arg (LR, FM), xf_fmc_arg (canonical),
-// xf_mvm_product (multi-view machine), each written once.  A flat predict kernel runs the loop over each row's token
-// indices.  A candidate kernel (xf_k_serve_cand*) runs it as a fold over positions (xf_serve_fold, xf_fmc_fold,
-// xf_mvm_fold): once over a request's context, then over each candidate's tokens from that state (see "Two forms of each
-// fold").  xf_launch_predict and xf_launch_candidates pick the instantiation (xf_with_precision, xf_with_lanes); the
+// xf_mvm_product (multi-view machine), xf_ffm_arg (field-aware FM), each written once.  A flat predict kernel runs the
+// loop over each row's token indices.  A candidate kernel (xf_k_serve_cand*) runs it as a fold over positions
+// (xf_serve_fold, xf_fmc_fold, xf_mvm_fold, xf_ffm_fold): once over a request's context, then over each candidate's
+// tokens from that state (see "Two forms of each fold").  xf_launch_predict and xf_launch_candidates pick the instantiation (xf_with_precision, xf_with_lanes); the
 // host entry points upload a batch as one image (xf_model_upload).
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -414,6 +420,179 @@ xf_k_serve_mvm(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, 
   }
 }
 
+// ---- field-aware FM rows {key, w, 0, v[L]}: the forward of xf_k_step_ffm (pass 1, pair sum, sigmoid) on the model's
+// rows.  Piece c of v is the key's vector for field c; F = C = L/4 fields.  The warp's field sums T[a][b] are F x F
+// float4 in shared memory (T[a * F + b]), Σwx and Q are warp-uniform.  The step kernel's arithmetic, spelled out as its
+// machine code does it (cuobjdump -sass of xf_k_step_ffm<C>, every C: the FMUL / FFMA / FADD of pass 1 and the pair sum):
+//   a_k = x v_k;  q = fma(a3, a3, fma(a2, a2, fma(a1, a1, a0 a0)))  (lane c == f);  wxt = w x  (lane c == 0)
+//   Σwx = Σwx + wxt, Q = Q + q and T[f][c]_k = T[f][c]_k + a_k, each in token order
+//   P = P + fma(u3, s3, fma(u2, s2, fma(u0, s0, u1 s1)))   u = T[a][b], s = T[b][a], a over the present fields ascending
+//   arg = fma(0.5, (xor 16 .. 1 warp sum of P) - Q, Σwx)
+// A token's w and piece c: its row found from the home slot the caller loaded (k, w, v), or the absent policy's row
+// (DEFAULT: w = 0 and the initial values; ZERO: zeros, its field still present)
+template <bool H>
+__device__ __forceinline__ void xf_ffm_serve_token(const XfTableView& m, int absent, uint64_t key, uint64_t k, float& w,
+                                                   float4& v, int c) {
+  if (xf_fmc_find<H>(m, key, k, w, v, c)) return;
+  w = 0.f;
+  if (absent == XF_ABSENT_ZERO) v = make_float4(0.f, 0.f, 0.f, 0.f);
+  else
+    v = make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
+                    xf_v_init(m, key, 4 * c + 3));
+}
+
+// One pass's tokens into the warp's state, as xf_k_step_ffm's pass 1: lane (token g, c) holds the token's field f,
+// piece c of v, w and x; the live tokens are the pass's first groups.  Σwx and Q take the live tokens in turn; a field's
+// tokens are ranked with __match_any_sync and added to T[f][*] a rank per round, lowest position first.
+template <int C>
+__device__ __forceinline__ void xf_ffm_add(float4* T, bool live, uint32_t f, float4 v, float w, float x, float& wx,
+                                           float& Q) {
+  constexpr int TP = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const int lead = lane & ~(C - 1);
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+  float q = 0.f, wxt = 0.f;
+  if (live) {
+    a = make_float4(__fmul_rn(v.x, x), __fmul_rn(v.y, x), __fmul_rn(v.z, x), __fmul_rn(v.w, x));
+    if (c == (int)f) q = __fmaf_rn(a.w, a.w, __fmaf_rn(a.z, a.z, __fmaf_rn(a.y, a.y, __fmul_rn(a.x, a.x))));
+    if (c == 0) wxt = __fmul_rn(w, x);
+  }
+  const float qt = __shfl_sync(0xffffffffu, q, lead + (int)f);  // the self term, from lane f of the token's group
+  const int n = __popc(__ballot_sync(0xffffffffu, live)) / C;
+  for (int g = 0; g < n; ++g) {
+    wx = __fadd_rn(wx, __shfl_sync(0xffffffffu, wxt, g * C));
+    Q = __fadd_rn(Q, __shfl_sync(0xffffffffu, qt, g * C));
+  }
+  int rank = 0, last = 0;
+  if (TP > 1) {
+    const unsigned peers = __match_any_sync(0xffffffffu, live ? f : 0xFFu);
+    rank = __popc(peers & ((1u << lead) - 1u)) / C;
+    last = (int)__reduce_max_sync(0xffffffffu, live ? (unsigned)rank : 0u);
+  }
+  for (int r = 0; r <= last; ++r) {
+    if (live && rank == r) {
+      float4 s = T[f * C + c];
+      s.x = __fadd_rn(s.x, a.x); s.y = __fadd_rn(s.y, a.y); s.z = __fadd_rn(s.z, a.z); s.w = __fadd_rn(s.w, a.w);
+      T[f * C + c] = s;
+    }
+    __syncwarp();
+  }
+}
+
+// the pair sum over the present fields and the sigmoid's argument (every lane returns it)
+template <int C>
+__device__ __forceinline__ float xf_ffm_arg(const float4* T, unsigned present, float wx, float Q) {
+  const int lane = threadIdx.x & 31;
+  float P = 0.f;
+  if (lane < C && ((present >> lane) & 1u))
+    for (unsigned q = present; q; q &= q - 1) {
+      const int fa = __ffs(q) - 1;
+      const float4 u = T[fa * C + lane], s = T[lane * C + fa];
+      P = __fadd_rn(P, __fmaf_rn(u.w, s.w, __fmaf_rn(u.z, s.z, __fmaf_rn(u.x, s.x, __fmul_rn(u.y, s.y)))));
+    }
+  return __fmaf_rn(0.5f, __fsub_rn(xf_warp_sum(P), Q), wx);
+}
+
+// The n tokens of a row from keys[beg] (vals NULL: every value 1) into the warp's state T, Σwx, Q, with
+// xf_k_serve_fmc's mapping, loads and probe, two passes in flight, each added as xf_ffm_add; returns the lane's fields
+// present (the caller reduces them over the warp).  Every token makes its field present.
+template <int C, bool H>
+__device__ __forceinline__ unsigned xf_ffm_fold(const XfTableView& m, int absent, const uint64_t* __restrict__ keys,
+                                                const uint8_t* __restrict__ fields, const float* __restrict__ vals,
+                                                uint32_t beg, uint32_t n, float4* T, float& wx, float& Q) {
+  constexpr uint32_t TP = 32 / C;
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const uint32_t tg = (uint32_t)(lane / C);
+  unsigned present = 0u;
+  for (uint32_t i0 = 0; i0 < n; i0 += 2u * TP) {
+    const uint32_t ia = i0 + tg, ib = ia + TP;
+    const bool va = ia < n, vb = ib < n;
+    const uint32_t ja = beg + ia, jb = beg + ib;
+    // streaming: do not displace model rows in L2
+    const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+    const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+    const uint32_t fa = va ? (uint32_t)__ldcs(fields + ja) & (C - 1) : 0u;
+    const uint32_t fb = vb ? (uint32_t)__ldcs(fields + jb) & (C - 1) : 0u;
+    const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+    const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+    // both home rows are in flight before either is resolved
+    uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+    float wa = 0.f, wb = 0.f;
+    float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
+    if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+    if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+    if (va) xf_ffm_serve_token<H>(m, absent, ka, ra, wa, pa, c);
+    if (vb) xf_ffm_serve_token<H>(m, absent, kb, rb, wb, pb, c);
+    present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
+    xf_ffm_add<C>(T, va, fa, pa, wa, xa, wx, Q);  // pass a, then pass b
+    xf_ffm_add<C>(T, vb, fb, pb, wb, xb, wx, Q);
+  }
+  return present;
+}
+
+// warps per CTA of the field-aware FM's flat kernel: C = 32 (L = 128) holds 16 KB of field sums per warp, 4 warps per
+// CTA (64 KB, opt-in) as xf_k_step_ffm; else 8.  Its candidate kernel holds twice that per warp (T and T0): 2 warps at
+// C = 32 (64 KB, opt-in), else 4.
+__host__ __device__ constexpr int xf_ffm_warps(int C) { return C == 32 ? 4 : 8; }
+__host__ __device__ constexpr int xf_cand_ffm_warps(int C) { return C == 32 ? 2 : 4; }
+
+// One warp per row; the row's field sums in dynamic shared memory, F x F float4 per warp.  After a row, lane b < F
+// clears T[a][b] for its present fields a.  No insert, no atomics.
+template <int C, bool H>
+__global__ void __launch_bounds__(32 * xf_ffm_warps(C))
+xf_k_serve_ffm(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
+               const uint8_t* __restrict__ fields, const float* __restrict__ vals, int B, float* __restrict__ pctr_out) {
+  constexpr int TP = 32 / C;
+  extern __shared__ float4 s_ffm[];
+  const int lane = threadIdx.x & 31;
+  const int c = lane & (C - 1);
+  const int tg = lane / C;
+  const int wib = threadIdx.x >> 5;
+  const int warps_per_block = blockDim.x >> 5;
+  const int gwarp = blockIdx.x * warps_per_block + wib;
+  const int nwarps = gridDim.x * warps_per_block;
+  float4* T = s_ffm + (size_t)wib * (C * C);
+  for (int i = lane; i < C * C; i += 32) T[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncwarp();
+  for (int row = gwarp; row < B; row += nwarps) {
+    const uint32_t beg = __ldg(row_ptr + row);
+    const uint32_t end = __ldg(row_ptr + row + 1);
+    unsigned present = 0u;
+    float wx = 0.f, Q = 0.f;
+    // xf_ffm_fold over the row in token indices (see "Two forms of each fold" above)
+    for (uint32_t j0 = beg; j0 < end; j0 += 2u * TP) {
+      const uint32_t ja = j0 + (uint32_t)tg, jb = ja + (uint32_t)TP;
+      const bool va = ja < end, vb = jb < end;
+      const uint64_t ka = va ? __ldcs(keys + ja) : 0ull;
+      const uint64_t kb = vb ? __ldcs(keys + jb) : 0ull;
+      const uint32_t fa = va ? (uint32_t)__ldcs(fields + ja) & (C - 1) : 0u;
+      const uint32_t fb = vb ? (uint32_t)__ldcs(fields + jb) & (C - 1) : 0u;
+      const float xa = (va && vals) ? __ldcs(vals + ja) : 1.0f;
+      const float xb = (vb && vals) ? __ldcs(vals + jb) : 1.0f;
+      uint64_t ra = XF_EMPTY_KEY, rb = XF_EMPTY_KEY;
+      float wa = 0.f, wb = 0.f;
+      float4 pa = make_float4(0.f, 0.f, 0.f, 0.f), pb = pa;
+      if (va) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, ka)), c, ra, wa, pa);
+      if (vb) xf_fmc_load<H>(xf_row(m, xf_home_slot(m, kb)), c, rb, wb, pb);
+      if (va) xf_ffm_serve_token<H>(m, absent, ka, ra, wa, pa, c);
+      if (vb) xf_ffm_serve_token<H>(m, absent, kb, rb, wb, pb, c);
+      present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
+      xf_ffm_add<C>(T, va, fa, pa, wa, xa, wx, Q);
+      xf_ffm_add<C>(T, vb, fb, pb, wb, xb, wx, Q);
+    }
+    present = __reduce_or_sync(0xffffffffu, present);
+    const float arg = xf_ffm_arg<C>(T, present, wx, Q);
+    if (lane == 0) pctr_out[row] = xf_sigmoid(arg);
+    // clear the rows of T this row used, for the warp's next row
+    __syncwarp();
+    if (lane < C)
+      for (unsigned q = present; q; q &= q - 1) T[(__ffs(q) - 1) * C + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+    __syncwarp();
+  }
+}
+
 // f(std::bool_constant<H>()) for a model's precision: H = true for binary16 latent fields
 template <typename F>
 static void xf_with_precision(const xf_model* m, F&& f) {
@@ -421,14 +600,33 @@ static void xf_with_precision(const xf_model* m, F&& f) {
   else f(std::false_type());
 }
 
-// the flat forward of any model on device arrays (fields: a multi-view machine's, which reads nothing else)
+// before the first field-aware FM launch at C = 32 on the current device (below)
+static void xf_ffm_opt_in();
+
+// CTAs of `warps` warps with `smem` bytes of dynamic shared memory each for `threads` threads of work: as many as fit
+// on the GPU at once, at most 8 per SM
+static int xf_ffm_grid(uint64_t threads, int warps, size_t smem) {
+  const int per_sm = (int)(227 * 1024 / (smem + 1024));
+  return xf_grid_for(threads, 32 * warps, per_sm < 8 ? per_sm : 8);
+}
+
+// the flat forward of any model on device arrays (fields: a multi-view machine's or a field-aware FM's, which read
+// nothing else)
 static void xf_launch_predict(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
                               const float* vals, uint32_t rows, float* pctr_out, cudaStream_t st) {
   if (rows == 0) return;
   const int grid = xf_grid_for((uint64_t)rows * 32, 256, 8);
   const int B = (int)rows;
   xf_with_precision(m, [&](auto H) {
-    if (m->fm == XF_SERVE_MVM)
+    if (m->fm == XF_SERVE_FFM)
+      xf_with_lanes<32>(m->view.K, [&](auto C) {
+        constexpr int warps = xf_ffm_warps(C);
+        constexpr size_t smem = (size_t)warps * C * C * sizeof(float4);
+        if (smem > 48 * 1024) xf_ffm_opt_in();
+        xf_k_serve_ffm<C, H><<<xf_ffm_grid((uint64_t)rows * 32, warps, smem), 32 * warps, smem, st>>>(
+            m->view, m->absent, row_ptr, keys, fields, vals, B, pctr_out);
+      });
+    else if (m->fm == XF_SERVE_MVM)
       xf_with_lanes<8>(m->view.K, [&](auto C) {
         xf_k_serve_mvm<C, H><<<grid, 256, 0, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, B, pctr_out);
       });
@@ -603,6 +801,80 @@ xf_k_serve_cand_mvm(XfTableView m, int absent, XfCandView b, float* __restrict__
                });
 }
 
+// Field-aware FM: a warp's working field sums T and a copy T0 of the context's, both in dynamic shared memory (2 F x F
+// float4 per warp: 32 KB at L = 128), the context's Σwx, Q and present fields in registers.  Each candidate continues
+// the fold from that state, forms the pair sum over the fields present in the context or the candidate, as
+// xf_k_serve_ffm, and puts the rows T[f][*] of its own fields back to the context's.  After a request's last candidate
+// in the run, its context's rows are cleared in both.  Every part of the state is a left fold in token order, so the
+// candidate tokens' lanes do not matter.
+template <int C, bool H>
+__global__ void __launch_bounds__(32 * xf_cand_ffm_warps(C), 1)
+xf_k_serve_cand_ffm(XfTableView m, int absent, XfCandView b, float* __restrict__ pctr_out) {
+  constexpr int W = xf_cand_ffm_warps(C);
+  extern __shared__ float4 s_ffm[];
+  const int lane = threadIdx.x & 31;
+  const int wib = threadIdx.x >> 5;
+  const int gwarp = blockIdx.x * W + wib;
+  float4* T = s_ffm + (size_t)wib * (2 * C * C);
+  float4* T0 = T + C * C;
+  for (int i = lane; i < 2 * C * C; i += 32) T[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncwarp();
+  struct Ctx { float wx, Q; unsigned present; };
+  xf_cand_walk(b, gwarp, gridDim.x * W,
+               [=](uint32_t q) {
+                 const uint32_t beg = __ldg(b.ctx_ptr + q), n = __ldg(b.ctx_ptr + q + 1) - beg;
+                 Ctx x{0.f, 0.f, 0u};
+                 x.present = __reduce_or_sync(
+                     0xffffffffu, xf_ffm_fold<C, H>(m, absent, b.ctx_keys, b.ctx_fields, b.ctx_vals, beg, n, T, x.wx, x.Q));
+                 __syncwarp();
+                 if (lane < C)
+                   for (unsigned f = x.present; f; f &= f - 1) T0[(__ffs(f) - 1) * C + lane] = T[(__ffs(f) - 1) * C + lane];
+                 return x;
+               },
+               [=](const Ctx& x, uint32_t c) {
+                 const uint32_t beg = __ldg(b.row_ptr + c), n = __ldg(b.row_ptr + c + 1) - beg;
+                 float wx = x.wx, Q = x.Q;
+                 __syncwarp();
+                 const unsigned own = __reduce_or_sync(
+                     0xffffffffu, xf_ffm_fold<C, H>(m, absent, b.keys, b.fields, b.vals, beg, n, T, wx, Q));
+                 __syncwarp();
+                 const float arg = xf_ffm_arg<C>(T, x.present | own, wx, Q);
+                 __syncwarp();  // every lane has read T before its candidate's rows go back
+                 if (lane < C)
+                   for (unsigned f = own; f; f &= f - 1) T[(__ffs(f) - 1) * C + lane] = T0[(__ffs(f) - 1) * C + lane];
+                 if (lane == 0) pctr_out[c] = xf_sigmoid(arg);
+               },
+               [=](const Ctx& x) {
+                 // the context leaves both copies before the warp's next request
+                 __syncwarp();
+                 if (lane < C)
+                   for (unsigned f = x.present; f; f &= f - 1)
+                     T[(__ffs(f) - 1) * C + lane] = T0[(__ffs(f) - 1) * C + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+                 __syncwarp();
+               });
+}
+
+// The field-aware FM kernels' dynamic shared memory at C = 32 is past the 48 KB a launch gets without opting in.  The
+// opt-in is per device and per kernel; it is made once per device, before the first such launch on it, however many
+// host threads launch at once.
+static void xf_ffm_opt_in() {
+  static std::mutex mu;
+  static std::vector<bool> done;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(mu);
+  if ((size_t)dev < done.size() && done[(size_t)dev]) return;
+  constexpr int flat = xf_ffm_warps(32) * 32 * 32 * (int)sizeof(float4);
+  constexpr int cand = xf_cand_ffm_warps(32) * 2 * 32 * 32 * (int)sizeof(float4);
+  cudaFuncSetAttribute(xf_k_serve_ffm<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, flat);
+  cudaFuncSetAttribute(xf_k_serve_ffm<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, flat);
+  cudaFuncSetAttribute(xf_k_serve_cand_ffm<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cand);
+  cudaFuncSetAttribute(xf_k_serve_cand_ffm<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cand);
+  if (done.size() <= (size_t)dev) done.resize((size_t)dev + 1, false);
+  done[(size_t)dev] = true;
+}
+
+
 // the candidate forward of any model on device arrays
 static void xf_launch_candidates(const xf_model* m, const XfCandView& b, float* pctr_out, cudaStream_t st) {
   if (b.candidates == 0) return;
@@ -610,7 +882,14 @@ static void xf_launch_candidates(const xf_model* m, const XfCandView& b, float* 
   constexpr int MVM_THREADS = 32 * XF_CAND_MVM_WARPS;
   const int grid = m->fm == XF_SERVE_MVM ? xf_grid_for(warps * 32, MVM_THREADS, 16) : xf_grid_for(warps * 32, 256, 8);
   xf_with_precision(m, [&](auto H) {
-    if (m->fm == XF_SERVE_MVM)
+    if (m->fm == XF_SERVE_FFM)
+      xf_with_lanes<32>(m->view.K, [&](auto C) {
+        constexpr int W = xf_cand_ffm_warps(C);
+        constexpr size_t smem = (size_t)W * 2 * C * C * sizeof(float4);
+        if (smem > 48 * 1024) xf_ffm_opt_in();
+        xf_k_serve_cand_ffm<C, H><<<xf_ffm_grid(warps * 32, W, smem), 32 * W, smem, st>>>(m->view, m->absent, b, pctr_out);
+      });
+    else if (m->fm == XF_SERVE_MVM)
       xf_with_lanes<8>(m->view.K, [&](auto C) {
         xf_k_serve_cand_mvm<C, H><<<grid, MVM_THREADS, 0, st>>>(m->view, m->absent, b, pctr_out);
       });
@@ -973,7 +1252,8 @@ XF_DLL int xf_freeze_config_default(xf_freeze_config* cfg) {
 }
 
 // the body of xf_table_freeze (latent = XF_SERVE_LR), xf_table_freeze_canonical (XF_SERVE_FMC), xf_table_freeze_mvm
-// (XF_SERVE_MVM) and xf_table_freeze_part (part): on failure the caller frees `m`
+// (XF_SERVE_MVM), xf_table_freeze_ffm (XF_SERVE_FFM: the canonical freeze, its rows are the canonical ones) and
+// xf_table_freeze_part (part): on failure the caller frees `m`
 static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, int latent, bool part, xf_model* m, const char* fn) {
   const int src_dev = t->cfg.device;
   XF_CUDA_TRY(cudaSetDevice(src_dev));
@@ -997,7 +1277,7 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, int latent, 
   uint64_t lo = 0, hi = 0;
   xf_shard_range(t->cfg.shard_index, t->cfg.num_shards, &lo, &hi);
 #define XF_FREEZE_LAUNCH(COUNT)                                                                                       \
-  if (fm == XF_SERVE_FMC) xf_k_freeze_fmc<COUNT, false><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
+  if (fm == XF_SERVE_FMC || fm == XF_SERVE_FFM) xf_k_freeze_fmc<COUNT, false><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
   else if (fm == XF_SERVE_MVM) xf_k_freeze_fmc<COUNT, true><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, d_counts, d_error); \
   else switch (xf_vec_for(tv.K)) {                                                                                         \
     case 4: xf_k_freeze<COUNT, 4><<<grid, 256, 0, st>>>(tv, m->view, m->absent, prune, lo, hi, d_counts, d_error); break; \
@@ -1053,9 +1333,9 @@ static int xf_freeze_into(xf_table* t, const xf_freeze_config& cfg, int latent, 
 }
 
 static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, int latent, bool part, xf_model** out) {
-  const bool canonical = latent == XF_SERVE_FMC, mvm = latent == XF_SERVE_MVM;
+  const bool canonical = latent == XF_SERVE_FMC, mvm = latent == XF_SERVE_MVM, ffm = latent == XF_SERVE_FFM;
   const char* fn = part ? "xf_table_freeze_part" : canonical ? "xf_table_freeze_canonical" : mvm ? "xf_table_freeze_mvm"
-                                                                                                 : "xf_table_freeze";
+                 : ffm ? "xf_table_freeze_ffm" : "xf_table_freeze";
   if (out) *out = nullptr;
   if (!t || !out) { xf_set_error("null argument"); return XF_ERR_ARG; }
   xf_freeze_config cfg;
@@ -1081,6 +1361,16 @@ static int xf_freeze(xf_table* t, const xf_freeze_config* cfg_in, int latent, bo
   }
   if (mvm && !xf_mvm_latent_ok(t->cfg.latent_dim)) {
     xf_set_error("xf_table_freeze_mvm: latent_dim = %d: the multi-view machine serves K = 4, 8, 16 or 32",
+                 t->cfg.latent_dim);
+    return XF_ERR_ARG;
+  }
+  if (ffm && !t->cfg.canonical_fm) {
+    xf_set_error("xf_table_freeze_ffm: the table is not canonical (canonical_fm = 0): the field-aware FM trains canonical "
+                 "tables only");
+    return XF_ERR_ARG;
+  }
+  if (ffm && !xf_fmc_latent_ok(t->cfg.latent_dim)) {
+    xf_set_error("xf_table_freeze_ffm: latent_dim = %d: the field-aware FM serves L = 4, 8, 16, 32, 64 or 128",
                  t->cfg.latent_dim);
     return XF_ERR_ARG;
   }
@@ -1112,6 +1402,10 @@ XF_DLL int xf_table_freeze_canonical(xf_table* t, const xf_freeze_config* cfg, x
 
 XF_DLL int xf_table_freeze_mvm(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
   return xf_freeze(t, cfg, XF_SERVE_MVM, false, out);
+}
+
+XF_DLL int xf_table_freeze_ffm(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
+  return xf_freeze(t, cfg, XF_SERVE_FFM, false, out);
 }
 
 XF_DLL int xf_table_freeze_part(xf_table* t, const xf_freeze_config* cfg, xf_model** out) {
@@ -1185,7 +1479,18 @@ static int xf_check_nondecreasing(const uint32_t* ptr, uint32_t n, const char* w
   return XF_OK;
 }
 
-static int xf_check_host_fields(const uint8_t* fields, uint32_t n, const char* what, const char* fn) {
+// the field ids of a model that reads them: below 32 for a multi-view machine's, below F = L / 4 for a field-aware FM's
+static int xf_check_host_fields(const xf_model* m, const uint8_t* fields, uint32_t n, const char* what, const char* fn) {
+  if (m->fm == XF_SERVE_FFM) {
+    const uint32_t F = (uint32_t)m->view.K / 4u;
+    for (uint32_t j = 0; j < n; ++j)
+      if (fields[j] >= F) {
+        xf_set_error("%s: %s: field id %u of token %u: a field-aware FM's model of latent_dim %d takes field ids below "
+                     "F = %u", fn, what, (unsigned)fields[j], j, m->view.K, F);
+        return XF_ERR_ARG;
+      }
+    return XF_OK;
+  }
   for (uint32_t j = 0; j < n; ++j)
     if (fields[j] >= XF_MVM_FIELDS) {
       xf_set_error("%s: %s: field id %u of token %u: a multi-view machine takes field ids below %d", fn, what,
@@ -1195,7 +1500,7 @@ static int xf_check_host_fields(const uint8_t* fields, uint32_t n, const char* w
   return XF_OK;
 }
 
-// feature values are read by canonical and multi-view machine models only: the LR and FM forwards ignore them
+// feature values are read by canonical, multi-view machine and field-aware FM models only: the LR and FM forwards ignore them
 static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
   if (vals && !xf_serve_latent_rows(m->fm)) {
     xf_set_error("%s: an %s model ignores feature values: pass vals = NULL (values need a model frozen with "
@@ -1205,18 +1510,22 @@ static int xf_check_vals(const xf_model* m, const void* vals, const char* fn) {
   return XF_OK;
 }
 
-// field ids are read by multi-view machine models, and those read nothing without them: the _fields entry points serve
-// them only, and every other entry point refuses them
+// the row kinds whose forward reads the tokens' field ids: the multi-view machine and the field-aware FM
+static bool xf_reads_fields(const xf_model* m) { return m->fm == XF_SERVE_MVM || m->fm == XF_SERVE_FFM; }
+
+// field ids are read by multi-view machine and field-aware FM models, and those read nothing without them: the _fields
+// entry points serve them only, and every other entry point refuses them
 static int xf_check_fields_kind(const xf_model* m, bool with_fields, const char* fn) {
-  if (m->fm == XF_SERVE_MVM && !with_fields) {
-    xf_set_error("%s: a multi-view machine's model reads the tokens' field ids: use xf_model_predict_host_fields or "
-                 "xf_model_predict_device_fields", fn);
+  static const char* const kind[] = {"LR", "FM", "canonical", "multi-view machine's", "field-aware FM's"};
+  static_assert(sizeof(kind) / sizeof(kind[0]) == XF_SERVE_FFM + 1, "a name for every row kind");
+  if (xf_reads_fields(m) && !with_fields) {
+    xf_set_error("%s: a %s model reads the tokens' field ids: use xf_model_predict_host_fields or "
+                 "xf_model_predict_device_fields", fn, kind[m->fm]);
     return XF_ERR_ARG;
   }
-  if (m->fm != XF_SERVE_MVM && with_fields) {
-    static const char* const kind[] = {"LR", "FM", "canonical"};
-    xf_set_error("%s: an %s model reads no field ids: field ids need a model frozen with xf_table_freeze_mvm", fn,
-                 kind[m->fm]);
+  if (!xf_reads_fields(m) && with_fields) {
+    xf_set_error("%s: an %s model reads no field ids: field ids need a model frozen with xf_table_freeze_mvm or "
+                 "xf_table_freeze_ffm", fn, kind[m->fm]);
     return XF_ERR_ARG;
   }
   return XF_OK;
@@ -1234,7 +1543,7 @@ static int xf_predict_host(xf_model* m, const uint32_t* row_ptr, const uint64_t*
   XF_TRY(xf_check_nondecreasing(row_ptr, rows, "row_ptr", fn));
   if (row_ptr[rows] > nnz) { xf_set_error("%s: row_ptr ends at %u, past nnz = %u", fn, row_ptr[rows], nnz); return XF_ERR_ARG; }
   XF_TRY(xf_check_host_keys(keys, nnz, fn));
-  if (with_fields) XF_TRY(xf_check_host_fields(fields, nnz, "fields", fn));
+  if (with_fields) XF_TRY(xf_check_host_fields(m, fields, nnz, "fields", fn));
   if (rows == 0) return XF_OK;
   std::lock_guard<std::mutex> lock(m->mu);
   XF_CUDA_TRY(cudaSetDevice(m->device));
@@ -1308,14 +1617,14 @@ XF_DLL int xf_model_predict_device_fields(xf_model* m, const uint32_t* d_row_ptr
 
 // what both candidate entry points check without reading the arrays: null pointers, a part, the model's kind
 static int xf_check_candidates(xf_model* m, const xf_candidate_batch* b, const void* pctr_out, const char* fn) {
-  const bool mvm = m && m->fm == XF_SERVE_MVM;
+  const bool reads = m && xf_reads_fields(m);
   if (!m || !b || !b->ctx_ptr || !b->cand_ptr || !b->row_ptr || (!b->ctx_keys && b->ctx_nnz) || (!b->keys && b->nnz) ||
-      (!pctr_out && b->candidates) || (mvm && ((!b->ctx_fields && b->ctx_nnz) || (!b->fields && b->nnz)))) {
+      (!pctr_out && b->candidates) || (reads && ((!b->ctx_fields && b->ctx_nnz) || (!b->fields && b->nnz)))) {
     xf_set_error("null argument");
     return XF_ERR_ARG;
   }
   XF_TRY(xf_refuse_part(m, fn));
-  XF_TRY(xf_check_fields_kind(m, mvm || b->ctx_fields || b->fields, fn));
+  XF_TRY(xf_check_fields_kind(m, reads || b->ctx_fields || b->fields, fn));
   XF_TRY(xf_check_vals(m, b->ctx_vals, fn));
   XF_TRY(xf_check_vals(m, b->vals, fn));
   return XF_OK;
@@ -1350,9 +1659,9 @@ static int xf_check_candidates_host(const xf_model* m, const xf_candidate_batch*
   XF_TRY(xf_check_host_keys(b->ctx_keys, b->ctx_nnz, what));
   snprintf(what, sizeof what, "%s: keys", fn);
   XF_TRY(xf_check_host_keys(b->keys, b->nnz, what));
-  if (m->fm == XF_SERVE_MVM) {
-    XF_TRY(xf_check_host_fields(b->ctx_fields, b->ctx_nnz, "ctx_fields", fn));
-    XF_TRY(xf_check_host_fields(b->fields, b->nnz, "fields", fn));
+  if (xf_reads_fields(m)) {
+    XF_TRY(xf_check_host_fields(m, b->ctx_fields, b->ctx_nnz, "ctx_fields", fn));
+    XF_TRY(xf_check_host_fields(m, b->fields, b->nnz, "fields", fn));
   }
   return XF_OK;
 }
@@ -1361,7 +1670,7 @@ static int xf_check_candidates_host(const xf_model* m, const xf_candidate_batch*
 // caller holds the model's mutex with its device current.
 static int xf_upload_candidates(xf_model* m, const xf_candidate_batch* b, XfCandView* v) {
   const uint32_t R = b->requests, N = b->candidates;
-  const bool mvm = m->fm == XF_SERVE_MVM;
+  const bool reads = xf_reads_fields(m);
   const XfUpload part[] = {
       {b->ctx_ptr, ((size_t)R + 1) * 4},
       {b->cand_ptr, ((size_t)R + 1) * 4},
@@ -1370,8 +1679,8 @@ static int xf_upload_candidates(xf_model* m, const xf_candidate_batch* b, XfCand
       {b->keys, (size_t)b->nnz * 8},
       {b->ctx_vals, b->ctx_vals ? (size_t)b->ctx_nnz * 4 : 0},
       {b->vals, b->vals ? (size_t)b->nnz * 4 : 0},
-      {b->ctx_fields, mvm ? (size_t)b->ctx_nnz : 0},
-      {b->fields, mvm ? (size_t)b->nnz : 0},
+      {b->ctx_fields, reads ? (size_t)b->ctx_nnz : 0},
+      {b->fields, reads ? (size_t)b->nnz : 0},
   };
   const void* d[9];
   XF_TRY(xf_model_upload(m, part, d));
@@ -1545,7 +1854,8 @@ XF_DLL int xf_model_lookup(xf_model* m, const uint64_t* keys, uint64_t n, float*
   if (xf_serve_latent_rows(m->fm)) {
     if (st || qt) {
       xf_set_error("xf_model_lookup: a %s model holds no st, qt: pass NULL, and read its latent rows with "
-                   "xf_model_lookup_latent", m->fm == XF_SERVE_MVM ? "multi-view machine's" : "canonical");
+                   "xf_model_lookup_latent", m->fm == XF_SERVE_MVM ? "multi-view machine's"
+                                             : m->fm == XF_SERVE_FFM ? "field-aware FM's" : "canonical");
       return XF_ERR_ARG;
     }
     XF_TRY(xf_check_host_keys(keys, n, "xf_model_lookup"));
@@ -1653,7 +1963,7 @@ int xf_file_size_check(FILE* f, const char* path, const char* file, uint64_t exp
 
 bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
   if (c.precision != XF_PRECISION_F32 && c.precision != XF_PRECISION_F16) return false;
-  if (c.fm == XF_SERVE_FMC) {
+  if (c.fm == XF_SERVE_FMC || c.fm == XF_SERVE_FFM) {
     if (!xf_fmc_latent_ok(c.latent_dim)) return false;
   } else if (c.fm == XF_SERVE_MVM) {
     if (!xf_mvm_latent_ok(c.latent_dim)) return false;

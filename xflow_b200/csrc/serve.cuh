@@ -12,9 +12,12 @@
 #include "internal.h"
 
 // what a model's rows hold (xf_model::fm, xf_model_info::fm, the files' fm field)
-enum { XF_SERVE_LR = 0, XF_SERVE_FM = 1, XF_SERVE_FMC = 2, XF_SERVE_MVM = 3 };
-// rows {key, word 8, v[K], 0...}: the canonical FM's (word 8: w) and the multi-view machine's (word 8: 0, no linear term)
-__host__ __device__ inline bool xf_serve_latent_rows(int fm) { return fm == XF_SERVE_FMC || fm == XF_SERVE_MVM; }
+enum { XF_SERVE_LR = 0, XF_SERVE_FM = 1, XF_SERVE_FMC = 2, XF_SERVE_MVM = 3, XF_SERVE_FFM = 4 };
+// rows {key, word 8, v[K], 0...}: the canonical FM's and the field-aware FM's (word 8: w) and the multi-view machine's
+// (word 8: 0, no linear term)
+__host__ __device__ inline bool xf_serve_latent_rows(int fm) {
+  return fm == XF_SERVE_FMC || fm == XF_SERVE_MVM || fm == XF_SERVE_FFM;
+}
 
 struct xf_model {
   XfTableView view{};      // base / mask / log2cap / bshift / stride of the model's rows; K, v_init, v_const, seed of the source;
@@ -75,7 +78,7 @@ inline const char* xf_compat_diff(const XfCompat& a, const XfCompat& b) {
 // 16 + 4K rounded up to 32, so that every row starts on a sector and lane c's piece v[4c .. 4c+3] lies at 16 + 16c.
 // F16 (FM and canonical only; w stays float32): FM {key, w, st, qt}: 16, no padding; canonical {key, w, 0, v[K], 0...}:
 // 16 + 2K rounded up to 32, lane c's piece at 16 + 8c.  A multi-view machine's row {key, u64 0, v[K], 0...} is the
-// canonical one with w = 0.
+// canonical one with w = 0; a field-aware FM's row is the canonical one.
 __host__ __device__ inline uint32_t xf_model_row_bytes(int fm, int K, int precision) {
   const uint32_t vb = precision == XF_PRECISION_F16 ? 2u : 4u;
   if (xf_serve_latent_rows(fm)) return (16u + vb * (uint32_t)K + 31u) & ~31u;
@@ -88,9 +91,9 @@ inline bool xf_fmc_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K ==
 inline bool xf_mvm_latent_ok(int K) { return K == 4 || K == 8 || K == 16 || K == 32; }
 // A packed row of a model (fm, K, precision, row_bytes) has zero bytes where its layout has padding: LR [12, 16); FM
 // [20, 32) at F32, none at F16; canonical [12, 16) and [16 + 4K, row_bytes) at F32, [16 + 2K, row_bytes) at F16; a
-// multi-view machine's as the canonical one's, and [8, 12) too.  Every model in memory keeps them zero (the fill writes
-// them, freeze and convert write fields only, the other passes copy whole rows), so that whole rows compare and hash as
-// their fields do.  Checked a word at a time: the 4-byte word after w (LR, canonical; for a multi-view machine's row
+// multi-view machine's as the canonical one's, and [8, 12) too; a field-aware FM's as the canonical one's.  Every model
+// in memory keeps them zero (the fill writes them, freeze and convert write fields only, the other passes copy whole
+// rows), so that whole rows compare and hash as their fields do.  Checked a word at a time: the 4-byte word after w (LR, canonical; for a multi-view machine's row
 // the word of w too) or qt (FM), then 8-byte words to the row's end.
 inline bool xf_model_padding_zero(const uint8_t* p, int fm, int K, int precision, uint32_t row_bytes) {
   if (fm == XF_SERVE_FM && precision == XF_PRECISION_F16) return true;
