@@ -1,6 +1,10 @@
 """The field-aware FM trainer (XF_MODEL_FFM, csrc/step_ffm.cu) on the device: parity with the float64 statement
 (ffm_model.FFM64) at every latent_dim and optimizer, the canonical FM at one field, the fixed-order forward, progressive
-validation, exact resume, launch counts and the refusals."""
+validation, exact resume, launch counts, two host threads training at once and the refusals."""
+import os
+import subprocess
+import sys
+
 import numpy as np
 import pytest
 
@@ -11,6 +15,7 @@ from xflow_b200 import api
 pytestmark = pytest.mark.gpu
 
 ERR_ARG = "error -1:"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _csr(lens):
@@ -277,6 +282,55 @@ def test_launch_counts_match_the_mvm():
         tr.set_validation(None)
         counts.append(got)
     assert counts[0] == counts[1] == [2, 1, 3]
+
+
+# Two host threads take the first L = 128 step of a fresh process at once (the step kernel's 64 KB shared-memory opt-in
+# is made then), each on its own table; the keys are distinct, so the state after the step has one value.
+_THREADS = r"""
+import threading
+import numpy as np
+from xflow_b200 import api
+L, B = 128, 4096
+rng = np.random.default_rng(11)
+lens = rng.integers(1, 40, B)
+rp = np.zeros(B + 1, np.uint32)
+rp[1:] = np.cumsum(lens)
+n = int(rp[-1])
+keys = api.hash_decimal_ids(rng.permutation(4 * n)[:n].astype(np.uint64) + 1)
+fields = rng.integers(0, 32, n).astype(np.uint8)
+x = rng.uniform(0.3, 1.5, n).astype(np.float32)
+lab = (rng.random(B) < 0.3).astype(np.uint8)
+
+def run(out, i, barrier=None):
+    t = api.Table(latent_dim=L, optimizer=api.OPT_FTRL, v_init=api.VINIT_COUNTER, seed=4, canonical_fm=1, capacity=1 << 18)
+    tr = api.Trainer(t, model=api.MODEL_FFM, max_rows=B, max_nnz=n, keep_loss=True)
+    if barrier is not None:
+        barrier.wait()
+    tr.step_host_fields(rp, keys, fields, x, lab)
+    ks = np.sort(t.list_keys())
+    e = t.export(ks)
+    out[i] = (tr.get_loss(B).tobytes(), ks.tobytes(), {k: np.ascontiguousarray(v).tobytes() for k, v in e.items()})
+    tr.close()
+    t.close()
+
+out = [None] * 3
+barrier = threading.Barrier(2)
+threads = [threading.Thread(target=run, args=(out, i, barrier)) for i in range(2)]
+for th in threads:
+    th.start()
+for th in threads:
+    th.join()
+run(out, 2)
+assert out[2] is not None and len(out[2][1]) == 8 * n
+assert out[0] == out[2] and out[1] == out[2]
+print("ok")
+"""
+
+
+def test_two_threads_first_step_on_the_device():
+    env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
+    r = subprocess.run([sys.executable, "-c", _THREADS], cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout + r.stderr
 
 
 def test_refusals_leave_the_table_unchanged():

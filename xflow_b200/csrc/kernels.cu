@@ -15,6 +15,10 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <mutex>
+#include <set>
+#include <utility>
+
 #include "kernels.h"
 #include "table.cuh"
 
@@ -432,6 +436,20 @@ int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm) {
   uint64_t cap = (uint64_t)xf_sms() * blocks_per_sm;
   if (want < 1) want = 1;
   return (int)(want < cap ? want : cap);
+}
+int xf_grid_smem(const void* kernel, uint64_t work_items, int block, size_t smem) {
+  if (smem > 48 * 1024) {
+    // the opt-in is per device and per kernel: made once each, however many host threads launch at once
+    static std::mutex mu;
+    static std::set<std::pair<int, const void*>> done;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> lock(mu);
+    if (done.insert({dev, kernel}).second)
+      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  }
+  const int per_sm = (int)(227 * 1024 / (smem + 1024));
+  return xf_grid_for(work_items, block, per_sm < 8 ? per_sm : 8);
 }
 
 int xf_vec_for(int K) { return K <= 0 ? 1 : (K % 4 == 0 ? 4 : (K % 2 == 0 ? 2 : 1)); }

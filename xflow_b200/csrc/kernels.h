@@ -63,6 +63,10 @@ void xf_launch_evict_hist(const XfTableView& t, const uint32_t* stamp, const XfE
 void xf_launch_list_keys(const XfTableView& t, uint64_t* keys_out, unsigned long long* count, uint64_t max_out,
                          cudaStream_t st);
 int xf_grid_for(uint64_t work_items, int block, int blocks_per_sm);
+// xf_grid_for for a kernel whose CTAs of `block` threads take `smem` bytes of dynamic shared memory each: as many CTAs
+// per SM as its 227 KB hold (1 KB of it reserved per CTA), at most 8.  Past the 48 KB a launch gets without opting in,
+// `kernel` is opted in to `smem` first, once per device and kernel, under a lock.
+int xf_grid_smem(const void* kernel, uint64_t work_items, int block, size_t smem);
 void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys,
                             const uint8_t* labels, int B, uint64_t nnz, int mode, uint32_t seq, uint64_t* rows_by_seq,
                             float* loss_out, float* pctr_out, float* abs_loss_sum, unsigned long long* unique_total,

@@ -27,10 +27,9 @@
 // A canonical model (xf_table_freeze_canonical, fm = XF_SERVE_FMC) serves the textbook FM with feature values
 // (step_fmc.cu), whose per-k sums do not collapse: its row is {key, w, 0, v[K]} padded to a multiple of 32 bytes.
 //   freeze   xf_k_freeze_fmc<COUNT>  the same two passes; v is the row's latent block or its initial values
-//   predict  xf_k_serve_fmc<C>       xf_k_step_fmc's mapping (C = K/4 lanes per token), its per-lane order, its
-//                                    reductions and its FMA contraction, spelled out (xf_fmc_add, xf_fmc_arg); the C
-//                                    lanes of a token load the head and their 16-byte piece of the home slot at once;
-//                                    two passes in flight
+//   predict  xf_k_serve_fmc<C>       xf_k_step_fmc's mapping (C = K/4 lanes per token), its per-lane order and its
+//                                    arithmetic (forward.cuh: xf_fmc_add, xf_fmc_arg); the C lanes of a token load the
+//                                    head and their 16-byte piece of the home slot at once; two passes in flight
 //
 // A multi-view machine's model (xf_table_freeze_mvm, fm = XF_SERVE_MVM) serves step_mvm.cu's forward on field ids and
 // feature values: its row is the canonical one with w = 0, {key, 0, v[K]} (the machine has no linear term).
@@ -43,7 +42,8 @@
 // feature values: its row is the canonical one, piece c of v the key's vector for field c.
 //   freeze   xf_k_freeze_fmc<COUNT, false>  the canonical freeze
 //   predict  xf_k_serve_ffm<C>              xf_k_serve_fmc's mapping, loads and probe; the field sums T[F][F] in dynamic
-//                                           shared memory, added in token order as xf_k_step_ffm adds them (xf_ffm_add)
+//                                           shared memory, in token order, with xf_k_step_ffm's arithmetic (forward.cuh:
+//                                           xf_ffm_add, xf_ffm_arg)
 //
 // An F16 model (xf_model_convert) holds its latent fields in binary16: FM {key, w, st, qt} in 16 bytes, canonical
 // {key, w, 0, v[K]} with 2-byte v.  Its predict and lookup kernels are the F32 ones' H = true instantiations, which widen
@@ -52,7 +52,8 @@
 //                                              converted and put into the result with xf_model_claim
 //
 // Each row kind's forward is a token loop and a finishing step: xf_serve_arg (LR, FM), xf_fmc_arg (canonical),
-// xf_mvm_product (multi-view machine), xf_ffm_arg (field-aware FM), each written once.  A flat predict kernel runs the
+// xf_mvm_product (multi-view machine), xf_ffm_arg (field-aware FM), each written once; the last three are forward.cuh's,
+// shared with the training steps.  A flat predict kernel runs the
 // loop over each row's token indices.  A candidate kernel (xf_k_serve_cand*) runs it as a fold over positions
 // (xf_serve_fold, xf_fmc_fold, xf_mvm_fold, xf_ffm_fold): once over a request's context, then over each candidate's
 // tokens from that state (see "Two forms of each fold").  xf_launch_predict and xf_launch_candidates pick the instantiation (xf_with_precision, xf_with_lanes); the
@@ -236,8 +237,7 @@ __device__ __forceinline__ void xf_fmc_serve_token(const XfTableView& m, int abs
     if (absent == XF_ABSENT_ZERO) return;
     // the row the table would insert: w = 0 and a latent block that is not materialised
     w = 0.f;
-    v = make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
-                    xf_v_init(m, key, 4 * c + 3));
+    v = xf_v_init_piece(m, key, c);
   }
   xf_fmc_add(v, x, w, c == 0, S, Q, wx);
 }
@@ -307,7 +307,7 @@ xf_k_serve_fmc(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, 
       if (va) xf_fmc_serve_token<H>(m, absent, ka, ra, wa, pa, xa, c, S, Q, wx);
       if (vb) xf_fmc_serve_token<H>(m, absent, kb, rb, wb, pb, xb, c, S, Q, wx);
     }
-    const float arg = xf_fmc_arg<C>(S, Q, wx);
+    const float arg = xf_fmc_arg(C, S, Q, wx);
     if (lane == 0) pctr_out[row] = xf_sigmoid(arg);
   }
 }
@@ -322,8 +322,7 @@ __device__ __forceinline__ float4 xf_mvm_serve_token(const XfTableView& m, int a
   float w;
   if (xf_fmc_find<H>(m, key, k, w, v, c)) return v;
   if (absent == XF_ABSENT_ZERO) return make_float4(0.f, 0.f, 0.f, 0.f);
-  return make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
-                     xf_v_init(m, key, 4 * c + 3));
+  return xf_v_init_piece(m, key, c);
 }
 
 // The n tokens of a row from keys[beg] (vals NULL: every value 1) into the warp's sums S, each entry in token order
@@ -421,13 +420,7 @@ xf_k_serve_mvm(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, 
 }
 
 // ---- field-aware FM rows {key, w, 0, v[L]}: the forward of xf_k_step_ffm (pass 1, pair sum, sigmoid) on the model's
-// rows.  Piece c of v is the key's vector for field c; F = C = L/4 fields.  The warp's field sums T[a][b] are F x F
-// float4 in shared memory (T[a * F + b]), Σwx and Q are warp-uniform.  The step kernel's arithmetic, spelled out as its
-// machine code does it (cuobjdump -sass of xf_k_step_ffm<C>, every C: the FMUL / FFMA / FADD of pass 1 and the pair sum):
-//   a_k = x v_k;  q = fma(a3, a3, fma(a2, a2, fma(a1, a1, a0 a0)))  (lane c == f);  wxt = w x  (lane c == 0)
-//   Σwx = Σwx + wxt, Q = Q + q and T[f][c]_k = T[f][c]_k + a_k, each in token order
-//   P = P + fma(u3, s3, fma(u2, s2, fma(u0, s0, u1 s1)))   u = T[a][b], s = T[b][a], a over the present fields ascending
-//   arg = fma(0.5, (xor 16 .. 1 warp sum of P) - Q, Σwx)
+// rows, with its arithmetic (xf_ffm_add, xf_ffm_arg).  Piece c of v is the key's vector for field c; F = C = L/4 fields.
 // A token's w and piece c: its row found from the home slot the caller loaded (k, w, v), or the absent policy's row
 // (DEFAULT: w = 0 and the initial values; ZERO: zeros, its field still present)
 template <bool H>
@@ -436,62 +429,7 @@ __device__ __forceinline__ void xf_ffm_serve_token(const XfTableView& m, int abs
   if (xf_fmc_find<H>(m, key, k, w, v, c)) return;
   w = 0.f;
   if (absent == XF_ABSENT_ZERO) v = make_float4(0.f, 0.f, 0.f, 0.f);
-  else
-    v = make_float4(xf_v_init(m, key, 4 * c), xf_v_init(m, key, 4 * c + 1), xf_v_init(m, key, 4 * c + 2),
-                    xf_v_init(m, key, 4 * c + 3));
-}
-
-// One pass's tokens into the warp's state, as xf_k_step_ffm's pass 1: lane (token g, c) holds the token's field f,
-// piece c of v, w and x; the live tokens are the pass's first groups.  Σwx and Q take the live tokens in turn; a field's
-// tokens are ranked with __match_any_sync and added to T[f][*] a rank per round, lowest position first.
-template <int C>
-__device__ __forceinline__ void xf_ffm_add(float4* T, bool live, uint32_t f, float4 v, float w, float x, float& wx,
-                                           float& Q) {
-  constexpr int TP = 32 / C;
-  const int lane = threadIdx.x & 31;
-  const int c = lane & (C - 1);
-  const int lead = lane & ~(C - 1);
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-  float q = 0.f, wxt = 0.f;
-  if (live) {
-    a = make_float4(__fmul_rn(v.x, x), __fmul_rn(v.y, x), __fmul_rn(v.z, x), __fmul_rn(v.w, x));
-    if (c == (int)f) q = __fmaf_rn(a.w, a.w, __fmaf_rn(a.z, a.z, __fmaf_rn(a.y, a.y, __fmul_rn(a.x, a.x))));
-    if (c == 0) wxt = __fmul_rn(w, x);
-  }
-  const float qt = __shfl_sync(0xffffffffu, q, lead + (int)f);  // the self term, from lane f of the token's group
-  const int n = __popc(__ballot_sync(0xffffffffu, live)) / C;
-  for (int g = 0; g < n; ++g) {
-    wx = __fadd_rn(wx, __shfl_sync(0xffffffffu, wxt, g * C));
-    Q = __fadd_rn(Q, __shfl_sync(0xffffffffu, qt, g * C));
-  }
-  int rank = 0, last = 0;
-  if (TP > 1) {
-    const unsigned peers = __match_any_sync(0xffffffffu, live ? f : 0xFFu);
-    rank = __popc(peers & ((1u << lead) - 1u)) / C;
-    last = (int)__reduce_max_sync(0xffffffffu, live ? (unsigned)rank : 0u);
-  }
-  for (int r = 0; r <= last; ++r) {
-    if (live && rank == r) {
-      float4 s = T[f * C + c];
-      s.x = __fadd_rn(s.x, a.x); s.y = __fadd_rn(s.y, a.y); s.z = __fadd_rn(s.z, a.z); s.w = __fadd_rn(s.w, a.w);
-      T[f * C + c] = s;
-    }
-    __syncwarp();
-  }
-}
-
-// the pair sum over the present fields and the sigmoid's argument (every lane returns it)
-template <int C>
-__device__ __forceinline__ float xf_ffm_arg(const float4* T, unsigned present, float wx, float Q) {
-  const int lane = threadIdx.x & 31;
-  float P = 0.f;
-  if (lane < C && ((present >> lane) & 1u))
-    for (unsigned q = present; q; q &= q - 1) {
-      const int fa = __ffs(q) - 1;
-      const float4 u = T[fa * C + lane], s = T[lane * C + fa];
-      P = __fadd_rn(P, __fmaf_rn(u.w, s.w, __fmaf_rn(u.z, s.z, __fmaf_rn(u.x, s.x, __fmul_rn(u.y, s.y)))));
-    }
-  return __fmaf_rn(0.5f, __fsub_rn(xf_warp_sum(P), Q), wx);
+  else v = xf_v_init_piece(m, key, c);
 }
 
 // The n tokens of a row from keys[beg] (vals NULL: every value 1) into the warp's state T, Σwx, Q, with
@@ -526,8 +464,8 @@ __device__ __forceinline__ unsigned xf_ffm_fold(const XfTableView& m, int absent
     if (va) xf_ffm_serve_token<H>(m, absent, ka, ra, wa, pa, c);
     if (vb) xf_ffm_serve_token<H>(m, absent, kb, rb, wb, pb, c);
     present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
-    xf_ffm_add<C>(T, va, fa, pa, wa, xa, wx, Q);  // pass a, then pass b
-    xf_ffm_add<C>(T, vb, fb, pb, wb, xb, wx, Q);
+    xf_ffm_add<C, true>(T, va, 0, fa, pa, wa, xa, wx, Q);  // pass a, then pass b
+    xf_ffm_add<C, true>(T, vb, 0, fb, pb, wb, xb, wx, Q);
   }
   return present;
 }
@@ -579,8 +517,8 @@ xf_k_serve_ffm(XfTableView m, int absent, const uint32_t* __restrict__ row_ptr, 
       if (va) xf_ffm_serve_token<H>(m, absent, ka, ra, wa, pa, c);
       if (vb) xf_ffm_serve_token<H>(m, absent, kb, rb, wb, pb, c);
       present |= (va ? 1u << fa : 0u) | (vb ? 1u << fb : 0u);
-      xf_ffm_add<C>(T, va, fa, pa, wa, xa, wx, Q);
-      xf_ffm_add<C>(T, vb, fb, pb, wb, xb, wx, Q);
+      xf_ffm_add<C, true>(T, va, 0, fa, pa, wa, xa, wx, Q);
+      xf_ffm_add<C, true>(T, vb, 0, fb, pb, wb, xb, wx, Q);
     }
     present = __reduce_or_sync(0xffffffffu, present);
     const float arg = xf_ffm_arg<C>(T, present, wx, Q);
@@ -600,16 +538,6 @@ static void xf_with_precision(const xf_model* m, F&& f) {
   else f(std::false_type());
 }
 
-// before the first field-aware FM launch at C = 32 on the current device (below)
-static void xf_ffm_opt_in();
-
-// CTAs of `warps` warps with `smem` bytes of dynamic shared memory each for `threads` threads of work: as many as fit
-// on the GPU at once, at most 8 per SM
-static int xf_ffm_grid(uint64_t threads, int warps, size_t smem) {
-  const int per_sm = (int)(227 * 1024 / (smem + 1024));
-  return xf_grid_for(threads, 32 * warps, per_sm < 8 ? per_sm : 8);
-}
-
 // the flat forward of any model on device arrays (fields: a multi-view machine's or a field-aware FM's, which read
 // nothing else)
 static void xf_launch_predict(const xf_model* m, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
@@ -620,11 +548,10 @@ static void xf_launch_predict(const xf_model* m, const uint32_t* row_ptr, const 
   xf_with_precision(m, [&](auto H) {
     if (m->fm == XF_SERVE_FFM)
       xf_with_lanes<32>(m->view.K, [&](auto C) {
-        constexpr int warps = xf_ffm_warps(C);
-        constexpr size_t smem = (size_t)warps * C * C * sizeof(float4);
-        if (smem > 48 * 1024) xf_ffm_opt_in();
-        xf_k_serve_ffm<C, H><<<xf_ffm_grid((uint64_t)rows * 32, warps, smem), 32 * warps, smem, st>>>(
-            m->view, m->absent, row_ptr, keys, fields, vals, B, pctr_out);
+        constexpr int block = 32 * xf_ffm_warps(C);
+        constexpr size_t smem = (size_t)xf_ffm_warps(C) * C * C * sizeof(float4);
+        xf_k_serve_ffm<C, H><<<xf_grid_smem((const void*)xf_k_serve_ffm<C, H>, (uint64_t)rows * 32, block, smem), block,
+                               smem, st>>>(m->view, m->absent, row_ptr, keys, fields, vals, B, pctr_out);
       });
     else if (m->fm == XF_SERVE_MVM)
       xf_with_lanes<8>(m->view.K, [&](auto C) {
@@ -744,7 +671,7 @@ xf_k_serve_cand_fmc(XfTableView m, int absent, XfCandView b, float* __restrict__
                  float S[4] = {x.S[0], x.S[1], x.S[2], x.S[3]};
                  float Q = x.Q, wx = x.wx;
                  xf_fmc_fold<C, H>(m, absent, b.keys, b.vals, beg, x.lo, x.lo + n, S, Q, wx);
-                 const float arg = xf_fmc_arg<C>(S, Q, wx);
+                 const float arg = xf_fmc_arg(C, S, Q, wx);
                  if (lane == 0) pctr_out[c] = xf_sigmoid(arg);
                },
                [](const Ctx&) {});
@@ -854,27 +781,6 @@ xf_k_serve_cand_ffm(XfTableView m, int absent, XfCandView b, float* __restrict__
                });
 }
 
-// The field-aware FM kernels' dynamic shared memory at C = 32 is past the 48 KB a launch gets without opting in.  The
-// opt-in is per device and per kernel; it is made once per device, before the first such launch on it, however many
-// host threads launch at once.
-static void xf_ffm_opt_in() {
-  static std::mutex mu;
-  static std::vector<bool> done;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lock(mu);
-  if ((size_t)dev < done.size() && done[(size_t)dev]) return;
-  constexpr int flat = xf_ffm_warps(32) * 32 * 32 * (int)sizeof(float4);
-  constexpr int cand = xf_cand_ffm_warps(32) * 2 * 32 * 32 * (int)sizeof(float4);
-  cudaFuncSetAttribute(xf_k_serve_ffm<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, flat);
-  cudaFuncSetAttribute(xf_k_serve_ffm<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, flat);
-  cudaFuncSetAttribute(xf_k_serve_cand_ffm<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cand);
-  cudaFuncSetAttribute(xf_k_serve_cand_ffm<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cand);
-  if (done.size() <= (size_t)dev) done.resize((size_t)dev + 1, false);
-  done[(size_t)dev] = true;
-}
-
-
 // the candidate forward of any model on device arrays
 static void xf_launch_candidates(const xf_model* m, const XfCandView& b, float* pctr_out, cudaStream_t st) {
   if (b.candidates == 0) return;
@@ -884,10 +790,10 @@ static void xf_launch_candidates(const xf_model* m, const XfCandView& b, float* 
   xf_with_precision(m, [&](auto H) {
     if (m->fm == XF_SERVE_FFM)
       xf_with_lanes<32>(m->view.K, [&](auto C) {
-        constexpr int W = xf_cand_ffm_warps(C);
-        constexpr size_t smem = (size_t)W * 2 * C * C * sizeof(float4);
-        if (smem > 48 * 1024) xf_ffm_opt_in();
-        xf_k_serve_cand_ffm<C, H><<<xf_ffm_grid(warps * 32, W, smem), 32 * W, smem, st>>>(m->view, m->absent, b, pctr_out);
+        constexpr int block = 32 * xf_cand_ffm_warps(C);
+        constexpr size_t smem = (size_t)xf_cand_ffm_warps(C) * 2 * C * C * sizeof(float4);
+        xf_k_serve_cand_ffm<C, H><<<xf_grid_smem((const void*)xf_k_serve_cand_ffm<C, H>, warps * 32, block, smem), block,
+                                    smem, st>>>(m->view, m->absent, b, pctr_out);
       });
     else if (m->fm == XF_SERVE_MVM)
       xf_with_lanes<8>(m->view.K, [&](auto C) {
@@ -957,8 +863,7 @@ xf_k_freeze(XfTableView t, XfTableView m, int absent, int prune, uint64_t lo, ui
 // materialised, else the initial values
 __device__ __forceinline__ float4 xf_fmc_piece(const XfTableView& t, uint64_t r, bool ready, uint64_t key, uint32_t q) {
   if (ready) return __ldcg(reinterpret_cast<const float4*>(xf_row(t, r) + 32) + q);
-  return make_float4(xf_v_init(t, key, 4 * q), xf_v_init(t, key, 4 * q + 1), xf_v_init(t, key, 4 * q + 2),
-                     xf_v_init(t, key, 4 * q + 3));
+  return xf_v_init_piece(t, key, q);
 }
 
 // xf_k_freeze for a canonical table: the model row is {key, w, 0, v[K]} with v resolved as xf_fmc_piece does.  Prune:

@@ -89,10 +89,10 @@ xf_k_det_fmc(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t
       const float x = vals ? __ldg(vals + j) : 1.0f;
       float4 v;
       if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(xf_row(t, slot) + 32) + c);
-      else v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
+      else v = xf_v_init_piece(t, key, c);
       xf_fmc_add(v, x, w, c == 0, S, Q, wx);
     }
-    const float pctr = xf_sigmoid(xf_fmc_arg<C>(S, Q, wx));
+    const float pctr = xf_sigmoid(xf_fmc_arg(C, S, Q, wx));
     const float loss = __fsub_rn(pctr, (float)labels[row]);
     if (lane == 0) {
       d.res[row] = loss;
@@ -155,7 +155,7 @@ xf_k_det_mvm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t
       if (on) {
         if (vals) x = __ldg(vals + j);
         if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(xf_row(t, slot) + 32) + c);
-        else v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
+        else v = xf_v_init_piece(t, key, c);
         present |= 1u << f;
       }
       xf_mvm_add<K>(S, on, f, c, v, x);

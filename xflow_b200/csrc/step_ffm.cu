@@ -18,13 +18,13 @@
 //     the token groups that share a field add in turn, lowest position first);
 //   - sum w x and Q: left folds from +0 in ascending position;
 //   - lane b adds <T[a][b], T[b][a]> over the present a ascending from +0, then the xor 16 .. 1 warp tree.
-// T starts zeroed; after a row only the rows T[a][*] of its present fields are cleared again.
+// T starts zeroed; after a row only the rows T[a][*] of its present fields are cleared again.  The forward's arithmetic
+// is forward.cuh's (xf_ffm_add, xf_ffm_arg), which the serving kernels run too.
 // Parity: a float64 numpy model (tests/ffm_model.py, tests/test_gpu_ffm.py).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "kernels.h"
-#include "table.cuh"
+#include "forward.cuh"
 
 #define XF_NO_SLOT 0xFFFFFFFFu
 
@@ -75,52 +75,19 @@ xf_k_step_ffm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
       f = __shfl_sync(0xffffffffu, f, lead);
       key = __shfl_sync(0xffffffffu, (unsigned long long)key, lead);
       const bool ok = live && slot != XF_NO_SLOT;
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-      float q = 0.f, wxt = 0.f;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      float x = 0.f;
       if (ok) {
-        const float x = vals ? __ldg(vals + j) : 1.0f;
-        float4 v;
+        x = vals ? __ldg(vals + j) : 1.0f;
         if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(xf_row(t, slot) + 32) + c);
-        else v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
-        a = make_float4(v.x * x, v.y * x, v.z * x, v.w * x);
-        if (c == (int)f) q = a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
-        if (c == 0) wxt = w * x;
+        else v = xf_v_init_piece(t, key, c);
       }
-      // the token's self term sits in lane lead + f: bring it to the lead lane, then add the pass's tokens in turn
-      const float qt = __shfl_sync(0xffffffffu, q, lead + (int)f);
-      const int n = (int)min((uint32_t)TP, end - j0);
-      for (int g = 0; g < n; ++g) {
-        wx += __shfl_sync(0xffffffffu, wxt, g * C);
-        Q += __shfl_sync(0xffffffffu, qt, g * C);
-      }
-      // T[f][c] += a, the token groups of one field in ascending position
-      int rank = 0, last = 0;
-      if (TP > 1) {
-        const unsigned peers = __match_any_sync(0xffffffffu, ok ? f : 0xFFu);
-        rank = __popc(peers & ((1u << lead) - 1u)) / C;
-        last = (int)__reduce_max_sync(0xffffffffu, ok ? (unsigned)rank : 0u);
-      }
-      for (int k = 0; k <= last; ++k) {
-        if (ok && rank == k) {
-          float4 s = T[f * F + c];
-          s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
-          T[f * F + c] = s;
-        }
-        __syncwarp();
-      }
+      // a live token without a row adds nothing to T and +0 to Σwx and Q
+      xf_ffm_add<C>(T, ok, (int)min((uint32_t)TP, end - j0), f, v, w, x, wx, Q);
       if (ok) present |= 1u << f;
     }
     present = __reduce_or_sync(0xffffffffu, present);
-    // y: lane b < F takes sum_a <T[a][b], T[b][a]> over the present fields
-    float P = 0.f;
-    if (lane < F && ((present >> lane) & 1u)) {
-      for (unsigned m = present; m; m &= m - 1) {
-        const int fa = __ffs(m) - 1;
-        const float4 u = T[fa * F + lane], s = T[lane * F + fa];
-        P += u.x * s.x + u.y * s.y + u.z * s.z + u.w * s.w;
-      }
-    }
-    const float pctr = xf_sigmoid(wx + 0.5f * (xf_warp_sum(P) - Q));
+    const float pctr = xf_sigmoid(xf_ffm_arg<C>(T, present, wx, Q));
     if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
     if (mode == 0) {
       const float loss = pctr - (float)labels[row];
@@ -148,7 +115,7 @@ xf_k_step_ffm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
           if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(rowp + 32) + c);
           else {
             const uint64_t key = __ldcs(keys + j);
-            v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
+            v = xf_v_init_piece(t, key, c);
           }
           d.x -= v.x * x; d.y -= v.y * x; d.z -= v.z * x; d.w -= v.w * x;
         }
@@ -177,37 +144,15 @@ xf_k_step_ffm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
   }
 }
 
-// C = 32 (L = 128) holds 16 KB of field sums per warp: 4 warps per CTA (64 KB, opt-in), 3 CTAs per SM
-template <int C>
-static void xf_launch_ffm(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
-                          const float* vals, const uint8_t* labels, int B, int mode, uint32_t* touched, float* loss_out,
-                          float* pctr_out, float* abs_loss_sum, cudaStream_t st) {
-  constexpr int block = C == 32 ? 128 : 256;
-  constexpr size_t smem = (size_t)(block / 32) * C * C * sizeof(float4);
-  if (smem > 48 * 1024) {
-    static bool opted[64] = {};  // per device; setting it twice is harmless
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 64 && !opted[dev]) {
-      cudaFuncSetAttribute(xf_k_step_ffm<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      opted[dev] = true;
-    }
-  }
-  const int per_sm = (int)(227 * 1024 / (smem + 1024));
-  xf_k_step_ffm<C><<<xf_grid_for((uint64_t)B * 32, block, per_sm < 8 ? per_sm : 8), block, smem, st>>>(
-      t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum);
-}
-
 void xf_launch_step_ffm(const XfTableView& t, const uint32_t* row_ptr, const uint64_t* keys, const uint8_t* fields,
                         const float* vals, const uint8_t* labels, int B, int mode, uint32_t* touched, float* loss_out,
                         float* pctr_out, float* abs_loss_sum, cudaStream_t st) {
   if (B <= 0) return;
-  switch (t.K) {
-    case 4: xf_launch_ffm<1>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-    case 8: xf_launch_ffm<2>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-    case 16: xf_launch_ffm<4>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-    case 32: xf_launch_ffm<8>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-    case 64: xf_launch_ffm<16>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-    default: xf_launch_ffm<32>(t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum, st); break;
-  }
+  xf_with_lanes<32>(t.K, [&](auto C) {
+    // C = 32 (L = 128) holds 16 KB of field sums per warp: 4 warps per CTA (64 KB, opt-in), 3 CTAs per SM
+    constexpr int block = C == 32 ? 128 : 256;
+    constexpr size_t smem = (size_t)(block / 32) * C * C * sizeof(float4);
+    xf_k_step_ffm<C><<<xf_grid_smem((const void*)xf_k_step_ffm<C>, (uint64_t)B * 32, block, smem), block, smem, st>>>(
+        t, row_ptr, keys, fields, vals, labels, B, mode, touched, loss_out, pctr_out, abs_loss_sum);
+  });
 }

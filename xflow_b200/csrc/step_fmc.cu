@@ -8,13 +8,13 @@
 //
 // One warp per row, C = K/4 lanes per token (each holds 4 latent coordinates = one 16-byte piece of the row: the
 // C lanes of a token read its latent row with ONE instruction), 32/C tokens per pass.  Pass 1: pull + per-k sums;
-// warp reductions; sigmoid.  Pass 2: the per-key sums with L2 atomics (one float4 RED per lane for A, two f64
-// atomics per token for G / L2); the token that finds G untouched records the slot for xf_k_update.
+// warp reductions; sigmoid (forward.cuh's xf_fmc_add and xf_fmc_arg, as the serving kernels).  Pass 2: the per-key
+// sums with L2 atomics (one float4 RED per lane for A, two f64 atomics per token for G / L2); the token that finds G
+// untouched records the slot for xf_k_update.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "kernels.h"
-#include "table.cuh"
+#include "forward.cuh"
 
 #define XF_NO_SLOT 0xFFFFFFFFu
 
@@ -61,21 +61,10 @@ xf_k_step_fmc(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
       const float x = vals ? __ldg(vals + j) : 1.0f;
       float4 v;
       if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(xf_row(t, slot) + 32) + c);
-      else v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
-      const float a0 = v.x * x, a1 = v.y * x, a2 = v.z * x, a3 = v.w * x;
-      S[0] += a0; S[1] += a1; S[2] += a2; S[3] += a3;
-      Q += a0 * a0 + a1 * a1 + a2 * a2 + a3 * a3;
-      if (c == 0) wx += w * x;
+      else v = xf_v_init_piece(t, key, c);
+      xf_fmc_add(v, x, w, c == 0, S, Q, wx);
     }
-    // S_k over the tokens (lanes with the same c), sum_k S_k^2 over the c's, Q and wx over the warp
-#pragma unroll
-    for (int e = 0; e < 4; ++e)
-      for (int o = C; o < 32; o <<= 1) S[e] += __shfl_xor_sync(0xffffffffu, S[e], o);
-    float s2 = S[0] * S[0] + S[1] * S[1] + S[2] * S[2] + S[3] * S[3];
-    for (int o = 1; o < C; o <<= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    Q = xf_warp_sum(Q);
-    wx = xf_warp_sum(wx);
-    const float pctr = xf_sigmoid(wx + 0.5f * (s2 - Q));
+    const float pctr = xf_sigmoid(xf_fmc_arg(C, S, Q, wx));
     if (lane == 0 && pctr_out) pctr_out[row] = pctr;  // training: only for progressive validation
     if (mode == 1) continue;
     const float loss = pctr - (float)labels[row];

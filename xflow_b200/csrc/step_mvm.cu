@@ -72,7 +72,7 @@ xf_k_step_mvm(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_
       const float x = vals ? __ldg(vals + j) : 1.0f;
       float4 v;
       if (flags & XF_FLAG_V_READY) v = __ldcg(reinterpret_cast<const float4*>(xf_row(t, slot) + 32) + c);
-      else v = make_float4(xf_v_init(t, key, 4 * c), xf_v_init(t, key, 4 * c + 1), xf_v_init(t, key, 4 * c + 2), xf_v_init(t, key, 4 * c + 3));
+      else v = xf_v_init_piece(t, key, c);
       atomicAdd(&S[f][4 * c + 0], v.x * x);
       atomicAdd(&S[f][4 * c + 1], v.y * x);
       atomicAdd(&S[f][4 * c + 2], v.z * x);

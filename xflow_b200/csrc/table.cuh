@@ -244,6 +244,11 @@ __device__ __forceinline__ float xf_v_init(const XfTableView& t, uint64_t key, u
   if (t.v_init == XF_INIT_ZERO) return 0.0f;
   return t.v_const;
 }
+// the initial values of latent piece q, coordinates 4q .. 4q+3 (the piece a lane of the canonical kernels holds)
+__device__ __forceinline__ float4 xf_v_init_piece(const XfTableView& t, uint64_t key, uint32_t q) {
+  return make_float4(xf_v_init(t, key, 4 * q), xf_v_init(t, key, 4 * q + 1), xf_v_init(t, key, 4 * q + 2),
+                     xf_v_init(t, key, 4 * q + 3));
+}
 
 // ---- row accessors
 __device__ __forceinline__ uint8_t* xf_row(const XfTableView& t, uint64_t slot) {
