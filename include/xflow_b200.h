@@ -1101,6 +1101,66 @@ XF_DLL int xf_pv_report_slices(xf_pv* pv, struct xf_pv_report* out, uint32_t n);
 XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv);
 
 /* ------------------------------------------------------------------------------------------------
+ * 9. Grouped test metric (csrc/group_metric.cu).  The exact AUC and logloss inside each group of a held-out set,
+ *    where a group is whatever one uint64 id per row names (a user, a request), and their mean over the groups
+ *    weighted by rows: group AUC, GAUC (Zhou et al., "Deep Interest Network for Click-Through Rate Prediction", KDD
+ *    2018).  A ranker orders candidates within a request, which a pooled AUC (xf_metric) does not judge.  The metric
+ *    sorts on the device, like xf_metric; with one id per segment it is a sliced xf_metric.
+ *
+ *    Rows.  A row (p, y, g): p the float prediction, y != 0 positive, g any uint64 (0 and 2^64 - 1 included).  A row
+ *    with p NaN counts in nan_rows and nothing else; it is in no group, and a group of NaN rows only does not exist.
+ *    Predictions tie when equal as floats (-0.0 ties with +0.0; +-Inf allowed, equal infinities tie).
+ *    Per group g, over its other rows: n_g rows, P_g positives, N_g negatives, and
+ *      U2_g      = sum over its negatives j of (2 #{positives i of g: p_i > p_j} + #{positives i of g: p_i == p_j}),
+ *                  twice the tie-aware Mann-Whitney U, an integer;
+ *      auc_g     = (double)U2_g / ((2.0 * (double)P_g) * (double)N_g) in IEEE double, NaN when P_g or N_g is 0 (the
+ *                  expression of xf_metric_finish's out[5]: rows that form one group report out[5] bit for bit);
+ *      L_i       = a row's logloss term in units of 2^-32: the pv's with weight 1 (section 8), l * 2^32 rounded to the
+ *                  nearest integer, l = -ln q (positive) or -ln(1 - q) (negative), q = p clamped to [1e-15, 1 - 1e-15];
+ *      S_g       = sum of L_i over the group, exact (128 bits);
+ *      logloss_g = (double)S_g / ((double)n_g * 2^32): S_g rounded to the nearest double, then one division.
+ *    Report, with "correctly rounded" the exact ratio rounded to nearest even, and NaN for a zero denominator:
+ *      rows = sum n_g, positives, negatives, nan_rows, groups;  scored_groups: groups with P_g > 0 and N_g > 0,
+ *      scored_rows: their sum of n_g;
+ *      logloss   = sum S_g / (2^32 rows), correctly rounded: byte for byte the logloss of an unweighted xf_pv fed the
+ *                  same rows;
+ *      gauc      = sum over scored groups of T_g / (2^32 scored_rows), correctly rounded,
+ *                  T_g = __double2ull_rn(((double)n_g * auc_g) * 2^32);
+ *      gauc_mean = sum over scored groups of M_g / (2^32 scored_groups), correctly rounded, M_g = __double2ull_rn(auc_g
+ *                  * 2^32).
+ *    Bounds: a metric holds fewer than 2^31 rows (xf_metric's limit), so sum T_g and sum M_g stay below 2^64, sum S_g
+ *    below 2^70 and U2_g, 2 P_g N_g below 2^63.  Every accumulator is an integer and every double a fixed function of
+ *    integers: the report and the per-group arrays depend only on the multiset of rows, not on how they were cut into
+ *    adds, their order, the streams, the grid or the order of atomics.
+ *    Memory: 13 bytes per held row; a finish adds 76 bytes of scratch per held row (two 16-byte sort keys, a 12-byte
+ *    scan, 32 bytes of per-group sums) and CUB's temporary storage, and keeps them for later calls.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct xf_group_metric xf_group_metric;
+/* the report of xf_group_metric_finish (a struct tag only, like xf_pv_report) */
+struct xf_group_report {
+  uint64_t rows, positives, negatives, nan_rows, groups, scored_groups, scored_rows;
+  double logloss, gauc, gauc_mean;
+};
+XF_DLL int xf_group_metric_create(xf_group_metric** out, int device);
+XF_DLL int xf_group_metric_destroy(xf_group_metric* m);
+/* drops every row; stream-ordered after every add enqueued so far, and before every later one */
+XF_DLL int xf_group_metric_reset(xf_group_metric* m);
+/* n predictions, labels (!= 0 positive) and group ids in device memory on m's device, copied into m on cuda_stream
+ * (cudaStream_t or NULL) without a synchronisation: the arrays must stay untouched until that stream has run the add.
+ * XF_ERR_ARG, naming the reason, leaving m unchanged, for a NULL array with n > 0 and for an add that would bring m to
+ * 2^31 rows or more. */
+XF_DLL int xf_group_metric_add_device(xf_group_metric* m, const float* d_pctr, const uint8_t* d_labels,
+                                      const uint64_t* d_groups, uint64_t n, void* cuda_stream);
+/* waits for every add enqueued so far, on any stream; does not reset.  An empty metric reports zero counts and NaN
+ * ratios. */
+XF_DLL int xf_group_metric_finish(xf_group_metric* m, struct xf_group_report* out);
+/* the groups of the last finish in ascending id order into host arrays of n elements, any of them NULL: id, n_g, P_g,
+ * auc_g, logloss_g.  XF_ERR_ARG unless n is that finish's `groups`; XF_ERR_STATE if no finish came after the last
+ * reset or add. */
+XF_DLL int xf_group_metric_groups(xf_group_metric* m, uint64_t n, uint64_t* ids, uint64_t* rows, uint64_t* positives,
+                                  double* auc, double* logloss);
+
+/* ------------------------------------------------------------------------------------------------
  * 1. Reference C API (src/c_api/c_api.h:26-29), unchanged signatures.
  *    XFCreate builds an LR worker on <train_path>-%05d / <test_path>-%05d (rank from XFLOW_RANK,
  *    default 0); paths are copied.  XFStartTrain trains `epochs` (default 60, lr_worker.h:63; env

@@ -78,6 +78,12 @@ class PvReport(C.Structure):
                 ("auc_lo", C.c_double), ("auc_hi", C.c_double)]
 
 
+class GroupReport(C.Structure):
+    _fields_ = [("rows", C.c_uint64), ("positives", C.c_uint64), ("negatives", C.c_uint64), ("nan_rows", C.c_uint64),
+                ("groups", C.c_uint64), ("scored_groups", C.c_uint64), ("scored_rows", C.c_uint64),
+                ("logloss", C.c_double), ("gauc", C.c_double), ("gauc_mean", C.c_double)]
+
+
 # name -> (restype, argtypes); also the list the symbol-export test checks against the header
 _vp, _u64, _u32, _i, _f = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_float
 SIGNATURES = {
@@ -212,6 +218,12 @@ SIGNATURES = {
     "xf_pv_add_device_rows": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _u64, _vp]),
     "xf_pv_report_slices": (_i, [_vp, _vp, _u32]),
     "xf_trainer_set_validation": (_i, [_vp, _vp]),
+    "xf_group_metric_create": (_i, [_vp, _i]),
+    "xf_group_metric_destroy": (_i, [_vp]),
+    "xf_group_metric_reset": (_i, [_vp]),
+    "xf_group_metric_add_device": (_i, [_vp, _vp, _vp, _vp, _u64, _vp]),
+    "xf_group_metric_finish": (_i, [_vp, _vp]),
+    "xf_group_metric_groups": (_i, [_vp, _u64, _vp, _vp, _vp, _vp, _vp]),
     "xf_trainer_set_deterministic": (_i, [_vp, _i]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
@@ -869,6 +881,54 @@ class ProgressiveValidation:
             r = PvReport.from_buffer_copy(raw)
             out.append({name: getattr(r, name) for name, _ in PvReport._fields_})
         return out
+
+
+class GroupMetric:
+    """Exact per-group AUC and logloss of held-out predictions on the device (xf_group_metric_*), keyed by one uint64
+    group id per row, and their row-weighted mean (GAUC).  The report depends only on the rows added."""
+
+    def __init__(self, device=0):
+        self.device = device
+        self.last_groups = 0  # the group count of the last finish
+        self.h = C.c_void_p()
+        _check(lib().xf_group_metric_create(C.byref(self.h), int(device)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            _check(lib().xf_group_metric_destroy(self.h))
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def add_device(self, d_pctr, d_labels, d_groups, n, stream=0):
+        """n predictions (float32), labels (uint8, != 0 positive) and group ids (uint64) at device addresses."""
+        _check(lib().xf_group_metric_add_device(self.h, _p(d_pctr), _p(d_labels), _p(d_groups), int(n),
+                                                _p(stream) if stream else None))
+
+    def finish_bytes(self):
+        """The raw struct xf_group_report, for byte comparisons."""
+        r = GroupReport()
+        _check(lib().xf_group_metric_finish(self.h, C.byref(r)))
+        self.last_groups = r.groups
+        return bytes(r)
+
+    def finish(self):
+        r = GroupReport.from_buffer_copy(self.finish_bytes())
+        return {name: getattr(r, name) for name, _ in GroupReport._fields_}
+
+    def groups(self, n=None):
+        """The last finish's groups in ascending id order: ids, rows, positives, auc, logloss (numpy arrays).  n
+        defaults to that finish's group count."""
+        n = self.last_groups if n is None else int(n)
+        out = dict(ids=np.empty(n, np.uint64), rows=np.empty(n, np.uint64), positives=np.empty(n, np.uint64),
+                   auc=np.empty(n, np.float64), logloss=np.empty(n, np.float64))
+        _check(lib().xf_group_metric_groups(self.h, n, _p(out["ids"]), _p(out["rows"]), _p(out["positives"]),
+                                            _p(out["auc"]), _p(out["logloss"])))
+        return out
+
+    def reset(self):
+        _check(lib().xf_group_metric_reset(self.h))
 
 
 class Trainer:

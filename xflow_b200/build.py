@@ -15,9 +15,9 @@ LIBDIR = os.path.join(ROOT, "xflow_b200", "lib")
 LIB = os.path.join(LIBDIR, "libxflow_b200.so")
 OBJDIR = os.path.join(ROOT, "build", "obj")
 
-CU_SOURCES = ["kernels.cu", "step.cu", "step_lazy.cu", "step_fmc.cu", "step_mvm.cu", "step_ffm.cu", "step_det.cu", "capi.cu", "comm.cu", "mg_kernels.cu", "ingest.cu", "metric.cu", "admit.cu", "evict.cu", "weight.cu", "checkpoint.cu", "serve.cu", "rank.cu", "delta.cu", "validate.cu"]
+CU_SOURCES = ["kernels.cu", "step.cu", "step_lazy.cu", "step_fmc.cu", "step_mvm.cu", "step_ffm.cu", "step_det.cu", "capi.cu", "comm.cu", "mg_kernels.cu", "ingest.cu", "metric.cu", "admit.cu", "evict.cu", "weight.cu", "checkpoint.cu", "serve.cu", "rank.cu", "delta.cu", "validate.cu", "group_metric.cu"]
 CC_SOURCES = ["loader.cc", "metrics.cc", "worker.cc"]
-HEADERS = ["table.cuh", "mg.cuh", "serve.cuh", "forward.cuh", "kernels.h", "internal.h", "hash.h", os.path.join(ROOT, "include", "xflow_b200.h"),
+HEADERS = ["table.cuh", "mg.cuh", "serve.cuh", "forward.cuh", "metric.cuh", "kernels.h", "internal.h", "hash.h", os.path.join(ROOT, "include", "xflow_b200.h"),
            os.path.join(ROOT, "include", "xflow", "xflow.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

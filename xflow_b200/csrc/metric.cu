@@ -20,7 +20,7 @@
 
 #include <cub/cub.cuh>
 
-#include "internal.h"
+#include "metric.cuh"
 
 struct xf_metric {
   int device = 0;
@@ -57,8 +57,7 @@ XF_DLL int xf_metric_reset(xf_metric* m) {
   return XF_OK;
 }
 
-// grow a buffer keeping its first `used` bytes (stream-ordered after everything queued on `st`)
-static int xf_grow_keep(XfDevBuf& b, size_t used, size_t want, cudaStream_t st) {
+int xf_grow_keep(XfDevBuf& b, size_t used, size_t want, cudaStream_t st) {
   if (want <= b.cap) return XF_OK;
   size_t ncap = std::max(want, b.cap * 2);
   void* np = nullptr;

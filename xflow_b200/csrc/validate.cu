@@ -15,7 +15,7 @@
 #include <mutex>
 #include <vector>
 
-#include "internal.h"
+#include "metric.cuh"
 
 typedef unsigned long long u64;
 
@@ -78,20 +78,6 @@ struct xf_pv {
   std::mutex mu;
 };
 
-__device__ __forceinline__ void xf_add128(u64& lo, u64& hi, u64 alo, u64 ahi) {
-  lo += alo;
-  hi += ahi + (lo < alo ? 1ull : 0ull);
-}
-
-// a multi-word atomic add: every word's carry is decided by the old value its own atomic returned, so the words hold
-// the exact sum (mod 2^(64 n)) whatever the order of the adds
-__device__ __forceinline__ void xf_atomic_add128(u64* w, u64 lo, u64 hi) {
-  if (lo) {
-    const u64 old = atomicAdd(w, lo);
-    if (old + lo < old) ++hi;
-  }
-  if (hi) atomicAdd(w + 1, hi);
-}
 __device__ __forceinline__ void xf_atomic_add192(u64* w, u64 a0, u64 a1, u64 a2) {
   if (a0) {
     const u64 old = atomicAdd(w, a0);
@@ -108,8 +94,8 @@ __device__ __forceinline__ double xf_u128_to_double(u64 lo, u64 hi) { return (do
 
 // a row's class and fixed-point terms (section 8): cls 0 / 1 for a scored negative / positive row, else one of the codes
 // below; bin, u (e), t (e * pc) and xl + 2^64 xh (e * l) are set for a scored row only.  The slice kernel's; xf_k_pv_add
-// keeps its own inline copy of the same arithmetic (through this function it compiles to 36 registers instead of 32),
-// and the tests hold the two to equal report bytes.
+// keeps its own inline copy of the classification and binning (through this function it compiles to 36 registers
+// instead of 32), and the tests hold the two to equal report bytes.  Both take e * l from xf_loss_units (metric.cuh).
 enum { XF_PV_SKIP = -1, XF_PV_OVERFLOW = -2, XF_PV_NAN = -3 };
 struct XfPvRow {
   int cls;
@@ -135,15 +121,7 @@ __device__ __forceinline__ XfPvRow xf_pv_row(float e, const float* __restrict__ 
   v.bin = (__float_as_uint(pc) >> (23 - m)) - first_bin;
   v.u = __double2ull_rn((double)e * 4294967296.0);
   v.t = __double2ull_rn((double)e * (double)pc * 4294967296.0);  // e * pc exact, < 2^63 units
-  const double q = fmin(fmax((double)p, 1e-15), 1.0 - 1e-15);
-  const double l = v.cls ? -log(q) : -log(1.0 - q);
-  const double x = (double)e * l * 4294967296.0;  // < 2^69 units
-  if (x < 0x1p64) {
-    v.xl = __double2ull_rn(x);
-  } else {  // an integer: the split is exact
-    v.xh = (u64)(x * 0x1p-64);
-    v.xl = (u64)(x - (double)v.xh * 0x1p64);
-  }
+  xf_loss_units(e, p, v.cls, v.xl, v.xh);
   return v;
 }
 
@@ -176,16 +154,8 @@ xf_k_pv_add(const float* __restrict__ pctr, const uint8_t* __restrict__ labels, 
             const u64 t = __double2ull_rn((double)e * (double)pc * 4294967296.0);  // e * pc exact, < 2^63 units
             ep0 += t;
             ep1 += ep0 < t ? 1ull : 0ull;
-            const double q = fmin(fmax((double)p, 1e-15), 1.0 - 1e-15);
-            const double l = cls ? -log(q) : -log(1.0 - q);
-            const double x = (double)e * l * 4294967296.0;  // < 2^69 units
-            u64 xl, xh = 0;
-            if (x < 0x1p64) {
-              xl = __double2ull_rn(x);
-            } else {  // an integer: the split is exact
-              xh = (u64)(x * 0x1p-64);
-              xl = (u64)(x - (double)xh * 0x1p64);
-            }
+            u64 xl, xh;
+            xf_loss_units(e, p, cls, xl, xh);
             el0 += xl;
             const u64 c = el0 < xl ? 1ull : 0ull;
             el1 += xh + c;
@@ -404,9 +374,7 @@ xf_k_pv_report(const XfPvBin* __restrict__ bins, uint32_t nbins, const XfPvSums*
 
 // ---- exact ratios on the host: num / den correctly rounded to double (round to nearest even), num and den < 2^192
 namespace {
-struct U256 {
-  uint64_t w[4] = {0, 0, 0, 0};
-};
+typedef XfU256 U256;
 int bitlen(const U256& a) {
   for (int k = 3; k >= 0; --k)
     if (a.w[k]) return 64 * k + 64 - __builtin_clzll(a.w[k]);
@@ -440,7 +408,7 @@ U256 u256(const u64* words, int n) {
 }
 }  // namespace
 
-static double xf_ratio(U256 num, U256 den) {
+double xf_ratio(U256 num, U256 den) {
   if (bitlen(den) == 0) return NAN;
   if (bitlen(num) == 0) return 0.0;
   // scale so that the quotient has 55 or 56 bits, then round it to 53 with the remainder as sticky bit
