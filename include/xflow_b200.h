@@ -1134,6 +1134,36 @@ XF_DLL int xf_trainer_set_validation(xf_trainer* tr, xf_pv* pv);
  *    adds, their order, the streams, the grid or the order of atomics.
  *    Memory: 13 bytes per held row; a finish adds 76 bytes of scratch per held row (two 16-byte sort keys, a 12-byte
  *    scan, 32 bytes of per-group sums) and CUB's temporary storage, and keeps them for later calls.
+ *
+ *    Ranking quality at a cutoff k (xf_group_metric_topk): NDCG@k, precision@k and recall@k of every group, over the
+ *    rows of the last finish.  The rows, the sort, NaN handling and the tie rule are the finish's.  Within group g, the
+ *    non-NaN rows are ordered by descending p, and equal floats tie (-0 ties with +0).  Positions are counted from 0.
+ *    Tie run r of g starts at position a_r; has c_r rows, of which m_r are positive (y != 0); and overlaps the top k
+ *    in o_r = min(max(k - a_r, 0), c_r) positions.  n_g is the group's rows, P_g its positives and N_g its negatives.
+ *      Discounts: d(i) = 2^32 / log2(i + 2), rounded to the nearest integer, for i = 0 .. 65535 (the table of
+ *                  xf_group_metric_discounts); D(i) = sum of d(j), j < i.  d(0) = 2^32 and D(65536) < 2^44.2.
+ *                  rn(x) is the exact rational x rounded to the nearest integer, ties to even, computed in 128-bit
+ *                  integers (m_r (D(a) - D(b)) reaches about 2^75).
+ *      Per-group integers, in units of 2^-32:
+ *        H_g = sum over runs of rn(m_r o_r 2^32 / c_r): the hits in the top k (only a run that straddles position k
+ *              rounds);
+ *        G_g = sum over runs of rn(m_r (D(a_r + o_r) - D(a_r)) / c_r): the DCG at k;
+ *        I_g = D(min(P_g, k)): the ideal DCG.
+ *      Per-group doubles, each one division of exactly representable values, all three NaN when P_g = 0:
+ *        ndcg_g      = (double)G_g / (double)I_g;
+ *        precision_g = (double)H_g / ((double)min(k, n_g) * 2^32): a request with fewer than k candidates can reach 1;
+ *        recall_g    = (double)H_g / ((double)P_g * 2^32).
+ *      These are the expectations over a uniformly random order inside each tie run, up to the units' rounding: a
+ *      run's positives are spread evenly over its positions, the top-k counterpart of the AUC's tied pair counting 1/2,
+ *      so a model that outputs many equal scores is not credited with a lucky order.
+ *      Report: the scored groups are the finish's (P_g > 0 and N_g > 0, so the numbers sit beside gauc; an
+ *      all-positive group scores 1 at every k and would inflate the mean).  For X in {ndcg, precision, recall}, built
+ *      as gauc and gauc_mean:
+ *        X      = sum over scored groups of __double2ull_rn(((double)n_g * X_g) * 2^32) / (2^32 scored_rows),
+ *        X_mean = sum over scored groups of __double2ull_rn(X_g * 2^32) / (2^32 scored_groups),
+ *      both correctly rounded, NaN for a zero denominator; every sum stays below 2^63 since rows < 2^31.  The same
+ *      bytes under any permutation, cut or stream of the adds, as the finish's.
+ *    Memory: a topk keeps 24 bytes per group for groups_topk and the metric keeps D (512 KB) once it has run one.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct xf_group_metric xf_group_metric;
 /* the report of xf_group_metric_finish (a struct tag only, like xf_pv_report) */
@@ -1159,6 +1189,25 @@ XF_DLL int xf_group_metric_finish(xf_group_metric* m, struct xf_group_report* ou
  * reset or add. */
 XF_DLL int xf_group_metric_groups(xf_group_metric* m, uint64_t n, uint64_t* ids, uint64_t* rows, uint64_t* positives,
                                   double* auc, double* logloss);
+enum { XF_GROUP_TOPK_MAX_K = 65536 };
+/* the report of xf_group_metric_topk: k, the finish's groups, scored_groups and scored_rows, and the means above */
+struct xf_group_topk_report {
+  uint32_t k;
+  uint64_t groups, scored_groups, scored_rows;
+  double ndcg, ndcg_mean, precision, precision_mean, recall, recall_mean;
+};
+/* evaluates the rows of the last finish at cutoff k, on m's stream; does not change what xf_group_metric_groups
+ * returns.  XF_ERR_STATE if no finish came after the last reset or add; XF_ERR_ARG, naming k, for k = 0 or
+ * k > XF_GROUP_TOPK_MAX_K.  A refused call leaves m unchanged.  An empty finish gives zero counts and NaN ratios. */
+XF_DLL int xf_group_metric_topk(xf_group_metric* m, uint32_t k, struct xf_group_topk_report* out);
+/* the last topk's ndcg_g, precision_g and recall_g in the order of xf_group_metric_groups (ascending id) into host
+ * arrays of n elements, any of them NULL.  XF_ERR_ARG unless n is the last finish's `groups`; XF_ERR_STATE if no topk
+ * came after the last finish, reset or add. */
+XF_DLL int xf_group_metric_groups_topk(xf_group_metric* m, uint64_t n, double* ndcg, double* precision,
+                                       double* recall);
+/* the discounts d(0 .. n-1) of the definition above, n <= XF_GROUP_TOPK_MAX_K (XF_ERR_ARG otherwise, or for d NULL
+ * with n > 0); host only, needs no device */
+XF_DLL int xf_group_metric_discounts(uint64_t* d, uint32_t n);
 
 /* ------------------------------------------------------------------------------------------------
  * 1. Reference C API (src/c_api/c_api.h:26-29), unchanged signatures.

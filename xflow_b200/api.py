@@ -84,6 +84,12 @@ class GroupReport(C.Structure):
                 ("logloss", C.c_double), ("gauc", C.c_double), ("gauc_mean", C.c_double)]
 
 
+class GroupTopkReport(C.Structure):
+    _fields_ = [("k", C.c_uint32), ("groups", C.c_uint64), ("scored_groups", C.c_uint64), ("scored_rows", C.c_uint64),
+                ("ndcg", C.c_double), ("ndcg_mean", C.c_double), ("precision", C.c_double),
+                ("precision_mean", C.c_double), ("recall", C.c_double), ("recall_mean", C.c_double)]
+
+
 # name -> (restype, argtypes); also the list the symbol-export test checks against the header
 _vp, _u64, _u32, _i, _f = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_float
 SIGNATURES = {
@@ -224,6 +230,9 @@ SIGNATURES = {
     "xf_group_metric_add_device": (_i, [_vp, _vp, _vp, _vp, _u64, _vp]),
     "xf_group_metric_finish": (_i, [_vp, _vp]),
     "xf_group_metric_groups": (_i, [_vp, _u64, _vp, _vp, _vp, _vp, _vp]),
+    "xf_group_metric_topk": (_i, [_vp, _u32, _vp]),
+    "xf_group_metric_groups_topk": (_i, [_vp, _u64, _vp, _vp, _vp]),
+    "xf_group_metric_discounts": (_i, [_vp, _u32]),
     "xf_trainer_set_deterministic": (_i, [_vp, _i]),
     "XFCreate": (_i, [_vp, C.c_char_p, C.c_char_p]),
     "XFStartTrain": (_i, [_vp]),
@@ -278,6 +287,14 @@ def hash_decimal_ids(ids):
 
 def shard_of(key, num_shards):
     return lib().xf_shard_of(int(key), int(num_shards))
+
+
+def group_discounts(n=65536):
+    """The grouped metric's top-k discounts d(0 .. n-1) = round(2^32 / log2(i + 2)) (uint64), n <= 65536
+    (xf_group_metric_discounts; header section 9)."""
+    out = np.empty(int(n), np.uint64)
+    _check(lib().xf_group_metric_discounts(_p(out), int(n)))
+    return out
 
 
 def auc_logloss(labels, pctr):
@@ -925,6 +942,27 @@ class GroupMetric:
                    auc=np.empty(n, np.float64), logloss=np.empty(n, np.float64))
         _check(lib().xf_group_metric_groups(self.h, n, _p(out["ids"]), _p(out["rows"]), _p(out["positives"]),
                                             _p(out["auc"]), _p(out["logloss"])))
+        return out
+
+    def topk_bytes(self, k):
+        """The raw struct xf_group_topk_report of topk(k), for byte comparisons."""
+        r = GroupTopkReport()
+        _check(lib().xf_group_metric_topk(self.h, int(k), C.byref(r)))
+        return bytes(r)
+
+    def topk(self, k):
+        """Ranking quality at cutoff k of the last finish's rows (xf_group_metric_topk): k, groups, scored_groups,
+        scored_rows and ndcg, precision, recall with their unweighted _mean, over the groups finish scores."""
+        r = GroupTopkReport.from_buffer_copy(self.topk_bytes(k))
+        return {name: getattr(r, name) for name, _ in GroupTopkReport._fields_}
+
+    def groups_topk(self, n=None):
+        """The last topk's per-group ndcg, precision and recall (numpy float64, NaN for a group without positives), in
+        the order of groups().  n defaults to the last finish's group count."""
+        n = self.last_groups if n is None else int(n)
+        out = dict(ndcg=np.empty(n, np.float64), precision=np.empty(n, np.float64), recall=np.empty(n, np.float64))
+        _check(lib().xf_group_metric_groups_topk(self.h, n, _p(out["ndcg"]), _p(out["precision"]),
+                                                 _p(out["recall"])))
         return out
 
     def reset(self):

@@ -11,7 +11,10 @@
 //                             units L_i, and the last row of a tie run adds gn (2 pb + gp) to U2
 //            xf_k_gm_groups   per group auc_g, logloss_g, T_g and M_g; the global integer sums by block reduction and
 //                             integer atomics
-//   The host only copies and turns the global sums into three correctly rounded ratios (xf_ratio).  Every
+//   topk     DeviceReduce::ReduceByKey  per group {H, G} over the finish's sorted rows and scan: the last row of a tie
+//                             run adds its overlap with the top k (xf_gm_run_end, as the U2 term)
+//            xf_k_gm_topk     per group ndcg_g, precision_g and recall_g, and the global sums as xf_k_gm_groups
+//   The host only copies and turns the global sums into correctly rounded ratios (xf_ratio).  Every
 // accumulator is an integer and every double a fixed function of integers, so the report and the per-group arrays
 // depend only on the multiset of rows: not on add cuts, streams, grid or atomic order.
 #include <cuda_runtime.h>
@@ -24,6 +27,7 @@
 #include <mutex>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
+#include <vector>
 
 #include "metric.cuh"
 
@@ -101,19 +105,73 @@ struct XfGmGroupOf {
   const XfGmKey* k;
   __host__ __device__ uint64_t operator()(uint32_t i) const { return k[i].g; }
 };
+
+// the tie run [start, i] that sorted row i ends, from the scan: its position in its group, its group's positives
+// before it (pb), its positives (gp) and rows
+struct XfGmRun {
+  u64 at, pb, gp, rows;
+};
+// false when row i is not the last row of its tie run (of n sorted rows)
+__device__ __forceinline__ bool xf_gm_run_end(const XfGmScan* s, uint32_t n, uint32_t i, XfGmRun& r) {
+  if (i + 1 != n && s[i + 1].run != i + 1) return false;
+  const XfGmScan h = s[i];
+  const u64 before_run = h.run ? s[h.run - 1].pos : 0u, before_grp = h.grp ? s[h.grp - 1].pos : 0u;
+  r.at = h.run - h.grp;
+  r.pb = before_run - before_grp;
+  r.gp = h.pos - before_run;
+  r.rows = i - h.run + 1;
+  return true;
+}
+
 struct XfGmRowTerms {
   const XfGmKey* k;
   const XfGmScan* s;
   uint32_t n;
   __device__ XfGmAgg operator()(uint32_t i) const {
     const XfGmKey c = k[i];
-    const XfGmScan h = s[i];
     XfGmAgg a{1ull | (u64)c.y << 32, 0ull, 0ull, 0ull};
     xf_loss_units(1.f, -c.negp, (int)c.y, a.s_lo, a.s_hi);
-    if (i + 1 == n || s[i + 1].run == i + 1) {  // the last row of its tie run [h.run, i]
-      const u64 before_run = h.run ? s[h.run - 1].pos : 0u, before_grp = h.grp ? s[h.grp - 1].pos : 0u;
-      const u64 pb = before_run - before_grp, gp = h.pos - before_run, gn = (i - h.run + 1) - gp;
-      a.u2 = gn * (2 * pb + gp);
+    XfGmRun r;
+    if (xf_gm_run_end(s, n, i, r)) a.u2 = (r.rows - r.gp) * (2 * r.pb + r.gp);
+    return a;
+  }
+};
+
+// ---- top k (xf_group_metric_topk): a group's integers H and G in units of 2^-32, summed over its tie runs
+struct XfGmTopkSums {
+  u64 h, g, zero;  // the third word keeps a group's sums in the place of its XfGmTopkOut
+};
+struct XfGmTopkSumOp {
+  __host__ __device__ XfGmTopkSums operator()(const XfGmTopkSums& a, const XfGmTopkSums& b) const {
+    return XfGmTopkSums{a.h + b.h, a.g + b.g, 0ull};
+  }
+};
+// the group's top-k results, written over its XfGmTopkSums by xf_k_gm_topk
+struct XfGmTopkOut {
+  double ndcg, precision, recall;
+};
+static_assert(sizeof(XfGmTopkSums) == sizeof(XfGmTopkOut), "a group's results take its sums' place");
+
+// x / c rounded to the nearest integer, ties to even; the quotient fits 64 bits
+__device__ __forceinline__ u64 xf_div_rn(unsigned __int128 x, u64 c) {
+  if (c == 1) return (u64)x;
+  const u64 q = (u64)(x / c), r = (u64)(x - (unsigned __int128)q * c);
+  return q + ((2 * r > c || (2 * r == c && (q & 1))) ? 1ull : 0ull);
+}
+
+// a tie run's terms at its last row: its m positives spread evenly over its c rows, o of which lie in the top k,
+// give rn(m o 2^32 / c) hits and rn(m (D(a + o) - D(a)) / c) DCG (D: the cumulative discounts, k <= 65536 entries)
+struct XfGmTopkTerms {
+  const XfGmScan* s;
+  const u64* D;
+  uint32_t n, k;
+  __device__ XfGmTopkSums operator()(uint32_t i) const {
+    XfGmTopkSums a{0ull, 0ull, 0ull};
+    XfGmRun r;
+    if (xf_gm_run_end(s, n, i, r) && r.gp && r.at < k) {
+      const u64 o = min((u64)k - r.at, r.rows);
+      a.h = xf_div_rn((unsigned __int128)(r.gp * o) << 32, r.rows);
+      a.g = xf_div_rn((unsigned __int128)r.gp * (D[r.at + o] - D[r.at]), r.rows);
     }
     return a;
   }
@@ -176,6 +234,77 @@ xf_k_gm_groups(XfGmAgg* __restrict__ groups, const uint32_t* __restrict__ n_grou
   }
 }
 
+// the top k's global sums (words of struct XfGmTopkTotals on the device): t and m of ndcg, precision and recall
+struct XfGmTopkTotals {
+  u64 groups, scored_groups, scored_rows, t[3], m[3];
+};
+constexpr int XF_GM_TOPK_WORDS = 9;
+static_assert(sizeof(XfGmTopkTotals) == 8 * XF_GM_TOPK_WORDS, "the top k's global sums are words");
+struct XfGmTopkTotalOp {
+  __device__ XfGmTopkTotals operator()(const XfGmTopkTotals& a, const XfGmTopkTotals& b) const {
+    XfGmTopkTotals r;
+    r.groups = a.groups + b.groups;
+    r.scored_groups = a.scored_groups + b.scored_groups;
+    r.scored_rows = a.scored_rows + b.scored_rows;
+    for (int x = 0; x < 3; ++x) {
+      r.t[x] = a.t[x] + b.t[x];
+      r.m[x] = a.m[x] + b.m[x];
+    }
+    return r;
+  }
+};
+
+// per group ndcg_g, precision_g and recall_g over its {H, G} (in place), from its rows and positives in the finish's
+// per-group results; the global integer sums by block reduction and integer atomics
+__global__ void __launch_bounds__(XF_GM_THREADS)
+xf_k_gm_topk(XfGmTopkSums* __restrict__ topk, const XfGmOut* __restrict__ groups, uint32_t G,
+             const u64* __restrict__ D, uint32_t k, u64* __restrict__ sums) {
+  XfGmTopkTotals acc{0, 0, 0, {0, 0, 0}, {0, 0, 0}};
+  for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < G; g += gridDim.x * blockDim.x) {
+    const XfGmTopkSums a = topk[g];
+    const u64 n = groups[g].rows, P = groups[g].positives, N = n - P;
+    XfGmTopkOut o;
+    o.ndcg = P ? (double)a.g / (double)D[P < k ? P : k] : NAN;
+    o.precision = P ? (double)a.h / ((double)(n < k ? n : k) * 4294967296.0) : NAN;
+    o.recall = P ? (double)a.h / ((double)P * 4294967296.0) : NAN;
+    reinterpret_cast<XfGmTopkOut*>(topk)[g] = o;
+    ++acc.groups;
+    if (P && N) {
+      ++acc.scored_groups;
+      acc.scored_rows += n;
+      const double x[3] = {o.ndcg, o.precision, o.recall};
+      for (int j = 0; j < 3; ++j) {
+        acc.t[j] += __double2ull_rn(((double)n * x[j]) * 4294967296.0);
+        acc.m[j] += __double2ull_rn(x[j] * 4294967296.0);
+      }
+    }
+  }
+  typedef cub::BlockReduce<XfGmTopkTotals, XF_GM_THREADS> R;
+  __shared__ typename R::TempStorage tmp;
+  const XfGmTopkTotals b = R(tmp).Reduce(acc, XfGmTopkTotalOp());
+  if (threadIdx.x == 0) {
+    const u64* w = reinterpret_cast<const u64*>(&b);
+    for (int j = 0; j < XF_GM_TOPK_WORDS; ++j)
+      if (w[j]) atomicAdd(sums + j, w[j]);
+  }
+}
+
+// d(i) = 2^32 / log2(i + 2) rounded to the nearest integer, and D(i) = sum of d(j), j < i: the header's table
+// (section 9), built once from long double log2l (64-bit mantissa)
+constexpr uint32_t XF_GM_TOPK_MAX_K = XF_GROUP_TOPK_MAX_K;
+const std::vector<u64>& xf_gm_discounts() {
+  static std::mutex mu;
+  static std::vector<u64> D;
+  std::lock_guard<std::mutex> lk(mu);
+  if (D.empty()) {
+    std::vector<u64> t(XF_GM_TOPK_MAX_K + 1, 0ull);
+    for (uint32_t i = 0; i < XF_GM_TOPK_MAX_K; ++i)
+      t[i + 1] = t[i] + (u64)llroundl(4294967296.0L / log2l((long double)i + 2.0L));
+    D.swap(t);
+  }
+  return D;
+}
+
 }  // namespace
 
 struct xf_group_metric {
@@ -187,10 +316,14 @@ struct xf_group_metric {
   // finish's scratch, kept for later calls: the sort's two key buffers (the group ids of the last finish end up in
   // the one the sort leaves free), the scan, the per-group sums and results, CUB's storage and the global sums
   XfDevBuf keys_a, keys_b, scan, agg, tmp, acc;
+  XfDevBuf topk, disc;              // the last topk's per-group results; the cumulative discounts D (uploaded once)
   const uint64_t* d_ids = nullptr;  // the last finish's group ids, in keys_a or keys_b
+  const XfGmKey* d_sorted = nullptr;  // the last finish's sorted rows, in the other one
   uint64_t n = 0;
   uint64_t groups = 0;              // of the last finish
+  uint32_t scored = 0;              // the last finish's sorted rows (its non-NaN rows)
   bool finished = false;            // a finish with no reset or add after it
+  bool topk_done = false;           // a topk with no finish, reset or add after it
   std::mutex mu;
 };
 
@@ -217,7 +350,8 @@ XF_DLL int xf_group_metric_destroy(xf_group_metric* m) {
   if (!m) return XF_OK;
   cudaSetDevice(m->device);
   if (m->stream) cudaStreamSynchronize(m->stream);
-  XfDevBuf* bufs[] = {&m->pctr, &m->lab, &m->grp, &m->keys_a, &m->keys_b, &m->scan, &m->agg, &m->tmp, &m->acc};
+  XfDevBuf* bufs[] = {&m->pctr, &m->lab, &m->grp, &m->keys_a, &m->keys_b, &m->scan, &m->agg, &m->tmp, &m->acc,
+                      &m->topk, &m->disc};
   for (XfDevBuf* b : bufs) b->release();
   if (m->added) cudaEventDestroy(m->added);
   if (m->cleared) cudaEventDestroy(m->cleared);
@@ -233,7 +367,7 @@ XF_DLL int xf_group_metric_reset(xf_group_metric* m) {
   // `stream` waits for every add so far; later adds wait for this
   XF_CUDA_TRY(cudaEventRecord(m->cleared, m->stream));
   m->n = 0;
-  m->finished = false;
+  m->finished = m->topk_done = false;
   return XF_OK;
 }
 
@@ -269,7 +403,7 @@ XF_DLL int xf_group_metric_add_device(xf_group_metric* m, const float* d_pctr, c
   XF_CUDA_TRY(cudaEventRecord(m->added, st));
   XF_CUDA_TRY(cudaStreamWaitEvent(m->stream, m->added, 0));
   m->n = total;
-  m->finished = false;
+  m->finished = m->topk_done = false;
   return XF_OK;
 }
 
@@ -279,7 +413,7 @@ XF_DLL int xf_group_metric_finish(xf_group_metric* m, struct xf_group_report* ou
   XF_CUDA_TRY(cudaSetDevice(m->device));
   cudaStream_t st = m->stream;
   const uint64_t n = m->n;
-  m->finished = false;
+  m->finished = m->topk_done = false;
   memset(out, 0, sizeof(*out));
   out->logloss = out->gauc = out->gauc_mean = NAN;
   // {XfGmSums, rows selected, groups}
@@ -340,6 +474,7 @@ XF_DLL int xf_group_metric_finish(xf_group_metric* m, struct xf_group_report* ou
     XF_CUDA_TRY(cudaMemcpyAsync(&h, m->acc.p, sizeof(XfGmSums), cudaMemcpyDeviceToHost, st));
     XF_CUDA_TRY(cudaStreamSynchronize(st));
     m->d_ids = ids;
+    m->d_sorted = sorted;
   }
   out->rows = h.rows;
   out->positives = h.positives;
@@ -360,6 +495,7 @@ XF_DLL int xf_group_metric_finish(xf_group_metric* m, struct xf_group_report* ou
   out->gauc = xf_ratio(t, srows);
   out->gauc_mean = xf_ratio(mm, sgroups);
   m->groups = h.groups;
+  m->scored = scored;
   m->finished = true;
   return XF_OK;
 }
@@ -387,5 +523,112 @@ XF_DLL int xf_group_metric_groups(xf_group_metric* m, uint64_t n, uint64_t* ids,
     if (dst[f])
       XF_CUDA_TRY(cudaMemcpy2DAsync(dst[f], 8, base + 8 * f, sizeof(XfGmOut), 8, n, cudaMemcpyDeviceToHost, st));
   XF_CUDA_TRY(cudaStreamSynchronize(st));
+  return XF_OK;
+}
+
+XF_DLL int xf_group_metric_topk(xf_group_metric* m, uint32_t k, struct xf_group_topk_report* out) {
+  if (!m || !out) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(m->mu);
+  if (!m->finished) {
+    xf_set_error("xf_group_metric_topk: no finish since the last reset or add (the top k ranks the rows of a finish)");
+    return XF_ERR_STATE;
+  }
+  if (k == 0 || k > XF_GM_TOPK_MAX_K) {
+    xf_set_error("xf_group_metric_topk: k = %u, outside 1 .. %u", k, XF_GM_TOPK_MAX_K);
+    return XF_ERR_ARG;
+  }
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  cudaStream_t st = m->stream;
+  const uint64_t G = m->groups;
+  m->topk_done = false;
+  memset(out, 0, sizeof(*out));
+  out->ndcg = out->ndcg_mean = out->precision = out->precision_mean = out->recall = out->recall_mean = NAN;
+  XfGmTopkTotals h{0, 0, 0, {0, 0, 0}, {0, 0, 0}};
+  if (G) {
+    if (!m->disc.p) {
+      const std::vector<u64>& D = xf_gm_discounts();
+      XF_TRY(m->disc.ensure(D.size() * 8));
+      XF_CUDA_TRY(cudaMemcpyAsync(m->disc.p, D.data(), D.size() * 8, cudaMemcpyHostToDevice, st));
+    }
+    XF_TRY(m->topk.ensure(G * sizeof(XfGmTopkSums)));
+    // {XfGmTopkTotals, groups found}: the finish's global sums, read already, leave room for these
+    XF_TRY(m->acc.ensure(sizeof(XfGmTopkTotals) + 4));
+    uint32_t* d_runs = reinterpret_cast<uint32_t*>(m->acc.as<char>() + sizeof(XfGmTopkTotals));
+    XfGmTopkSums* sums = m->topk.as<XfGmTopkSums>();
+    const u64* D = m->disc.as<u64>();
+    const int nv = (int)m->scored;
+    // the unique ids go to the free half of the ids' buffer: 16 bytes per sorted row hold 8 per group twice
+    uint64_t* ids_again = const_cast<uint64_t*>(m->d_ids) + G;
+    const auto ids_in = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0), XfGmGroupOf{m->d_sorted});
+    const auto terms = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0),
+                                                       XfGmTopkTerms{m->scan.as<XfGmScan>(), D, (uint32_t)nv, k});
+    size_t need = 0;
+    XF_CUDA_TRY(cub::DeviceReduce::ReduceByKey(nullptr, need, ids_in, ids_again, terms, sums, d_runs, XfGmTopkSumOp(),
+                                               nv, st));
+    XF_TRY(m->tmp.ensure(need));
+    size_t tb = m->tmp.cap;
+    XF_CUDA_TRY(cub::DeviceReduce::ReduceByKey(m->tmp.p, tb, ids_in, ids_again, terms, sums, d_runs, XfGmTopkSumOp(),
+                                               nv, st));
+    XF_CUDA_TRY(cudaMemsetAsync(m->acc.p, 0, sizeof(XfGmTopkTotals), st));
+    xf_k_gm_topk<<<xf_grid_for(G, XF_GM_THREADS, 4), XF_GM_THREADS, 0, st>>>(sums, m->agg.as<XfGmOut>(), (uint32_t)G,
+                                                                           D, k, m->acc.as<u64>());
+    XF_CUDA_TRY(cudaGetLastError());
+    XF_CUDA_TRY(cudaMemcpyAsync(&h, m->acc.p, sizeof(XfGmTopkTotals), cudaMemcpyDeviceToHost, st));
+    XF_CUDA_TRY(cudaStreamSynchronize(st));
+  }
+  out->k = k;
+  out->groups = h.groups;
+  out->scored_groups = h.scored_groups;
+  out->scored_rows = h.scored_rows;
+  XfU256 srows, sgroups;  // units of 2^-32; every count is below 2^31
+  srows.w[0] = h.scored_rows << 32;
+  sgroups.w[0] = h.scored_groups << 32;
+  double* ratios[3][2] = {{&out->ndcg, &out->ndcg_mean}, {&out->precision, &out->precision_mean},
+                          {&out->recall, &out->recall_mean}};
+  for (int x = 0; x < 3; ++x) {
+    XfU256 t, mm;
+    t.w[0] = h.t[x];
+    mm.w[0] = h.m[x];
+    *ratios[x][0] = xf_ratio(t, srows);
+    *ratios[x][1] = xf_ratio(mm, sgroups);
+  }
+  m->topk_done = true;
+  return XF_OK;
+}
+
+XF_DLL int xf_group_metric_groups_topk(xf_group_metric* m, uint64_t n, double* ndcg, double* precision,
+                                       double* recall) {
+  if (!m) return XF_ERR_ARG;
+  std::lock_guard<std::mutex> lk(m->mu);
+  if (!m->topk_done) {
+    xf_set_error("xf_group_metric_groups_topk: no topk since the last finish, reset or add (the values are those of "
+                 "a topk)");
+    return XF_ERR_STATE;
+  }
+  if (n != m->groups) {
+    xf_set_error("xf_group_metric_groups_topk: n = %llu, but the last finish found %llu groups", (unsigned long long)n,
+                 (unsigned long long)m->groups);
+    return XF_ERR_ARG;
+  }
+  if (n == 0) return XF_OK;
+  XF_CUDA_TRY(cudaSetDevice(m->device));
+  cudaStream_t st = m->stream;
+  const char* base = m->topk.as<char>();
+  double* dst[3] = {ndcg, precision, recall};
+  for (int f = 0; f < 3; ++f)  // field f of every XfGmTopkOut
+    if (dst[f])
+      XF_CUDA_TRY(cudaMemcpy2DAsync(dst[f], 8, base + 8 * f, sizeof(XfGmTopkOut), 8, n, cudaMemcpyDeviceToHost, st));
+  XF_CUDA_TRY(cudaStreamSynchronize(st));
+  return XF_OK;
+}
+
+XF_DLL int xf_group_metric_discounts(uint64_t* d, uint32_t n) {
+  if (n > XF_GM_TOPK_MAX_K || (n && !d)) {
+    xf_set_error("xf_group_metric_discounts: n = %u with d %s (n <= %u and d set when n > 0)", n, d ? "set" : "NULL",
+                 XF_GM_TOPK_MAX_K);
+    return XF_ERR_ARG;
+  }
+  const std::vector<u64>& D = xf_gm_discounts();
+  for (uint32_t i = 0; i < n; ++i) d[i] = D[i + 1] - D[i];
   return XF_OK;
 }
