@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libxflow_b200.so")
 
 MODEL_LR, MODEL_FM, MODEL_FM_CANONICAL, MODEL_MVM, MODEL_FFM = 0, 1, 2, 3, 4
-OPT_FTRL, OPT_SGD = 0, 1
+OPT_FTRL, OPT_SGD, OPT_ADAGRAD = 0, 1, 2
 VINIT_DEFAULT, VINIT_COUNTER, VINIT_ZERO = 0, 1, 3
 ADMIT_ALL, ADMIT_POISSON, ADMIT_BLOOM = 0, 1, 2
 ABSENT_DEFAULT, ABSENT_ZERO = 0, 1

@@ -259,9 +259,21 @@ int xf_table::ensure_room(uint64_t incoming) {
 XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   if (!out || !cfg) { xf_set_error("null argument"); return XF_ERR_ARG; }
   if (cfg->latent_dim < 0 || cfg->latent_dim > 1024 || cfg->num_shards < 1 || cfg->shard_index < 0 ||
-      cfg->shard_index >= cfg->num_shards || (cfg->optimizer != XF_OPTIMIZER_FTRL && cfg->optimizer != XF_OPTIMIZER_SGD)) {
+      cfg->shard_index >= cfg->num_shards ||
+      (cfg->optimizer != XF_OPTIMIZER_FTRL && cfg->optimizer != XF_OPTIMIZER_SGD && cfg->optimizer != XF_OPTIMIZER_ADAGRAD)) {
     xf_set_error("bad table config");
     return XF_ERR_ARG;
+  }
+  if (cfg->optimizer == XF_OPTIMIZER_ADAGRAD) {
+    // beta is the accumulator's start: sqrt(beta + n) must be a positive finite divisor from the first step on
+    if (!(isfinite(cfg->beta) && cfg->beta > 0.0f)) {
+      xf_set_error("AdaGrad needs beta finite and above 0 (got %g)", (double)cfg->beta);
+      return XF_ERR_ARG;
+    }
+    if (!isfinite(cfg->learning_rate)) {
+      xf_set_error("AdaGrad needs a finite learning_rate (got %g)", (double)cfg->learning_rate);
+      return XF_ERR_ARG;
+    }
   }
   if (cfg->canonical_fm) {
     const int K = cfg->latent_dim;
@@ -286,14 +298,14 @@ XF_DLL int xf_table_create(xf_table** out, const xf_table_config* cfg) {
   XF_CUDA_TRY(cudaMemsetAsync(t->d_error, 0, sizeof(int), t->stream));
   XfTableView& v = t->view;
   v.K = cfg->latent_dim;
-  v.opt = cfg->optimizer == XF_OPTIMIZER_FTRL ? XF_OPT_FTRL : XF_OPT_SGD;
+  v.opt = cfg->optimizer == XF_OPTIMIZER_FTRL ? XF_OPT_FTRL : (cfg->optimizer == XF_OPTIMIZER_ADAGRAD ? XF_OPT_ADAGRAD : XF_OPT_SGD);
   v.alpha = cfg->alpha; v.beta = cfg->beta; v.lambda1 = cfg->lambda1; v.lambda2 = cfg->lambda2;
   v.learning_rate = cfg->learning_rate;
   v.seed = cfg->seed;
   v.v_const = 0.001f;  // sgd.h:68-70
   if (cfg->v_init == XF_VINIT_ZERO) v.v_init = XF_INIT_ZERO;
   else if (cfg->v_init == XF_VINIT_COUNTER) v.v_init = XF_INIT_COUNTER;
-  else v.v_init = (v.opt == XF_OPT_FTRL) ? XF_INIT_COUNTER : XF_INIT_DEFAULT;
+  else v.v_init = (v.opt == XF_OPT_SGD) ? XF_INIT_DEFAULT : XF_INIT_COUNTER;  // SGD: the constant of sgd.h:68-70
   v.size = t->d_size;
   v.error = t->d_error;
   v.canon = cfg->canonical_fm ? 1 : 0;
@@ -668,6 +680,7 @@ XF_DLL int xf_table_list_keys(xf_table* t, uint64_t* keys_out, uint64_t max_keys
 }
 
 // checkpoint file: "XFTB" u64 n, u32 K, u32 has_nz, keys[n], w[n], (nw,zw), v[n*K], (nv,zv), present[n]
+// (has_nz: FTRL and AdaGrad; an AdaGrad table writes its zw and zv as zeros)
 XF_DLL int xf_table_save(xf_table* t, const char* path) {
   if (!t || !path) return XF_ERR_ARG;
   uint64_t n = 0;
@@ -678,7 +691,7 @@ XF_DLL int xf_table_save(xf_table* t, const char* path) {
   n = std::min(n, got);
   std::sort(keys.begin(), keys.begin() + n);
   const size_t K = (size_t)t->view.K;
-  const uint32_t has_nz = t->view.opt == XF_OPT_FTRL ? 1 : 0;
+  const uint32_t has_nz = t->view.opt != XF_OPT_SGD ? 1 : 0;
   std::vector<float> w(n), nw(n), zw(n), v(n * K), nv(n * K), zv(n * K);
   std::vector<uint8_t> present(n);
   XF_TRY(xf_table_export(t, keys.data(), n, w.data(), nw.data(), zw.data(), K ? v.data() : nullptr,

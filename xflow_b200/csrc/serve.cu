@@ -1877,7 +1877,7 @@ bool xf_compat_sane(const XfCompat& c, uint32_t row_bytes) {
   }
   if (row_bytes != xf_model_row_bytes(c.fm, c.latent_dim, c.precision)) return false;
   if (c.absent != XF_ABSENT_DEFAULT && c.absent != XF_ABSENT_ZERO) return false;
-  if (c.optimizer != XF_OPT_FTRL && c.optimizer != XF_OPT_SGD) return false;
+  if (c.optimizer != XF_OPT_FTRL && c.optimizer != XF_OPT_SGD && c.optimizer != XF_OPT_ADAGRAD) return false;
   return c.v_init == 0 || c.v_init == XF_INIT_COUNTER || c.v_init == XF_INIT_ZERO;
 }
 

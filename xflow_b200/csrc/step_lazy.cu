@@ -107,7 +107,8 @@ __device__ __forceinline__ void xf_group_sync(int grp, int n) {
 // WEIGHT = true (importance weighting, weight.cu; training only): a row with wv.e[row] = 0 is skipped before phase A
 // (no probe, no insert, no admission, no stamp, no deposit; loss_out 0); every other row deposits the weighted
 // residual e x (pctr - label), and the fixed-point unit comes from the device bound *wv.W instead of fix_shift.
-template <bool ADMIT, bool STAMP, bool WEIGHT>
+// ADAGRAD = true for AdaGrad tables, false for FTRL and SGD ones (xf_lazy_fold_t).
+template <bool ADMIT, bool STAMP, bool WEIGHT, bool ADAGRAD>
 __global__ void __launch_bounds__(256, 4)
 xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uint64_t* __restrict__ keys,
                   const uint8_t* __restrict__ labels, int B, int mode, uint32_t seq, uint64_t* rows_by_seq, int fix_shift,
@@ -178,7 +179,7 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
       // the weight this batch pulls = the row with its pending step applied (computed, not stored)
       uint64_t a2n = a2;
       float w = 0.f;
-      if (s != XF_NO_SLOT) w = xf_lazy_fold(t, a1, a2, a3, mode == 1 ? 0xFFFFFFFFu : seq, a2n);
+      if (s != XF_NO_SLOT) w = xf_lazy_fold_t<ADAGRAD>(t, a1, a2, a3, mode == 1 ? 0xFFFFFFFFu : seq, a2n);
       s_w[threadIdx.x] = w;
       if (mode == 0) {
         // lanes with the same slot elect their lowest lane; invalid lanes get unique dummy values
@@ -260,11 +261,11 @@ xf_k_step_lr_lazy(XfTableView t, const uint32_t* __restrict__ row_ptr, const uin
 }
 
 // CTAs of the kernel that fit on one SM at once
-template <bool A, bool S, bool W>
+template <bool A, bool S, bool W, bool G>
 static int xf_lazy_ctas_per_sm() {
   static const int n = [] {
     int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, xf_k_step_lr_lazy<A, S, W>, 256, 0) != cudaSuccess || v < 1) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, xf_k_step_lr_lazy<A, S, W, G>, 256, 0) != cudaSuccess || v < 1) {
       cudaGetLastError();
       v = 1;
     }
@@ -287,13 +288,19 @@ void xf_launch_step_lr_lazy(const XfTableView& t, const uint32_t* row_ptr, const
   const int gshift = nnz <= 64ull * (uint64_t)B ? 6 : 7;
 #define XF_LAZY_ARGS t, row_ptr, keys, labels, B, mode, seq, rows_by_seq, fs, gshift, loss_out, pctr_out, abs_loss_sum, unique_total, a, sv, wv
   // a grid of the CTAs that fit on the GPU at once (or fewer, for a small batch): each group strides over the rows
-#define XF_LAZY_LAUNCH(A, S, W)                                                                                        \
-  xf_k_step_lr_lazy<A, S, W><<<xf_grid_for((uint64_t)B << gshift, 256, xf_lazy_ctas_per_sm<A, S, W>()), 256, 0, st>>>( \
-      XF_LAZY_ARGS)
-#define XF_LAZY_LAUNCH_W(A, S)            \
-  do {                                    \
-    if (wv.e) XF_LAZY_LAUNCH(A, S, true); \
-    else XF_LAZY_LAUNCH(A, S, false);     \
+#define XF_LAZY_LAUNCH(A, S, W, G)                                                                                   \
+  xf_k_step_lr_lazy<A, S, W, G>                                                                                       \
+      <<<xf_grid_for((uint64_t)B << gshift, 256, xf_lazy_ctas_per_sm<A, S, W, G>()), 256, 0, st>>>(XF_LAZY_ARGS)
+  // AdaGrad tables run instances of their own (xf_lazy_fold_t)
+#define XF_LAZY_LAUNCH_W(A, S)                        \
+  do {                                                \
+    if (t.opt == XF_OPT_ADAGRAD) {                    \
+      if (wv.e) XF_LAZY_LAUNCH(A, S, true, true);     \
+      else XF_LAZY_LAUNCH(A, S, false, true);         \
+    } else {                                          \
+      if (wv.e) XF_LAZY_LAUNCH(A, S, true, false);    \
+      else XF_LAZY_LAUNCH(A, S, false, false);        \
+    }                                                 \
   } while (0)
   const bool stamp = sv.stamp != nullptr;
   if (adm && stamp) XF_LAZY_LAUNCH_W(true, true);

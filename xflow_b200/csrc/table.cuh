@@ -13,8 +13,8 @@
 //                                more accurate than the reference's own sequential float sum).
 //                                (LAZY tables keep their sum elsewhere, see below)
 //   byte 16  f32  w              app-0 weight                         (FTRLEntry_w::w / SGDEntry_w::w)
-//   byte 20  f32  n              FTRL accumulator of w (unused by SGD)
-//   byte 24  f32  z              FTRL accumulator of w (unused by SGD)
+//   byte 20  f32  n              FTRL / AdaGrad accumulator of w (unused by SGD)
+//   byte 24  f32  z              FTRL accumulator of w (unused by SGD; 0 under AdaGrad)
 //   byte 28  u32  flags          bit0 = latent block materialised (V_READY)
 //   LAZY tables (LR, K == 0, "update on next touch", step_lazy.cu) use bytes 16..31 differently, so that ONE
 //   128-bit compare-and-swap on that aligned word can fold a pending optimizer step in, stamp the row for the
@@ -22,6 +22,7 @@
 //     byte 16  f32 n, byte 20 f32 z   (FTRL; the weight is not stored: w = f(z, n), the closed form the
 //                                      reference's handle evaluates after every push, ftrl.h:66-74)
 //              f32 w, byte 20 unused  (SGD)
+//              f32 w, byte 20 f32 n   (AdaGrad)
 //     byte  8  f32 w_given, u32 check   a weight set from outside (xf_table_import) that is NOT f(z, n): it stands
 //                                      for w until the first optimizer step after the import is folded in
 //                                      (check = a digest of bytes 16..23, re-marked by the batch that first opens
@@ -42,9 +43,9 @@
 //                                  L_i = sum_occ loss_s and Aq_i = sum_occ loss_s * S_s: two f64
 //                                  accumulators per key instead of K float ones (3 atomics per token
 //                                  instead of 1 + K/4 vector ones, and no second read of v).
-//   byte A + 16        f32 nv[K]   (FTRL only)
+//   byte A + 16        f32 nv[K]   (FTRL and AdaGrad)
 //   byte A + 16 + 4K   f32 zv[K]   (FTRL only)
-//   row stride = round_up(A + 16 + (FTRL ? 8K : 0), 32): K = 16 FTRL -> 256 B.
+//   row stride = round_up(A + 16 + (FTRL ? 8K : AdaGrad ? 4K : 0), 32): K = 16 FTRL -> 256 B, AdaGrad -> 192 B.
 //
 // Missing keys are inserted on first touch by a pull OR a push, like `store[key]`
 // (ftrl.h:56,114-120 ; sgd.h:48,92).  Default contents: w = n = z = 0 ; v per init mode.  The latent
@@ -61,7 +62,7 @@
 #define XF_NEG_ZERO_BITS64 0x8000000000000000ull
 #define XF_MAX_PROBE 8192
 
-enum { XF_OPT_FTRL = 0, XF_OPT_SGD = 1 };
+enum { XF_OPT_FTRL = 0, XF_OPT_SGD = 1, XF_OPT_ADAGRAD = 2 };  // = XF_OPTIMIZER_*
 enum { XF_INIT_DEFAULT = 0, XF_INIT_COUNTER = 1, XF_INIT_ZERO = 3 };
 
 struct XfTableView {
@@ -149,8 +150,10 @@ __host__ __device__ inline int xf_fix_shift(uint64_t nnz) {
 }
 
 __host__ __device__ inline uint32_t xf_acc_off(int K) { return (32u + 4u * (uint32_t)K + 15u) & ~15u; }
+// floats of optimizer state per latent coordinate behind the accumulators: nv, zv (FTRL), nv (AdaGrad), none (SGD)
+__host__ __device__ inline uint32_t xf_latent_state(int opt) { return opt == XF_OPT_FTRL ? 2u : (opt == XF_OPT_ADAGRAD ? 1u : 0u); }
 __host__ __device__ inline uint32_t xf_ca_off(int K, int opt) {  // canonical FM: the A[K] accumulators
-  return xf_acc_off(K) + 16u + ((opt == XF_OPT_FTRL) ? 8u * (uint32_t)K : 0u);
+  return xf_acc_off(K) + 16u + 4u * xf_latent_state(opt) * (uint32_t)K;
 }
 __host__ __device__ inline uint32_t xf_row_stride(int K, int opt, int canon = 0) {
   if (K <= 0) return 32u;
@@ -499,8 +502,16 @@ __device__ __forceinline__ void xf_sgd_coord(const XfTableView& t, float g, floa
   w = __fsub_rn(w, __fmul_rn(t.learning_rate, g));
 }
 
+// AdaGrad coordinate update (include/xflow_b200.h, section 2): eta = learning_rate, beta = the accumulator's start
+//   n' = n + g*g,  w' = w - eta*g / sqrt(beta + n'),  every operation rounded to nearest on its own (no FMA)
+__device__ __forceinline__ void xf_adagrad_coord(const XfTableView& t, float g, float& w, float& n) {
+  n = __fadd_rn(n, __fmul_rn(g, g));
+  w = __fsub_rn(w, __fdiv_rn(__fmul_rn(t.learning_rate, g), __fsqrt_rn(__fadd_rn(t.beta, n))));
+}
+
 __device__ __forceinline__ void xf_opt_coord(const XfTableView& t, float g, float& w, float& n, float& z) {
   if (t.opt == XF_OPT_FTRL) xf_ftrl_coord(t, g, w, n, z);
+  else if (t.opt == XF_OPT_ADAGRAD) xf_adagrad_coord(t, g, w, n);
   else xf_sgd_coord(t, g, w);
 }
 
@@ -571,8 +582,11 @@ __device__ __forceinline__ void xf_lazy_mark_open(uint8_t* rowp, uint64_t q1, ui
 // What batch `seq` pulls from a lazy row whose second half is (q2, q3): the weight with the pending optimizer
 // step (the Push of the batch named by the tag, gradient = (float)(residual sum) / rows, lr_worker.cc:116-118)
 // applied.  q2_new = the first word the row gets when it is opened (its state after that step).  Pure.
-__device__ __forceinline__ float xf_lazy_fold(const XfTableView& t, uint64_t q1, uint64_t q2, uint64_t q3, uint32_t seq,
-                                              uint64_t& q2_new) {
+// ADAGRAD: the table's optimizer is AdaGrad; otherwise it is FTRL or SGD, told apart at run time.  The lazy LR step
+// instantiates both, so that its FTRL and SGD code does not carry AdaGrad's branch.
+template <bool ADAGRAD>
+__device__ __forceinline__ float xf_lazy_fold_t(const XfTableView& t, uint64_t q1, uint64_t q2, uint64_t q3, uint32_t seq,
+                                                uint64_t& q2_new) {
   const uint32_t tag = (uint32_t)(q3 & XF_TAG_MASK);
   const bool pending = tag != 0u && tag != seq;
   float g = 0.f;
@@ -584,6 +598,12 @@ __device__ __forceinline__ float xf_lazy_fold(const XfTableView& t, uint64_t q1,
     g = xf_div_rows_plain((float)((double)gfix * xf_pow2(-(int)(rs >> 32))), (double)(uint32_t)rs);
   }
   const float a = __uint_as_float((uint32_t)q2), b = __uint_as_float((uint32_t)(q2 >> 32));
+  if (ADAGRAD) {  // the weight itself and its accumulator
+    float w = a, n = b;
+    if (pending) xf_adagrad_coord(t, g, w, n);
+    q2_new = (uint64_t)__float_as_uint(w) | ((uint64_t)__float_as_uint(n) << 32);
+    return w;
+  }
   if (t.opt == XF_OPT_FTRL) {
     float n = a, z = b;
     float w = xf_lazy_given(q1, q2, q3) ? __uint_as_float((uint32_t)q1) : xf_ftrl_w(t, z, n);
@@ -596,6 +616,11 @@ __device__ __forceinline__ float xf_lazy_fold(const XfTableView& t, uint64_t q1,
   q2_new = (uint64_t)__float_as_uint(w);
   return w;
 }
+__device__ __forceinline__ float xf_lazy_fold(const XfTableView& t, uint64_t q1, uint64_t q2, uint64_t q3, uint32_t seq,
+                                              uint64_t& q2_new) {
+  return t.opt == XF_OPT_ADAGRAD ? xf_lazy_fold_t<true>(t, q1, q2, q3, seq, q2_new)
+                                 : xf_lazy_fold_t<false>(t, q1, q2, q3, seq, q2_new);
+}
 // A raw-loaded head of a lazy row -> the row as the reference's server would hold it right now (pending step
 // applied): canonical fields w, n, z; flags = 0; g = 0.  Every reader outside the step kernels goes through this.
 __device__ __forceinline__ void xf_apply_pending(const XfTableView& t, XfHead& h) {
@@ -607,7 +632,7 @@ __device__ __forceinline__ void xf_apply_pending(const XfTableView& t, XfHead& h
     h.n = __uint_as_float((uint32_t)q2n);
     h.z = __uint_as_float((uint32_t)(q2n >> 32));
   } else {
-    h.n = 0.f;
+    h.n = t.opt == XF_OPT_ADAGRAD ? __uint_as_float((uint32_t)(q2n >> 32)) : 0.f;
     h.z = 0.f;
   }
   h.flags = 0u;
@@ -619,7 +644,8 @@ __device__ __forceinline__ bool xf_lazy_has_pending(const XfHead& raw) { return 
 __device__ __forceinline__ void xf_lazy_store(const XfTableView& t, uint8_t* rowp, const XfHead& h, bool keep_w = false) {
   const bool ftrl = t.opt == XF_OPT_FTRL;
   const uint64_t q2 = ftrl ? ((uint64_t)__float_as_uint(h.n) | ((uint64_t)__float_as_uint(h.z) << 32))
-                           : (uint64_t)__float_as_uint(h.w);
+                    : t.opt == XF_OPT_ADAGRAD ? ((uint64_t)__float_as_uint(h.w) | ((uint64_t)__float_as_uint(h.n) << 32))
+                                              : (uint64_t)__float_as_uint(h.w);
   uint64_t q1 = 0ull;
   if (keep_w && ftrl && __float_as_uint(h.w) != __float_as_uint(xf_ftrl_w(t, h.z, h.n)))
     q1 = (uint64_t)__float_as_uint(h.w) | ((uint64_t)xf_lazy_check(q2) << 32);
